@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py -- ICP registrations/s, 131072-point scan vs 524288-point rolling map, 30 iterations
-(BASELINE.json configs[1]) on N B200s, one independent track per GPU.
+(BASELINE.json configs[1]) on N H100s, independent tracks batched per GPU.
 
 A "step" = one scan-to-local-map registration (LaserTrack::localScanToSubMap -> icp_.compute,
 reference laser_slam/src/laser_track.cpp:466-519) of the next scan of a synthetic HDL-64-shaped sequence.
@@ -9,7 +9,9 @@ reference laser_slam/src/laser_track.cpp:466-519) of the next scan of a syntheti
           from pinned host memory (ls_map_push_scan) and reads the 4x4 result + stats back.
   --impl reference : the reference's CPU algorithm (oracle port: kd-tree 1-NN, nth_element trim,
           point-to-plane) on the host cores -- the reference's own libraries are absent (SURVEY.md §8c).
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR also writes what the last timed step of the resident arm returned
+(every track's final transform, status and ICP statistics) as DIR/<name>.npy, so two builds can be compared output for
+output: the inputs are seeded and identical from run to run for the same arguments.
 """
 import argparse
 import json
@@ -26,7 +28,7 @@ sys.path.insert(0, ROOT)
 
 # BASELINE.json configs[1] (default) and configs[4] (--config 5): scan size, scans per map, ICP iterations, sensor
 WORKLOADS = {
-    2: dict(n_scan=131072, k_map=4, iters=30, sensor=0, pool=24, tracks=74,
+    2: dict(n_scan=131072, k_map=4, iters=30, sensor=0, pool=24, tracks=None,   # None: one track per 4 co-resident CTAs
             name="configs[1]: scan-to-local-map ICP, 131072-pt scan vs 524288-pt rolling map (4 scans), 30 iterations",
             metric="ICP registrations/s (131072-pt scan vs 524288-pt map, 30 iterations)"),
     5: dict(n_scan=262144, k_map=8, iters=50, sensor=1, pool=14, tracks=8,
@@ -51,7 +53,7 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
@@ -238,6 +240,22 @@ def cpu_baseline_sample():
                       f"single-thread (libpointmatcher default): {out[1]:.3f} registrations/s"}
 
 
+def dump_outputs(out_dir, touts, outs):
+    """What ls_icp_register_submap_batch_end hands the caller, per track in track order (the groups are contiguous):
+    T (B,4,4) final transforms, status (B,) per-problem return codes, and the deterministic ICP statistics."""
+    import laser_slam_b200 as ls
+    os.makedirs(out_dir, exist_ok=True)
+    T = np.concatenate([np.stack([ls.from_colmajor(t) for t in tg]) for tg in touts]).astype(np.float32)
+    status = np.concatenate([o[0] for o in outs]).astype(np.float64)
+    stats = [st for o in outs for st in o[1]]
+    arrays = {"T": T, "status": status}
+    for f in ("iterations", "converged", "max_iter_reached", "last_kept", "last_limit", "used_ratio", "grid_cells",
+              "grid_tables", "grid_overflow"):
+        arrays[f] = np.array([getattr(st, f) for st in stats], np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -245,15 +263,21 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours")
     ap.add_argument("--tracks", type=int, default=0, help="independent sequences (tracks) hosted per GPU, batched per "
-                    "launch (default: 74 for config 2 = 4 of the 296 co-resident CTAs each, 8 for config 5)")
+                    "launch (default: config 2 gives each track 4 of the device's co-resident ICP CTAs, i.e. 66 on an "
+                    "H100 SXM, at most 160; config 5 hosts 8)")
     ap.add_argument("--contexts", type=int, default=1,
                     help="device contexts the tracks of a GPU are split over, each with 1/contexts of the co-resident CTAs "
-                         "(experiment: measured on B200, cooperative launches of different contexts do NOT overlap -- 2 contexts "
-                         "run at 0.66x -- so the default is 1)")
+                         "(experiment; the default is 1)")
     ap.add_argument("--config", type=int, default=2, choices=(2, 3, 4, 5),
                     help="BASELINE.json workload: 2 scan-to-map ICP (default, the headline metric), 3 batched trajectories "
                          "feeding the shared estimator, 4 pose-graph solve, 5 dense-sensor stress")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's results (configs 2 and 5) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.config not in (2, 5):
+        ap.error("--dump-outputs is implemented for configs 2 and 5")
     if args.config == 4:
         import bench_posegraph
         return bench_posegraph.main(args)
@@ -261,8 +285,6 @@ def main():
         import bench_trajectory
         return bench_trajectory.main(args)
     wl = select_workload(args.config)
-    if args.tracks <= 0:
-        args.tracks = wl["tracks"]
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -277,9 +299,12 @@ def main():
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    ctx0 = ls.Context(local)
+    if args.tracks <= 0:
+        args.tracks = wl["tracks"] or min(160, ctx0.set_icp_cta_budget(0) // 4)   # 160: most problems per launch
     B = args.tracks
     G = max(1, min(args.contexts, B))
-    ctxs = [ls.Context(local) for _ in range(G)]
+    ctxs = [ctx0] + [ls.Context(local) for _ in range(G - 1)]
     ctx = ctxs[0]
     if G > 1:
         full = ctx.set_icp_cta_budget(0)
@@ -350,12 +375,14 @@ def main():
             prepared[g].append(mps[g].prepare_begin_batch(probs, prm))
     dev_ms, icp_ms = [], []
     last_touts = [None] * G
+    last_out = [None] * G   # (statuses, stats) of each group's most recent launch
 
     def finish(g, s, record):
         rc, statuses, touts, stats = prepared[g][s][1]()
         if rc != 0 or statuses.any():
             raise RuntimeError(f"registration failed rc={rc} {list(statuses)}")
         last_touts[g] = touts.copy()
+        last_out[g] = (statuses.copy(), [stats[b] for b in range(len(members[g]))])
         if world > 1 and g == 0:
             share_pose_delta(ls.from_colmajor(touts[0]))
         if record:
@@ -392,6 +419,8 @@ def main():
     idx, ref = staged[0][n_total - 1][0], staged[0][n_total - 1][1]
     truth_rel = np.linalg.inv(tracks[0][0][ref]) @ tracks[0][0][idx]
     pose_err = float(np.abs(ls.from_colmajor(last_touts[0][0])[:3, 3] - truth_rel[:3, 3]).max())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_touts, last_out)
 
     # parity of what was just timed, outside the clock: one problem of the last batched step against the oracle
     parity = None
@@ -468,6 +497,12 @@ def main():
     barrier()
     t_e2e = time.perf_counter() - t0
     clocks = sampler.summary()
+    # The host layer below opens its own context with B workspaces (hundreds of MB each for config 2): release the C-ABI arms'
+    # rings and workspaces first, so that the two never have to fit the 80 GB of an H100 together.
+    for m in mps + mp2:
+        m.close()
+    for c in ctxs:
+        c.close()
 
     # ------------------------------------------------------------------ the same through the C++ host layer
     # laser_slam::IncrementalEstimator::processPosesAndLaserScans (libls_host.so): what laser_slam_ros would call.  Host
@@ -498,7 +533,7 @@ def main():
                     [nrms[t][idxs[t]].data_ptr() for t in range(B)], [N_SCAN] * B), [pose7(tracks[t][1][idxs[t]]) for t in range(B)]
 
         # the same scans as the C-ABI arm's timed steps: its step s registers scan walk(s + K_MAP + 1)
-        n_host = max(3, min(args.steps, 60))
+        n_host = args.steps
         w_host = args.warmup + K_MAP + 1
         hargs = [host_args(s) for s in range(w_host + n_host + 1)]   # marshalled before the clock, like the C-ABI arm's
 
@@ -540,31 +575,6 @@ def main():
     peak, peak_src = load_peaks()
     t_icp = float(np.mean(icp_ms)) * 1e-3
     t_dev = float(np.mean(dev_ms)) * 1e-3
-    # ncu DRAM bytes of one launch of the same shape (8 registrations per launch has its own capture: eight maps do
-    # not fit L2 together, one does)
-    traffic, traffic_note = None, None
-    import glob
-    import re
-    caps = {}
-    for prof in glob.glob(os.path.join(ROOT, "profiles", f"r2_icp_kernel_cfg{args.config}_batch*_summary.json")):
-        m = re.search(r"_batch(\d+)_summary", prof)
-        if m:
-            caps[int(m.group(1))] = prof
-    if caps:
-        regs = min(caps, key=lambda r: (abs(r - B // G), -r))   # the capture closest in shape to what was timed
-        try:
-            per_launch = float(json.load(open(caps[regs])).get("dram_bytes_per_launch"))
-            fname = os.path.basename(caps[regs])
-            if regs == B // G:
-                traffic = per_launch
-                traffic_note = f"ncu dram__bytes_read+write of one launch with {regs} registration(s) (profiles/{fname})"
-            else:
-                traffic = per_launch * (B // G) / regs
-                traffic_note = (f"no ncu capture with {B // G} registrations per launch: scaled per registration from the capture with "
-                                f"{regs} per launch (profiles/{fname}: {per_launch / 1e9:.2f} GB for {regs}); the working sets "
-                                "of > 3 registrations already exceed L2, so DRAM bytes per registration are flat from there on")
-        except Exception:
-            traffic, traffic_note = None, None
     Bg = B / G   # registrations per launch
     t_step = t_res / args.steps
     # G launches (one per context, B/G registrations and 1/G of the co-resident CTAs each) run side by side, so the device-level
@@ -574,7 +584,6 @@ def main():
                                       f"{Bg:.0f} registrations per launch, {G} launches side by side)",
             "achieved": B * ALG_BYTES_ICP / t_step / 1e9, "peak": peak, "unit": "GB/s",
             "frac": B * ALG_BYTES_ICP / t_step / 1e9 / peak,
-            "traffic": traffic, "traffic_note": traffic_note,
             "peak_source": peak_src, "algorithmic_bytes_per_step": B * ALG_BYTES_ICP, "step_ms": t_step * 1e3,
             "per_launch": {"registrations": Bg, "algorithmic_bytes": Bg * ALG_BYTES_ICP, "kernel_ms": t_icp * 1e3,
                            "achieved": Bg * ALG_BYTES_ICP / t_icp / 1e9, "sm_share": 1.0 / G,

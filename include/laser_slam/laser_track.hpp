@@ -1,5 +1,5 @@
 // LaserTrack -- public interface of reference laser_slam/include/laser_slam/laser_track.hpp:17-236, implemented
-// over the B200 C ABI (include/ls_b200.h): scans live in a device ring (ls_map_*), the scan-to-sub-map ICP is
+// over the C ABI of include/ls_b200.h: scans live in a device ring (ls_map_*), the scan-to-sub-map ICP is
 // ls_icp_register_submap, factors are ls_factor records.
 #ifndef LASER_SLAM_LASER_TRACK_HPP_
 #define LASER_SLAM_LASER_TRACK_HPP_

@@ -1,4 +1,4 @@
-/* ls_b200.h -- C ABI of the B200-native laser_slam hot path (libls_b200.so).
+/* ls_b200.h -- C ABI of the H100-native laser_slam hot path (libls_b200.so).
  *
  * Plain C, plain pointers and sizes; no torch / CUDA types cross this boundary.  Each entry point
  * names the reference interface it replaces (paths relative to the reference repo root).

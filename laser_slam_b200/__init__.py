@@ -1,7 +1,7 @@
-"""laser_slam_b200 -- B200-native scan-to-local-map ICP + pose-graph hot path of ethz-asl/laser_slam.
+"""laser_slam_b200 -- H100-native scan-to-local-map ICP + pose-graph hot path of ethz-asl/laser_slam.
 
 This package is a thin ctypes front-end over the C ABI in include/ls_b200.h (libls_b200.so, built by
-laser_slam_b200/csrc/Makefile for sm_100a).  The compute path is the CUDA library; there is NO CPU
+laser_slam_b200/csrc/Makefile for sm_90a).  The compute path is the CUDA library; there is NO CPU
 fallback: loading fails loudly when the shared library is missing and ls_b200_init fails when no
 CUDA device is usable.
 """
@@ -59,7 +59,7 @@ FACTOR_PRIOR, FACTOR_BETWEEN = 0, 1
 
 
 def build(force=False):
-    """Compile libls_b200.so in-tree (nvcc cross-compiles sm_100a without a GPU)."""
+    """Compile libls_b200.so in-tree (nvcc cross-compiles sm_90a without a GPU)."""
     src_dir = os.path.join(_HERE, "csrc")
     srcs = [os.path.join(src_dir, f) for f in os.listdir(src_dir)] + [os.path.join(_HERE, "..", "include", "ls_b200.h")]
     stale = (not os.path.exists(LIB_PATH)) or os.path.getmtime(LIB_PATH) < max(os.path.getmtime(s) for s in srcs)

@@ -168,9 +168,14 @@ struct Scratch {  // freed on every exit path
   }
 };
 
+// grid-stride kernels: at most 8 CTAs of 256 threads per SM of the current device (set by every entry point)
 inline int blocks(int n) {
-  int b = (n + 255) / 256;
-  return b < 1 ? 1 : (b > 148 * 8 ? 148 * 8 : b);
+  int dev = 0, sms = 1;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      sms < 1)
+    sms = 1;
+  const int b = (n + 255) / 256;
+  return b < 1 ? 1 : (b > sms * 8 ? sms * 8 : b);
 }
 
 #define FCU(call)                              \

@@ -17,7 +17,7 @@
 // every cell is one contiguous range and a row of x-adjacent fine cells is one contiguous candidate run.
 // Why two levels with a wide table (round 1 went through a three-level 4x4x4 design first): the query is
 // latency bound on DEPENDENT loads; top entry -> row entries (all independent) -> candidates is three round
-// trips, where the 4-ary hierarchy needed one more per sub-cell of every level (profiles/r1_history.md).
+// trips, where the 4-ary hierarchy needed one more per sub-cell of every level.
 //
 // Exactness: the query is a ball query around a real candidate (the previous iteration's match, or a seed found
 // by descending the grid), radius sqrt(best).  Loop bounds come from the same monotone float cell-coordinate
@@ -38,8 +38,7 @@
 #include "ls_math.cuh"
 
 #ifndef LS_FB
-#define LS_FB 8  // fine cells per level-0 cell edge (8: 12.5 cm at H0 = 1 m; 16 was measured too: faster warm
-                 // iterations, slower build and cold iteration, 8x the table memory)
+#define LS_FB 8  // fine cells per level-0 cell edge (8: 12.5 cm at H0 = 1 m; 16 costs 8x the table memory)
 #endif
 #define LS_FB3 (LS_FB * LS_FB * LS_FB)
 
@@ -193,8 +192,7 @@ LS_HD float gap(float q, float lo, float hi, float m) {
 
 LS_HD float ball_radius(float best_d2, float margin) { return sqrtf(best_d2) * 1.000001f + margin; }
 
-// The candidate test (for Best: branch-free selects; a data-dependent branch per candidate was measured ~1.6x
-// slower).
+// The candidate test (for Best: branch-free selects rather than a data-dependent branch per candidate).
 LS_HD void Best::offer_pt(float d, const float4& c, int p) { offer(d, f2i(c.w), p); }
 LS_HD void TopK::offer_pt(float dist, const float4& c, int p) { offer(dist, f2i(c.w), p); }
 template <class Acc>
@@ -207,7 +205,6 @@ LS_HD void consider(const float4* pts, int pos, float qx, float qy, float qz, Ac
 }
 
 // candidates are independent loads: issue four before touching any (memory-level parallelism).
-// (A single loop with a predicated tail was measured 1.6x slower than this main loop + scalar tail.)
 template <class Acc>
 LS_HD void scan_range(const float4* pts, uint32_t a, uint32_t e, float qx, float qy, float qz, Acc& b) {
   uint32_t pos = a;

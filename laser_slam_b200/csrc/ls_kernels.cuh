@@ -1,4 +1,4 @@
-// CUDA kernels of the registration hot path (sm_100a).  No tensor cores: there is no dense
+// CUDA kernels of the registration hot path (sm_90a).  No tensor cores: there is no dense
 // contraction on this path; every kernel is an HBM/L2-bound gather, scatter, histogram or reduction.
 //
 //   K0  assemble_kernel      sub-map = concat_p( T_p * scan_p ), exact mean sums, bounding box

@@ -1,4 +1,4 @@
-// IncrementalEstimator over the B200 C ABI.  Control flow follows reference
+// IncrementalEstimator over the ls_b200 C ABI.  Control flow follows reference
 // laser_slam/src/incremental_estimator.cpp (cited per function); gtsam::ISAM2 is replaced by the device pose
 // graph (ls_pg_*): every update runs three Gauss-Newton iterations over the whole graph, mirroring
 // isam2_.update(new) + update() + update() (reference :156-159, :258-262, :272-289).

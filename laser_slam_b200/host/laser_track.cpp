@@ -1,4 +1,4 @@
-// LaserTrack over the B200 C ABI.  Control flow follows reference laser_slam/src/laser_track.cpp (cited per
+// LaserTrack over the ls_b200 C ABI.  Control flow follows reference laser_slam/src/laser_track.cpp (cited per
 // function); the heavy steps call include/ls_b200.h instead of libpointmatcher:
 //   laser_scans_ copies + RigidTransformation::compute + concatenate  ->  ls_map_push_scan / device assembly
 //   icp_.compute                                                       ->  ls_icp_register_submap
