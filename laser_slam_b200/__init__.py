@@ -12,7 +12,7 @@ import subprocess
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("LS_B200_LIB") or os.path.join(_HERE, "_build", "libls_b200.so")  # override: A/B builds
+LIB_PATH = os.path.join(_HERE, "_build", "libls_b200.so")
 _lib = None
 
 LS_OK, LS_ERR_CONVERGENCE = 0, 1

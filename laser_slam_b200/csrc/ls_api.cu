@@ -24,10 +24,7 @@ struct Workspace {
   int n_cap = 0, m_cap = 0, cells_cap = 0, tab_cap = 0, hist_cap = 0;
   BuildArrays A{};
   BuildState* bs = nullptr;
-  float4 *reading = nullptr, *rd = nullptr;               // raw reading (one-shot path), pre-transformed reading
-  float4 *ref_stage = nullptr, *ref_nrm_stage = nullptr;  // one-shot reference staging (scan frame)
-  float* nrm_raw = nullptr;                               // raw normals staging
-  size_t nrm_raw_cap = 0;
+  float4* rd = nullptr;  // pre-transformed reading
   int* pos = nullptr;
   float4 *vq = nullptr, *vpts = nullptr;                   // certified candidate lists (ls_grid.cuh VLists)
   float* d2 = nullptr;
@@ -35,8 +32,6 @@ struct Workspace {
   float* d2_out = nullptr;
   IcpWork* work = nullptr;
   float* T_hist = nullptr;
-  unsigned long long* phase_ns = nullptr;  // debug (LS_PHASE_TIMING=1)
-  float* T0_dev = nullptr;
   BuildJob* job_host = nullptr;  // pinned; this workspace's slot of the context's job array
   BuildJob* job_dev = nullptr;
   IcpWork* h_work = nullptr;  // pinned host mirrors of the small results
@@ -58,6 +53,13 @@ struct ls_ctx {
   BuildJob* jobs_dev = nullptr;      // [kMaxBatch]: workspace b stages its build in slot b
   BuildJob* jobs_host = nullptr;     // pinned
   IcpWork* work_pool = nullptr;      // [kMaxBatch] contiguous, so one memset clears a whole batch
+  // staging of the entry points that take host clouds (used on workspace 0's stream; ensure_staging)
+  float4* reading = nullptr;                               // raw reading
+  float4 *ref_stage = nullptr, *ref_nrm_stage = nullptr;  // reference points and normals (scan frame)
+  int reading_cap = 0, ref_cap = 0;
+  float* nrm_raw = nullptr;                                // raw normals (upload_normals)
+  size_t nrm_raw_cap = 0;
+  float* T0_dev = nullptr;                                 // 16 floats: ls_transform_cloud's transformation
   // query-sharded registration: this GPU's exchange buffer (shard_count slots + the arrival counter) and the peers'
   unsigned char* xbuf = nullptr;
   unsigned char* xpeer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -69,7 +71,6 @@ struct ls_ctx {
   int pending_batch = 0;
   std::vector<int> pending_n;
   std::vector<float> pending_T0;
-  ls_icp_params pending_prm;
   // ring slots (map, slot index) the in-flight batch reads: an asynchronous upload must not overwrite them
   std::vector<std::pair<const ls_map*, int>> pending_slots;
 };
@@ -153,7 +154,6 @@ int ensure_capacity(ls_ctx* ctx, Workspace* w, int n, int m, int max_cells, int 
   if (n > w->n_cap) {
     const int cap = n + n / 8 + 1024;
     int rc;
-    if ((rc = dev_alloc(ctx, &w->reading, (size_t)cap))) return rc;
     if ((rc = dev_alloc(ctx, &w->rd, (size_t)cap))) return rc;
     if ((rc = dev_alloc(ctx, &w->pos, (size_t)cap))) return rc;
     if ((rc = dev_alloc(ctx, &w->d2, (size_t)cap))) return rc;
@@ -174,8 +174,6 @@ int ensure_capacity(ls_ctx* ctx, Workspace* w, int n, int m, int max_cells, int 
     if ((rc = dev_alloc(ctx, &w->A.srt_pts, (size_t)cap))) return rc;
     if ((rc = dev_alloc(ctx, &w->A.srt_nrm, (size_t)cap))) return rc;
     if ((rc = dev_alloc(ctx, &w->A.pkey, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->ref_stage, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->ref_nrm_stage, (size_t)cap))) return rc;
     // a fine table exists only for a level-0 cell with > leaf_split (>= 16) points; the pool is also capped at
     // ~1.5 GB (cells beyond the pool stay leaves: slower, still exact, flagged in stats.grid_overflow)
     int tcap = cap / 17 + 1024;
@@ -207,6 +205,23 @@ int ensure_capacity(ls_ctx* ctx, Workspace* w, int n, int m, int max_cells, int 
     int rc;
     if ((rc = dev_alloc(ctx, &w->T_hist, (size_t)max_iter * 16))) return rc;
     w->hist_cap = max_iter;
+  }
+  return LS_OK;
+}
+
+// The context's staging for a host reading of n points and a host reference of m points, grown like the workspaces.
+int ensure_staging(ls_ctx* ctx, int n, int m) {
+  int rc;
+  if (n > ctx->reading_cap) {
+    const int cap = n + n / 8 + 1024;
+    if ((rc = dev_alloc(ctx, &ctx->reading, (size_t)cap))) return rc;
+    ctx->reading_cap = cap;
+  }
+  if (m > ctx->ref_cap) {
+    const int cap = m + m / 8 + 1024;
+    if ((rc = dev_alloc(ctx, &ctx->ref_stage, (size_t)cap))) return rc;
+    if ((rc = dev_alloc(ctx, &ctx->ref_nrm_stage, (size_t)cap))) return rc;
+    ctx->ref_cap = cap;
   }
   return LS_OK;
 }
@@ -313,20 +328,20 @@ int upload_normals(ls_ctx* ctx, Workspace* w, const float* normals, int stride, 
   // the descriptor block may be addressed at a row offset (normals = descriptors.data() + row, stride = D): the last
   // point's normal ends (n-1)*stride + 3 floats after `normals`, and nothing beyond that may be read
   const size_t need = n > 0 ? (stride <= 8 ? (size_t)(n - 1) * (size_t)stride + 3 : (size_t)n * 3) : 0;
-  if (need > w->nrm_raw_cap) {
+  if (need > ctx->nrm_raw_cap) {
     int rc;
-    if ((rc = dev_alloc(ctx, &w->nrm_raw, need + 4096))) return rc;
-    w->nrm_raw_cap = need + 4096;
+    if ((rc = dev_alloc(ctx, &ctx->nrm_raw, need + 4096))) return rc;
+    ctx->nrm_raw_cap = need + 4096;
   }
   int dstride = stride;
   if (stride <= 8) {
-    CU(cudaMemcpyAsync(w->nrm_raw, normals, need * sizeof(float), cudaMemcpyHostToDevice, w->stream));
+    CU(cudaMemcpyAsync(ctx->nrm_raw, normals, need * sizeof(float), cudaMemcpyHostToDevice, w->stream));
   } else {
-    CU(cudaMemcpy2DAsync(w->nrm_raw, 3 * sizeof(float), normals, (size_t)stride * sizeof(float), 3 * sizeof(float),
+    CU(cudaMemcpy2DAsync(ctx->nrm_raw, 3 * sizeof(float), normals, (size_t)stride * sizeof(float), 3 * sizeof(float),
                          (size_t)n, cudaMemcpyHostToDevice, w->stream));
     dstride = 3;
   }
-  expand_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->nrm_raw, dstride, n, dst);
+  expand_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->nrm_raw, dstride, n, dst);
   LAUNCH_CHECK();
   return LS_OK;
 }
@@ -362,14 +377,7 @@ int fill_problem(ls_ctx* ctx, Workspace* w, const ls_icp_params* prm, int n, con
     w->stream_dirty = true;
   }
   hp.want_matches = want_matches ? 1 : 0;
-  const bool want_phase = getenv("LS_PHASE_TIMING") != nullptr;
-  if (want_phase) {
-    if (w->phase_ns) cudaFree(w->phase_ns);
-    CU(cudaMalloc((void**)&w->phase_ns, (size_t)prm->max_iterations * 6 * sizeof(unsigned long long)));
-    CU(cudaMemsetAsync(w->phase_ns, 0, (size_t)prm->max_iterations * 6 * sizeof(unsigned long long), w->stream));
-    w->stream_dirty = true;
-  }
-  hp.phase_ns = want_phase ? w->phase_ns : nullptr;
+  hp.phase_ns = nullptr;
   std::memcpy(hp.T0, T0, sizeof(hp.T0));
   return LS_OK;
 }
@@ -408,7 +416,6 @@ int launch_icp(ls_ctx* ctx, const ls_icp_params* prm, int batch, int n_max, bool
   if (ctas < 1) ctas = 1;
   const IcpProblem* probs = ctx->probs_dev;
   int dynamic = batch > 1 ? 1 : 0;  // several problems: warps pull work from per-problem counters
-  if (const char* e = getenv("LS_DYNAMIC")) dynamic = atoi(e);  // experiment
   void* args[] = {(void*)&probs, (void*)&ctas, (void*)&dp, (void*)&dynamic};
   if (sharded) {  // narrow the staged problem to this shard's queries (cuts at cell starts, computed on the device)
     shard_slice_kernel<<<1, 32, 0, w0->stream>>>(ctx->probs_dev, w0->job_dev, w0->hp.shard_rank, w0->hp.shard_count);
@@ -430,22 +437,9 @@ int launch_icp(ls_ctx* ctx, const ls_icp_params* prm, int batch, int n_max, bool
 }
 
 // After launch_icp + a synchronise of workspace 0's stream: unpack one problem's results.
-int fetch_icp(ls_ctx* ctx, Workspace* w, const ls_icp_params* prm, int n, const float T0[16], float T_out[16],
-              ls_icp_stats* stats, bool batch_timing = false) {
+int fetch_icp(ls_ctx* ctx, Workspace* w, int n, const float T0[16], float T_out[16], ls_icp_stats* stats,
+              bool batch_timing = false) {
   const IcpWork& wk = *w->h_work;
-  if (getenv("LS_PHASE_TIMING") && w->phase_ns) {
-    std::vector<unsigned long long> ph((size_t)prm->max_iterations * 6);
-    cudaMemcpy(ph.data(), w->phase_ns, ph.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[ls] phase us per iteration: A(nn) B(sel1) C(sel2) D(sel3+acc) E(solve) | total\n");
-    for (int it = 0; it < wk.iterations && it < prm->max_iterations; ++it) {
-      const unsigned long long* q = &ph[(size_t)it * 6];
-      fprintf(stderr, "[ls] it %2d: %8.1f %8.1f %8.1f %8.1f %8.1f | %8.1f\n", it, (q[1] - q[0]) * 1e-3, (q[2] - q[1]) * 1e-3,
-              (q[3] - q[2]) * 1e-3, (q[4] - q[3]) * 1e-3, (q[5] - q[4]) * 1e-3, (q[5] - q[0]) * 1e-3);
-    }
-  }
-  if (getenv("LS_DEBUG"))
-    fprintf(stderr, "[ls] status %d fail_code %d iters %d kept %d limit %g\n", wk.status, wk.fail_code, wk.iterations, wk.last_kept,
-            wk.last_limit);
   std::memcpy(T_out, wk.T_out, 16 * sizeof(float));
   if (stats) {
     std::memset(stats, 0, sizeof(*stats));
@@ -476,7 +470,7 @@ int fetch_icp(ls_ctx* ctx, Workspace* w, const ls_icp_params* prm, int n, const 
 
 // single problem: stage on workspace 0, launch, optional arrays, fetch
 int run_icp(ls_ctx* ctx, const ls_icp_params* prm, const float4* reading_dev, int n, const float T0[16],
-            float T_out[16], ls_icp_stats* stats, int32_t* opt_ids, float* opt_d2, float* opt_T_hist, int m) {
+            float T_out[16], ls_icp_stats* stats, int32_t* opt_ids, float* opt_d2, float* opt_T_hist) {
   Workspace* w = ctx->ws[0];
   int rc;
   if ((rc = prep_icp(ctx, w, prm, reading_dev, n, T0, opt_ids || opt_d2, opt_T_hist != nullptr))) return rc;
@@ -487,8 +481,7 @@ int run_icp(ls_ctx* ctx, const ls_icp_params* prm, const float4* reading_dev, in
     CU(cudaMemcpyAsync(opt_T_hist, w->T_hist, (size_t)prm->max_iterations * 16 * sizeof(float), cudaMemcpyDeviceToHost,
                        w->stream));
   CU(cudaStreamSynchronize(w->stream));
-  (void)m;
-  return fetch_icp(ctx, w, prm, n, T0, T_out, stats);
+  return fetch_icp(ctx, w, n, T0, T_out, stats);
 }
 
 bool is_identity16(const float* T) {
@@ -548,7 +541,6 @@ Workspace* new_workspace(ls_ctx* ctx, int index) {
             cudaEventCreate(&w->ev0) == cudaSuccess && cudaEventCreate(&w->ev1) == cudaSuccess &&
             cudaEventCreate(&w->ev2) == cudaSuccess && cudaEventCreate(&w->ev_launch) == cudaSuccess &&
             cudaMalloc((void**)&w->bs, sizeof(BuildState)) == cudaSuccess &&
-            cudaMalloc((void**)&w->T0_dev, 64 * sizeof(float)) == cudaSuccess &&
             cudaMallocHost((void**)&w->h_work, sizeof(IcpWork)) == cudaSuccess &&
             cudaMallocHost((void**)&w->h_grid, sizeof(Grid)) == cudaSuccess;
   if (!ok) return nullptr;  // partially built workspace is leaked only on an out-of-memory init failure
@@ -558,8 +550,8 @@ void free_workspace(Workspace* w) {
   if (!w) return;
   if (w->stream) cudaStreamSynchronize(w->stream);
   void* bufs[] = {w->A.sub_pts, w->A.sub_nrm, w->A.srt_pts, w->A.srt_nrm, w->A.pkey, w->A.top, w->A.cnt0, w->A.tab1, w->A.cnt1,
-                  w->A.tab1_cell, w->A.pyr, w->A.topmask, w->bs, w->reading, w->rd, w->ref_stage, w->ref_nrm_stage, w->nrm_raw, w->pos, w->d2,
-                  w->ids, w->vq, w->vpts, w->T_hist, w->T0_dev, w->phase_ns, w->d2_out, w->A.qkey, w->A.qperm, w->A.rd_s,
+                  w->A.tab1_cell, w->A.pyr, w->A.topmask, w->bs, w->rd, w->pos, w->d2,
+                  w->ids, w->vq, w->vpts, w->T_hist, w->d2_out, w->A.qkey, w->A.qperm, w->A.rd_s,
                   w->A.qtab_local, w->A.qtab_total, w->A.qtop_start};
   for (void* b : bufs)
     if (b) cudaFree(b);
@@ -609,6 +601,7 @@ int ls_b200_init(int device, ls_ctx** out) {
   if (cudaMalloc((void**)&ctx->jobs_dev, sizeof(BuildJob) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (cudaMallocHost((void**)&ctx->jobs_host, sizeof(BuildJob) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (cudaMalloc((void**)&ctx->work_pool, sizeof(IcpWork) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (cudaMalloc((void**)&ctx->T0_dev, 16 * sizeof(float)) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (ensure_workspaces(ctx, 1) != LS_OK) return bail(LS_ERR_NOMEM);
   *out = ctx;
   return LS_OK;
@@ -623,6 +616,9 @@ void ls_b200_destroy(ls_ctx* ctx) {
   if (ctx->jobs_dev) cudaFree(ctx->jobs_dev);
   if (ctx->jobs_host) cudaFreeHost(ctx->jobs_host);
   if (ctx->work_pool) cudaFree(ctx->work_pool);
+  void* stage[] = {ctx->reading, ctx->ref_stage, ctx->ref_nrm_stage, ctx->nrm_raw, ctx->T0_dev};
+  for (void* b : stage)
+    if (b) cudaFree(b);
   ls_shard_exchange_close(ctx);
   delete ctx;
 }
@@ -673,20 +669,21 @@ int ls_icp_register(ls_ctx* ctx, const ls_icp_params* prm, const float* reading4
   Workspace* w = ctx->ws[0];
   const Resolved r = resolve(prm);
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
+  if ((rc = ensure_staging(ctx, n, m))) return rc;
   CU(cudaEventRecord(w->ev0, w->stream));
-  CU(cudaMemcpyAsync(w->reading, reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemcpyAsync(w->ref_stage, ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  if ((rc = upload_normals(ctx, w, ref_normals, normals_stride, m, w->ref_nrm_stage))) return rc;
+  CU(cudaMemcpyAsync(ctx->reading, reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemcpyAsync(ctx->ref_stage, ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if ((rc = upload_normals(ctx, w, ref_normals, normals_stride, m, ctx->ref_nrm_stage))) return rc;
   Parts parts;
   std::memset(&parts, 0, sizeof(parts));
   parts.n_parts = 1;
   parts.offset[0] = 0;
   parts.offset[1] = m;
-  parts.pts[0] = w->ref_stage;
-  parts.nrm[0] = w->ref_nrm_stage;
+  parts.pts[0] = ctx->ref_stage;
+  parts.nrm[0] = ctx->ref_nrm_stage;
   parts.identity[0] = 1;
   if ((rc = enqueue_build(ctx, w, parts, r, T0))) return rc;
-  return run_icp(ctx, prm, w->reading, n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist, m);
+  return run_icp(ctx, prm, ctx->reading, n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist);
 }
 
 int ls_nn_query(ls_ctx* ctx, const ls_icp_params* prm, const float* reading4, int n, const float* ref4, int m,
@@ -705,18 +702,19 @@ int ls_nn_query(ls_ctx* ctx, const ls_icp_params* prm, const float* reading4, in
   Workspace* w = ctx->ws[0];
   const Resolved r = resolve(prm);
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, 1))) return rc;
-  CU(cudaMemcpyAsync(w->reading, reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemcpyAsync(w->ref_stage, ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemsetAsync(w->ref_nrm_stage, 0, (size_t)m * sizeof(float4), w->stream));
+  if ((rc = ensure_staging(ctx, n, m))) return rc;
+  CU(cudaMemcpyAsync(ctx->reading, reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemcpyAsync(ctx->ref_stage, ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemsetAsync(ctx->ref_nrm_stage, 0, (size_t)m * sizeof(float4), w->stream));
   Parts parts;
   std::memset(&parts, 0, sizeof(parts));
   parts.n_parts = 1;
   parts.offset[1] = m;
-  parts.pts[0] = w->ref_stage;
-  parts.nrm[0] = w->ref_nrm_stage;
+  parts.pts[0] = ctx->ref_stage;
+  parts.nrm[0] = ctx->ref_nrm_stage;
   parts.identity[0] = 1;
   if ((rc = enqueue_build(ctx, w, parts, r, T0))) return rc;
-  w->job_host->reading = w->reading;
+  w->job_host->reading = ctx->reading;
   w->job_host->n = n;
   CU(cudaMemcpyAsync(w->job_dev, w->job_host, sizeof(BuildJob), cudaMemcpyHostToDevice, w->stream));
   reading_kernel<<<dim3(blocks_for(n, 256, ctx->sm_count * 8), 1), 256, 0, w->stream>>>(w->job_dev);
@@ -741,11 +739,12 @@ int ls_transform_cloud(ls_ctx* ctx, const float T[16], const float* in4, const f
   Workspace* w = ctx->ws[0];
   int rc;
   if ((rc = ensure_capacity(ctx, w, n, n, 64, 1))) return rc;
-  CU(cudaMemcpyAsync(w->T0_dev + 16, T, 16 * sizeof(float), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemcpyAsync(w->reading, in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  if (normals && (rc = upload_normals(ctx, w, normals, normals_stride, n, w->ref_nrm_stage))) return rc;
+  if ((rc = ensure_staging(ctx, n, n))) return rc;
+  CU(cudaMemcpyAsync(ctx->T0_dev, T, 16 * sizeof(float), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemcpyAsync(ctx->reading, in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if (normals && (rc = upload_normals(ctx, w, normals, normals_stride, n, ctx->ref_nrm_stage))) return rc;
   transform_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(
-      w->T0_dev + 16, w->reading, normals ? w->ref_nrm_stage : nullptr, n, w->rd, w->A.sub_nrm);
+      ctx->T0_dev, ctx->reading, normals ? ctx->ref_nrm_stage : nullptr, n, w->rd, w->A.sub_nrm);
   LAUNCH_CHECK();
   CU(cudaMemcpyAsync(out4, w->rd, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
   if (normals) {
@@ -949,9 +948,10 @@ int ls_estimate_normals(ls_ctx* ctx, const float* features4, int n, int knn, flo
   Workspace* w = ctx->ws[0];
   int rc;
   if ((rc = ensure_capacity(ctx, w, n, n, 64, 1))) return rc;
-  CU(cudaMemcpyAsync(w->reading, features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  if ((rc = enqueue_normals(ctx, w, w->reading, n, knn, w->ref_nrm_stage))) return rc;
-  pack_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->ref_nrm_stage, n, (float*)w->A.srt_nrm);
+  if ((rc = ensure_staging(ctx, n, n))) return rc;
+  CU(cudaMemcpyAsync(ctx->reading, features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if ((rc = enqueue_normals(ctx, w, ctx->reading, n, knn, ctx->ref_nrm_stage))) return rc;
+  pack_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->ref_nrm_stage, n, (float*)w->A.srt_nrm);
   LAUNCH_CHECK();
   CU(cudaMemcpyAsync(out_normals3, w->A.srt_nrm, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
   CU(cudaStreamSynchronize(w->stream));
@@ -1015,7 +1015,7 @@ int ls_icp_register_submap(ls_ctx* ctx, const ls_icp_params* prm, const ls_map* 
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
   CU(cudaEventRecord(w->ev0, w->stream));
   if ((rc = enqueue_build(ctx, w, parts, r, T0))) return rc;
-  return run_icp(ctx, prm, rs->pts, n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist, m);
+  return run_icp(ctx, prm, rs->pts, n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist);
 }
 
 // ---- query-sharded registration (SURVEY.md 8 e-2) -------------------------------------------------------------
@@ -1130,7 +1130,7 @@ int ls_icp_register_submap_sharded(ls_ctx* ctx, const ls_icp_params* prm, const 
   if ((rc = launch_icp(ctx, prm, 1, 1 << 30, shard_count > 1))) return rc;
   CU(cudaStreamSynchronize(w->stream));
   ctx->xflag_base += w->h_work->xsignals;
-  return fetch_icp(ctx, w, prm, n, T0, T_out, stats);
+  return fetch_icp(ctx, w, n, T0, T_out, stats);
 }
 
 // Sub-map <-> sub-map registration with both clouds assembled on the device (SURVEY.md 8 f2: the loop-closure ICP of
@@ -1159,11 +1159,12 @@ int ls_icp_register_submaps(ls_ctx* ctx, const ls_icp_params* prm, const ls_map*
   if (n == 0 || m == 0) return fail(ctx, LS_ERR_CONVERGENCE, "empty reading or reference");
   const Resolved r = resolve(prm);
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
+  if ((rc = ensure_staging(ctx, n, 0))) return rc;
   CU(cudaEventRecord(w->ev0, w->stream));
-  assemble_points_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(rd, w->reading);
+  assemble_points_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(rd, ctx->reading);
   LAUNCH_CHECK();
   if ((rc = enqueue_build(ctx, w, ref, r, T0))) return rc;
-  return run_icp(ctx, prm, w->reading, n, T0, T_out, stats, nullptr, nullptr, nullptr, m);
+  return run_icp(ctx, prm, ctx->reading, n, T0, T_out, stats, nullptr, nullptr, nullptr);
 }
 
 // Several independent scan -> sub-map registrations in ONE cooperative launch (the multi-robot case: the
@@ -1185,7 +1186,6 @@ int ls_icp_register_submap_batch_begin(ls_ctx* ctx, const ls_icp_params* prm, co
   const Resolved r = resolve(prm);
   ctx->pending_n.assign(batch, 0);
   ctx->pending_T0.assign(T0s, T0s + 16 * (size_t)batch);
-  ctx->pending_prm = *prm;
   ctx->pending_slots.clear();
   // validate every problem before anything is enqueued
   {
@@ -1256,7 +1256,7 @@ int ls_icp_register_submap_batch_end(ls_ctx* ctx, float* T_outs, ls_icp_stats* s
   CU(cudaSetDevice(ctx->device));
   CU(cudaStreamSynchronize(ctx->ws[0]->stream));
   for (int b = 0; b < batch; ++b) {
-    const int st = fetch_icp(ctx, ctx->ws[b], &ctx->pending_prm, ctx->pending_n[b], ctx->pending_T0.data() + 16 * b, T_outs + 16 * b,
+    const int st = fetch_icp(ctx, ctx->ws[b], ctx->pending_n[b], ctx->pending_T0.data() + 16 * b, T_outs + 16 * b,
                              stats ? stats + b : nullptr, true);
     if (st < 0) return st;
     statuses[b] = st;

@@ -37,9 +37,7 @@
 
 #include "ls_math.cuh"
 
-#ifndef LS_FB
-#define LS_FB 8  // fine cells per level-0 cell edge (8: 12.5 cm at H0 = 1 m; 16 costs 8x the table memory)
-#endif
+#define LS_FB 8  // fine cells per level-0 cell edge (12.5 cm at H0 = 1 m); a table's 8x8 rows fill GridView::topmask
 #define LS_FB3 (LS_FB * LS_FB * LS_FB)
 
 namespace ls {
@@ -74,8 +72,8 @@ struct GridView {
   const Entry* tab1;  // fine tables, LS_FB3 entries each (all leaves)
   const float4* pts;  // sorted {x,y,z,idx}
   const unsigned long long* pyr;  // occupancy masks, levels 1..n_pyr
-  // per level-0 cell that owns a fine table: bit (z*LS_FB + y) set iff row (z, y) of the table holds a point (LS_FB == 8:
-  // 64 rows).  Surfaces leave most rows of a table empty; the mask -- fetched together with the cell's entry, same
+  // per level-0 cell that owns a fine table: bit (z*LS_FB + y) set iff row (z, y) of the table holds a point (64
+  // rows).  Surfaces leave most rows of a table empty; the mask -- fetched together with the cell's entry, same
   // index -- lets the ball query skip them without touching their entries.  Meaningless for other cells.
   const unsigned long long* topmask;
 };
@@ -236,9 +234,7 @@ LS_HD void visit_fine(const Grid& g, const Entry* tab, unsigned long long rows, 
     if (gz2 * LS_SHRINK > b.bound()) continue;
     const Entry* row = tab + (z * LS_FB + y0) * LS_FB;
     for (int y = y0; y <= y1; ++y, row += LS_FB) {
-#if LS_FB == 8
       if (!((rows >> (z * LS_FB + y)) & 1ull)) continue;  // empty row
-#endif
       const float gy = gap(qy, cell_lo(loy, y, g.H1), cell_lo(loy, y + 1, g.H1), g.margin);
       const float lb = gy * gy + gz2;
       if (lb * LS_SHRINK > b.bound()) continue;

@@ -22,10 +22,7 @@ namespace ls {
 constexpr int kMaxParts = 16;
 constexpr int kScanTile = 4096;       // level-0 cells per scan block
 constexpr int kScanThreads = 512;
-#ifndef LS_ICP_THREADS
-#define LS_ICP_THREADS 512
-#endif
-constexpr int kIcpThreads = LS_ICP_THREADS;
+constexpr int kIcpThreads = 512;
 constexpr int kIcpCtasPerSm = 1024 / kIcpThreads;
 constexpr int kMaxSmooth = 15;
 constexpr uint32_t kTag1 = 1u << 31, kKeyMask = (1u << 31) - 1u;  // pkey: tag | key (fine keys < 2^31)
@@ -103,7 +100,7 @@ struct alignas(16) IcpWork {
   float last_limit;
   int fail_code;       // 1 no finite match, 2 nothing kept, 3 non-finite solve, 4 NaN in checker, 5 non-finite T
   unsigned int xsignals;  // query-sharded: arrivals this registration consumed from the local exchange flag
-  unsigned int dbg_total, dbg_bin[3], dbg_rem[3];
+  unsigned int dbg_total, dbg_bin[3], dbg_rem[3];  // written by CTA 0 in phase E, read by nothing (see LS_STAMP)
   double dbg_A[6], dbg_x[6];
 };
 
@@ -138,7 +135,7 @@ struct IcpProblem {
   ShardLink link;
   float* T_hist;  // max_iterations*16 floats or null
   int want_matches;  // 1: finish with an uncapped NN pass so ids/d2 hold every point's true match
-  unsigned long long* phase_ns;  // debug: max_iterations*6 globaltimer stamps (CTA 0) or null
+  unsigned long long* phase_ns;  // always null (see LS_STAMP)
   float T0[16];
 };
 
@@ -458,7 +455,7 @@ __global__ void __launch_bounds__(256) tables_kernel(const BuildJob* __restrict_
   BuildState* bs = jobs[blockIdx.y].bs;
   const BuildArrays A = jobs[blockIdx.y].A;
   const int n_tab = min(bs->grid.n_tab1, A.tab_cap);
-  constexpr int per = LS_FB3 / 256;  // 2 (LS_FB 8) or 16 (LS_FB 16) consecutive cells per thread
+  constexpr int per = LS_FB3 / 256;  // 2 consecutive cells per thread
   __shared__ unsigned int ws[8];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int t = blockIdx.x; t < n_tab; t += gridDim.x) {
@@ -490,7 +487,6 @@ __global__ void __launch_bounds__(256) tables_kernel(const BuildJob* __restrict_
       tab[threadIdx.x * per + k] = e;
       run += c[k];
     }
-#if LS_FB == 8
     // non-empty rows: a row is 8 consecutive cells = 4 consecutive threads; warp w covers rows 8w .. 8w+7
     const unsigned int occ = __ballot_sync(0xffffffffu, loc != 0u);
     unsigned int rows8 = 0u;
@@ -505,7 +501,6 @@ __global__ void __launch_bounds__(256) tables_kernel(const BuildJob* __restrict_
       for (int w = 0; w < 8; ++w) m |= (unsigned long long)ws[w] << (8 * w);
       A.topmask[A.tab1_cell[t]] = m;
     }
-#endif
   }
 }
 
@@ -844,6 +839,9 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+// Per-phase globaltimer stamps of CTA 0 into IcpProblem::phase_ns, which the library always sets to null.  Neither these
+// sites nor the IcpWork::dbg_* stores of phase E contribute to the result, but removing them changes icp_kernel's register
+// allocation, and the batched launch then ran about 1% slower (H100 SXM, 700 W power limit, bench.py configs 2 and 5).
 #define LS_STAMP(slot)                                                                   \
   do {                                                                                   \
     if (P.phase_ns && cta == 0 && tid == 0) P.phase_ns[iter * 6 + (slot)] = globaltimer_ns(); \
@@ -1094,17 +1092,10 @@ __device__ __noinline__ long long consume_pairs(const float* recs, int head, int
 
 // Warp-collective (all 32 lanes, converged): lanes with sign != 0 queue the pair (query at s, matched point q at sorted
 // position pos, its normal fetched here).
-template <int site>
 __device__ __forceinline__ void push_pairs(const IcpProblem& P, PairQueue& Q, int sign, float sx, float sy, float sz,
                                            const float4 q, int pos) {
   const unsigned int m = __ballot_sync(0xffffffffu, sign != 0);
   if (m == 0u) return;  // warp-uniform
-#ifdef LS_DEBUG_PAIRS
-  if (sign && (pos < 0 || pos >= P.bs->grid.m)) {
-    printf("[ls] push_pairs: sign %d pos %d site %d block %d thread %d q.w %d\n", sign, pos, site, (int)blockIdx.x, (int)threadIdx.x, __float_as_int(q.w));
-    sign = 0;
-  }
-#endif
   if (sign) {
     float f[6], e;
     residual_terms(sx, sy, sz, q, __ldg(P.nrm + pos), f, e);
@@ -1161,7 +1152,6 @@ __device__ __noinline__ void phase_a_search(const Grid* gp, const IcpProblem* Pp
 
 // Warp-collective: the queries just searched (j < 0: none on this lane) whose match lies inside the accumulation
 // limit queue their pairs.  The match is read back from the query's state, written by this very thread.
-template <int site>
 __device__ __forceinline__ void push_searched(const IcpProblem& P, PairQueue& Q, const float* T_iter, int j, float acc_limit) {
   if (!(acc_limit >= 0.0f)) return;  // uniform: nothing enters the normal equations during phase A
   float d = INFINITY;
@@ -1177,7 +1167,7 @@ __device__ __forceinline__ void push_searched(const IcpProblem& P, PairQueue& Q,
     xform_point(T_iter, r.x, r.y, r.z, sx, sy, sz);
     q = __ldg(P.view.pts + pos);
   }
-  push_pairs<site>(P, Q, keep ? 1 : 0, sx, sy, sz, q, pos);
+  push_pairs(P, Q, keep ? 1 : 0, sx, sy, sz, q, pos);
 }
 
 // After the loop, when the caller asked for correspondences: every point's true (uncapped) match under T.
@@ -1348,7 +1338,7 @@ icp_kernel(const IcpProblem* __restrict__ probs, int ctas_per_problem, IcpParams
           hit = vlist_query(P.lists, P.view.pts, i, v, c0, sx, sy, sz, cap, b, c);
           if (hit) phase_a_record(P, i, b, &hs, pred_bin1, pred_pref12);
         }
-        push_pairs<0>(P, Q, (hit && b.pos >= 0 && b.d2 <= acc_limit) ? 1 : 0, sx, sy, sz, c, b.pos);
+        push_pairs(P, Q, (hit && b.pos >= 0 && b.d2 <= acc_limit) ? 1 : 0, sx, sy, sz, c, b.pos);
         const unsigned int mm = __ballot_sync(0xffffffffu, valid && !hit);
         if (mm) {
           if (valid && !hit) mq[n_miss + __popc(mm & ((1u << lane) - 1u))] = i;
@@ -1359,7 +1349,7 @@ icp_kernel(const IcpProblem* __restrict__ probs, int ctas_per_problem, IcpParams
             const int j = mq[n_miss + lane];
             __syncwarp();
             phase_a_search(&g, &P, T_iter, T_prev, j, cap, &hs, pred_bin1, pred_pref12);
-            push_searched<1>(P, Q, T_iter, j, acc_limit);
+            push_searched(P, Q, T_iter, j, acc_limit);
           }
         }
       }
@@ -1368,7 +1358,7 @@ icp_kernel(const IcpProblem* __restrict__ probs, int ctas_per_problem, IcpParams
         const int j = lane < n_miss ? mq[lane] : -1;
         phase_a_search(&g, &P, T_iter, T_prev, j, cap, &hs, pred_bin1, pred_pref12);
         __syncwarp();
-        push_searched<2>(P, Q, T_iter, j, acc_limit);
+        push_searched(P, Q, T_iter, j, acc_limit);
       }
     }
     drain_pairs(Q, acc_w[tid >> 5]);
@@ -1473,7 +1463,7 @@ icp_kernel(const IcpProblem* __restrict__ probs, int ctas_per_problem, IcpParams
         xform_point(T_iter, r.x, r.y, r.z, sx, sy, sz);
         q = __ldg(P.view.pts + pos);
       }
-      push_pairs<3>(P, Q, sign, sx, sy, sz, q, pos);
+      push_pairs(P, Q, sign, sx, sy, sz, q, pos);
     }
     drain_pairs(Q, acc_w[tid >> 5]);
     flush_slabs(acc_w, X->acc[par]);

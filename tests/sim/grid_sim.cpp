@@ -86,7 +86,7 @@ void build(SimGrid& S, const float* refc3, int m, float cell, int max_cells, int
   for (int c = 0; c < g.n_cells0; ++c)
     if (tabidx0[c] >= 0)
       for (int f = 0; f < LS_FB3; ++f)
-        if (cnt1[(size_t)tabidx0[c] * LS_FB3 + f] > 0 && LS_FB == 8) S.topmask[c] |= 1ull << (f / LS_FB);
+        if (cnt1[(size_t)tabidx0[c] * LS_FB3 + f] > 0) S.topmask[c] |= 1ull << (f / LS_FB);
   // occupancy pyramid
   S.pyr.assign(g.n_pyr_cells, 0ull);
   for (int l = 1; l <= g.n_pyr; ++l) {
