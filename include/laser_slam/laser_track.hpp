@@ -123,6 +123,8 @@ class LaserTrack {
   size_t scanIndexAtTime(const curves::Time& time_ns) const;
   uint64_t residentScan(size_t index) const;  // device id of laser_scans_[index], uploading it if it was evicted
   uint64_t uploadScan(const DataPoints& cloud) const;
+  // the input filters on the device (ls_map_push_scan_filtered) into the ring; *filtered = the slot's cloud, downloaded
+  int pushFiltered(const DataPoints& raw, uint64_t* id, DataPoints* filtered);
   void describeSubMapAroundTime(const curves::Time& time_ns, const unsigned int sub_maps_radius, std::vector<size_t>* scan_indices,
                                 std::vector<PointMatcher::TransformationParameters>* Ts) const;
   void assembleSubMap(const std::vector<size_t>& scan_indices, const std::vector<PointMatcher::TransformationParameters>& Ts,
@@ -139,6 +141,7 @@ class LaserTrack {
   std::map<Time, double> scan_matching_times_;
   LaserTrackParams params_;
   ls_icp_params icp_params_;
+  std::vector<ls_point_filter> input_filters_;  // icp_input_filters_file (reference :24-30); empty: scans are stored as given
   ls_icp_stats last_icp_stats_;
   // device side
   ls_ctx* ctx_ = nullptr;

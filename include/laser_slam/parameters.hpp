@@ -15,7 +15,8 @@ struct LaserTrackParams {
   bool add_m_estimator_on_icp = true;
 
   std::string icp_configuration_file;   // libpointmatcher chain YAML; unreadable -> icp_default.yaml values
-  std::string icp_input_filters_file;   // input filters are upstream of the path here: scans must carry normals
+  std::string icp_input_filters_file;   // DataPointsFilters YAML run on every scan on the device; without a normal filter
+                                        // in it (or without the file) scans must carry normals
   bool use_icp_factors = true;
   bool use_odom_factors = true;
   int nscan_in_sub_map = 4;

@@ -259,6 +259,65 @@ int ls_voxel_grid(int device, const float* in4, int n, const float leaf_size[3],
 int ls_deskew_revolution(int device, const float* points4, const int* packet_offsets, int n_packets, const float* T_packets,
                          const float T_final[16], float* out4);
 
+/* ---- per-scan input filters (reference laser_slam/src/laser_track.cpp:24-30 loads them from
+ * LaserTrackParams::icp_input_filters_file, :81 and :146 apply them to every scan before it is stored) ----------------
+ * A chain is an array of ls_point_filter records applied in order; each filter sees the cloud the previous one produced,
+ * every compaction keeps the input order and normals travel with their points.  The rules (oracle/INPUT_FILTERS.md):
+ *   LS_PF_REMOVE_NAN          drop a point whose x, y or z is NaN (+-inf is left to the distance filters)
+ *   LS_PF_MAX_DIST            dim -1: keep iff (x*x + y*y) + z*z < dist*dist (float32, each operation rounded);
+ *                             dim 0/1/2: keep iff |coord| < dist
+ *   LS_PF_MIN_DIST            the same with >
+ *   LS_PF_BOUNDING_BOX        inside iff box[2a] < coord_a < box[2a+1] on all three axes; keeps the outside points
+ *                             (remove_inside != 0) or the inside ones
+ *   LS_PF_RANDOM_SAMPLING     keep iff ls_keep_point(i, 0x7e11, prob), i = index in the cloud entering the filter
+ *   LS_PF_FIX_STEP_SAMPLING   keep iff i % step == 0
+ *   LS_PF_VOXEL_GRID          ls_voxel_grid's centroids with edge leaf[3]; normals, when present, are averaged the same
+ *                             exact way (not renormalised)
+ *   LS_PF_SURFACE_NORMAL      normals as ls_estimate_normals with knn clamped to [3, 16]
+ *   LS_PF_SAMPLING_SURFACE_NORMAL  the same, then keep iff ls_keep_point(i, 0x5a17, prob) */
+#define LS_PF_REMOVE_NAN 1
+#define LS_PF_MAX_DIST 2
+#define LS_PF_MIN_DIST 3
+#define LS_PF_BOUNDING_BOX 4
+#define LS_PF_RANDOM_SAMPLING 5
+#define LS_PF_FIX_STEP_SAMPLING 6
+#define LS_PF_VOXEL_GRID 7
+#define LS_PF_SURFACE_NORMAL 8
+#define LS_PF_SAMPLING_SURFACE_NORMAL 9
+
+typedef struct ls_point_filter {
+  int32_t type;          /* LS_PF_* */
+  int32_t dim;           /* Max/MinDist: -1 = distance to the origin, 0/1/2 = one axis */
+  int32_t knn;           /* (Sampling)SurfaceNormal */
+  int32_t step;          /* FixStepSampling: startStep */
+  int32_t remove_inside; /* BoundingBox */
+  int32_t reserved;
+  float dist;            /* maxDist / minDist */
+  float prob;            /* RandomSampling: prob; SamplingSurfaceNormal: ratio */
+  float box[6];          /* BoundingBox: xMin, xMax, yMin, yMax, zMin, zMax */
+  float leaf[3];         /* VoxelGrid: vSizeX, vSizeY, vSizeZ */
+  float reserved_f;
+} ls_point_filter;
+
+/* Parse a libpointmatcher DataPointsFilters YAML list (`- NameDataPointsFilter:` followed by `key: value` lines, or
+ * `{key: value, ...}` on the same line).  Host code: needs no GPU.  Absent keys take libpointmatcher's defaults except
+ * knn 10, prob 1 and ratio 1, which keep the values PointMatcher::DataPointsFilters used before (oracle/INPUT_FILTERS.md).  out
+ * may be NULL (count only).  On success *n_out = number of filters.  LS_ERR_ARG for a filter this path does not run
+ * (any other name), a key value it cannot honour (FixStep endStep != startStep or stepMult != 1, VoxelGrid useCentroid 0,
+ * ...) or more filters than `capacity`; *n_out is then the index of the offending filter. */
+int ls_point_filters_from_yaml(const char* yaml_text, ls_point_filter* out, int capacity, int* n_out);
+/* Run a chain on the device: host cloud in (normals through (pointer, stride) as ls_map_push_scan; may be NULL), host
+ * cloud out.  out4 holds up to n points, out_normals3 (may be NULL) 3 floats per point; *n_out = points kept.  Asking
+ * for out_normals3 when neither the input nor a normal filter provides normals returns LS_ERR_ARG. */
+int ls_filter_cloud(ls_ctx* ctx, const ls_point_filter* filters, int n_filters, const float* in4, const float* normals,
+                    int normals_stride, int n, float* out4, float* out_normals3, int* n_out);
+/* Push a raw scan through a chain into the next ring slot: one upload, the whole chain on the device, the result in the
+ * slot (synchronous, like ls_map_push_scan_estimate_normals).  The chain must leave normals (given, or a normal filter)
+ * and at most max_pts_per_scan points; otherwise LS_ERR_ARG and no slot is taken.  A chain that keeps nothing stores an
+ * empty scan (*n_kept 0; registrations against it return LS_ERR_CONVERGENCE). */
+int ls_map_push_scan_filtered(ls_map* map, const ls_point_filter* filters, int n_filters, const float* in4, const float* normals,
+                              int normals_stride, int n, uint64_t* scan_id, int* n_kept);
+
 /* ---- pose graph ------------------------------------------------------------------------------------
  * Replaces gtsam::ISAM2 as IncrementalEstimator uses it (laser_slam/src/incremental_estimator.cpp:17-20,
  * 151-163 estimate, 165-266 estimateAndRemove, 268-291 registerPrior).  Poses are 7 doubles

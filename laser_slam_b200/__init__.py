@@ -58,6 +58,18 @@ class PgStats(ctypes.Structure):
 FACTOR_PRIOR, FACTOR_BETWEEN = 0, 1
 
 
+class PointFilter(ctypes.Structure):
+    """ls_point_filter: one filter of a per-scan input chain (include/ls_b200.h, LS_PF_*)."""
+    _fields_ = [("type", ctypes.c_int32), ("dim", ctypes.c_int32), ("knn", ctypes.c_int32), ("step", ctypes.c_int32),
+                ("remove_inside", ctypes.c_int32), ("reserved", ctypes.c_int32), ("dist", ctypes.c_float),
+                ("prob", ctypes.c_float), ("box", ctypes.c_float * 6), ("leaf", ctypes.c_float * 3),
+                ("reserved_f", ctypes.c_float)]
+
+
+PF_REMOVE_NAN, PF_MAX_DIST, PF_MIN_DIST, PF_BOUNDING_BOX, PF_RANDOM_SAMPLING = 1, 2, 3, 4, 5
+PF_FIX_STEP_SAMPLING, PF_VOXEL_GRID, PF_SURFACE_NORMAL, PF_SAMPLING_SURFACE_NORMAL = 6, 7, 8, 9
+
+
 def build(force=False):
     """Compile libls_b200.so in-tree (nvcc cross-compiles sm_90a without a GPU)."""
     src_dir = os.path.join(_HERE, "csrc")
@@ -135,6 +147,9 @@ def lib():
         L.ls_filter_cylinder.argtypes = [ci, vp, ci, vp, ctypes.c_double, ctypes.c_double, ci, vp, ctypes.POINTER(ci)]
         L.ls_voxel_grid.argtypes = [ci, vp, ci, vp, vp, ctypes.POINTER(ci)]
         L.ls_deskew_revolution.argtypes = [ci, vp, vp, ci, vp, vp, vp]
+        L.ls_point_filters_from_yaml.argtypes = [ctypes.c_char_p, vp, ci, ctypes.POINTER(ci)]
+        L.ls_filter_cloud.argtypes = [vp, vp, ci, vp, vp, ci, ci, vp, vp, ctypes.POINTER(ci)]
+        L.ls_map_push_scan_filtered.argtypes = [vp, vp, ci, vp, vp, ci, ci, ctypes.POINTER(u64), ctypes.POINTER(ci)]
         _lib = L
     return _lib
 
@@ -159,6 +174,28 @@ def keep_mask(n, salt, prob):
     """ls_keep_point for indices 0..n-1: the deterministic RandomSamplingDataPointsFilter rule (host side of the C ABI)."""
     f = lib().ls_keep_point
     return np.fromiter((f(i, salt, prob) for i in range(n)), dtype=bool, count=n)
+
+
+def point_filters_from_yaml(text):
+    """Parse a DataPointsFilters YAML list (LaserTrackParams::icp_input_filters_file) into a chain of PointFilter records
+    (ls_point_filters_from_yaml).  Host code, no GPU needed.  Raises LsError naming the index of a refused filter."""
+    n = ctypes.c_int(0)
+    rc = lib().ls_point_filters_from_yaml(text.encode(), None, 0, ctypes.byref(n))
+    if rc != 0:
+        raise LsError(f"unsupported input filter #{n.value} (rc={rc})")
+    arr = (PointFilter * max(n.value, 1))()
+    rc = lib().ls_point_filters_from_yaml(text.encode(), ctypes.cast(arr, ctypes.c_void_p), n.value, ctypes.byref(n))
+    if rc != 0:
+        raise LsError(f"unsupported input filter #{n.value} (rc={rc})")
+    return list(arr[:n.value])
+
+
+def _chain(filters):
+    if isinstance(filters, str):
+        filters = point_filters_from_yaml(filters)
+    filters = list(filters)
+    arr = (PointFilter * max(len(filters), 1))(*filters)
+    return arr, len(filters)
 
 
 READING_SALT, REFERENCE_SALT = 0x7e11, 0x5a17   # the salts PointMatcher::DataPointsFilters uses (compat.hpp)
@@ -356,6 +393,22 @@ class Context:
         self._check(lib().ls_estimate_normals(self._h, pts4.ctypes.data, pts4.shape[0], knn, out.ctypes.data))
         return out[:pts4.shape[0]]
 
+    def filter_cloud(self, filters, pts4, normals3=None, want_normals=None):
+        """Run a per-scan input chain (PointFilter list or its YAML text) on the device: ls_filter_cloud.  Returns
+        (points (m,4), normals (m,3) or None).  want_normals defaults to: the input has normals or the chain makes them."""
+        arr, nf = _chain(filters)
+        pts4 = _f32c(pts4, 4)
+        n = pts4.shape[0]
+        nrm = None if normals3 is None else _f32c(normals3, 3)
+        if want_normals is None:
+            want_normals = nrm is not None or any(f.type in (PF_SURFACE_NORMAL, PF_SAMPLING_SURFACE_NORMAL) for f in arr[:nf])
+        out = np.empty((max(n, 1), 4), np.float32)
+        nout = np.empty((max(n, 1), 3), np.float32) if want_normals else None
+        m = ctypes.c_int(0)
+        self._check(lib().ls_filter_cloud(self._h, ctypes.cast(arr, ctypes.c_void_p), nf, pts4.ctypes.data, _ptr(nrm), 3, n,
+                                          out.ctypes.data, _ptr(nout), ctypes.byref(m)))
+        return out[:m.value].copy(), (nout[:m.value].copy() if want_normals else None)
+
     def create_map(self, capacity_scans, max_pts_per_scan):
         return Map(self, capacity_scans, max_pts_per_scan)
 
@@ -394,6 +447,17 @@ class Map:
         sid = ctypes.c_uint64(0)
         self.ctx._check(lib().ls_map_push_scan_estimate_normals(self._h, f.ctypes.data, f.shape[0], knn, ctypes.byref(sid)))
         return sid.value
+
+    def push_scan_filtered(self, filters, features4, normals3=None):
+        """ls_map_push_scan_filtered: a raw scan through a per-scan input chain (PointFilter list or its YAML text) into
+        the next slot, all on the device.  Returns (scan id, points kept)."""
+        arr, nf = _chain(filters)
+        f = _f32c(features4, 4)
+        nrm = None if normals3 is None else _f32c(normals3, 3)
+        sid, kept = ctypes.c_uint64(0), ctypes.c_int(0)
+        self.ctx._check(lib().ls_map_push_scan_filtered(self._h, ctypes.cast(arr, ctypes.c_void_p), nf, f.ctypes.data, _ptr(nrm), 3,
+                                                        f.shape[0], ctypes.byref(sid), ctypes.byref(kept)))
+        return sid.value, kept.value
 
     def push_scan_raw(self, feat_ptr, nrm_ptr, nrm_stride, n):
         """Pointer form (e.g. torch pinned tensors' data_ptr()) -- no numpy conversion on the way."""

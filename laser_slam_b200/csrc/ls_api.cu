@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/ls_b200.h"
+#include "ls_filters.cuh"
 #include "ls_kernels.cuh"
 
 using namespace ls;
@@ -73,6 +74,8 @@ struct ls_ctx {
   std::vector<float> pending_T0;
   // ring slots (map, slot index) the in-flight batch reads: an asynchronous upload must not overwrite them
   std::vector<std::pair<const ls_map*, int>> pending_slots;
+  // device scratch of the per-scan input filters (ls_filter_cloud / ls_map_push_scan_filtered)
+  lsf::ChainBuffers chain;
 };
 constexpr int kMaxBatch = 160;
 
@@ -619,6 +622,7 @@ void ls_b200_destroy(ls_ctx* ctx) {
   void* stage[] = {ctx->reading, ctx->ref_stage, ctx->ref_nrm_stage, ctx->nrm_raw, ctx->T0_dev};
   for (void* b : stage)
     if (b) cudaFree(b);
+  lsf::release(ctx->chain);
   ls_shard_exchange_close(ctx);
   delete ctx;
 }
@@ -983,6 +987,144 @@ int ls_map_push_scan_estimate_normals(ls_map* map, const float* features4, int n
   s.id = id;
   s.used = true;
   *scan_id = id;
+  return LS_OK;
+}
+
+// ---- per-scan input filters -----------------------------------------------------------------------------------------
+namespace {
+bool chain_valid(const ls_point_filter* f, int n_filters) {
+  if (n_filters < 0 || (n_filters > 0 && !f)) return false;
+  for (int k = 0; k < n_filters; ++k)
+    if (f[k].type < LS_PF_REMOVE_NAN || f[k].type > LS_PF_SAMPLING_SURFACE_NORMAL) return false;
+  return true;
+}
+bool chain_makes_normals(const ls_point_filter* f, int n_filters) {
+  for (int k = 0; k < n_filters; ++k)
+    if (f[k].type == LS_PF_SURFACE_NORMAL || f[k].type == LS_PF_SAMPLING_SURFACE_NORMAL) return true;
+  return false;
+}
+
+// Upload a host cloud (and its normals) into the chain buffers and run the chain on workspace 0's stream.  On return the
+// result is in ctx->chain.pts[*cur] / nrm[*cur] (normals valid iff *has_nrm), *n_out points; nothing has been copied back
+// but counts.  Runs of mask filters are one flag launch per point-wise run / sampler plus one compaction; the voxel grid
+// and the normals work on the device buffers in place of ls_voxel_grid / ls_estimate_normals' host round trips.
+int run_chain(ls_ctx* ctx, const ls_point_filter* f, int n_filters, const float* in4, const float* normals, int normals_stride,
+              int n, int* cur, bool* has_nrm, int* n_out) {
+  Workspace* w = ctx->ws[0];
+  lsf::ChainBuffers& b = ctx->chain;
+  CU(lsf::reserve(b, n));
+  *cur = 0;
+  *has_nrm = normals != nullptr;
+  *n_out = n;
+  if (n == 0) return LS_OK;
+  int rc;
+  CU(cudaMemcpyAsync(b.pts[0], in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if (normals && (rc = upload_normals(ctx, w, normals, normals_stride, n, b.nrm[0]))) return rc;
+  int k = 0, m = n, c = 0;
+  while (k < n_filters && m > 0) {
+    const ls_point_filter& fk = f[k];
+    if (lsf::is_mask_filter(fk.type)) {
+      int used = 0;
+      CU(lsf::enqueue_mask_run(f + k, n_filters - k, b.pts[c], *has_nrm ? b.nrm[c] : nullptr, m, b.pts[1 - c], b.nrm[1 - c], b,
+                               w->stream, &used, &ctx->launches));
+      CU(cudaMemcpyAsync(&m, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, w->stream));
+      CU(cudaStreamSynchronize(w->stream));
+      c = 1 - c;
+      k += used;
+    } else if (fk.type == LS_PF_VOXEL_GRID) {
+      int v = 0;
+      rc = lsf::enqueue_voxel_grid(b.pts[c], *has_nrm ? b.nrm[c] : nullptr, m, fk.leaf, b.pts[1 - c], b.nrm[1 - c],
+                                   lsf::voxel_buffers(b), w->stream, &v, &ctx->launches);
+      if (rc == LS_ERR_ARG) return fail(ctx, rc, "filter %d: voxel leaf too small for the cloud's extent", k);
+      if (rc) return fail(ctx, rc, "filter %d: voxel grid: %s", k, cudaGetErrorString(cudaGetLastError()));
+      m = v;
+      c = 1 - c;
+      ++k;
+    } else {  // (Sampling)SurfaceNormal: exact k-NN normals of the current cloud, then the sampling of the Sampling variant
+      const int knn = fk.knn < 3 ? 3 : (fk.knn > LS_KNN_MAX ? LS_KNN_MAX : fk.knn);
+      if ((rc = enqueue_normals(ctx, w, b.pts[c], m, knn, b.nrm[c]))) return rc;
+      *has_nrm = true;
+      if (fk.type == LS_PF_SAMPLING_SURFACE_NORMAL && fk.prob < 1.0f) {
+        int used = 0;
+        CU(lsf::enqueue_mask_run(&fk, 1, b.pts[c], b.nrm[c], m, b.pts[1 - c], b.nrm[1 - c], b, w->stream, &used,
+                                 &ctx->launches));
+        CU(cudaMemcpyAsync(&m, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, w->stream));
+        CU(cudaStreamSynchronize(w->stream));
+        c = 1 - c;
+      }
+      ++k;
+    }
+  }
+  for (; k < n_filters; ++k)  // the cloud is empty: a normal filter further on still defines (zero) normals
+    if (f[k].type == LS_PF_SURFACE_NORMAL || f[k].type == LS_PF_SAMPLING_SURFACE_NORMAL) *has_nrm = true;
+  *cur = c;
+  *n_out = m;
+  return LS_OK;
+}
+}  // namespace
+
+int ls_filter_cloud(ls_ctx* ctx, const ls_point_filter* filters, int n_filters, const float* in4, const float* normals,
+                    int normals_stride, int n, float* out4, float* out_normals3, int* n_out) {
+  if (!ctx) return LS_ERR_ARG;
+  BUSY_CHECK(ctx);
+  if (!chain_valid(filters, n_filters) || !in4 || !out4 || !n_out || n < 0 || (normals && normals_stride < 3))
+    return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (out_normals3 && !normals && !chain_makes_normals(filters, n_filters))
+    return fail(ctx, LS_ERR_ARG, "normals requested from a cloud without normals and a chain without a normal filter");
+  *n_out = 0;
+  CU(cudaSetDevice(ctx->device));
+  Workspace* w = ctx->ws[0];
+  int cur = 0, m = 0, rc;
+  bool has_nrm = false;
+  if ((rc = run_chain(ctx, filters, n_filters, in4, normals, normals_stride, n, &cur, &has_nrm, &m))) return rc;
+  if (m > 0) {
+    CU(cudaMemcpyAsync(out4, ctx->chain.pts[cur], (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
+    if (out_normals3) {
+      pack_normals_kernel<<<blocks_for(m, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->chain.nrm[cur], m,
+                                                                                           (float*)ctx->chain.nrm[1 - cur]);
+      LAUNCH_CHECK();
+      CU(cudaMemcpyAsync(out_normals3, ctx->chain.nrm[1 - cur], (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
+    }
+    CU(cudaStreamSynchronize(w->stream));
+  }
+  *n_out = m;
+  return LS_OK;
+}
+
+int ls_map_push_scan_filtered(ls_map* map, const ls_point_filter* filters, int n_filters, const float* in4, const float* normals,
+                              int normals_stride, int n, uint64_t* scan_id, int* n_kept) {
+  if (!map) return LS_ERR_ARG;
+  ls_ctx* ctx = map->ctx;
+  BUSY_CHECK(ctx);
+  if (!chain_valid(filters, n_filters) || !in4 || !scan_id || !n_kept || n < 0 || (normals && normals_stride < 3))
+    return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!normals && !chain_makes_normals(filters, n_filters))
+    return fail(ctx, LS_ERR_ARG, "a scan without normals needs a normal filter in its chain (a slot must serve as a reference)");
+  *n_kept = 0;
+  CU(cudaSetDevice(ctx->device));
+  Workspace* w = ctx->ws[0];
+  int cur = 0, m = 0, rc;
+  bool has_nrm = false;
+  if ((rc = run_chain(ctx, filters, n_filters, in4, normals, normals_stride, n, &cur, &has_nrm, &m))) return rc;
+  if (m > map->max_pts) return fail(ctx, LS_ERR_ARG, "the chain kept %d points, more than a slot holds (%d)", m, map->max_pts);
+  // the batch in flight cannot read the slot this evicts: BUSY_CHECK above; an asynchronous upload into it may still run
+  const uint64_t id = map->next_id++;
+  ls_scan_slot& s = map->slots[id % (uint64_t)map->capacity];
+  s.used = false;
+  if (s.async) {
+    CU(cudaEventSynchronize(s.ready));
+    s.async = false;
+  }
+  if (m > 0) {
+    CU(cudaMemcpyAsync(s.pts, ctx->chain.pts[cur], (size_t)m * sizeof(float4), cudaMemcpyDeviceToDevice, w->stream));
+    CU(cudaMemcpyAsync(s.nrm, ctx->chain.nrm[cur], (size_t)m * sizeof(float4), cudaMemcpyDeviceToDevice, w->stream));
+    CU(cudaStreamSynchronize(w->stream));
+  }
+  s.n = m;
+  s.id = id;
+  s.used = true;
+  *scan_id = id;
+  *n_kept = m;
   return LS_OK;
 }
 

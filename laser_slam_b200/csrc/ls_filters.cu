@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/ls_b200.h"
+#include "ls_filters.cuh"
 
 namespace {
 
@@ -47,10 +48,84 @@ __global__ void cylinder_flag_kernel(const float4* __restrict__ in, int n, doubl
   }
 }
 
-__global__ void compact_kernel(const float4* __restrict__ in, const int* __restrict__ keep, const int* __restrict__ pos, int n,
-                               float4* __restrict__ out) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-    if (keep[i]) out[pos[i]] = in[i];
+// Stable compaction by the exclusive scan `pos` of `keep`; normals (may be NULL) move with their points, and the thread of
+// the last point stores the number kept (count may be NULL).
+__global__ void compact_kernel(const float4* __restrict__ in, const float4* __restrict__ in_nrm, const int* __restrict__ keep,
+                               const int* __restrict__ pos, int n, float4* __restrict__ out, float4* __restrict__ out_nrm,
+                               int* __restrict__ count) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (keep[i]) {
+      out[pos[i]] = in[i];
+      if (in_nrm) out_nrm[pos[i]] = in_nrm[i];
+    }
+    if (count && i == n - 1) *count = pos[i] + keep[i];
+  }
+}
+
+// ---- per-scan input filters (ls_point_filter): one flag kernel per run of point-wise tests, samplers on the rank the
+// preceding exclusive scan gives each point
+constexpr int kMaxPw = 8;
+struct PwOp {
+  int type, dim, remove_inside, pad;
+  float dist;
+  float box[6];
+};
+struct MaskStage {
+  int n_pw;
+  int sampler;  // 0, LS_PF_RANDOM_SAMPLING, LS_PF_FIX_STEP_SAMPLING or LS_PF_SAMPLING_SURFACE_NORMAL
+  float prob;
+  uint32_t salt;
+  int step;
+  PwOp pw[kMaxPw];
+};
+
+// ls_keep_point (ls_yaml.cpp) on the device
+__device__ __forceinline__ bool keep_point_dev(uint32_t index, uint32_t salt, float prob) {
+  if (!(prob < 1.0f)) return true;
+  if (!(prob > 0.0f)) return false;
+  uint32_t h = index * 0x9E3779B1u + salt * 0x85EBCA77u + 0x165667B1u;
+  h ^= h >> 15; h *= 0x2C1B3C6Du;
+  h ^= h >> 12; h *= 0x297A2D39u;
+  h ^= h >> 15;
+  return (double)h < (double)prob * 4294967296.0;
+}
+
+// float32, each operation rounded (the library is built with -fmad=false): fl(fl(fl(x*x) + fl(y*y)) + fl(z*z))
+__device__ __forceinline__ bool pass_pw(const PwOp& o, const float4 p) {
+  if (o.type == LS_PF_REMOVE_NAN) return !(isnan(p.x) || isnan(p.y) || isnan(p.z));
+  if (o.type == LS_PF_MAX_DIST || o.type == LS_PF_MIN_DIST) {
+    float v, lim;
+    if (o.dim < 0) {
+      const float a = p.x * p.x, b = p.y * p.y, c = p.z * p.z;
+      v = a + b;
+      v = v + c;
+      lim = o.dist * o.dist;
+    } else {
+      v = fabsf(o.dim == 0 ? p.x : (o.dim == 1 ? p.y : p.z));
+      lim = o.dist;
+    }
+    return o.type == LS_PF_MAX_DIST ? v < lim : v > lim;
+  }
+  // LS_PF_BOUNDING_BOX: a point on a face is outside
+  const bool inside = o.box[0] < p.x && p.x < o.box[1] && o.box[2] < p.y && p.y < o.box[3] && o.box[4] < p.z && p.z < o.box[5];
+  return o.remove_inside ? !inside : inside;
+}
+
+// keep_out[i] = keep_in[i] (1 if NULL) && sampler(rank[i] (i if NULL)) && every point-wise test.  keep_in may be keep_out.
+__global__ void mask_kernel(const float4* __restrict__ pts, int n, const int* keep_in, const int* __restrict__ rank, MaskStage s,
+                            int* keep_out) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    bool k = keep_in ? keep_in[i] != 0 : true;
+    if (k && s.sampler) {
+      const uint32_t r = rank ? (uint32_t)rank[i] : (uint32_t)i;
+      k = s.sampler == LS_PF_FIX_STEP_SAMPLING ? (r % (uint32_t)s.step) == 0u : keep_point_dev(r, s.salt, s.prob);
+    }
+    if (k && s.n_pw) {
+      const float4 p = pts[i];
+      for (int j = 0; j < s.n_pw; ++j) k = k && pass_pw(s.pw[j], p);
+    }
+    keep_out[i] = k ? 1 : 0;
+  }
 }
 
 // ---- de-skew of one revolution: out = T_final (x) (T_packet (x) p), two float32 transforms in the reference's order
@@ -132,25 +207,38 @@ __global__ void voxel_head_kernel(const unsigned long long* __restrict__ key, in
 }
 
 // slot[i] = inclusive scan of head - 1: every sorted point adds its exact fixed-point coordinates to its voxel
-__global__ void voxel_accumulate_kernel(const float4* __restrict__ in, const unsigned long long* __restrict__ key,
-                                        const int* __restrict__ idx, const int* __restrict__ slot, int n,
-                                        unsigned long long* __restrict__ sums /* 4 per voxel: x, y, z, count */) {
+// Normals (nrm != NULL) are summed the same way into sums[4..6] of a voxel (stride 7 then, 4 without).
+__global__ void voxel_accumulate_kernel(const float4* __restrict__ in, const float4* __restrict__ nrm,
+                                        const unsigned long long* __restrict__ key, const int* __restrict__ idx,
+                                        const int* __restrict__ slot, int n, int stride,
+                                        unsigned long long* __restrict__ sums /* per voxel: x, y, z, count[, nx, ny, nz] */) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     if (key[i] == ~0ull) continue;
     const float4 p = in[idx[i]];
-    unsigned long long* s = sums + 4 * (size_t)(slot[i] - 1);
+    unsigned long long* s = sums + (size_t)stride * (size_t)(slot[i] - 1);
     atomicAdd(&s[0], (unsigned long long)__double2ll_rn((double)p.x * 16777216.0));
     atomicAdd(&s[1], (unsigned long long)__double2ll_rn((double)p.y * 16777216.0));
     atomicAdd(&s[2], (unsigned long long)__double2ll_rn((double)p.z * 16777216.0));
     atomicAdd(&s[3], 1ull);
+    if (nrm) {
+      const float4 q = nrm[idx[i]];
+      atomicAdd(&s[4], (unsigned long long)__double2ll_rn((double)q.x * 16777216.0));
+      atomicAdd(&s[5], (unsigned long long)__double2ll_rn((double)q.y * 16777216.0));
+      atomicAdd(&s[6], (unsigned long long)__double2ll_rn((double)q.z * 16777216.0));
+    }
   }
 }
 
-__global__ void voxel_centroid_kernel(const unsigned long long* __restrict__ sums, int m, float4* __restrict__ out) {
+__global__ void voxel_centroid_kernel(const unsigned long long* __restrict__ sums, int m, int stride, float4* __restrict__ out,
+                                      float4* __restrict__ out_nrm) {
   for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < m; v += gridDim.x * blockDim.x) {
-    const double c = (double)sums[4 * (size_t)v + 3] * 16777216.0;
-    out[v] = make_float4((float)((double)(long long)sums[4 * (size_t)v] / c), (float)((double)(long long)sums[4 * (size_t)v + 1] / c),
-                         (float)((double)(long long)sums[4 * (size_t)v + 2] / c), 1.0f);
+    const unsigned long long* s = sums + (size_t)stride * (size_t)v;
+    const double c = (double)s[3] * 16777216.0;
+    out[v] = make_float4((float)((double)(long long)s[0] / c), (float)((double)(long long)s[1] / c),
+                         (float)((double)(long long)s[2] / c), 1.0f);
+    if (out_nrm)  // mean of the voxel's normals, one rounding, not renormalised
+      out_nrm[v] = make_float4((float)((double)(long long)s[4] / c), (float)((double)(long long)s[5] / c),
+                               (float)((double)(long long)s[6] / c), 0.0f);
   }
 }
 
@@ -229,7 +317,7 @@ int ls_filter_cylinder(int device, const float* in4, int n, const double center[
   void* d_tmp;
   FCU(s.alloc((unsigned char**)&d_tmp, tmp_bytes));
   FCU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_keep, d_pos, n));
-  compact_kernel<<<blocks(n), 256>>>(d_in, d_keep, d_pos, n, d_out);
+  compact_kernel<<<blocks(n), 256>>>(d_in, nullptr, d_keep, d_pos, n, d_out, nullptr, nullptr);
   int last_pos = 0, last_keep = 0;
   FCU(cudaMemcpy(&last_pos, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost));
   FCU(cudaMemcpy(&last_keep, d_keep + (n - 1), sizeof(int), cudaMemcpyDeviceToHost));
@@ -276,50 +364,187 @@ int ls_voxel_grid(int device, const float* in4, int n, const float leaf_size[3],
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return LS_ERR_CUDA;
   FCU(cudaSetDevice(device));
-  const float ix = 1.0f / leaf_size[0], iy = 1.0f / leaf_size[1], iz = 1.0f / leaf_size[2];  // PCL: inverse_leaf_size_
   Scratch s;
   float4 *d_in, *d_out;
-  int *d_mm, *d_idx, *d_idx2, *d_head, *d_slot;
-  unsigned long long *d_key, *d_key2, *d_sums;
+  lsf::VoxelBuffers vb;
   FCU(s.alloc(&d_in, (size_t)n));
   FCU(s.alloc(&d_out, (size_t)n));
-  FCU(s.alloc(&d_mm, 6));
-  FCU(s.alloc(&d_idx, (size_t)n));
-  FCU(s.alloc(&d_idx2, (size_t)n));
-  FCU(s.alloc(&d_head, (size_t)n));
-  FCU(s.alloc(&d_slot, (size_t)n));
-  FCU(s.alloc(&d_key, (size_t)n));
-  FCU(s.alloc(&d_key2, (size_t)n));
+  FCU(s.alloc(&vb.mm, 6));
+  FCU(s.alloc(&vb.idx, (size_t)n));
+  FCU(s.alloc(&vb.idx2, (size_t)n));
+  FCU(s.alloc(&vb.head, (size_t)n));
+  FCU(s.alloc(&vb.slot, (size_t)n));
+  FCU(s.alloc(&vb.key, (size_t)n));
+  FCU(s.alloc(&vb.key2, (size_t)n));
+  FCU(s.alloc(&vb.sums, (size_t)n * 4));
+  vb.tmp_bytes = lsf::voxel_temp_bytes(n);
+  FCU(s.alloc((unsigned char**)&vb.tmp, vb.tmp_bytes));
   FCU(cudaMemcpy(d_in, in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice));
-  const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-  FCU(cudaMemcpy(d_mm, init, sizeof(init), cudaMemcpyHostToDevice));
-  minmax_kernel<<<blocks(n), 256>>>(d_in, n, d_mm, d_mm + 3, ix, iy, iz);
-  int mm[6];
-  FCU(cudaMemcpy(mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost));
-  if (mm[0] > mm[3]) return LS_OK;  // no finite point
-  const double cells = ((double)mm[3] - mm[0] + 1) * ((double)mm[4] - mm[1] + 1) * ((double)mm[5] - mm[2] + 1);
-  if (cells >= 9.0e18) return LS_ERR_ARG;  // PCL: "Leaf size is too small for the input dataset"
-  voxel_key_kernel<<<blocks(n), 256>>>(d_in, n, d_mm, d_mm + 3, ix, iy, iz, d_key, d_idx);
-  size_t tmp_bytes = 0, tmp2 = 0;
-  FCU(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_key, d_key2, d_idx, d_idx2, n));
-  FCU(cub::DeviceScan::InclusiveSum(nullptr, tmp2, d_head, d_slot, n));
-  void* d_tmp;
-  FCU(s.alloc((unsigned char**)&d_tmp, tmp_bytes > tmp2 ? tmp_bytes : tmp2));
-  FCU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_key, d_key2, d_idx, d_idx2, n));  // stable: input order inside a voxel
-  voxel_head_kernel<<<blocks(n), 256>>>(d_key2, n, d_head);
-  FCU(cub::DeviceScan::InclusiveSum(d_tmp, tmp2, d_head, d_slot, n));
+  uint64_t launches = 0;
   int m = 0;
-  FCU(cudaMemcpy(&m, d_slot + (n - 1), sizeof(int), cudaMemcpyDeviceToHost));
-  if (m > 0) {
-    FCU(s.alloc(&d_sums, (size_t)m * 4));
-    FCU(cudaMemset(d_sums, 0, (size_t)m * 4 * sizeof(unsigned long long)));
-    voxel_accumulate_kernel<<<blocks(n), 256>>>(d_in, d_key2, d_idx2, d_slot, n, d_sums);
-    voxel_centroid_kernel<<<blocks(m), 256>>>(d_sums, m, d_out);
-    FCU(cudaMemcpy(out4, d_out, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost));
-  }
-  FCU(cudaGetLastError());
+  const int rc = lsf::enqueue_voxel_grid(d_in, nullptr, n, leaf_size, d_out, nullptr, vb, 0, &m, &launches);
+  if (rc != LS_OK) return rc;
+  if (m > 0) FCU(cudaMemcpy(out4, d_out, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost));
   *n_out = m;
   return LS_OK;
 }
 
 }  // extern "C"
+
+// ---- per-scan input filters: what ls_api.cu enqueues ----------------------------------------------------------------
+namespace lsf {
+
+namespace {
+bool is_pointwise(int type) {
+  return type == LS_PF_REMOVE_NAN || type == LS_PF_MAX_DIST || type == LS_PF_MIN_DIST || type == LS_PF_BOUNDING_BOX;
+}
+size_t scan_temp_bytes(int n) {
+  size_t a = 0, b = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, a, (const int*)nullptr, (int*)nullptr, n);
+  cub::DeviceScan::InclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, n);
+  return a > b ? a : b;
+}
+template <typename T>
+cudaError_t grow(T** p, size_t count) {
+  return cudaMalloc((void**)p, (count ? count : 1) * sizeof(T));
+}
+}  // namespace
+
+bool is_mask_filter(int type) {
+  return is_pointwise(type) || type == LS_PF_RANDOM_SAMPLING || type == LS_PF_FIX_STEP_SAMPLING;
+}
+
+size_t voxel_temp_bytes(int n) {
+  size_t sort = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, sort, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                  (const int*)nullptr, (int*)nullptr, n);
+  const size_t scan = scan_temp_bytes(n);
+  return sort > scan ? sort : scan;
+}
+
+void release(ChainBuffers& b) {
+  void* all[] = {b.pts[0], b.pts[1], b.nrm[0], b.nrm[1], b.keep, b.pos, b.small, b.key, b.key2, b.idx, b.idx2, b.head, b.slot, b.sums, b.tmp};
+  for (void* p : all)
+    if (p) cudaFree(p);
+  b = ChainBuffers();
+}
+
+cudaError_t reserve(ChainBuffers& b, int n) {
+  if (n <= b.cap && b.pts[0]) return cudaSuccess;
+  release(b);
+  const int cap = n + n / 8 + 1024;
+  const size_t c = (size_t)cap;
+  cudaError_t e;
+  if ((e = grow(&b.pts[0], c)) || (e = grow(&b.pts[1], c)) || (e = grow(&b.nrm[0], c)) || (e = grow(&b.nrm[1], c)) ||
+      (e = grow(&b.keep, c)) || (e = grow(&b.pos, c)) || (e = grow(&b.small, 8)) || (e = grow(&b.key, c)) ||
+      (e = grow(&b.key2, c)) || (e = grow(&b.idx, c)) || (e = grow(&b.idx2, c)) || (e = grow(&b.head, c)) ||
+      (e = grow(&b.slot, c)) || (e = grow(&b.sums, 7 * c))) {
+    release(b);
+    return e;
+  }
+  b.tmp_bytes = voxel_temp_bytes(cap);
+  if ((e = grow((unsigned char**)&b.tmp, b.tmp_bytes))) {
+    release(b);
+    return e;
+  }
+  b.cap = cap;
+  return cudaSuccess;
+}
+
+VoxelBuffers voxel_buffers(const ChainBuffers& b) {
+  VoxelBuffers v;
+  v.mm = b.small;
+  v.key = b.key;
+  v.key2 = b.key2;
+  v.sums = b.sums;
+  v.idx = b.idx;
+  v.idx2 = b.idx2;
+  v.head = b.head;
+  v.slot = b.slot;
+  v.tmp = b.tmp;
+  v.tmp_bytes = b.tmp_bytes;
+  return v;
+}
+
+cudaError_t enqueue_mask_run(const ls_point_filter* filters, int n_filters, const float4* pts, const float4* nrm, int n,
+                             float4* out, float4* out_nrm, ChainBuffers& b, cudaStream_t st, int* used, uint64_t* launches) {
+  cudaError_t e;
+  int j = 0;
+  bool have_keep = false;
+  while (j < n_filters && (j == 0 || is_mask_filter(filters[j].type))) {
+    MaskStage s;
+    memset(&s, 0, sizeof(s));
+    const int* rank = nullptr;
+    const int t = filters[j].type;
+    if (!is_pointwise(t)) {  // a sampler: rank of every point in the cloud entering it = exclusive scan of the flags so far
+      if (have_keep) {
+        if ((e = cub::DeviceScan::ExclusiveSum(b.tmp, b.tmp_bytes, b.keep, b.pos, n, st))) return e;
+        rank = b.pos;
+      }
+      s.sampler = t;
+      s.prob = filters[j].prob;
+      s.salt = t == LS_PF_SAMPLING_SURFACE_NORMAL ? 0x5a17u : 0x7e11u;
+      s.step = filters[j].step;
+      ++j;
+    }
+    while (j < n_filters && is_pointwise(filters[j].type) && s.n_pw < kMaxPw) {
+      const ls_point_filter& f = filters[j++];
+      PwOp& o = s.pw[s.n_pw++];
+      o.type = f.type;
+      o.dim = f.dim;
+      o.remove_inside = f.remove_inside;
+      o.dist = f.dist;
+      for (int a = 0; a < 6; ++a) o.box[a] = f.box[a];
+    }
+    mask_kernel<<<blocks(n), 256, 0, st>>>(pts, n, have_keep ? b.keep : nullptr, rank, s, b.keep);
+    ++*launches;
+    if ((e = cudaGetLastError())) return e;
+    have_keep = true;
+  }
+  *used = j;
+  if ((e = cub::DeviceScan::ExclusiveSum(b.tmp, b.tmp_bytes, b.keep, b.pos, n, st))) return e;
+  compact_kernel<<<blocks(n), 256, 0, st>>>(pts, nrm, b.keep, b.pos, n, out, out_nrm, b.small + 6);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+int enqueue_voxel_grid(const float4* in, const float4* in_nrm, int n, const float leaf[3], float4* out, float4* out_nrm,
+                       const VoxelBuffers& b, cudaStream_t st, int* m_out, uint64_t* launches) {
+  *m_out = 0;
+  if (n == 0) return LS_OK;
+  const float ix = 1.0f / leaf[0], iy = 1.0f / leaf[1], iz = 1.0f / leaf[2];  // PCL: inverse_leaf_size_
+  const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+  FCU(cudaMemcpyAsync(b.mm, init, sizeof(init), cudaMemcpyHostToDevice, st));
+  minmax_kernel<<<blocks(n), 256, 0, st>>>(in, n, b.mm, b.mm + 3, ix, iy, iz);
+  ++*launches;
+  int mm[6];
+  FCU(cudaMemcpyAsync(mm, b.mm, sizeof(mm), cudaMemcpyDeviceToHost, st));
+  FCU(cudaStreamSynchronize(st));
+  if (mm[0] > mm[3]) return LS_OK;  // no finite point
+  const double cells = ((double)mm[3] - mm[0] + 1) * ((double)mm[4] - mm[1] + 1) * ((double)mm[5] - mm[2] + 1);
+  if (cells >= 9.0e18) return LS_ERR_ARG;  // PCL: "Leaf size is too small for the input dataset"
+  voxel_key_kernel<<<blocks(n), 256, 0, st>>>(in, n, b.mm, b.mm + 3, ix, iy, iz, b.key, b.idx);
+  ++*launches;
+  size_t bytes = b.tmp_bytes;
+  // stable: input order inside a voxel
+  FCU(cub::DeviceRadixSort::SortPairs(b.tmp, bytes, b.key, b.key2, b.idx, b.idx2, n, 0, (int)sizeof(unsigned long long) * 8, st));
+  voxel_head_kernel<<<blocks(n), 256, 0, st>>>(b.key2, n, b.head);
+  ++*launches;
+  bytes = b.tmp_bytes;
+  FCU(cub::DeviceScan::InclusiveSum(b.tmp, bytes, b.head, b.slot, n, st));
+  int m = 0;
+  FCU(cudaMemcpyAsync(&m, b.slot + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+  FCU(cudaStreamSynchronize(st));
+  if (m > 0) {
+    const int stride = in_nrm ? 7 : 4;
+    FCU(cudaMemsetAsync(b.sums, 0, (size_t)m * stride * sizeof(unsigned long long), st));
+    voxel_accumulate_kernel<<<blocks(n), 256, 0, st>>>(in, in_nrm, b.key2, b.idx2, b.slot, n, stride, b.sums);
+    voxel_centroid_kernel<<<blocks(m), 256, 0, st>>>(b.sums, m, stride, out, in_nrm ? out_nrm : nullptr);
+    *launches += 2;
+  }
+  FCU(cudaGetLastError());
+  *m_out = m;
+  return LS_OK;
+}
+
+}  // namespace lsf

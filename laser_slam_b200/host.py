@@ -21,7 +21,7 @@ def lib():
         L = ctypes.CDLL(LIB_PATH)
         vp, ci, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
         L.lsh_create.restype = vp
-        L.lsh_create.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ctypes.c_char_p, ctypes.c_char_p, ci]
+        L.lsh_create.argtypes = [ci, ci, ci, ci, ci, ci, ci, ci, ctypes.c_char_p, ctypes.c_char_p, ctypes.c_char_p, ci]
         L.lsh_destroy.argtypes = [vp]
         L.lsh_destroy.restype = None
         L.lsh_last_error.argtypes = [vp]
@@ -43,11 +43,15 @@ class Estimator:
     """laser_slam::IncrementalEstimator with n_workers LaserTracks."""
 
     def __init__(self, n_workers=1, nscan_in_sub_map=4, use_icp_factors=True, use_odom_factors=True, robust_icp=True,
-                 device=0, do_icp_step_on_loop_closures=False, loop_closures_sub_maps_radius=2, icp_yaml_path=None):
+                 device=0, do_icp_step_on_loop_closures=False, loop_closures_sub_maps_radius=2, icp_yaml_path=None,
+                 icp_input_filters_path=None):
+        """icp_input_filters_path: a DataPointsFilters YAML list (LaserTrackParams::icp_input_filters_file) every scan
+        goes through on the device before the track stores it."""
         err = ctypes.create_string_buffer(512)
         self._h = lib().lsh_create(n_workers, nscan_in_sub_map, int(use_icp_factors), int(use_odom_factors), int(robust_icp),
                                    device, int(do_icp_step_on_loop_closures), loop_closures_sub_maps_radius,
-                                   icp_yaml_path.encode() if icp_yaml_path else None, err, 512)
+                                   icp_yaml_path.encode() if icp_yaml_path else None,
+                                   icp_input_filters_path.encode() if icp_input_filters_path else None, err, 512)
         if not self._h:
             raise LsError(err.value.decode() or "lsh_create failed")
 
@@ -69,15 +73,16 @@ class Estimator:
             raise LsError(lib().lsh_last_error(self._h).decode())
         return rc
 
-    def step(self, worker, time_ns, pose7, features4, normals3):
-        """One scan callback; returns (icp T_a_b as 7 doubles, IcpStats)."""
+    def step(self, worker, time_ns, pose7, features4, normals3=None):
+        """One scan callback; returns (icp T_a_b as 7 doubles, IcpStats).  normals3=None passes a raw scan (the input
+        filters must then estimate the normals)."""
         f = np.ascontiguousarray(features4, np.float32)
-        nr = np.ascontiguousarray(normals3, np.float32)
+        nr = None if normals3 is None else np.ascontiguousarray(normals3, np.float32)
         p = np.ascontiguousarray(pose7, np.float64)
         out = np.zeros(7, np.float64)
         st = IcpStats()
-        self._check(lib().lsh_step(self._h, worker, int(time_ns), p.ctypes.data, f.ctypes.data, nr.ctypes.data, f.shape[0],
-                                   out.ctypes.data, ctypes.byref(st)))
+        self._check(lib().lsh_step(self._h, worker, int(time_ns), p.ctypes.data, f.ctypes.data,
+                                   None if nr is None else nr.ctypes.data, f.shape[0], out.ctypes.data, ctypes.byref(st)))
         return out, st
 
     def step_batch(self, workers, times_ns, poses7, feat_ptrs, nrm_ptrs, ns, with_estimator=True, views=False):

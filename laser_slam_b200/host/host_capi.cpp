@@ -41,7 +41,8 @@ int guarded(Handle* h, F f) {
 extern "C" {
 
 void* lsh_create(int n_workers, int nscan_in_sub_map, int use_icp_factors, int use_odom_factors, int robust_icp, int device,
-                 int do_icp_step_on_loop_closures, int loop_closures_sub_maps_radius, const char* icp_yaml_path, char* err, int errlen) {
+                 int do_icp_step_on_loop_closures, int loop_closures_sub_maps_radius, const char* icp_yaml_path,
+                 const char* icp_input_filters_path, char* err, int errlen) {
   try {
     EstimatorParams p;
     p.laser_track_params.nscan_in_sub_map = nscan_in_sub_map;
@@ -50,6 +51,7 @@ void* lsh_create(int n_workers, int nscan_in_sub_map, int use_icp_factors, int u
     p.laser_track_params.add_m_estimator_on_icp = robust_icp != 0;
     p.laser_track_params.cuda_device = device;
     p.laser_track_params.icp_configuration_file = icp_yaml_path ? icp_yaml_path : "";
+    p.laser_track_params.icp_input_filters_file = icp_input_filters_path ? icp_input_filters_path : "";
     p.do_icp_step_on_loop_closures = do_icp_step_on_loop_closures != 0;
     p.loop_closures_sub_maps_radius = loop_closures_sub_maps_radius;
     Handle* h = new Handle();
@@ -64,7 +66,8 @@ void* lsh_create(int n_workers, int nscan_in_sub_map, int use_icp_factors, int u
 void lsh_destroy(void* hv) { delete static_cast<Handle*>(hv); }
 const char* lsh_last_error(void* hv) { return static_cast<Handle*>(hv)->err.c_str(); }
 
-// One scan callback.  pose7 = odometry pose T_w (qw,qx,qy,qz,tx,ty,tz).  out_icp7 (may be NULL) receives the ICP
+// One scan callback.  pose7 = odometry pose T_w (qw,qx,qy,qz,tx,ty,tz); normals3 may be NULL (raw scan: the track's
+// input filters must then make the normals).  out_icp7 (may be NULL) receives the ICP
 // T_a_b of this step (identity for the first scan); out_stats (may be NULL) the device-side ICP statistics.
 int lsh_step(void* hv, int worker, int64_t time_ns, const double* pose7, const float* feat4, const float* normals3, int n,
              double* out_icp7, ls_icp_stats* out_stats) {

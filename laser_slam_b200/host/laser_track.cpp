@@ -2,8 +2,10 @@
 // function); the heavy steps call include/ls_b200.h instead of libpointmatcher:
 //   laser_scans_ copies + RigidTransformation::compute + concatenate  ->  ls_map_push_scan / device assembly
 //   icp_.compute                                                       ->  ls_icp_register_submap
-// Scans must arrive with a "normals" descriptor: the reference computes it in its input / reference filters
-// (icp_default.yaml:5-7), which are upstream of this path (SURVEY.md §8 row f1).
+//   input_filters_.apply(scan) (:81, :146)                             ->  ls_map_push_scan_filtered
+// The input filters of icp_input_filters_file run on the device straight into the scan's ring slot; the track keeps the
+// filtered cloud (downloaded once), as the reference stores the filtered scan.  Without filters -- or without a normal
+// filter among them -- scans must arrive with a "normals" descriptor.
 #include "laser_slam/laser_track.hpp"
 
 #include <atomic>
@@ -63,8 +65,15 @@ LaserTrack::LaserTrack(const LaserTrackParams& parameters, unsigned int laser_tr
     icp_params_.smooth_length = 3;
   }
   // reference :24-30 is fatal when the input-filter file cannot be opened; an empty name means "no filters".
-  if (!params_.icp_input_filters_file.empty() && readFile(params_.icp_input_filters_file).empty())
-    throw std::runtime_error("Could not open ICP input filters configuration file.");
+  if (!params_.icp_input_filters_file.empty()) {
+    if (!std::ifstream(params_.icp_input_filters_file.c_str()).good())
+      throw std::runtime_error("Could not open ICP input filters configuration file.");
+    const std::string text = readFile(params_.icp_input_filters_file);
+    int n = 0;
+    if (ls_point_filters_from_yaml(text.c_str(), nullptr, 0, &n) != LS_OK ||
+        (input_filters_.resize((size_t)n), ls_point_filters_from_yaml(text.c_str(), input_filters_.data(), n, &n)) != LS_OK)
+      throw std::runtime_error("unsupported input filter #" + std::to_string(n) + " in " + params_.icp_input_filters_file);
+  }
   // noise models (reference :36-64)
   using namespace gtsam::noiseModel;
   odometry_noise_model_ = Diagonal::Sigmas(params_.odometry_noise_model);
@@ -130,17 +139,26 @@ void LaserTrack::beginPoseAndLaserScan(const Pose& pose, const LaserScan& in_sca
   LS_CHECK(pending != NULL, "null pending");
   *pending = PendingIcp();
   pending->t_start_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-  LS_CHECK(in_scan.scan.descriptorExists("normals"), "scans must carry a 'normals' descriptor");
+  const bool filtered = !input_filters_.empty();
+  auto pf = prefetched_.find(in_scan.time_ns);
+  // the input filters (reference :146) before anything is stored; the normals check comes after them
+  LaserScan stored;
+  uint64_t filtered_id = 0;
+  if (filtered && pf == prefetched_.end()) {
+    stored.time_ns = in_scan.time_ns;
+    stored.key = in_scan.key;
+    throwOnError(ctx_, pushFiltered(in_scan.scan, &filtered_id, &stored.scan), "ls_map_push_scan_filtered");
+  }
+  LS_CHECK(filtered || in_scan.scan.descriptorExists("normals"), "scans must carry a 'normals' descriptor");
   pending->pose = pose;
-  laser_scans_.push_back(in_scan);  // the one copy the track keeps (the reference copies twice, :143 and :197)
+  laser_scans_.push_back(filtered_id ? stored : in_scan);  // the one copy the track keeps (the reference copies twice, :143 and :197)
   LaserScan& scan = laser_scans_.back();
   pose_measurements_.push_back(pose);
-  auto pf = prefetched_.find(scan.time_ns);
+  if (filtered_id) resident_[laser_scans_.size() - 1u] = filtered_id;
   if (pf != prefetched_.end()) {  // already on the device (prefetchLaserScan); share the storage that upload reads from
-    if (*map_p_ && ls_map_scan_size(*map_p_, pf->second.first) >= 0) {
-      scan.scan = pf->second.second.scan;
-      resident_[laser_scans_.size() - 1u] = pf->second.first;
-    }
+    const bool resident = *map_p_ && ls_map_scan_size(*map_p_, pf->second.first) >= 0;
+    if (resident || filtered) scan.scan = pf->second.second.scan;  // a filtered hint holds the chain's output either way
+    if (resident) resident_[laser_scans_.size() - 1u] = pf->second.first;
     prefetched_.erase(pf);
   }
 
@@ -410,14 +428,47 @@ uint64_t LaserTrack::uploadScan(const DataPoints& c) const {
   return id;
 }
 
+// A filtered scan goes through the chain on the device into a fresh slot of the ring; the ring's slots hold a whole raw
+// scan, so the chain's output always fits.  Returns the C ABI's code (LS_ERR_STATE: the context is busy with a batch).
+int LaserTrack::pushFiltered(const DataPoints& raw, uint64_t* id, DataPoints* filtered) {
+  const size_t n = raw.getNbPoints();
+  ensureRing(n);
+  const int off = raw.descriptorOffset("normals");
+  int kept = 0;
+  int rc = ls_map_push_scan_filtered(*map_p_, input_filters_.data(), (int)input_filters_.size(), raw.features.data(),
+                                     off >= 0 ? raw.descriptors.data() + off : NULL, (int)raw.descriptorDim, (int)n, id, &kept);
+  if (rc != LS_OK) return rc;
+  // the track's copy is the slot's cloud, bit for bit (ls_map_assemble of the one scan, identity: copied verbatim)
+  std::vector<float> feat(4 * std::max<size_t>(1, (size_t)kept)), nrm(3 * std::max<size_t>(1, (size_t)kept));
+  const PointMatcher::TransformationParameters I;
+  int m = 0;
+  if (kept > 0 && (rc = ls_map_assemble(ctx_, *map_p_, 1, id, I.data(), feat.data(), nrm.data(), &m)) != LS_OK) return rc;
+  *filtered = DataPoints::fromArrays(feat.data(), nrm.data(), (size_t)m);
+  return LS_OK;
+}
+
 void LaserTrack::prefetchLaserScan(const LaserScan& scan) {
   std::lock_guard<std::recursive_mutex> lock(full_laser_track_mutex_);
-  if (!params_.use_icp_factors || scan.scan.getNbPoints() == 0 || !scan.scan.descriptorExists("normals")) return;
+  const bool filtered = !input_filters_.empty();
+  if (!params_.use_icp_factors || scan.scan.getNbPoints() == 0 || (!filtered && !scan.scan.descriptorExists("normals"))) return;
   if (prefetched_.count(scan.time_ns)) return;
   if (!*map_p_ || (int)scan.scan.getNbPoints() > *map_max_pts_p_) return;  // no ring yet, or it would have to grow: not now
   if (prefetched_.size() >= 2) {  // hints that were never followed up
     ls_map_sync(*map_p_);         // their uploads may still be reading the storage about to be released
     prefetched_.erase(prefetched_.begin());
+  }
+  if (filtered) {
+    // the chain needs the context's workspace: while a batch is in flight (between beginPosesAndLaserScans and
+    // endPosesAndLaserScans) the hint is dropped and the scan is filtered in its own call
+    LaserScan f;
+    f.time_ns = scan.time_ns;
+    f.key = scan.key;
+    uint64_t id = 0;
+    const int rc = pushFiltered(scan.scan, &id, &f.scan);
+    if (rc == LS_ERR_STATE) return;
+    throwOnError(ctx_, rc, "ls_map_push_scan_filtered");
+    prefetched_[scan.time_ns] = std::make_pair(id, f);
+    return;
   }
   std::pair<uint64_t, LaserScan>& slot = prefetched_[scan.time_ns];
   slot.second = scan;  // shares the storage (copy-on-write)
