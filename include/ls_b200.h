@@ -85,7 +85,9 @@ int ls_b200_version(void);
  * default).  Two contexts that each take half of the device run their cooperative launches side by side, so the map build
  * and host-side staging of one overlap the ICP iterations of the other (bench.py drives two such contexts). */
 int ls_b200_set_icp_cta_budget(ls_ctx* ctx, int ctas);
-int ls_b200_icp_cta_budget(const ls_ctx* ctx); /* CTAs the next launch will use at most */
+/* The budget in force.  A launch of B problems gives each max(1, budget / B) CTAs (fewer for a small reading), so it
+ * stays within the budget unless B exceeds it: then every problem still gets one CTA and the launch uses B. */
+int ls_b200_icp_cta_budget(const ls_ctx* ctx);
 /* Number of this library's kernel launches issued on the context so far (bench "gpu_launches"). */
 uint64_t ls_b200_launch_count(const ls_ctx* ctx);
 
@@ -180,7 +182,9 @@ int ls_icp_register_submap(ls_ctx* ctx, const ls_icp_params* prm, const ls_map* 
  * GPU: the reference's n_laser_slam_workers tracks, laser_slam/src/incremental_estimator.cpp:22-26).  Problem b
  * uses reading_ids[b], its n_parts[b] parts follow each other in part_ids / T_parts (16 floats per part),
  * T0s / T_outs hold 16 floats per problem, statuses[b] is LS_OK or LS_ERR_CONVERGENCE (then T_out == T0).
- * Results are bit-identical to separate ls_icp_register_submap calls.  1 <= batch <= 160. */
+ * Results are bit-identical to separate ls_icp_register_submap calls.  1 <= batch <= 160.  A problem whose reading or
+ * sub-map is empty is left out of the launch and gets LS_ERR_CONVERGENCE, T_out == T0 and zeroed stats, as its single
+ * call would; the other problems run unchanged.  If every problem is empty nothing is launched. */
 int ls_icp_register_submap_batch(ls_ctx* ctx, const ls_icp_params* prm, const ls_map* map, int batch,
                                  const uint64_t* reading_ids, const int* n_parts, const uint64_t* part_ids,
                                  const float* T_parts, const float* T0s, float* T_outs, ls_icp_stats* stats,
@@ -314,7 +318,8 @@ int ls_filter_cloud(ls_ctx* ctx, const ls_point_filter* filters, int n_filters, 
 /* Push a raw scan through a chain into the next ring slot: one upload, the whole chain on the device, the result in the
  * slot (synchronous, like ls_map_push_scan_estimate_normals).  The chain must leave normals (given, or a normal filter)
  * and at most max_pts_per_scan points; otherwise LS_ERR_ARG and no slot is taken.  A chain that keeps nothing stores an
- * empty scan (*n_kept 0; registrations against it return LS_ERR_CONVERGENCE). */
+ * empty scan (*n_kept 0; a registration with it as the reading or as its whole sub-map returns LS_ERR_CONVERGENCE,
+ * also as one problem of a batch). */
 int ls_map_push_scan_filtered(ls_map* map, const ls_point_filter* filters, int n_filters, const float* in4, const float* normals,
                               int normals_stride, int n, uint64_t* scan_id, int* n_kept);
 

@@ -70,7 +70,8 @@ struct ls_ctx {
   // a batch between ls_icp_register_submap_batch_begin and _end: the workspaces are busy
   bool pending = false;
   int pending_batch = 0;
-  std::vector<int> pending_n;
+  std::vector<int> pending_ws;  // per problem of the caller: its workspace, or -1 (empty reading or sub-map: not launched)
+  std::vector<int> pending_n;   // per launched problem (workspace order)
   std::vector<float> pending_T0;
   // ring slots (map, slot index) the in-flight batch reads: an asynchronous upload must not overwrite them
   std::vector<std::pair<const ls_map*, int>> pending_slots;
@@ -1314,6 +1315,8 @@ int ls_icp_register_submaps(ls_ctx* ctx, const ls_icp_params* prm, const ls_map*
 // Problem b stages on its own stream (assembly + hash build overlap across problems); the persistent kernel's
 // grid is split into `batch` CTA groups, each with its own barrier, so one problem's barrier / solve latency is
 // filled by the others' search.  Results are bit-identical to `batch` separate ls_icp_register_submap calls.
+// A problem with an empty reading or an empty sub-map is not launched: like the single call it ends in
+// LS_ERR_CONVERGENCE with T_out == T0, and the others run as if it were not there.
 int ls_icp_register_submap_batch_begin(ls_ctx* ctx, const ls_icp_params* prm, const ls_map* map, int batch,
                                        const uint64_t* reading_ids, const int* n_parts, const uint64_t* part_ids,
                                        const float* T_parts, const float* T0s) {
@@ -1324,19 +1327,18 @@ int ls_icp_register_submap_batch_begin(ls_ctx* ctx, const ls_icp_params* prm, co
   int rc = check_params(ctx, prm);
   if (rc) return rc;
   CU(cudaSetDevice(ctx->device));
-  if ((rc = ensure_workspaces(ctx, batch))) return rc;
   const Resolved r = resolve(prm);
-  ctx->pending_n.assign(batch, 0);
+  ctx->pending_ws.assign(batch, -1);
   ctx->pending_T0.assign(T0s, T0s + 16 * (size_t)batch);
   ctx->pending_slots.clear();
-  // validate every problem before anything is enqueued
+  // validate every problem before anything is enqueued; the non-empty ones get workspaces 0.. in the caller's order
+  int launched = 0;
   {
     int po = 0;
     for (int b = 0; b < batch; ++b) {
       if (n_parts[b] < 1 || n_parts[b] > kMaxParts) return fail(ctx, LS_ERR_ARG, "n_parts must be in [1,%d]", kMaxParts);
       const ls_scan_slot* rs = find_slot(map, reading_ids[b]);
       if (!rs) return fail(ctx, LS_ERR_STATE, "reading scan %llu is not resident", (unsigned long long)reading_ids[b]);
-      if (rs->n == 0) return fail(ctx, LS_ERR_ARG, "empty reading in a batch (use the single call)");
       ctx->pending_slots.emplace_back(map, (int)(rs - map->slots.data()));
       long long m = 0;
       for (int p = 0; p < n_parts[b]; ++p) {
@@ -1345,44 +1347,53 @@ int ls_icp_register_submap_batch_begin(ls_ctx* ctx, const ls_icp_params* prm, co
         ctx->pending_slots.emplace_back(map, (int)(s - map->slots.data()));
         m += s->n;
       }
-      if (m == 0) return fail(ctx, LS_ERR_ARG, "empty reference in a batch (use the single call)");
+      if (rs->n > 0 && m > 0) ctx->pending_ws[b] = launched++;
       po += n_parts[b];
     }
   }
+  ctx->pending_n.assign(launched, 0);
+  ctx->pending_batch = batch;
+  if (launched == 0) {  // every problem is empty: nothing to launch, _end reports LS_ERR_CONVERGENCE for each
+    ctx->pending = true;
+    return LS_OK;
+  }
+  if ((rc = ensure_workspaces(ctx, launched))) return rc;
   // stage every problem's job on the host, then ONE upload and ONE launch per build phase for the whole batch
   Workspace* w0 = ctx->ws[0];
   int n_max = 0, m_max = 0, part_off = 0;
   for (int b = 0; b < batch; ++b) {
-    Workspace* w = ctx->ws[b];
+    const int k = ctx->pending_ws[b];
+    const int np = n_parts[b];
+    part_off += np;
+    if (k < 0) continue;
+    Workspace* w = ctx->ws[k];
     const float* T0 = T0s + 16 * b;
     const ls_scan_slot* rs = find_slot(map, reading_ids[b]);
     Parts parts;
-    if ((rc = make_parts(ctx, map, n_parts[b], part_ids + part_off, T_parts + 16 * (size_t)part_off, &parts, w0->stream)))
+    if ((rc = make_parts(ctx, map, np, part_ids + (part_off - np), T_parts + 16 * (size_t)(part_off - np), &parts, w0->stream)))
       return rc;
     if (wait_slot(rs, w0->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
-    part_off += n_parts[b];
-    const int n = rs->n, m = parts.offset[n_parts[b]];
-    ctx->pending_n[b] = n;
+    const int n = rs->n, m = parts.offset[np];
+    ctx->pending_n[k] = n;
     n_max = n > n_max ? n : n_max;
     m_max = m > m_max ? m : m_max;
     if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
     fill_job(w, parts, T0, rs->pts, n);
     if ((rc = fill_problem(ctx, w, prm, n, T0, false, false))) return rc;
   }
-  for (int b = 1; b < batch; ++b) {  // allocation-time clears a workspace enqueued on its own stream come first
-    if (!ctx->ws[b]->stream_dirty) continue;
-    CU(cudaEventRecord(ctx->ws[b]->ev2, ctx->ws[b]->stream));
-    CU(cudaStreamWaitEvent(w0->stream, ctx->ws[b]->ev2, 0));
-    ctx->ws[b]->stream_dirty = false;
+  for (int k = 1; k < launched; ++k) {  // allocation-time clears a workspace enqueued on its own stream come first
+    if (!ctx->ws[k]->stream_dirty) continue;
+    CU(cudaEventRecord(ctx->ws[k]->ev2, ctx->ws[k]->stream));
+    CU(cudaStreamWaitEvent(w0->stream, ctx->ws[k]->ev2, 0));
+    ctx->ws[k]->stream_dirty = false;
   }
   CU(cudaEventRecord(w0->ev0, w0->stream));
-  CU(cudaMemcpyAsync(ctx->jobs_dev, ctx->jobs_host, sizeof(BuildJob) * (size_t)batch, cudaMemcpyHostToDevice, w0->stream));
-  if ((rc = launch_build(ctx, ctx->jobs_dev, batch, m_max, r, w0->stream))) return rc;
-  if ((rc = launch_reading_sort(ctx, ctx->jobs_dev, batch, n_max, r, w0->stream))) return rc;
+  CU(cudaMemcpyAsync(ctx->jobs_dev, ctx->jobs_host, sizeof(BuildJob) * (size_t)launched, cudaMemcpyHostToDevice, w0->stream));
+  if ((rc = launch_build(ctx, ctx->jobs_dev, launched, m_max, r, w0->stream))) return rc;
+  if ((rc = launch_reading_sort(ctx, ctx->jobs_dev, launched, n_max, r, w0->stream))) return rc;
   CU(cudaEventRecord(w0->ev1, w0->stream));
-  CU(cudaMemsetAsync(ctx->work_pool, 0, sizeof(IcpWork) * (size_t)batch, w0->stream));
-  if ((rc = launch_icp(ctx, prm, batch, n_max))) return rc;
-  ctx->pending_batch = batch;
+  CU(cudaMemsetAsync(ctx->work_pool, 0, sizeof(IcpWork) * (size_t)launched, w0->stream));
+  if ((rc = launch_icp(ctx, prm, launched, n_max))) return rc;
   ctx->pending = true;
   return LS_OK;
 }
@@ -1398,7 +1409,13 @@ int ls_icp_register_submap_batch_end(ls_ctx* ctx, float* T_outs, ls_icp_stats* s
   CU(cudaSetDevice(ctx->device));
   CU(cudaStreamSynchronize(ctx->ws[0]->stream));
   for (int b = 0; b < batch; ++b) {
-    const int st = fetch_icp(ctx, ctx->ws[b], ctx->pending_n[b], ctx->pending_T0.data() + 16 * b, T_outs + 16 * b,
+    const int k = ctx->pending_ws[b];
+    if (k < 0) {  // not launched: T_out is already T0
+      if (stats) std::memset(stats + b, 0, sizeof(*stats));
+      statuses[b] = fail(ctx, LS_ERR_CONVERGENCE, "empty reading or reference");
+      continue;
+    }
+    const int st = fetch_icp(ctx, ctx->ws[k], ctx->pending_n[k], ctx->pending_T0.data() + 16 * b, T_outs + 16 * b,
                              stats ? stats + b : nullptr, true);
     if (st < 0) return st;
     statuses[b] = st;
