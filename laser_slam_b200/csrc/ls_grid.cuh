@@ -11,8 +11,8 @@
 //   level 0  dense array of cells of edge H0 over the bounding box                (Entry top[nx*ny*nz])
 //   level 1  a cell holding more than `leaf_split` points owns ONE direct table of LS_FB^3 fine cells of
 //            edge H0/LS_FB (LS_FB = 8: 12.5 cm at H0 = 1 m)
-//   above    occupancy pyramid: 64-bit child masks at edges H0*4^l up to a single root (empty-space skipping
-//            for wide balls, greedy seed for cold queries)
+//   above    occupancy pyramid: 64-bit child masks at edges H0*4^l, at most LS_PYR_LEVELS levels, up to a single
+//            root or a row of top cells (empty-space skipping for wide balls, greedy seed for cold queries)
 // Points are stored sorted by (level-0 cell, fine cell), x fastest, as float4 {x, y, z, original index bits}:
 // every cell is one contiguous range and a row of x-adjacent fine cells is one contiguous candidate run.
 // Why two levels with a wide table (round 1 went through a three-level 4x4x4 design first): the query is
@@ -39,6 +39,10 @@
 
 #define LS_FB 8  // fine cells per level-0 cell edge (12.5 cm at H0 = 1 m); a table's 8x8 rows fill GridView::topmask
 #define LS_FB3 (LS_FB * LS_FB * LS_FB)
+// occupancy pyramid levels above level 0, at most.  A top cell covers 4^7 = 16384 level-0 cells per axis, so the top
+// level of a map longer than that along one axis (up to 2^22 cells: the device caps max_cells there) holds several
+// cells; pyramid_query and seed_query walk all of them.
+#define LS_PYR_LEVELS 7
 
 namespace ls {
 
@@ -60,10 +64,11 @@ struct Grid {
   int n_tab1;
   int overflow;     // set if a table pool was exhausted (cells then stay leaves: slower, still exact)
   // occupancy pyramid above level 0: level l (1..n_pyr) has cells of edge H0*4^l, each a 64-bit mask
-  // of its non-empty 4x4x4 children; the top level is a single cell.
+  // of its non-empty 4x4x4 children; the top level is a single cell unless an axis spans more than 4^LS_PYR_LEVELS
+  // level-0 cells.
   int n_pyr;
-  int pdim[8][3];   // pdim[0] == dim
-  int poff[8];      // offset of level l's masks in GridView::pyr (poff[0] unused)
+  int pdim[LS_PYR_LEVELS + 1][3];   // pdim[0] == dim
+  int poff[LS_PYR_LEVELS + 1];      // offset of level l's masks in GridView::pyr (poff[0] unused)
   int n_pyr_cells;
 };
 
@@ -270,33 +275,39 @@ LS_HD void visit_top_cell(const Grid& g, const GridView& v, int x, int y, int z,
 // 64 cells instead of one entry load per cell) -------------------------------------------------------
 template <class Acc>
 LS_HDN void pyramid_query(const Grid& g, const GridView& v, float qx, float qy, float qz, Acc& b) {
-  int lvl[8], bx[8], by[8], bz[8];
-  unsigned long long mk[8];
-  int sp = 0;
-  lvl[0] = g.n_pyr;
-  bx[0] = by[0] = bz[0] = 0;
-  mk[0] = ld_mask(v.pyr + g.poff[g.n_pyr]);
-  while (sp >= 0) {
-    if (mk[sp] == 0ull) { --sp; continue; }
-    const int bit = ctz64(mk[sp]);
-    mk[sp] &= mk[sp] - 1ull;
-    LS_CNT_STEP();
-    const int cl = lvl[sp] - 1;  // level of the child cell
-    const int cx = bx[sp] + (bit & 3), cy = by[sp] + ((bit >> 2) & 3), cz = bz[sp] + (bit >> 4);
-    const float Hc = g.H0 * (float)(1 << (2 * cl));
-    const float lx = cell_lo(g.org[0], cx, Hc), ly = cell_lo(g.org[1], cy, Hc), lz = cell_lo(g.org[2], cz, Hc);
-    const float gx = gap(qx, lx, cell_lo(g.org[0], cx + 1, Hc), g.margin);
-    const float gy = gap(qy, ly, cell_lo(g.org[1], cy + 1, Hc), g.margin);
-    const float gz = gap(qz, lz, cell_lo(g.org[2], cz + 1, Hc), g.margin);
-    const float lb = gx * gx + (gy * gy + gz * gz);
-    if (lb * LS_SHRINK > b.bound()) continue;
-    if (cl == 0) {
-      visit_top_cell(g, v, cx, cy, cz, lx, ly, lz, qx, qy, qz, b);
-    } else {
-      ++sp;
-      lvl[sp] = cl;
-      bx[sp] = cx * 4; by[sp] = cy * 4; bz[sp] = cz * 4;
-      mk[sp] = ld_mask(v.pyr + g.poff[cl] + ((size_t)cz * g.pdim[cl][1] + cy) * g.pdim[cl][0] + cx);
+  int lvl[LS_PYR_LEVELS + 1], bx[LS_PYR_LEVELS + 1], by[LS_PYR_LEVELS + 1], bz[LS_PYR_LEVELS + 1];
+  unsigned long long mk[LS_PYR_LEVELS + 1];
+  const int* td = g.pdim[g.n_pyr];
+  const int n_top = td[0] * td[1] * td[2];  // 1 unless an axis spans more than 4^LS_PYR_LEVELS level-0 cells
+  for (int t = 0; t < n_top; ++t) {
+    int sp = 0;
+    lvl[0] = g.n_pyr;
+    bx[0] = (t % td[0]) * 4;
+    by[0] = ((t / td[0]) % td[1]) * 4;
+    bz[0] = (t / (td[0] * td[1])) * 4;
+    mk[0] = ld_mask(v.pyr + g.poff[g.n_pyr] + t);
+    while (sp >= 0) {
+      if (mk[sp] == 0ull) { --sp; continue; }
+      const int bit = ctz64(mk[sp]);
+      mk[sp] &= mk[sp] - 1ull;
+      LS_CNT_STEP();
+      const int cl = lvl[sp] - 1;  // level of the child cell
+      const int cx = bx[sp] + (bit & 3), cy = by[sp] + ((bit >> 2) & 3), cz = bz[sp] + (bit >> 4);
+      const float Hc = g.H0 * (float)(1 << (2 * cl));
+      const float lx = cell_lo(g.org[0], cx, Hc), ly = cell_lo(g.org[1], cy, Hc), lz = cell_lo(g.org[2], cz, Hc);
+      const float gx = gap(qx, lx, cell_lo(g.org[0], cx + 1, Hc), g.margin);
+      const float gy = gap(qy, ly, cell_lo(g.org[1], cy + 1, Hc), g.margin);
+      const float gz = gap(qz, lz, cell_lo(g.org[2], cz + 1, Hc), g.margin);
+      const float lb = gx * gx + (gy * gy + gz * gz);
+      if (lb * LS_SHRINK > b.bound()) continue;
+      if (cl == 0) {
+        visit_top_cell(g, v, cx, cy, cz, lx, ly, lz, qx, qy, qz, b);
+      } else {
+        ++sp;
+        lvl[sp] = cl;
+        bx[sp] = cx * 4; by[sp] = cy * 4; bz[sp] = cz * 4;
+        mk[sp] = ld_mask(v.pyr + g.poff[cl] + ((size_t)cz * g.pdim[cl][1] + cy) * g.pdim[cl][0] + cx);
+      }
     }
   }
 }
@@ -343,6 +354,21 @@ LS_HDN void seed_query(const Grid& g, const GridView& v, float qx, float qy, flo
     // empty level-0 cell: greedy descent of the occupancy pyramid towards the nearest occupied child
     // at every level; the first point of the level-0 cell reached is a real (if loose) candidate.
     int X = 0, Y = 0, Z = 0;
+    const int* td = g.pdim[g.n_pyr];
+    const int n_top = td[0] * td[1] * td[2];
+    if (n_top > 1) {  // several top cells (an axis spans more than 4^LS_PYR_LEVELS cells): start in the nearest occupied one
+      const float Ht = g.H0 * (float)(1 << (2 * g.n_pyr));
+      float best_lb = INFINITY;
+      for (int t = 0; t < n_top; ++t) {
+        if (ld_mask(v.pyr + g.poff[g.n_pyr] + t) == 0ull) continue;
+        const int tx = t % td[0], ty = (t / td[0]) % td[1], tz = t / (td[0] * td[1]);
+        const float gx = gap(qx, cell_lo(g.org[0], tx, Ht), cell_lo(g.org[0], tx + 1, Ht), 0.f);
+        const float gy = gap(qy, cell_lo(g.org[1], ty, Ht), cell_lo(g.org[1], ty + 1, Ht), 0.f);
+        const float gz = gap(qz, cell_lo(g.org[2], tz, Ht), cell_lo(g.org[2], tz + 1, Ht), 0.f);
+        const float lb = gx * gx + (gy * gy + gz * gz);
+        if (lb < best_lb) { best_lb = lb; X = tx; Y = ty; Z = tz; }
+      }
+    }
     for (int l = g.n_pyr; l >= 1; --l) {
       unsigned long long mask = ld_mask(v.pyr + g.poff[l] + ((size_t)Z * g.pdim[l][1] + Y) * g.pdim[l][0] + X);
       const float Hc = g.H0 * (float)(1 << (2 * (l - 1)));
@@ -574,10 +600,13 @@ LS_HDN void grid_setup(Grid& g, const float* lo, const float* hi, float cell_siz
     emax = fmaxf(emax, ext[a]);
     oabs = fmaxf(oabs, fmaxf(fabsf(lo[a]), fabsf(hi[a])));
   }
-  // grow H (powers of two) until the dense level-0 array fits the budget
+  // grow H (powers of two) until the dense level-0 array fits the budget.  The cells are counted with the float
+  // expression that sets `dim` below, so n_cells0 <= max_cells holds exactly (for a cell size that is not a power of
+  // two, floor(ext / H) in double can be one less than floorf(ext * (1 / H)) in float).
   for (int it = 0; it < 40; ++it) {
+    const float inv = 1.0f / H;
     double cells = 1.0;
-    for (int a = 0; a < 3; ++a) cells *= floor((double)ext[a] / (double)H) + 1.0;
+    for (int a = 0; a < 3; ++a) cells *= (double)floorf(ext[a] * inv) + 1.0;
     if (cells <= (double)max_cells) break;
     H = H * 2.0f;
   }
@@ -607,7 +636,7 @@ LS_HDN void grid_setup(Grid& g, const float* lo, const float* hi, float cell_siz
     for (int a = 0; a < 3; ++a) g.pdim[l][a] = (g.pdim[l - 1][a] + 3) / 4;
     g.poff[l] = off;
     off += g.pdim[l][0] * g.pdim[l][1] * g.pdim[l][2];
-  } while ((g.pdim[l][0] > 1 || g.pdim[l][1] > 1 || g.pdim[l][2] > 1) && l < 7);
+  } while ((g.pdim[l][0] > 1 || g.pdim[l][1] > 1 || g.pdim[l][2] > 1) && l < LS_PYR_LEVELS);
   g.n_pyr = l;
   g.n_pyr_cells = off;
 }

@@ -146,6 +146,49 @@ void sim_nn(const float* q3, int n, const float* refc3, int m, float cell, int m
   }
 }
 
+// The geometry grid_setup derives from a centred bounding box [lo, hi]: H0 (and the m/leaf_split it is given) go to
+// H0_out; out (int32) = dim[3], n_cells0, n_pyr, n_pyr_cells, then pdim[l][3] and poff[l] for l = 0..L, where L (the
+// return value) is the deepest pyramid level Grid has room for.
+int sim_grid(const float* lo, const float* hi, float cell, int max_cells, int split, int m, float* H0_out,
+             int32_t* out) {
+  ls::Grid g;
+  ls::grid_setup(g, lo, hi, cell, max_cells, split, m);
+  const int levels = (int)(sizeof(g.pdim) / sizeof(g.pdim[0])) - 1;
+  *H0_out = g.H0;
+  int k = 0;
+  for (int a = 0; a < 3; ++a) out[k++] = g.dim[a];
+  out[k++] = g.n_cells0;
+  out[k++] = g.n_pyr;
+  out[k++] = g.n_pyr_cells;
+  for (int l = 0; l <= levels; ++l) {
+    for (int a = 0; a < 3; ++a) out[k++] = l <= g.n_pyr ? g.pdim[l][a] : 0;
+    out[k++] = l <= g.n_pyr ? g.poff[l] : 0;
+  }
+  return levels;
+}
+
+// Exact K nearest neighbours (knn_search, the normals' query) of n queries over the centred reference: ids/d2 are n x k,
+// ascending by (d2, index); a map with fewer than k points leaves INT_MAX / +inf in the tail.  stats as sim_nn.
+void sim_knn(const float* q3, int n, const float* refc3, int m, float cell, int max_cells, int split, int k,
+             int32_t* ids, float* d2, double* stats) {
+  SimGrid S;
+  build(S, refc3, m, cell, max_cells, split);
+  ls::GridView v{S.top.data(), S.tab1.data(), S.pts.data(), S.pyr.data(), S.topmask.data()};
+  for (int i = 0; i < n; ++i) {
+    ls::TopK t;
+    ls::knn_search(S.g, v, q3[3 * i], q3[3 * i + 1], q3[3 * i + 2], k, t);
+    for (int j = 0; j < k; ++j) {
+      ids[(size_t)i * k + j] = t.id[j];
+      d2[(size_t)i * k + j] = t.d[j];
+    }
+  }
+  if (stats) {
+    stats[3] = S.g.n_tab1;
+    stats[4] = S.g.H0;
+    stats[5] = S.g.n_cells0;
+  }
+}
+
 // Certified candidate lists over a sequence of poses: queries rd3 (n x 3) are moved by T_seq[t] (column-major 4x4,
 // n_iter of them); iteration t answers every query through vlist_query when its certificate holds and through
 // nn_search (+ vlist_build) otherwise, exactly as the ICP kernel's phase A does, and checks each answer against
