@@ -106,6 +106,10 @@ class LaserTrack {
   const RelativePoseVector& getIcpTransformations() const { return icp_transformations_; }
   const ls_icp_stats& getLastIcpStats() const { return last_icp_stats_; }
   ls_ctx* context() const { return ctx_; }
+  // (new) the device copy of the scan at time_ns (scanIndexAtTime): its id in ring(), uploaded again if it was evicted.
+  // What a resident local map (include/laser_slam/local_map.hpp) reads instead of the host cloud.
+  uint64_t residentScanAtTime(const curves::Time& time_ns) const;
+  const ls_map* ring() const { return *map_p_; }
   unsigned int id() const { return laser_track_id_; }
 
  private:
@@ -116,7 +120,7 @@ class LaserTrack {
   gtsam::ExpressionFactor<SE3> makeMeasurementFactor(const Pose& pose_measurement, gtsam::noiseModel::Base::shared_ptr noise_model) const;
   void stageLocalScanToSubMap(PendingIcp* pending);
   void finishLocalScanToSubMap(const PendingIcp& pending, int rc, const float* T_out16);
-  void ensureRing(size_t max_pts);
+  void ensureRing(size_t max_pts) const;  // the ring is a device cache of laser_scans_ (reached through map_p_)
   const Pose& findPose(const Time& timestamp_ns) const;
   Pose& findPose(const Time& timestamp_ns);
   Key extendTrajectory(const Time& timestamp_ns, const SE3& value);

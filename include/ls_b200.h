@@ -263,6 +263,64 @@ int ls_voxel_grid(int device, const float* in4, int n, const float leaf_size[3],
 int ls_deskew_revolution(int device, const float* points4, const int* packet_offsets, int n_packets, const float* T_packets,
                          const float T_final[16], float* out4);
 
+/* ---- resident local map: the map maintenance of LaserSlamWorker (laser_slam_ros/src/laser_slam_worker.cpp) ------------
+ * The worker's local_map_, local_map_filtered_, distant_map_ and local_map_queue_ kept on the device next to a ring, so the
+ * scans reach the map and the map reaches the filters without crossing PCIe.  Only counts return to the host until a
+ * cloud is downloaded.  The rules (oracle/LOCAL_MAP.md):
+ *   ls_local_map_add_scan    scanCallback (:195-246): the slot's scan moved by T_w_scan (float32, the ls_map_assemble
+ *                            arithmetic; an exact identity copies it verbatim); with remove_ground_from_local_map a point is
+ *                            kept iff (double)z > robot_z - ground_distance_to_robot_center_m; input order kept; the cloud is
+ *                            appended to LOCAL and queued as one cloud, unless nothing is left (then neither)
+ *   ls_local_map_filter      getFilteredMap (:415-488): snapshot = LOCAL; LOCAL := the snapshot inside the cylinder around
+ *                            `center` of radius distance_to_consider_fixed and height 40 (ls_filter_cylinder's <= rule);
+ *                            with separate_distant_map, v = voxel grid of the SNAPSHOT (ls_voxel_grid's rule, voxels with
+ *                            fewer than minimum_point_number_per_voxel points dropped), LOCAL_FILTERED := inside(v) (<=),
+ *                            DISTANT += outside(v) (>=; a centroid on the boundary lands in both), FILTERED_MAP =
+ *                            LOCAL_FILTERED ++ DISTANT; without it FILTERED_MAP = the snapshot and LOCAL_FILTERED is kept
+ *   ls_local_map_transform   updateLocalMap (:522-540): LOCAL and LOCAL_FILTERED moved by T in place (float32, no
+ *                            correctTransformationMatrix); DISTANT and the queue are not moved, as in the reference
+ *   ls_local_map_clear       clearLocalMap (:496-506): empties LOCAL and LOCAL_FILTERED; DISTANT and the queue stay
+ *   ls_local_map_take_queue  getQueuedPoints (:407-412): the queued clouds in order (cloud k = points
+ *                            [cloud_offsets[k], cloud_offsets[k+1])), then the queue is empty
+ * FILTERED_MAP is the cloud the last ls_local_map_filter returned; it is kept as a value, unaffected by later calls.
+ * The local map has its own stream and device buffers (grown geometrically, never per call) and uses none of the context's
+ * workspaces, so its calls are legal between ls_icp_register_submap_batch_begin and _end.  Calls are synchronous.  Errors:
+ * LS_ERR_STATE for a scan no longer in the ring, LS_ERR_ARG for a ring on another device, a too-small buffer or bad
+ * parameters, LS_ERR_NOMEM when a buffer cannot grow; the map is unchanged after any error.  The voxel grid refuses a
+ * snapshot whose cell index space reaches 9e18 (LS_ERR_ARG) like ls_voxel_grid; it does not fall back to the unfiltered
+ * cloud as pcl::VoxelGrid does past INT32_MAX cells. */
+#define LS_LM_LOCAL 0          /* local_map_ */
+#define LS_LM_LOCAL_FILTERED 1 /* local_map_filtered_ */
+#define LS_LM_DISTANT 2        /* distant_map_ */
+#define LS_LM_FILTERED_MAP 3   /* what the last ls_local_map_filter returned */
+#define LS_LM_QUEUE 4          /* local_map_queue_, all clouds concatenated */
+
+typedef struct ls_local_map ls_local_map;
+typedef struct ls_local_map_params { /* LaserSlamWorkerParams (laser_slam_ros/include/laser_slam_ros/common.hpp:20-31) */
+  double distance_to_consider_fixed;        /* cylinder radius [m], >= 0 */
+  int separate_distant_map;
+  double voxel_size_m;                      /* leaf [m], > 0 (used with separate_distant_map) */
+  int minimum_point_number_per_voxel;       /* >= 0; 0 and 1 keep every voxel */
+  int remove_ground_from_local_map;
+  double ground_distance_to_robot_center_m;
+  int initial_capacity_points;              /* first size of every buffer; <= 0: 262144 */
+} ls_local_map_params;
+
+int ls_local_map_create(ls_ctx* ctx, const ls_local_map_params* params, ls_local_map** out);
+void ls_local_map_destroy(ls_local_map* lm);
+/* T_w_scan: the track's pose at the scan's time after correctTransformationMatrix (LaserTrack::getLocalCloudInWorldFrame);
+ * robot_z: the current pose's z.  *n_added = points appended (0: nothing appended or queued). */
+int ls_local_map_add_scan(ls_local_map* lm, const ls_map* ring, uint64_t scan_id, const float T_w_scan[16], double robot_z,
+                          int* n_added);
+/* center: the current pose's position (rounded to float32 by the caller, as the reference's PclPoint does). */
+int ls_local_map_filter(ls_local_map* lm, const double center[3], int* n_filtered_map);
+int ls_local_map_size(const ls_local_map* lm, int which); /* points in LS_LM_*, < 0 on a bad argument */
+/* cap: points out4 can hold (4 floats each); LS_ERR_ARG without a copy if the cloud is larger. */
+int ls_local_map_download(const ls_local_map* lm, int which, float* out4, int cap, int* n);
+int ls_local_map_take_queue(ls_local_map* lm, float* out4, int cap_points, int* cloud_offsets, int cap_clouds, int* n_clouds);
+int ls_local_map_transform(ls_local_map* lm, const float T[16]);
+int ls_local_map_clear(ls_local_map* lm);
+
 /* ---- per-scan input filters (reference laser_slam/src/laser_track.cpp:24-30 loads them from
  * LaserTrackParams::icp_input_filters_file, :81 and :146 apply them to every scan before it is stored) ----------------
  * A chain is an array of ls_point_filter records applied in order; each filter sees the cloud the previous one produced,

@@ -70,6 +70,19 @@ PF_REMOVE_NAN, PF_MAX_DIST, PF_MIN_DIST, PF_BOUNDING_BOX, PF_RANDOM_SAMPLING = 1
 PF_FIX_STEP_SAMPLING, PF_VOXEL_GRID, PF_SURFACE_NORMAL, PF_SAMPLING_SURFACE_NORMAL = 6, 7, 8, 9
 
 
+class LocalMapParams(ctypes.Structure):
+    """ls_local_map_params: the map fields of LaserSlamWorkerParams (reference laser_slam_ros/include/laser_slam_ros/
+    common.hpp:20-31) plus the first buffer size."""
+    _fields_ = [("distance_to_consider_fixed", ctypes.c_double), ("separate_distant_map", ctypes.c_int),
+                ("voxel_size_m", ctypes.c_double), ("minimum_point_number_per_voxel", ctypes.c_int),
+                ("remove_ground_from_local_map", ctypes.c_int), ("ground_distance_to_robot_center_m", ctypes.c_double),
+                ("initial_capacity_points", ctypes.c_int)]
+
+
+LM_LOCAL, LM_LOCAL_FILTERED, LM_DISTANT, LM_FILTERED_MAP, LM_QUEUE = 0, 1, 2, 3, 4
+LS_ERR_NOMEM, LS_ERR_STATE = -3, -4
+
+
 def build(force=False):
     """Compile libls_b200.so in-tree (nvcc cross-compiles sm_90a without a GPU)."""
     src_dir = os.path.join(_HERE, "csrc")
@@ -150,6 +163,16 @@ def lib():
         L.ls_point_filters_from_yaml.argtypes = [ctypes.c_char_p, vp, ci, ctypes.POINTER(ci)]
         L.ls_filter_cloud.argtypes = [vp, vp, ci, vp, vp, ci, ci, vp, vp, ctypes.POINTER(ci)]
         L.ls_map_push_scan_filtered.argtypes = [vp, vp, ci, vp, vp, ci, ci, ctypes.POINTER(u64), ctypes.POINTER(ci)]
+        L.ls_local_map_create.argtypes = [vp, ctypes.POINTER(LocalMapParams), ctypes.POINTER(vp)]
+        L.ls_local_map_destroy.argtypes = [vp]
+        L.ls_local_map_destroy.restype = None
+        L.ls_local_map_add_scan.argtypes = [vp, vp, u64, vp, ctypes.c_double, ctypes.POINTER(ci)]
+        L.ls_local_map_filter.argtypes = [vp, vp, ctypes.POINTER(ci)]
+        L.ls_local_map_size.argtypes = [vp, ci]
+        L.ls_local_map_download.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
+        L.ls_local_map_take_queue.argtypes = [vp, vp, ci, vp, ci, ctypes.POINTER(ci)]
+        L.ls_local_map_transform.argtypes = [vp, vp]
+        L.ls_local_map_clear.argtypes = [vp]
         _lib = L
     return _lib
 
@@ -412,6 +435,9 @@ class Context:
     def create_map(self, capacity_scans, max_pts_per_scan):
         return Map(self, capacity_scans, max_pts_per_scan)
 
+    def create_local_map(self, **params):
+        return LocalMap(self, **params)
+
 
 class Map:
     """Device-resident ring of the last `capacity_scans` scans (LaserTrack::laser_scans_ on the GPU)."""
@@ -648,6 +674,84 @@ class Map:
         self.ctx._check(lib().ls_map_assemble(self.ctx._h, self._h, len(ids_arr), ids_arr.ctypes.data, tp.ctypes.data,
                                               out.ctypes.data, _ptr(nout), ctypes.byref(mo)))
         return out[:mo.value], (nout[:mo.value] if want_normals else None)
+
+
+class LocalMap:
+    """LaserSlamWorker's local map on the device (ls_local_map_*): local_map_, local_map_filtered_, distant_map_ and
+    local_map_queue_ next to a Map ring.  Keyword arguments are the LocalMapParams fields; the defaults are
+    LaserSlamWorkerParams' usual values."""
+
+    def __init__(self, ctx, distance_to_consider_fixed=20.0, separate_distant_map=True, voxel_size_m=0.1,
+                 minimum_point_number_per_voxel=0, remove_ground_from_local_map=False,
+                 ground_distance_to_robot_center_m=1.0, initial_capacity_points=0):
+        self.ctx = ctx
+        self.params = LocalMapParams(float(distance_to_consider_fixed), int(bool(separate_distant_map)), float(voxel_size_m),
+                                     int(minimum_point_number_per_voxel), int(bool(remove_ground_from_local_map)),
+                                     float(ground_distance_to_robot_center_m), int(initial_capacity_points))
+        self._h = ctypes.c_void_p()
+        ctx._check(lib().ls_local_map_create(ctx._h, ctypes.byref(self.params), ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().ls_local_map_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add_scan(self, ring, scan_id, T_w_scan, robot_z):
+        """scanCallback's map part: scan `scan_id` of `ring` moved by T_w_scan (4x4, already corrected) appended and queued,
+        ground removed against robot_z.  Returns the points added."""
+        t = colmajor(T_w_scan)
+        n = ctypes.c_int(0)
+        self.ctx._check(lib().ls_local_map_add_scan(self._h, ring._h, int(scan_id), t.ctypes.data, float(robot_z), ctypes.byref(n)))
+        return n.value
+
+    def filter(self, center):
+        """getFilteredMap around `center` (the pose's position, rounded to float32 as the reference's PclPoint): returns the
+        number of points of the filtered map (download(LM_FILTERED_MAP) holds them)."""
+        c = np.ascontiguousarray(np.asarray(center, np.float32), np.float64)
+        n = ctypes.c_int(0)
+        self.ctx._check(lib().ls_local_map_filter(self._h, c.ctypes.data, ctypes.byref(n)))
+        return n.value
+
+    def get_filtered_map(self, center):
+        self.filter(center)
+        return self.download(LM_FILTERED_MAP)
+
+    def size(self, which):
+        n = int(lib().ls_local_map_size(self._h, which))
+        if n < 0:
+            raise LsError(f"ls_local_map_size: rc={n}")
+        return n
+
+    def download(self, which, cap=None):
+        n = self.size(which) if cap is None else int(cap)
+        out = np.empty((max(n, 1), 4), np.float32)
+        got = ctypes.c_int(0)
+        self.ctx._check(lib().ls_local_map_download(self._h, which, out.ctypes.data, n, ctypes.byref(got)))
+        return out[:got.value].copy()
+
+    def take_queue(self):
+        """getQueuedPoints: the queued clouds in order (a list of (k,4) arrays); the queue is empty afterwards."""
+        n = self.size(LM_QUEUE)
+        out = np.empty((max(n, 1), 4), np.float32)
+        cap_clouds = n + 1  # every queued cloud holds at least one point
+        offs = np.zeros(cap_clouds + 1, np.int32)
+        k = ctypes.c_int(0)
+        self.ctx._check(lib().ls_local_map_take_queue(self._h, out.ctypes.data, n, offs.ctypes.data, cap_clouds, ctypes.byref(k)))
+        return [out[offs[j]:offs[j + 1]].copy() for j in range(k.value)]
+
+    def transform(self, T):
+        """updateLocalMap's move: local_map_ and local_map_filtered_ by T (4x4 float32, not corrected)."""
+        t = colmajor(T)
+        self.ctx._check(lib().ls_local_map_transform(self._h, t.ctypes.data))
+
+    def clear(self):
+        self.ctx._check(lib().ls_local_map_clear(self._h))
 
 
 def check_rigid(T):

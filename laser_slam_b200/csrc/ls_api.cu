@@ -1,5 +1,6 @@
 // C-ABI implementation (include/ls_b200.h): context, device memory, kernel launches.
 // There is no CPU fallback anywhere in this file: every entry point needs a live CUDA device.
+#include <cmath>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -1034,7 +1035,7 @@ int run_chain(ls_ctx* ctx, const ls_point_filter* f, int n_filters, const float*
       k += used;
     } else if (fk.type == LS_PF_VOXEL_GRID) {
       int v = 0;
-      rc = lsf::enqueue_voxel_grid(b.pts[c], *has_nrm ? b.nrm[c] : nullptr, m, fk.leaf, b.pts[1 - c], b.nrm[1 - c],
+      rc = lsf::enqueue_voxel_grid(b.pts[c], *has_nrm ? b.nrm[c] : nullptr, m, fk.leaf, b.pts[1 - c], b.nrm[1 - c], 0,
                                    lsf::voxel_buffers(b), w->stream, &v, &ctx->launches);
       if (rc == LS_ERR_ARG) return fail(ctx, rc, "filter %d: voxel leaf too small for the cloud's extent", k);
       if (rc) return fail(ctx, rc, "filter %d: voxel grid: %s", k, cudaGetErrorString(cudaGetLastError()));
@@ -1463,6 +1464,272 @@ int ls_map_assemble(ls_ctx* ctx, const ls_map* map, int n_parts, const uint64_t*
     CU(cudaMemcpyAsync(out_normals3, w->A.srt_nrm, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
   }
   CU(cudaStreamSynchronize(w->stream));
+  return LS_OK;
+}
+
+}  // extern "C"
+
+// ---- resident local map (LaserSlamWorker's map maintenance) -------------------------------------------------------------
+// local[cur] is local_map_.  A filter crops it into local[1 - cur] and flips `cur`, so the old buffer is the snapshot
+// without a copy; without a separate distant map that snapshot is also the filter's result and stays untouched until the
+// next filter.  With one, the result is copied into `result` so later transforms and clears do not change it.
+struct ls_local_map {
+  ls_ctx* ctx = nullptr;
+  ls_local_map_params prm{};
+  int initial_cap = 0;
+  cudaStream_t stream = nullptr;
+  float4* local[2] = {nullptr, nullptr};
+  int local_cap[2] = {0, 0};
+  int cur = 0, n_local = 0;
+  float4* filt = nullptr;  // local_map_filtered_
+  int filt_cap = 0, n_filt = 0;
+  float4* dist = nullptr;  // distant_map_
+  int dist_cap = 0, n_dist = 0;
+  float4* queue = nullptr;  // local_map_queue_, clouds back to back
+  int queue_cap = 0, n_queue = 0;
+  std::vector<int> queue_sizes;
+  float4* result = nullptr;  // the last filter's result (separate distant map only)
+  int result_cap = 0, n_result = 0;
+  lsf::ChainBuffers scratch;  // per-call flags, scans and voxel arrays, sized for the largest cloud seen
+};
+
+namespace {
+// Grows a persistent cloud to hold `need` points (doubling), keeping its first `keep` points.  If the allocation fails the
+// old buffer is left as it was.
+int grow_cloud(ls_local_map* lm, float4** p, int* cap, long long need, int keep) {
+  ls_ctx* ctx = lm->ctx;
+  if (need <= *cap) return LS_OK;
+  if (need > 0x7fffffffLL) return fail(ctx, LS_ERR_NOMEM, "local map cloud of %lld points", need);
+  long long c = *cap > lm->initial_cap ? *cap : lm->initial_cap;
+  while (c < need) c *= 2;
+  if (c > 0x7fffffffLL) c = 0x7fffffffLL;
+  float4* q = nullptr;
+  if (cudaMalloc((void**)&q, (size_t)c * sizeof(float4)) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(ctx, LS_ERR_NOMEM, "local map growth to %lld points failed", c);
+  }
+  if (keep > 0 && cudaMemcpyAsync(q, *p, (size_t)keep * sizeof(float4), cudaMemcpyDeviceToDevice, lm->stream) != cudaSuccess) {
+    cudaFree(q);
+    return fail(ctx, LS_ERR_CUDA, "local map growth copy failed");
+  }
+  CU(cudaStreamSynchronize(lm->stream));
+  if (*p) cudaFree(*p);
+  *p = q;
+  *cap = (int)c;
+  return LS_OK;
+}
+
+int reserve_scratch(ls_local_map* lm, int n) {
+  ls_ctx* ctx = lm->ctx;
+  const int want = n > lm->initial_cap ? n : lm->initial_cap;
+  if (want <= lm->scratch.cap && lm->scratch.pts[0]) return LS_OK;
+  CU(cudaStreamSynchronize(lm->stream));
+  if (lsf::reserve(lm->scratch, want) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(lm->ctx, LS_ERR_NOMEM, "local map scratch for %d points failed", want);
+  }
+  return LS_OK;
+}
+
+// LS_LM_* -> (device pointer, points)
+bool lm_cloud(const ls_local_map* lm, int which, const float4** p, int* n) {
+  switch (which) {
+    case LS_LM_LOCAL: *p = lm->local[lm->cur]; *n = lm->n_local; return true;
+    case LS_LM_LOCAL_FILTERED: *p = lm->filt; *n = lm->n_filt; return true;
+    case LS_LM_DISTANT: *p = lm->dist; *n = lm->n_dist; return true;
+    case LS_LM_FILTERED_MAP:
+      *p = lm->prm.separate_distant_map ? lm->result : lm->local[1 - lm->cur];
+      *n = lm->n_result;
+      return true;
+    case LS_LM_QUEUE: *p = lm->queue; *n = lm->n_queue; return true;
+    default: return false;
+  }
+}
+}  // namespace
+
+extern "C" {
+
+int ls_local_map_create(ls_ctx* ctx, const ls_local_map_params* params, ls_local_map** out) {
+  if (!ctx || !out) return LS_ERR_ARG;
+  *out = nullptr;
+  if (!params) return fail(ctx, LS_ERR_ARG, "bad argument");
+  const ls_local_map_params& p = *params;
+  if (!(p.distance_to_consider_fixed >= 0.0) || !((float)p.voxel_size_m > 0.0f) || !std::isfinite(p.voxel_size_m) ||
+      p.minimum_point_number_per_voxel < 0 || !std::isfinite(p.ground_distance_to_robot_center_m))
+    return fail(ctx, LS_ERR_ARG, "bad local map parameters (radius >= 0, leaf > 0, minimum >= 0)");
+  CU(cudaSetDevice(ctx->device));
+  ls_local_map* lm = new ls_local_map();
+  lm->ctx = ctx;
+  lm->prm = p;
+  lm->initial_cap = p.initial_capacity_points > 0 ? p.initial_capacity_points : 262144;
+  if (cudaStreamCreateWithFlags(&lm->stream, cudaStreamNonBlocking) != cudaSuccess) {
+    cudaGetLastError();
+    ls_local_map_destroy(lm);
+    return fail(ctx, LS_ERR_NOMEM, "local map creation failed");
+  }
+  *out = lm;
+  return LS_OK;
+}
+
+void ls_local_map_destroy(ls_local_map* lm) {
+  if (!lm) return;
+  cudaSetDevice(lm->ctx->device);
+  if (lm->stream) cudaStreamSynchronize(lm->stream);
+  void* bufs[] = {lm->local[0], lm->local[1], lm->filt, lm->dist, lm->queue, lm->result};
+  for (void* b : bufs)
+    if (b) cudaFree(b);
+  lsf::release(lm->scratch);
+  if (lm->stream) cudaStreamDestroy(lm->stream);
+  delete lm;
+}
+
+int ls_local_map_add_scan(ls_local_map* lm, const ls_map* ring, uint64_t scan_id, const float T_w_scan[16], double robot_z,
+                          int* n_added) {
+  if (!lm) return LS_ERR_ARG;
+  ls_ctx* ctx = lm->ctx;
+  if (!ring || !T_w_scan || !n_added) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (ring->ctx->device != ctx->device)
+    return fail(ctx, LS_ERR_ARG, "the ring is on device %d, the local map on device %d", ring->ctx->device, ctx->device);
+  CU(cudaSetDevice(ctx->device));
+  const ls_scan_slot* s = find_slot(ring, scan_id);
+  if (!s) return fail(ctx, LS_ERR_STATE, "scan %llu is not resident (evicted or never pushed)", (unsigned long long)scan_id);
+  *n_added = 0;
+  const int n = s->n;
+  if (n == 0) return LS_OK;
+  int rc;
+  const int c = lm->cur;
+  if ((rc = grow_cloud(lm, &lm->local[c], &lm->local_cap[c], (long long)lm->n_local + n, lm->n_local))) return rc;
+  if ((rc = grow_cloud(lm, &lm->queue, &lm->queue_cap, (long long)lm->n_queue + n, lm->n_queue))) return rc;
+  if ((rc = reserve_scratch(lm, n))) return rc;
+  if (wait_slot(s, lm->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
+  int kept = 0;
+  const double z_min = robot_z - lm->prm.ground_distance_to_robot_center_m;
+  rc = lsf::enqueue_local_map_append(s->pts, n, T_w_scan, is_identity16(T_w_scan), lm->prm.remove_ground_from_local_map != 0,
+                                     z_min, lm->local[c] + lm->n_local, lm->queue + lm->n_queue, lm->scratch, lm->stream, &kept,
+                                     &ctx->launches);
+  if (rc) return fail(ctx, rc, "local map append failed");
+  if (kept > 0) {
+    lm->n_local += kept;
+    lm->n_queue += kept;
+    lm->queue_sizes.push_back(kept);
+  }
+  *n_added = kept;
+  return LS_OK;
+}
+
+int ls_local_map_filter(ls_local_map* lm, const double center[3], int* n_filtered_map) {
+  if (!lm) return LS_ERR_ARG;
+  ls_ctx* ctx = lm->ctx;
+  if (!center || !n_filtered_map) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  const bool separate = lm->prm.separate_distant_map != 0;
+  const double radius = lm->prm.distance_to_consider_fixed, height = 40.0;  // the reference hard-codes the height
+  const int c = lm->cur, n = lm->n_local;
+  const float4* snap = lm->local[c];
+  int rc;
+  // every buffer this call can write, before anything changes (the previous result is kept until the new one exists)
+  if ((rc = grow_cloud(lm, &lm->local[1 - c], &lm->local_cap[1 - c], n, separate ? 0 : lm->n_result))) return rc;
+  if ((rc = reserve_scratch(lm, n))) return rc;
+  if (separate) {
+    if ((rc = grow_cloud(lm, &lm->filt, &lm->filt_cap, n, lm->n_filt))) return rc;
+    if ((rc = grow_cloud(lm, &lm->dist, &lm->dist_cap, (long long)lm->n_dist + n, lm->n_dist))) return rc;
+    if ((rc = grow_cloud(lm, &lm->result, &lm->result_cap, (long long)lm->n_dist + 2LL * n, lm->n_result))) return rc;
+  }
+  int n_cropped = 0;
+  if ((rc = lsf::enqueue_cylinder_crop(snap, n, center, radius, height, lm->local[1 - c], lm->scratch, lm->stream, &n_cropped,
+                                       &ctx->launches)))
+    return fail(ctx, rc, "local map crop failed");
+  if (!separate) {  // the result is the snapshot itself, uncropped and not voxelised
+    lm->cur = 1 - c;
+    lm->n_local = n_cropped;
+    lm->n_result = n;
+    *n_filtered_map = n;
+    return LS_OK;
+  }
+  const float leaf[3] = {(float)lm->prm.voxel_size_m, (float)lm->prm.voxel_size_m, (float)lm->prm.voxel_size_m};
+  lsf::VoxelBuffers vb = lsf::voxel_buffers(lm->scratch);
+  vb.cent = lm->scratch.nrm[0];
+  float4* vox = lm->scratch.pts[1];
+  int m = 0;
+  if ((rc = lsf::enqueue_voxel_grid(snap, nullptr, n, leaf, vox, nullptr, lm->prm.minimum_point_number_per_voxel, vb, lm->stream,
+                                    &m, &ctx->launches)))
+    return fail(ctx, rc, rc == LS_ERR_ARG ? "leaf too small for the local map's extent" : "local map voxel grid failed");
+  int n_in = 0, n_out = 0;
+  if ((rc = lsf::enqueue_cylinder_split(vox, m, center, radius, height, lm->filt, lm->dist + lm->n_dist, lm->scratch, lm->stream,
+                                        &n_in, &n_out, &ctx->launches)))
+    return fail(ctx, rc, "local map split failed");
+  lm->cur = 1 - c;
+  lm->n_local = n_cropped;
+  lm->n_filt = n_in;
+  lm->n_dist += n_out;
+  if (n_in > 0) CU(cudaMemcpyAsync(lm->result, lm->filt, (size_t)n_in * sizeof(float4), cudaMemcpyDeviceToDevice, lm->stream));
+  if (lm->n_dist > 0)
+    CU(cudaMemcpyAsync(lm->result + n_in, lm->dist, (size_t)lm->n_dist * sizeof(float4), cudaMemcpyDeviceToDevice, lm->stream));
+  CU(cudaStreamSynchronize(lm->stream));
+  lm->n_result = n_in + lm->n_dist;
+  *n_filtered_map = lm->n_result;
+  return LS_OK;
+}
+
+int ls_local_map_size(const ls_local_map* lm, int which) {
+  if (!lm) return LS_ERR_ARG;
+  const float4* p;
+  int n;
+  return lm_cloud(lm, which, &p, &n) ? n : LS_ERR_ARG;
+}
+
+int ls_local_map_download(const ls_local_map* lm, int which, float* out4, int cap, int* n_out) {
+  if (!lm) return LS_ERR_ARG;
+  ls_ctx* ctx = lm->ctx;
+  const float4* p;
+  int n;
+  if (!n_out || !lm_cloud(lm, which, &p, &n)) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (n > cap || (n > 0 && !out4)) return fail(ctx, LS_ERR_ARG, "buffer of %d points for a cloud of %d", cap, n);
+  CU(cudaSetDevice(ctx->device));
+  if (n > 0) CU(cudaMemcpyAsync(out4, p, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, lm->stream));
+  CU(cudaStreamSynchronize(lm->stream));
+  *n_out = n;
+  return LS_OK;
+}
+
+int ls_local_map_take_queue(ls_local_map* lm, float* out4, int cap_points, int* cloud_offsets, int cap_clouds, int* n_clouds) {
+  if (!lm) return LS_ERR_ARG;
+  ls_ctx* ctx = lm->ctx;
+  if (!cloud_offsets || !n_clouds) return fail(ctx, LS_ERR_ARG, "bad argument");
+  const int k = (int)lm->queue_sizes.size();
+  if (lm->n_queue > cap_points || k > cap_clouds || (lm->n_queue > 0 && !out4))
+    return fail(ctx, LS_ERR_ARG, "buffers of %d points / %d clouds for a queue of %d / %d", cap_points, cap_clouds, lm->n_queue, k);
+  CU(cudaSetDevice(ctx->device));
+  if (lm->n_queue > 0)
+    CU(cudaMemcpyAsync(out4, lm->queue, (size_t)lm->n_queue * sizeof(float4), cudaMemcpyDeviceToHost, lm->stream));
+  CU(cudaStreamSynchronize(lm->stream));
+  cloud_offsets[0] = 0;
+  for (int j = 0; j < k; ++j) cloud_offsets[j + 1] = cloud_offsets[j] + lm->queue_sizes[j];
+  *n_clouds = k;
+  lm->queue_sizes.clear();
+  lm->n_queue = 0;
+  return LS_OK;
+}
+
+int ls_local_map_transform(ls_local_map* lm, const float T[16]) {
+  if (!lm) return LS_ERR_ARG;
+  ls_ctx* ctx = lm->ctx;
+  if (!T) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  float4* clouds[2] = {lm->local[lm->cur], lm->filt};
+  const int counts[2] = {lm->n_local, lm->n_filt};
+  for (int k = 0; k < 2; ++k) {
+    const int rc = lsf::enqueue_transform_in_place(clouds[k], counts[k], T, lm->stream, &ctx->launches);
+    if (rc) return fail(ctx, rc, "local map transform failed");
+  }
+  CU(cudaStreamSynchronize(lm->stream));
+  return LS_OK;
+}
+
+int ls_local_map_clear(ls_local_map* lm) {
+  if (!lm) return LS_ERR_ARG;
+  lm->n_local = 0;
+  lm->n_filt = 0;
   return LS_OK;
 }
 

@@ -242,6 +242,77 @@ __global__ void voxel_centroid_kernel(const unsigned long long* __restrict__ sum
   }
 }
 
+// pcl::VoxelGrid's minimum point number: keep[v] = 1 iff voxel v holds at least min_points points
+__global__ void voxel_min_count_kernel(const unsigned long long* __restrict__ sums, int m, int stride, int min_points,
+                                       int* __restrict__ keep) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < m; v += gridDim.x * blockDim.x)
+    keep[v] = sums[(size_t)stride * (size_t)v + 3] >= (unsigned long long)min_points ? 1 : 0;
+}
+
+// ---- local map (ls_local_map_*): the map maintenance of LaserSlamWorker
+// The scan of a ring slot moved into the world frame (xform3: the xform_point order of ls_map_assemble; an exact identity
+// copies verbatim), and keep[i] = 0 for a ground point: (double)z <= z_min when remove_ground.
+struct Xform16 {
+  float T[16];
+};
+__global__ void local_map_append_kernel(const float4* __restrict__ in, int n, Xform16 T, int identity, int remove_ground,
+                                        double z_min, float4* __restrict__ out, int* __restrict__ keep) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float4 p = in[i];
+    if (!identity) {
+      float x, y, z;
+      xform3(T.T, p.x, p.y, p.z, x, y, z);
+      p.x = x; p.y = y; p.z = z;
+    }
+    out[i] = p;
+    keep[i] = (!remove_ground || (double)p.z > z_min) ? 1 : 0;
+  }
+}
+
+// updateLocalMap's move, in place: every thread reads its point and writes it back (no restrict pointers)
+__global__ void local_map_transform_kernel(float4* pts, int n, Xform16 T) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float4 p = pts[i];
+    float x, y, z;
+    xform3(T.T, p.x, p.y, p.z, x, y, z);
+    p.x = x; p.y = y; p.z = z;
+    pts[i] = p;
+  }
+}
+
+// Two-way split of the voxelised map by the cylinder: flag[i] = inside (d_xy^2 <= r^2 and |dz| <= h/2) in the low word,
+// outside (>= on either) in the high word -- a point exactly on the boundary is both, as in the reference.  One 64-bit
+// exclusive scan then places both streams at once.
+__global__ void split_flag_kernel(const float4* __restrict__ in, int n, double cx, double cy, double cz, double r2, double hh,
+                                  unsigned long long* __restrict__ flag) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float4 p = in[i];
+    const double dx = (double)p.x - cx, dy = (double)p.y - cy;
+    const double d2 = dx * dx + dy * dy;
+    const double dz = fabs((double)p.z - cz);
+    const bool inside = d2 <= r2 && dz <= hh;
+    const bool outside = d2 >= r2 || dz >= hh;
+    flag[i] = (inside ? 1ull : 0ull) | (outside ? (1ull << 32) : 0ull);
+  }
+}
+
+// Scatter by the exclusive scan `pos` of `flag`: inside points to in_out[lo], outside points to out_out[hi]; the thread of
+// the last point stores both totals in counts[0..1].
+__global__ void split_scatter_kernel(const float4* __restrict__ in, const unsigned long long* __restrict__ flag,
+                                     const unsigned long long* __restrict__ pos, int n, float4* __restrict__ in_out,
+                                     float4* __restrict__ out_out, int* __restrict__ counts) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const unsigned long long f = flag[i], q = pos[i];
+    if (f & 0xffffffffull) in_out[q & 0xffffffffull] = in[i];
+    if (f >> 32) out_out[q >> 32] = in[i];
+    if (i == n - 1) {
+      const unsigned long long t = q + f;
+      counts[0] = (int)(t & 0xffffffffull);
+      counts[1] = (int)(t >> 32);
+    }
+  }
+}
+
 struct Scratch {  // freed on every exit path
   void* p[12] = {};
   int n = 0;
@@ -382,7 +453,7 @@ int ls_voxel_grid(int device, const float* in4, int n, const float leaf_size[3],
   FCU(cudaMemcpy(d_in, in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice));
   uint64_t launches = 0;
   int m = 0;
-  const int rc = lsf::enqueue_voxel_grid(d_in, nullptr, n, leaf_size, d_out, nullptr, vb, 0, &m, &launches);
+  const int rc = lsf::enqueue_voxel_grid(d_in, nullptr, n, leaf_size, d_out, nullptr, 0, vb, 0, &m, &launches);
   if (rc != LS_OK) return rc;
   if (m > 0) FCU(cudaMemcpy(out4, d_out, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost));
   *n_out = m;
@@ -399,10 +470,12 @@ bool is_pointwise(int type) {
   return type == LS_PF_REMOVE_NAN || type == LS_PF_MAX_DIST || type == LS_PF_MIN_DIST || type == LS_PF_BOUNDING_BOX;
 }
 size_t scan_temp_bytes(int n) {
-  size_t a = 0, b = 0;
+  size_t a = 0, b = 0, c = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, a, (const int*)nullptr, (int*)nullptr, n);
   cub::DeviceScan::InclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, n);
-  return a > b ? a : b;
+  cub::DeviceScan::ExclusiveSum(nullptr, c, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, n);  // split
+  a = a > b ? a : b;
+  return a > c ? a : c;
 }
 template <typename T>
 cudaError_t grow(T** p, size_t count) {
@@ -509,8 +582,10 @@ cudaError_t enqueue_mask_run(const ls_point_filter* filters, int n_filters, cons
 }
 
 int enqueue_voxel_grid(const float4* in, const float4* in_nrm, int n, const float leaf[3], float4* out, float4* out_nrm,
-                       const VoxelBuffers& b, cudaStream_t st, int* m_out, uint64_t* launches) {
+                       int min_points, const VoxelBuffers& b, cudaStream_t st, int* m_out, uint64_t* launches) {
   *m_out = 0;
+  const bool min_filter = min_points > 1;  // 0 and 1 keep every voxel: exactly the kernels of the plain grid
+  if (min_filter && (in_nrm || !b.cent)) return LS_ERR_ARG;
   if (n == 0) return LS_OK;
   const float ix = 1.0f / leaf[0], iy = 1.0f / leaf[1], iz = 1.0f / leaf[2];  // PCL: inverse_leaf_size_
   const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
@@ -539,11 +614,83 @@ int enqueue_voxel_grid(const float4* in, const float4* in_nrm, int n, const floa
     const int stride = in_nrm ? 7 : 4;
     FCU(cudaMemsetAsync(b.sums, 0, (size_t)m * stride * sizeof(unsigned long long), st));
     voxel_accumulate_kernel<<<blocks(n), 256, 0, st>>>(in, in_nrm, b.key2, b.idx2, b.slot, n, stride, b.sums);
-    voxel_centroid_kernel<<<blocks(m), 256, 0, st>>>(b.sums, m, stride, out, in_nrm ? out_nrm : nullptr);
+    voxel_centroid_kernel<<<blocks(m), 256, 0, st>>>(b.sums, m, stride, min_filter ? b.cent : out, in_nrm ? out_nrm : nullptr);
     *launches += 2;
+    if (min_filter) {  // flag, scan, stable compaction of the voxels (head / slot are free again after the accumulation)
+      voxel_min_count_kernel<<<blocks(m), 256, 0, st>>>(b.sums, m, stride, min_points, b.head);
+      bytes = b.tmp_bytes;
+      FCU(cub::DeviceScan::ExclusiveSum(b.tmp, bytes, b.head, b.slot, m, st));
+      compact_kernel<<<blocks(m), 256, 0, st>>>(b.cent, nullptr, b.head, b.slot, m, out, nullptr, b.mm);
+      *launches += 2;
+      FCU(cudaMemcpyAsync(&m, b.mm, sizeof(int), cudaMemcpyDeviceToHost, st));
+      FCU(cudaStreamSynchronize(st));
+    }
   }
   FCU(cudaGetLastError());
   *m_out = m;
+  return LS_OK;
+}
+
+int enqueue_local_map_append(const float4* scan, int n, const float T[16], bool identity, bool remove_ground, double z_min,
+                             float4* local_tail, float4* queue_tail, ChainBuffers& b, cudaStream_t st, int* kept,
+                             uint64_t* launches) {
+  *kept = 0;
+  if (n == 0) return LS_OK;
+  Xform16 x;
+  memcpy(x.T, T, sizeof(x.T));
+  local_map_append_kernel<<<blocks(n), 256, 0, st>>>(scan, n, x, identity ? 1 : 0, remove_ground ? 1 : 0, z_min, b.pts[0], b.keep);
+  size_t bytes = b.tmp_bytes;
+  FCU(cub::DeviceScan::ExclusiveSum(b.tmp, bytes, b.keep, b.pos, n, st));
+  // one compaction fills both: the local map's tail as the points, the queue's tail as the "normals" of the same points
+  compact_kernel<<<blocks(n), 256, 0, st>>>(b.pts[0], b.pts[0], b.keep, b.pos, n, local_tail, queue_tail, b.small + 6);
+  *launches += 2;
+  FCU(cudaGetLastError());
+  FCU(cudaMemcpyAsync(kept, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+  FCU(cudaStreamSynchronize(st));
+  return LS_OK;
+}
+
+int enqueue_transform_in_place(float4* pts, int n, const float T[16], cudaStream_t st, uint64_t* launches) {
+  if (n == 0) return LS_OK;
+  Xform16 x;
+  memcpy(x.T, T, sizeof(x.T));
+  local_map_transform_kernel<<<blocks(n), 256, 0, st>>>(pts, n, x);
+  ++*launches;
+  FCU(cudaGetLastError());
+  return LS_OK;
+}
+
+int enqueue_cylinder_crop(const float4* in, int n, const double center[3], double radius_m, double height_m, float4* out,
+                          ChainBuffers& b, cudaStream_t st, int* kept, uint64_t* launches) {
+  *kept = 0;
+  if (n == 0) return LS_OK;
+  cylinder_flag_kernel<<<blocks(n), 256, 0, st>>>(in, n, center[0], center[1], center[2], radius_m * radius_m, height_m / 2.0, 0,
+                                                  b.keep);
+  size_t bytes = b.tmp_bytes;
+  FCU(cub::DeviceScan::ExclusiveSum(b.tmp, bytes, b.keep, b.pos, n, st));
+  compact_kernel<<<blocks(n), 256, 0, st>>>(in, nullptr, b.keep, b.pos, n, out, nullptr, b.small + 6);
+  *launches += 2;
+  FCU(cudaGetLastError());
+  FCU(cudaMemcpyAsync(kept, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+  FCU(cudaStreamSynchronize(st));
+  return LS_OK;
+}
+
+int enqueue_cylinder_split(const float4* in, int n, const double center[3], double radius_m, double height_m, float4* inside,
+                           float4* outside, ChainBuffers& b, cudaStream_t st, int* n_inside, int* n_outside, uint64_t* launches) {
+  *n_inside = *n_outside = 0;
+  if (n == 0) return LS_OK;
+  split_flag_kernel<<<blocks(n), 256, 0, st>>>(in, n, center[0], center[1], center[2], radius_m * radius_m, height_m / 2.0, b.key);
+  size_t bytes = b.tmp_bytes;
+  FCU(cub::DeviceScan::ExclusiveSum(b.tmp, bytes, b.key, b.key2, n, st));
+  split_scatter_kernel<<<blocks(n), 256, 0, st>>>(in, b.key, b.key2, n, inside, outside, b.small + 6);
+  *launches += 2;
+  FCU(cudaGetLastError());
+  int c[2];
+  FCU(cudaMemcpyAsync(c, b.small + 6, sizeof(c), cudaMemcpyDeviceToHost, st));
+  FCU(cudaStreamSynchronize(st));
+  *n_inside = c[0];
+  *n_outside = c[1];
   return LS_OK;
 }
 

@@ -39,17 +39,38 @@ bool is_mask_filter(int type);
 // pcl::VoxelGrid centroids (ls_voxel_grid) of n device points, with the normals averaged alongside when in_nrm != NULL.
 // Synchronises `st` twice (cell bounds, voxel count).  *m_out = voxels written to out / out_nrm.  Returns LS_OK,
 // LS_ERR_ARG (leaf too small for the cloud's extent) or LS_ERR_CUDA.
+// min_points > 1 keeps only the voxels with at least that many points (pcl::VoxelGrid::setMinimumPointsNumberPerVoxel):
+// the centroids go to b.cent first, then one flag / scan / compaction into out, and `st` is synchronised a third time.
+// It needs b.cent (n float4) and no normals.  min_points 0 or 1 launches exactly the kernels of the plain grid.
 struct VoxelBuffers {
   int* mm;  // 6 ints
   unsigned long long *key, *key2, *sums;
   int *idx, *idx2, *head, *slot;
   void* tmp;
   size_t tmp_bytes;
+  float4* cent = nullptr;  // centroids before the minimum-count compaction
 };
 size_t voxel_temp_bytes(int n);
 int enqueue_voxel_grid(const float4* in, const float4* in_nrm, int n, const float leaf[3], float4* out, float4* out_nrm,
-                       const VoxelBuffers& b, cudaStream_t st, int* m_out, uint64_t* launches);
+                       int min_points, const VoxelBuffers& b, cudaStream_t st, int* m_out, uint64_t* launches);
 VoxelBuffers voxel_buffers(const ChainBuffers& b);
+
+// ---- local map (ls_local_map_*): scratch is a ChainBuffers reserved for the largest cloud of the call; each helper
+// synchronises `st` once and returns LS_OK or LS_ERR_CUDA.
+// Append: the n points of a ring slot moved by T (an exact identity when `identity`: verbatim) into b.pts[0], ground points
+// ((double)z <= z_min) dropped when remove_ground, the rest compacted in order to BOTH local_tail and queue_tail.
+int enqueue_local_map_append(const float4* scan, int n, const float T[16], bool identity, bool remove_ground, double z_min,
+                             float4* local_tail, float4* queue_tail, ChainBuffers& b, cudaStream_t st, int* kept,
+                             uint64_t* launches);
+// updateLocalMap's move of n device points in place (the xform_point order, no identity shortcut); enqueued only.
+int enqueue_transform_in_place(float4* pts, int n, const float T[16], cudaStream_t st, uint64_t* launches);
+// ls_filter_cylinder's inside rule (d_xy^2 <= r^2 and |dz| <= h/2) from device `in` to device `out`, input order kept.
+int enqueue_cylinder_crop(const float4* in, int n, const double center[3], double radius_m, double height_m, float4* out,
+                          ChainBuffers& b, cudaStream_t st, int* kept, uint64_t* launches);
+// One stable two-way partition: the inside points (<=) to `inside`, the outside points (>= on either) to `outside`; a
+// point on the boundary goes to both.  Uses b.key / b.key2 as its 64-bit flags and their scan.
+int enqueue_cylinder_split(const float4* in, int n, const double center[3], double radius_m, double height_m, float4* inside,
+                           float4* outside, ChainBuffers& b, cudaStream_t st, int* n_inside, int* n_outside, uint64_t* launches);
 
 }  // namespace lsf
 

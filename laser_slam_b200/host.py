@@ -137,20 +137,26 @@ class Estimator:
         p = np.ascontiguousarray(w_T_a_b7, np.float64)
         self._check(lib().lsh_loop_closure(self._h, track_a, int(time_a), track_b, int(time_b), p.ctypes.data))
 
+    def _count(self, n):
+        """A hook that returns a count: only a negative value is an error (1 is one node, not LS_ERR_CONVERGENCE)."""
+        if n < 0:
+            self._check(n)
+        return n
+
     def trajectory(self, worker=0):
-        n = self._check(lib().lsh_trajectory(self._h, worker, None, None, 0))
+        n = self._count(lib().lsh_trajectory(self._h, worker, None, None, 0))
         times = np.zeros(max(n, 1), np.int64)
         poses = np.zeros((max(n, 1), 7), np.float64)
-        self._check(lib().lsh_trajectory(self._h, worker, times.ctypes.data, poses.ctypes.data, n))
+        self._count(lib().lsh_trajectory(self._h, worker, times.ctypes.data, poses.ctypes.data, n))
         return times[:n], poses[:n]
 
     def num_scans(self, worker=0):
-        return self._check(lib().lsh_num_scans(self._h, worker))
+        return self._count(lib().lsh_num_scans(self._h, worker))
 
     def build_submap(self, worker, time_ns, radius, cap_points):
         f = np.zeros((cap_points, 4), np.float32)
         nr = np.zeros((cap_points, 3), np.float32)
-        m = self._check(lib().lsh_build_submap(self._h, worker, int(time_ns), radius, f.ctypes.data, nr.ctypes.data, cap_points))
+        m = self._count(lib().lsh_build_submap(self._h, worker, int(time_ns), radius, f.ctypes.data, nr.ctypes.data, cap_points))
         return f[:m], nr[:m]
 
 
@@ -186,3 +192,75 @@ class Assembler:
         if self._h:
             lib().lsh_assembler_destroy(self._h)
             self._h = None
+
+
+LM_LOCAL, LM_LOCAL_FILTERED, LM_DISTANT, LM_FILTERED_MAP = 0, 1, 2, 3   # include/ls_b200.h LS_LM_*
+
+
+class LocalMap:
+    """laser_slam::LocalMap (include/laser_slam/local_map.hpp) on one worker's track of an Estimator: the worker's map
+    maintenance, each call taking its pose, centre or transform from the track.  Close it before the estimator."""
+
+    def __init__(self, estimator, worker, distance_to_consider_fixed=20.0, separate_distant_map=True, create_filtered_map=True,
+                 voxel_size_m=0.1, minimum_point_number_per_voxel=0, remove_ground_from_local_map=False,
+                 ground_distance_to_robot_center_m=1.0):
+        L = lib()
+        if not hasattr(L, "_lm_bound"):
+            vp, ci, cd = ctypes.c_void_p, ctypes.c_int, ctypes.c_double
+            L.lsh_local_map_create.restype = vp
+            L.lsh_local_map_create.argtypes = [vp, ci, cd, ci, ci, cd, ci, ci, cd, ctypes.c_char_p, ci]
+            L.lsh_local_map_destroy.argtypes = [vp]
+            L.lsh_local_map_destroy.restype = None
+            L.lsh_local_map_last_error.argtypes = [vp]
+            L.lsh_local_map_last_error.restype = ctypes.c_char_p
+            for f in ("add_scan", "filter", "take_queue", "clear"):
+                getattr(L, "lsh_local_map_" + f).argtypes = [vp]
+            L.lsh_local_map_get.argtypes = [vp, ci, vp, ci]
+            L.lsh_local_map_queued.argtypes = [vp, ci, vp, ci]
+            L.lsh_local_map_update.argtypes = [vp, vp, ctypes.c_int64]
+            L._lm_bound = True
+        err = ctypes.create_string_buffer(512)
+        self._h = L.lsh_local_map_create(estimator._h, worker, float(distance_to_consider_fixed), int(bool(separate_distant_map)),
+                                         int(bool(create_filtered_map)), float(voxel_size_m), int(minimum_point_number_per_voxel),
+                                         int(bool(remove_ground_from_local_map)), float(ground_distance_to_robot_center_m), err, 512)
+        if not self._h:
+            raise LsError(err.value.decode() or "lsh_local_map_create failed")
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().lsh_local_map_destroy(self._h)
+            self._h = None
+
+    def _check(self, rc):
+        if rc < 0:
+            raise LsError(lib().lsh_local_map_last_error(self._h).decode())
+        return rc
+
+    @staticmethod
+    def _read(fn):
+        n = fn(None, 0)
+        out = np.zeros((max(n, 1), 4), np.float32)
+        if n > 0:
+            fn(out.ctypes.data, n)
+        return out[:n]
+
+    def add_scan(self):
+        self._check(lib().lsh_local_map_add_scan(self._h))
+
+    def get_filtered_map(self):
+        self._check(lib().lsh_local_map_filter(self._h))
+        return self.get(LM_FILTERED_MAP)
+
+    def get(self, which):
+        return self._read(lambda p, cap: self._check(lib().lsh_local_map_get(self._h, which, p, cap)))
+
+    def get_queued_points(self):
+        k = self._check(lib().lsh_local_map_take_queue(self._h))
+        return [self._read(lambda p, cap, j=j: self._check(lib().lsh_local_map_queued(self._h, j, p, cap))) for j in range(k)]
+
+    def update_local_map(self, last_pose_before_update7, time_ns):
+        p = np.ascontiguousarray(last_pose_before_update7, np.float64)
+        self._check(lib().lsh_local_map_update(self._h, p.ctypes.data, int(time_ns)))
+
+    def clear_local_map(self):
+        self._check(lib().lsh_local_map_clear(self._h))

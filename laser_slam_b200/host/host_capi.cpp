@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "laser_slam/incremental_estimator.hpp"
+#include "laser_slam/local_map.hpp"
 #include "laser_slam/velodyne_assembler.hpp"
 
 using namespace laser_slam;
@@ -252,6 +253,100 @@ int lsh_build_submap(void* hv, int worker, int64_t time_ns, int radius, float* f
   });
 }
 
+// ---- laser_slam::LocalMap (include/laser_slam/local_map.hpp) on one worker's track, for the tests.  Destroy it before
+// the estimator: the map lives on the estimator's context.
+}  // extern "C"
+
+namespace {
+struct LocalMapHandle {
+  std::shared_ptr<LaserTrack> track;
+  std::unique_ptr<LocalMap> map;
+  DataPoints filtered;                 // what the last lsh_local_map_filter returned
+  std::vector<DataPoints> queue;       // what the last lsh_local_map_take_queue took
+  std::string err;
+};
+int copy_cloud(const DataPoints& d, float* out4, int cap) {
+  const int n = (int)d.getNbPoints();
+  if (out4 && n <= cap) std::memcpy(out4, d.features.data(), sizeof(float) * 4 * (size_t)n);
+  return n;
+}
+template <typename F>
+int guarded_lm(LocalMapHandle* h, F f) {
+  try {
+    return f();
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+}  // namespace
+
+extern "C" {
+
+void* lsh_local_map_create(void* hv, int worker, double distance_to_consider_fixed, int separate_distant_map,
+                           int create_filtered_map, double voxel_size_m, int minimum_point_number_per_voxel,
+                           int remove_ground_from_local_map, double ground_distance_to_robot_center_m, char* err, int errlen) {
+  try {
+    LocalMapParams p;
+    p.distance_to_consider_fixed = distance_to_consider_fixed;
+    p.separate_distant_map = separate_distant_map != 0;
+    p.create_filtered_map = create_filtered_map != 0;
+    p.voxel_size_m = voxel_size_m;
+    p.minimum_point_number_per_voxel = minimum_point_number_per_voxel;
+    p.remove_ground_from_local_map = remove_ground_from_local_map != 0;
+    p.ground_distance_to_robot_center_m = ground_distance_to_robot_center_m;
+    LocalMapHandle* h = new LocalMapHandle();
+    h->track = static_cast<Handle*>(hv)->est->getLaserTrack((unsigned int)worker);
+    h->map.reset(new LocalMap(p, *h->track));
+    return h;
+  } catch (const std::exception& e) {
+    if (err && errlen > 0) std::strncpy(err, e.what(), (size_t)errlen - 1), err[errlen - 1] = 0;
+    return nullptr;
+  }
+}
+void lsh_local_map_destroy(void* lv) { delete static_cast<LocalMapHandle*>(lv); }
+const char* lsh_local_map_last_error(void* lv) { return static_cast<LocalMapHandle*>(lv)->err.c_str(); }
+
+int lsh_local_map_add_scan(void* lv) {
+  LocalMapHandle* h = static_cast<LocalMapHandle*>(lv);
+  return guarded_lm(h, [&]() { h->map->addScan(); return LS_OK; });
+}
+// getFilteredMap; returns its number of points (read it with lsh_local_map_get(LS_LM_FILTERED_MAP))
+int lsh_local_map_filter(void* lv) {
+  LocalMapHandle* h = static_cast<LocalMapHandle*>(lv);
+  return guarded_lm(h, [&]() { h->map->getFilteredMap(&h->filtered); return (int)h->filtered.getNbPoints(); });
+}
+// LS_LM_LOCAL / _LOCAL_FILTERED / _DISTANT / _FILTERED_MAP: returns the number of points, written to out4 if <= cap
+int lsh_local_map_get(void* lv, int which, float* out4, int cap) {
+  LocalMapHandle* h = static_cast<LocalMapHandle*>(lv);
+  return guarded_lm(h, [&]() {
+    DataPoints d;
+    if (which == LS_LM_LOCAL) h->map->getLocalMap(&d);
+    else if (which == LS_LM_LOCAL_FILTERED) h->map->getLocalMapFiltered(&d);
+    else if (which == LS_LM_DISTANT) h->map->getDistantMap(&d);
+    else if (which == LS_LM_FILTERED_MAP) d = h->filtered;
+    else return LS_ERR_ARG;
+    return copy_cloud(d, out4, cap);
+  });
+}
+// getQueuedPoints; returns the number of clouds taken (read cloud k with lsh_local_map_queued)
+int lsh_local_map_take_queue(void* lv) {
+  LocalMapHandle* h = static_cast<LocalMapHandle*>(lv);
+  return guarded_lm(h, [&]() { h->queue = h->map->getQueuedPoints(); return (int)h->queue.size(); });
+}
+int lsh_local_map_queued(void* lv, int k, float* out4, int cap) {
+  LocalMapHandle* h = static_cast<LocalMapHandle*>(lv);
+  if (k < 0 || k >= (int)h->queue.size()) return LS_ERR_ARG;
+  return copy_cloud(h->queue[(size_t)k], out4, cap);
+}
+int lsh_local_map_update(void* lv, const double* last_pose_before_update7, int64_t time_ns) {
+  LocalMapHandle* h = static_cast<LocalMapHandle*>(lv);
+  return guarded_lm(h, [&]() { h->map->updateLocalMap(SE3::fromArray7(last_pose_before_update7), time_ns); return LS_OK; });
+}
+int lsh_local_map_clear(void* lv) {
+  LocalMapHandle* h = static_cast<LocalMapHandle*>(lv);
+  return guarded_lm(h, [&]() { h->map->clearLocalMap(); return LS_OK; });
+}
 
 // ---- laser_slam::VelodyneAssembler (include/laser_slam/velodyne_assembler.hpp) for the tests
 void* lsh_assembler_create(const float* T_sensor_base16, int naive, int device) {

@@ -413,6 +413,17 @@ uint64_t LaserTrack::residentScan(size_t index) const {
   return id;
 }
 
+uint64_t LaserTrack::residentScanAtTime(const curves::Time& time_ns) const {
+  std::lock_guard<std::recursive_mutex> lock(full_laser_track_mutex_);
+  const size_t index = scanIndexAtTime(time_ns);
+  // the ring exists from the first registration on; a reader of the first scan creates it, sized as the staging does
+  const size_t n = laser_scans_.size();
+  size_t max_pts = 0;
+  for (size_t i = (n > 16 ? n - 16 : 0); i < n; ++i) max_pts = std::max(max_pts, laser_scans_[i].scan.getNbPoints());
+  ensureRing(max_pts);
+  return residentScan(index);
+}
+
 uint64_t LaserTrack::uploadScan(const DataPoints& c) const {
   const int off = c.descriptorOffset("normals");
   LS_CHECK(off >= 0, "scan without normals");
@@ -477,7 +488,7 @@ void LaserTrack::prefetchLaserScan(const LaserScan& scan) {
 
 // device ring large enough for the sub-map + the reading; (re)created when a larger scan shows up.  A track of its own
 // keeps nscan_in_sub_map + 3 slots; a hosted track shares its host's ring (ring_slots_per_track_ slots per track).
-void LaserTrack::ensureRing(size_t max_pts) {
+void LaserTrack::ensureRing(size_t max_pts) const {
   const int want_cap = owns_ctx_ ? std::max(8, params_.nscan_in_sub_map + 3) : *map_capacity_p_;
   if (!*map_p_ || (int)max_pts > *map_max_pts_p_ || want_cap > *map_capacity_p_) {
     LS_CHECK(owns_ctx_ || !*map_p_, "a scan larger than the shared ring's slots arrived (the host sizes the ring from the first scans)");

@@ -1,5 +1,5 @@
 """Workload for compute-sanitizer (memcheck / racecheck / synccheck): the smoke registration plus one batched launch of four
-small scan-to-sub-map problems, a normals estimate, a pose-graph solve with marginals and the input-side kernels -- every kernel family of the
+small scan-to-sub-map problems, a normals estimate, a pose-graph solve with marginals, the input-side kernels and a short local-map sequence -- every kernel family of the
 library on inputs small enough for the tool's ~100x slow-down.  Results are still checked against the oracle."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -46,4 +46,22 @@ offs = [0, 100, 100, 1500, 4096]
 Tp = [np.eye(4, dtype=np.float32)] + [(np.linalg.inv(truth[0]) @ truth[k]).astype(np.float32) for k in (1, 2, 3)]
 Tf = oracle.rigid_inverse_f32(Tp[3])
 assert np.array_equal(ls.deskew_revolution(pts, offs, Tp, Tf), oracle.deskew_revolution(pts, offs, Tp, Tf))
+# resident local map: append, crop, voxel grid with a minimum count, split, transform, queue (one regrowth)
+from oracle import local_map as olm
+lmp = dict(distance_to_consider_fixed=12.0, voxel_size_m=0.5, minimum_point_number_per_voxel=2, remove_ground_from_local_map=True)
+lm, olmap = ls.LocalMap(ctx, initial_capacity_points=4096, **lmp), olm.LocalMap(**lmp)
+for k in range(4):
+    Tw = ls.correct_rigid(truth[k].astype(np.float32))
+    assert lm.add_scan(mp, sid[k], Tw, float(truth[k][2, 3])) == olmap.add_scan(sc[k][0], Tw, float(truth[k][2, 3]))
+    if k == 2:
+        lm.transform(Tp[1])
+        olmap.update_local_map(Tp[1])
+        assert len(olmap.local_map_filtered) > 0
+        assert np.array_equal(lm.download(ls.LM_LOCAL_FILTERED), olmap.local_map_filtered)
+    if k % 2 == 1:
+        assert np.array_equal(lm.get_filtered_map(truth[k][:3, 3]), olmap.get_filtered_map(truth[k][:3, 3]))
+        assert np.array_equal(lm.download(ls.LM_LOCAL), olmap.local_map)
+        q, oq = lm.take_queue(), olmap.get_queued_points()
+        assert len(q) == len(oq) and all(np.array_equal(a, b) for a, b in zip(q, oq))
+lm.close()
 print("sanitize workload ok:", g["stats"].iterations, "iterations;", len(batch), "batched problems;", ctx.launch_count, "launches")
