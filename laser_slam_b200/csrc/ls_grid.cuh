@@ -486,9 +486,9 @@ struct Collector {
 
 // Try to answer the capped query (qx,qy,qz) from list i, whose header `v` = vq[i] and first candidate `c0` =
 // vpts[i] the caller has already loaded (both addresses are known up front, so the common case -- a one-candidate
-// list -- costs a single round trip to memory).  true: `b` is exactly what nn_search(.., cap_d2) returns (b.pos < 0:
-// nothing within the cap; b.idx is NOT filled in) and cbest = the match's {x, y, z, sorted position}.  false: no valid
-// certificate, run the search.
+// list -- costs a single round trip to memory; a longer list costs one more, its other planes being loaded together).
+// true: `b` is exactly what nn_search(.., cap_d2) returns (b.pos < 0: nothing within the cap; b.idx is NOT filled in)
+// and cbest = the match's {x, y, z, sorted position}.  false: no valid certificate, run the search.
 LS_HD bool vlist_query(const VLists& L, const float4* pts, int i, const float4 v, const float4 c0, float qx, float qy,
                        float qz, float cap_d2, Best& b, float4& cbest) {
   const unsigned int bits = (unsigned int)f2i(v.w);
@@ -501,8 +501,7 @@ LS_HD bool vlist_query(const VLists& L, const float4* pts, int i, const float4 v
   b.d2 = cap_d2;
   b.idx = INT_MAX;
   b.pos = -1;
-  for (int k = 0; k < cnt; ++k) {
-    const float4 c = k == 0 ? c0 : ld_state4(L.vpts + (size_t)k * L.n + i);
+  auto take = [&](const float4 c) {  // candidates in ascending k: the order decides nothing but ties
     const float d = dist2(qx, qy, qz, c.x, c.y, c.z);
     const int cpos = f2i(c.w);
     if (d < b.d2) {
@@ -516,6 +515,18 @@ LS_HD bool vlist_query(const VLists& L, const float4* pts, int i, const float4 v
         cbest = c;
       }
     }
+  };
+  if (cnt > 0) take(c0);  // cnt == 0: nothing within R_v, plane 0 holds no candidate of this list
+  // The other planes are independent loads: issue four before comparing any (fixed slots, as in scan_range).  Seven
+  // slots, the whole list in one group, measured no faster on the H100 (DESIGN.md §7).
+  for (int k0 = 1; k0 < cnt; k0 += 4) {
+    float4 cs[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u)  // every slot assigned: a slot left unwritten put the array in local memory
+      cs[u] = k0 + u < cnt ? ld_state4(L.vpts + (size_t)(k0 + u) * L.n + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+      if (k0 + u < cnt) take(cs[u]);
   }
   // b.d2 == cap_d2 when nothing was accepted: then the certificate must cover the whole cap
   return b.d2 * 1.00001f <= Rc * Rc;
