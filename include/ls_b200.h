@@ -321,6 +321,63 @@ int ls_local_map_take_queue(ls_local_map* lm, float* out4, int cap_points, int* 
 int ls_local_map_transform(ls_local_map* lm, const float T[16]);
 int ls_local_map_clear(ls_local_map* lm);
 
+/* ---- resident occupancy map: laser_to_octomap's insertion loop (laser_slam_tools/src/laser_to_octomap.cpp) ------------
+ * Every scan of a trajectory inserted at its pose into a voxel map of float log-odds, the job volumetric_mapping's
+ * OctomapManager does for the tool on one CPU thread.  The rules (oracle/OCCUPANCY.md):
+ *   points      the slot's scan moved by T_w_scan (float32, the ls_map_assemble arithmetic; an exact identity copies it);
+ *               the ray origin is T_w_scan's translation column; a point with a non-finite coordinate casts no ray
+ *   keys        floor(c * (1/resolution)) + 32768 per axis in double, valid iff in [0, 65535]; packed kx | ky<<16 | kz<<32;
+ *               a voxel's centre is (float)((k - 32768 + 0.5) * resolution)
+ *   one ray     within max_range (or max_range < 0): free cells = the DDA keys from the origin to the point, the point's key
+ *               occupied if valid; beyond it: free cells only, to origin + dir * max_range.  The DDA is octomap's
+ *               computeRayKeys (origin key and every key stepped into before the end key; none when an end key is invalid
+ *               or both ends share a key)
+ *   one scan    a point whose endpoint key an earlier in-range point of the scan already has casts no ray; occupied wins
+ *               over free; each touched voxel gets one update v = clamp(v + L_hit or L_miss, L_min, L_max) (float32,
+ *               starting from 0) and becomes known.  A voxel is occupied iff known and v >= L_occ
+ * L = (float)log(p / (1 - p)) of the probabilities below, computed on the host in double.  Scans apply in call order.
+ * The map has its own stream and device buffers and uses none of the context's workspaces, so its calls are legal between
+ * ls_icp_register_submap_batch_begin and _end.  Calls are synchronous; per insert only counters return to the host.
+ * Errors: LS_ERR_STATE for a scan no longer in the ring, LS_ERR_ARG for a ring on another device, a too-small buffer or bad
+ * parameters, LS_ERR_NOMEM when the map cannot grow; the known voxels and their log-odds are unchanged after any error. */
+#define LS_OCC_KNOWN 1    /* every voxel that has had an update */
+#define LS_OCC_OCCUPIED 2 /* known voxels with log-odds >= the occupancy threshold */
+
+typedef struct ls_occupancy ls_occupancy;
+typedef struct ls_occupancy_params {
+  double resolution;          /* voxel edge [m], > 0 (laser_to_octomap: 0.075) */
+  double prob_hit;            /* 0.9 */
+  double prob_miss;           /* 0.4 */
+  double clamp_min;           /* 0.12 */
+  double clamp_max;           /* 0.97 */
+  double occupancy_threshold; /* 0.7 */
+  double max_range;           /* [m]; < 0: unlimited (laser_to_octomap: 20) */
+  int initial_capacity;       /* bricks of 8x8x8 voxels the map starts with; <= 0: 32768.  It grows by doubling */
+} ls_occupancy_params;
+
+typedef struct ls_occupancy_stats {
+  int64_t rays_cast;        /* points that cast a ray */
+  int64_t rays_skipped;     /* points that did not: non-finite, or an endpoint key already occupied in this scan */
+  int64_t free_updates;     /* voxels updated as free by this scan */
+  int64_t occupied_updates; /* voxels updated as occupied by this scan */
+  int64_t known_voxels;     /* known voxels of the map after the scan */
+  int64_t bricks;           /* bricks in use */
+  int64_t device_bytes;     /* device memory the map holds */
+  float device_ms;          /* the insert on the map's stream */
+} ls_occupancy_stats;
+
+void ls_occupancy_default_params(ls_occupancy_params* out);
+int ls_occupancy_create(ls_ctx* ctx, const ls_occupancy_params* params, ls_occupancy** out);
+void ls_occupancy_destroy(ls_occupancy* om);
+/* T_w_scan: the scan's pose (float32, column-major), not corrected.  stats may be NULL. */
+int ls_occupancy_insert_scan(ls_occupancy* om, const ls_map* ring, uint64_t scan_id, const float T_w_scan[16],
+                             ls_occupancy_stats* stats);
+int ls_occupancy_size(ls_occupancy* om, int which, int64_t* n); /* voxels in LS_OCC_* */
+/* The voxels of LS_OCC_* by ascending packed key (x fastest): keys, log-odds and centres {x, y, z, 1}; any output may be
+ * NULL.  cap: voxels the outputs can hold; LS_ERR_ARG without a copy if there are more. */
+int ls_occupancy_download(ls_occupancy* om, int which, uint64_t* keys, float* log_odds, float* centres4, int64_t cap,
+                          int64_t* n);
+
 /* ---- per-scan input filters (reference laser_slam/src/laser_track.cpp:24-30 loads them from
  * LaserTrackParams::icp_input_filters_file, :81 and :146 apply them to every scan before it is stored) ----------------
  * A chain is an array of ls_point_filter records applied in order; each filter sees the cloud the previous one produced,

@@ -80,6 +80,23 @@ class LocalMapParams(ctypes.Structure):
 
 
 LM_LOCAL, LM_LOCAL_FILTERED, LM_DISTANT, LM_FILTERED_MAP, LM_QUEUE = 0, 1, 2, 3, 4
+
+
+class OccupancyParams(ctypes.Structure):
+    """ls_occupancy_params: laser_to_octomap's resolution, hit, miss and max range, volumetric_mapping's clamping and
+    occupancy threshold, and the first number of 8x8x8 bricks."""
+    _fields_ = [("resolution", ctypes.c_double), ("prob_hit", ctypes.c_double), ("prob_miss", ctypes.c_double),
+                ("clamp_min", ctypes.c_double), ("clamp_max", ctypes.c_double), ("occupancy_threshold", ctypes.c_double),
+                ("max_range", ctypes.c_double), ("initial_capacity", ctypes.c_int)]
+
+
+class OccupancyStats(ctypes.Structure):
+    _fields_ = [("rays_cast", ctypes.c_int64), ("rays_skipped", ctypes.c_int64), ("free_updates", ctypes.c_int64),
+                ("occupied_updates", ctypes.c_int64), ("known_voxels", ctypes.c_int64), ("bricks", ctypes.c_int64),
+                ("device_bytes", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
+OCC_KNOWN, OCC_OCCUPIED = 1, 2
 LS_ERR_NOMEM, LS_ERR_STATE = -3, -4
 
 
@@ -173,6 +190,15 @@ def lib():
         L.ls_local_map_take_queue.argtypes = [vp, vp, ci, vp, ci, ctypes.POINTER(ci)]
         L.ls_local_map_transform.argtypes = [vp, vp]
         L.ls_local_map_clear.argtypes = [vp]
+        i64p = ctypes.POINTER(ctypes.c_int64)
+        L.ls_occupancy_default_params.argtypes = [ctypes.POINTER(OccupancyParams)]
+        L.ls_occupancy_default_params.restype = None
+        L.ls_occupancy_create.argtypes = [vp, ctypes.POINTER(OccupancyParams), ctypes.POINTER(vp)]
+        L.ls_occupancy_destroy.argtypes = [vp]
+        L.ls_occupancy_destroy.restype = None
+        L.ls_occupancy_insert_scan.argtypes = [vp, vp, u64, vp, ctypes.POINTER(OccupancyStats)]
+        L.ls_occupancy_size.argtypes = [vp, ci, i64p]
+        L.ls_occupancy_download.argtypes = [vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
         _lib = L
     return _lib
 
@@ -437,6 +463,9 @@ class Context:
 
     def create_local_map(self, **params):
         return LocalMap(self, **params)
+
+    def create_occupancy_map(self, **params):
+        return OccupancyMap(self, **params)
 
 
 class Map:
@@ -752,6 +781,84 @@ class LocalMap:
 
     def clear(self):
         self.ctx._check(lib().ls_local_map_clear(self._h))
+
+
+class OccupancyMap:
+    """laser_to_octomap's occupancy map on the device (ls_occupancy_*): scans of a Map ring inserted at their poses into
+    voxels of float log-odds.  Keyword arguments are the OccupancyParams fields; the defaults are laser_to_octomap's."""
+
+    def __init__(self, ctx, **params):
+        self.ctx = ctx
+        self.params = OccupancyParams()
+        lib().ls_occupancy_default_params(ctypes.byref(self.params))
+        for k, v in params.items():
+            if not hasattr(self.params, k):
+                raise TypeError(f"unknown occupancy map parameter {k!r}")
+            setattr(self.params, k, v)
+        self._h = ctypes.c_void_p()
+        ctx._check(lib().ls_occupancy_create(ctx._h, ctypes.byref(self.params), ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().ls_occupancy_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def insert_scan(self, ring, scan_id, T_w_scan):
+        """Scan `scan_id` of `ring` at pose T_w_scan (4x4, cast to float32, not corrected).  Returns OccupancyStats."""
+        t = colmajor(T_w_scan)
+        st = OccupancyStats()
+        self.ctx._check(lib().ls_occupancy_insert_scan(self._h, ring._h, int(scan_id), t.ctypes.data, ctypes.byref(st)))
+        return st
+
+    def size(self, which=OCC_KNOWN):
+        n = ctypes.c_int64(0)
+        self.ctx._check(lib().ls_occupancy_size(self._h, int(which), ctypes.byref(n)))
+        return n.value
+
+    def download(self, which=OCC_KNOWN, cap=None):
+        """(keys uint64, log-odds float32, centres (n,4) float32) by ascending packed key."""
+        n = self.size(which) if cap is None else int(cap)
+        keys = np.empty(max(n, 1), np.uint64)
+        lo = np.empty(max(n, 1), np.float32)
+        cen = np.empty((max(n, 1), 4), np.float32)
+        got = ctypes.c_int64(0)
+        self.ctx._check(lib().ls_occupancy_download(self._h, int(which), keys.ctypes.data, lo.ctypes.data, cen.ctypes.data, n,
+                                                    ctypes.byref(got)))
+        m = got.value
+        return keys[:m].copy(), lo[:m].copy(), cen[:m].copy()
+
+    def save_point_cloud(self, path):
+        """The occupied voxels' centres as ASCII .pcd (v0.7, FIELDS x y z) or .ply, chosen by the extension (the job of
+        octomap_to_point_cloud).  Returns the number of points written."""
+        ext = os.path.splitext(path)[1].lower()
+        if ext not in (".pcd", ".ply"):
+            raise ValueError(f"unsupported point cloud extension {ext!r} (.pcd or .ply)")
+        pts = self.download(OCC_OCCUPIED)[2][:, :3]
+        write_point_cloud(path, pts)
+        return len(pts)
+
+
+def write_point_cloud(path, xyz):
+    """ASCII .pcd (v0.7, FIELDS x y z) or .ply of an (n,3) float32 array, by the extension of `path`."""
+    xyz = np.asarray(xyz, np.float32).reshape(-1, 3)
+    ext = os.path.splitext(path)[1].lower()
+    n = len(xyz)
+    if ext == ".pcd":
+        head = ("# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z\nSIZE 4 4 4\nTYPE F F F\n"
+                f"COUNT 1 1 1\nWIDTH {n}\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS {n}\nDATA ascii\n")
+    elif ext == ".ply":
+        head = f"ply\nformat ascii 1.0\nelement vertex {n}\nproperty float x\nproperty float y\nproperty float z\nend_header\n"
+    else:
+        raise ValueError(f"unsupported point cloud extension {ext!r} (.pcd or .ply)")
+    with open(path, "w") as f:
+        f.write(head)
+        np.savetxt(f, xyz, fmt="%.9g")  # nine significant digits give a float32 back exactly
 
 
 def check_rigid(T):

@@ -13,6 +13,7 @@
 #include "../../include/ls_b200.h"
 #include "ls_filters.cuh"
 #include "ls_kernels.cuh"
+#include "ls_occupancy.cuh"
 
 using namespace ls;
 
@@ -1730,6 +1731,134 @@ int ls_local_map_clear(ls_local_map* lm) {
   if (!lm) return LS_ERR_ARG;
   lm->n_local = 0;
   lm->n_filt = 0;
+  return LS_OK;
+}
+
+}  // extern "C"
+
+// ---- resident occupancy map (laser_to_octomap's insertion loop; kernels in ls_occupancy.cu) ------------------------------
+struct ls_occupancy {
+  ls_ctx* ctx = nullptr;
+  lso::Params prm{};
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  lso::Map map;
+};
+
+extern "C" {
+
+void ls_occupancy_default_params(ls_occupancy_params* out) {
+  if (!out) return;
+  out->resolution = 0.075;  // laser_to_octomap.cpp:18-21
+  out->prob_hit = 0.9;
+  out->prob_miss = 0.4;
+  out->max_range = 20.0;
+  out->clamp_min = 0.12;  // volumetric_mapping's defaults
+  out->clamp_max = 0.97;
+  out->occupancy_threshold = 0.7;
+  out->initial_capacity = 0;
+}
+
+int ls_occupancy_create(ls_ctx* ctx, const ls_occupancy_params* params, ls_occupancy** out) {
+  if (!ctx || !out) return LS_ERR_ARG;
+  *out = nullptr;
+  if (!params) return fail(ctx, LS_ERR_ARG, "bad argument");
+  const ls_occupancy_params& p = *params;
+  auto prob = [](double x) { return x > 0.0 && x < 1.0; };
+  if (!(p.resolution > 0.0) || !std::isfinite(p.resolution) || !prob(p.prob_hit) || !prob(p.prob_miss) || !prob(p.clamp_min) ||
+      !prob(p.clamp_max) || !prob(p.occupancy_threshold) || !(p.clamp_min <= p.clamp_max) || std::isnan(p.max_range))
+    return fail(ctx, LS_ERR_ARG, "bad occupancy map parameters (resolution > 0, probabilities in (0, 1), clamp_min <= clamp_max)");
+  CU(cudaSetDevice(ctx->device));
+  auto logodds = [](double x) { return (float)std::log(x / (1.0 - x)); };
+  ls_occupancy* om = new ls_occupancy();
+  om->ctx = ctx;
+  om->prm = lso::Params{p.resolution, 1.0 / p.resolution, p.max_range, logodds(p.prob_hit), logodds(p.prob_miss),
+                        logodds(p.clamp_min), logodds(p.clamp_max), logodds(p.occupancy_threshold)};
+  int bricks = 32768;
+  if (p.initial_capacity > 0) bricks = p.initial_capacity < (1 << 24) ? p.initial_capacity : (1 << 24);
+  int rc = LS_OK;
+  if (cudaStreamCreateWithFlags(&om->stream, cudaStreamNonBlocking) != cudaSuccess ||
+      cudaEventCreate(&om->ev0) != cudaSuccess || cudaEventCreate(&om->ev1) != cudaSuccess) {
+    cudaGetLastError();
+    rc = LS_ERR_NOMEM;
+  }
+  if (!rc) rc = lso::init(om->map, bricks, om->stream);
+  if (rc) {
+    ls_occupancy_destroy(om);
+    return fail(ctx, rc, "occupancy map creation failed");
+  }
+  *out = om;
+  return LS_OK;
+}
+
+void ls_occupancy_destroy(ls_occupancy* om) {
+  if (!om) return;
+  cudaSetDevice(om->ctx->device);
+  if (om->stream) cudaStreamSynchronize(om->stream);
+  lso::release(om->map);
+  if (om->ev0) cudaEventDestroy(om->ev0);
+  if (om->ev1) cudaEventDestroy(om->ev1);
+  if (om->stream) cudaStreamDestroy(om->stream);
+  delete om;
+}
+
+int ls_occupancy_insert_scan(ls_occupancy* om, const ls_map* ring, uint64_t scan_id, const float T_w_scan[16],
+                             ls_occupancy_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!ring || !T_w_scan) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (ring->ctx->device != ctx->device)
+    return fail(ctx, LS_ERR_ARG, "the ring is on device %d, the occupancy map on device %d", ring->ctx->device, ctx->device);
+  CU(cudaSetDevice(ctx->device));
+  const ls_scan_slot* s = find_slot(ring, scan_id);
+  if (!s) return fail(ctx, LS_ERR_STATE, "scan %llu is not resident (evicted or never pushed)", (unsigned long long)scan_id);
+  if (wait_slot(s, om->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
+  CU(cudaEventRecord(om->ev0, om->stream));
+  lso::Counters c;
+  const int rc = lso::insert(om->map, om->prm, s->pts, s->n, T_w_scan, is_identity16(T_w_scan), om->stream, &c, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "occupancy map growth failed" : "occupancy map insert failed");
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    stats->rays_cast = c.rays_cast;
+    stats->rays_skipped = c.rays_skipped;
+    stats->free_updates = (int64_t)c.free_upd;
+    stats->occupied_updates = (int64_t)c.occ_upd;
+    stats->known_voxels = om->map.n_known;
+    stats->bricks = om->map.pool_n;
+    stats->device_bytes = (int64_t)lso::device_bytes(om->map);
+    stats->device_ms = ms;
+  }
+  return LS_OK;
+}
+
+int ls_occupancy_size(ls_occupancy* om, int which, int64_t* n) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!n || (which != LS_OCC_KNOWN && which != LS_OCC_OCCUPIED)) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  long long m = 0;
+  const int rc = lso::count(om->map, om->prm, which, &m, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "occupancy map count failed");
+  *n = m;
+  return LS_OK;
+}
+
+int ls_occupancy_download(ls_occupancy* om, int which, uint64_t* keys, float* log_odds, float* centres4, int64_t cap,
+                          int64_t* n) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!n || (which != LS_OCC_KNOWN && which != LS_OCC_OCCUPIED)) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  long long m = 0;
+  int rc = lso::count(om->map, om->prm, which, &m, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "occupancy map count failed");
+  if (m > cap) return fail(ctx, LS_ERR_ARG, "buffers of %lld voxels for %lld", (long long)cap, m);
+  rc = lso::download(om->map, om->prm, which, m, keys, log_odds, centres4, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "occupancy map download failed");
+  *n = m;
   return LS_OK;
 }
 

@@ -1,0 +1,69 @@
+// Resident occupancy map (ls_occupancy_*): laser_to_octomap's scan insertion on the device.  The rules are
+// oracle/OCCUPANCY.md; the layout and kernels are described in ls_occupancy.cu and DESIGN.md.
+#pragma once
+#include <cstddef>
+#include <cstdint>
+
+#include <cuda_runtime.h>
+
+namespace lso {
+
+// The rules' constants: log-odds computed on the host in double and rounded to float once.
+struct Params {
+  double res, inv, max_range;
+  float l_hit, l_miss, l_min, l_max, l_occ;
+};
+
+// Device counters of one insert (or export), copied back whole.
+struct Counters {
+  unsigned long long free_upd, occ_upd, new_known, n_out;
+  int pool_n, n_touched, overflow, rays_cast, rays_skipped, pad[3];
+};
+
+// Bricks of 8x8x8 voxels.  The hash maps a brick key (13 bits per axis) to a pool index; per brick the pool holds 512
+// float log-odds, 16 words of known bits and 16 + 16 words of per-scan free / occupied marks.
+struct Map {
+  int tab_cap = 0;  // power of two
+  unsigned long long* tab_keys = nullptr;
+  int* tab_vals = nullptr;
+  int pool_cap = 0, pool_n = 0;
+  float* lo = nullptr;
+  unsigned *known = nullptr, *mfree = nullptr, *mocc = nullptr;
+  unsigned long long* bkey = nullptr;  // brick key of each pool brick
+  unsigned* touched = nullptr;         // per brick: marked in this scan
+  int* tlist = nullptr;                // bricks marked in this scan
+  // per-scan scratch: ray ends, endpoint keys and classes; the endpoint-key -> first point index table
+  int pt_cap = 0;
+  float4* ends = nullptr;
+  unsigned long long* pkey = nullptr;
+  int* cls = nullptr;
+  int ep_cap = 0;
+  unsigned long long* ep_keys = nullptr;
+  int* ep_min = nullptr;
+  // export scratch
+  long long ex_cap = 0;
+  unsigned long long* ex_k[2] = {nullptr, nullptr};
+  unsigned* ex_v[2] = {nullptr, nullptr};
+  float4* ex_c = nullptr;
+  void* cub_tmp = nullptr;
+  size_t cub_bytes = 0;
+  Counters* cnt_dev = nullptr;
+  Counters* cnt_host = nullptr;  // pinned
+  long long n_known = 0;
+};
+
+// All return LS_OK, LS_ERR_NOMEM or LS_ERR_CUDA (include/ls_b200.h) and count their launches in *launches.
+int init(Map& m, int initial_bricks, cudaStream_t st);
+void release(Map& m);
+// One scan of n points (device, float4) moved by T (column-major float32; identity: copied).  Synchronous; *out holds the
+// scan's counters.  On an error the known voxels and their log-odds are unchanged.
+int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16], bool identity, cudaStream_t st, Counters* out,
+           uint64_t* launches);
+// which: LS_OCC_KNOWN or LS_OCC_OCCUPIED.  count() gives the number of voxels; download() writes n of them (as counted)
+// by ascending packed key: keys, log-odds and centres {x, y, z, 1}, each output may be NULL.
+int count(Map& m, const Params& P, int which, long long* n, cudaStream_t st, uint64_t* launches);
+int download(Map& m, const Params& P, int which, long long n, uint64_t* keys, float* log_odds, float* centres4, cudaStream_t st,
+             uint64_t* launches);
+size_t device_bytes(const Map& m);
+
+}  // namespace lso

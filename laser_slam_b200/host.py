@@ -264,3 +264,57 @@ class LocalMap:
 
     def clear_local_map(self):
         self._check(lib().lsh_local_map_clear(self._h))
+
+
+class OccupancyMap:
+    """laser_slam::OccupancyMap (include/laser_slam/occupancy_map.hpp) on an Estimator: laser_to_octomap's insertion of
+    every track's scans.  Keyword arguments are laser_slam_b200.OccupancyParams' fields.  Close it before the estimator."""
+
+    def __init__(self, estimator, resolution=0.075, prob_hit=0.9, prob_miss=0.4, clamp_min=0.12, clamp_max=0.97,
+                 occupancy_threshold=0.7, max_range=20.0, initial_capacity=0):
+        L = lib()
+        if not hasattr(L, "_occ_bound"):
+            vp, ci, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
+            L.lsh_occupancy_create.restype = vp
+            L.lsh_occupancy_create.argtypes = [vp, vp, ci, ctypes.c_char_p, ci]
+            L.lsh_occupancy_destroy.argtypes = [vp]
+            L.lsh_occupancy_destroy.restype = None
+            L.lsh_occupancy_last_error.argtypes = [vp]
+            L.lsh_occupancy_last_error.restype = ctypes.c_char_p
+            L.lsh_occupancy_insert_laser_tracks.argtypes = [vp]
+            L.lsh_occupancy_voxels.argtypes = [vp, ci, vp, vp, i64]
+            L.lsh_occupancy_voxels.restype = i64
+            L.lsh_occupancy_occupied_cloud.argtypes = [vp, vp, ci]
+            L._occ_bound = True
+        prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range], np.float64)
+        err = ctypes.create_string_buffer(512)
+        self._h = L.lsh_occupancy_create(estimator._h, prm.ctypes.data, int(initial_capacity), err, 512)
+        if not self._h:
+            raise LsError(err.value.decode() or "lsh_occupancy_create failed")
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().lsh_occupancy_destroy(self._h)
+            self._h = None
+
+    def _check(self, rc):
+        if rc < 0:
+            raise LsError(lib().lsh_occupancy_last_error(self._h).decode())
+        return rc
+
+    def insert_laser_tracks(self):
+        return self._check(lib().lsh_occupancy_insert_laser_tracks(self._h))
+
+    def voxels(self, which=1):
+        """(keys uint64, log-odds float32) of LS_OCC_KNOWN (1) or LS_OCC_OCCUPIED (2), by ascending key."""
+        n = self._check(lib().lsh_occupancy_voxels(self._h, which, None, None, 0))
+        keys = np.zeros(max(n, 1), np.uint64)
+        lo = np.zeros(max(n, 1), np.float32)
+        self._check(lib().lsh_occupancy_voxels(self._h, which, keys.ctypes.data, lo.ctypes.data, n))
+        return keys[:n], lo[:n]
+
+    def occupied_cloud(self):
+        n = self._check(lib().lsh_occupancy_occupied_cloud(self._h, None, 0))
+        out = np.zeros((max(n, 1), 4), np.float32)
+        self._check(lib().lsh_occupancy_occupied_cloud(self._h, out.ctypes.data, n))
+        return out[:n]

@@ -8,6 +8,7 @@
 
 #include "laser_slam/incremental_estimator.hpp"
 #include "laser_slam/local_map.hpp"
+#include "laser_slam/occupancy_map.hpp"
 #include "laser_slam/velodyne_assembler.hpp"
 
 using namespace laser_slam;
@@ -372,6 +373,80 @@ int lsh_assembler_add_packet(void* av, const float* pts4, int n, const float* T_
     if (stamp_out) *stamp_out = (int64_t)st;
     return 1;
   } catch (const std::exception&) {
+    return LS_ERR_STATE;
+  }
+}
+
+// ---- laser_slam::OccupancyMap (include/laser_slam/occupancy_map.hpp) on an estimator, for the tests.  Destroy it before
+// the estimator.  prm: resolution, hit, miss, clamp min, clamp max, occupancy threshold, max range.
+struct OccupancyHandle {
+  std::unique_ptr<OccupancyMap> map;
+  std::string err;
+};
+
+void* lsh_occupancy_create(void* hv, const double* prm, int initial_capacity_bricks, char* err, int errlen) {
+  try {
+    OccupancyMapParams p;
+    p.resolution = prm[0];
+    p.probability_hit = prm[1];
+    p.probability_miss = prm[2];
+    p.clamping_thres_min = prm[3];
+    p.clamping_thres_max = prm[4];
+    p.occupancy_thres = prm[5];
+    p.sensor_max_range = prm[6];
+    p.initial_capacity_bricks = initial_capacity_bricks;
+    OccupancyHandle* h = new OccupancyHandle();
+    h->map.reset(new OccupancyMap(p, *static_cast<Handle*>(hv)->est));
+    return h;
+  } catch (const std::exception& e) {
+    if (err && errlen > 0) std::strncpy(err, e.what(), (size_t)errlen - 1), err[errlen - 1] = 0;
+    return nullptr;
+  }
+}
+void lsh_occupancy_destroy(void* ov) { delete static_cast<OccupancyHandle*>(ov); }
+const char* lsh_occupancy_last_error(void* ov) { return static_cast<OccupancyHandle*>(ov)->err.c_str(); }
+
+// insertLaserTracks; returns the scans inserted
+int lsh_occupancy_insert_laser_tracks(void* ov) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    return (int)h->map->insertLaserTracks();
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// getVoxels (keys / log_odds may be NULL: count only); returns the number of voxels, written when it is <= cap
+int64_t lsh_occupancy_voxels(void* ov, int which, uint64_t* keys, float* log_odds, int64_t cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<uint64_t> k;
+    std::vector<float> v;
+    h->map->getVoxels(which, &k, &v);
+    const int64_t n = (int64_t)k.size();
+    if (keys && log_odds && n <= cap) {
+      std::memcpy(keys, k.data(), sizeof(uint64_t) * (size_t)n);
+      std::memcpy(log_odds, v.data(), sizeof(float) * (size_t)n);
+    }
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// getOccupiedCloud; returns its number of points, written when it is <= cap
+int lsh_occupancy_occupied_cloud(void* ov, float* out4, int cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    DataPoints d;
+    h->map->getOccupiedCloud(&d);
+    const int n = (int)d.getNbPoints();
+    if (out4 && n <= cap) std::memcpy(out4, static_cast<const DataPoints&>(d).features.data(), sizeof(float) * 4 * (size_t)n);
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
     return LS_ERR_STATE;
   }
 }

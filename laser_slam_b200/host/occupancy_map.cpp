@@ -1,0 +1,96 @@
+// laser_slam::OccupancyMap over ls_occupancy_* (include/laser_slam/occupancy_map.hpp).
+#include "laser_slam/occupancy_map.hpp"
+
+#include <algorithm>
+#include <stdexcept>
+#include <string>
+#include <tuple>
+
+namespace laser_slam {
+
+namespace {
+void throwOnError(ls_ctx* ctx, int rc, const char* what) {
+  if (rc < 0) throw std::runtime_error(std::string(what) + ": " + ls_b200_last_error(ctx));
+}
+}  // namespace
+
+OccupancyMap::OccupancyMap(const OccupancyMapParams& params, IncrementalEstimator& estimator)
+    : params_(params), estimator_(estimator), ctx_(estimator.trackContext()) {
+  ls_occupancy_params p;
+  ls_occupancy_default_params(&p);
+  p.resolution = params.resolution;
+  p.prob_hit = params.probability_hit;
+  p.prob_miss = params.probability_miss;
+  p.clamp_min = params.clamping_thres_min;
+  p.clamp_max = params.clamping_thres_max;
+  p.occupancy_threshold = params.occupancy_thres;
+  p.max_range = params.sensor_max_range;
+  p.initial_capacity = params.initial_capacity_bricks;
+  throwOnError(ctx_, ls_occupancy_create(ctx_, &p, &map_), "ls_occupancy_create");
+}
+
+OccupancyMap::~OccupancyMap() { ls_occupancy_destroy(map_); }
+
+void OccupancyMap::insertScan(const LaserTrack& laser_track, const Time& time_ns, ls_occupancy_stats* stats) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  Trajectory trajectory;
+  laser_track.getTrajectory(&trajectory);
+  const PointMatcher::TransformationParameters T =
+      PointMatcher::TransformationParameters::cast(trajectory.at(time_ns).getTransformationMatrix());
+  const uint64_t id = laser_track.residentScanAtTime(time_ns);
+  throwOnError(ctx_, ls_occupancy_insert_scan(map_, laser_track.ring(), id, T.data(), stats), "ls_occupancy_insert_scan");
+}
+
+size_t OccupancyMap::insertLaserTracks() {
+  std::vector<std::shared_ptr<LaserTrack> > tracks = estimator_.getAllLaserTracks();
+  std::vector<std::tuple<Time, size_t, size_t> > order;  // (time, track, scan)
+  for (size_t k = 0; k < tracks.size(); ++k) {
+    const std::vector<LaserScan>& scans = tracks[k]->getLaserScans();
+    for (size_t j = 0; j < scans.size(); ++j) order.emplace_back(scans[j].time_ns, k, j);
+  }
+  std::sort(order.begin(), order.end());
+  bool zero_added = false;
+  size_t inserted = 0;
+  for (const auto& e : order) {
+    const Time t = std::get<0>(e);
+    if (t == 0u) {
+      if (zero_added) continue;
+      zero_added = true;
+    }
+    insertScan(*tracks[std::get<1>(e)], t);
+    ++inserted;
+  }
+  return inserted;
+}
+
+void OccupancyMap::download(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds,
+                            std::vector<float>* centres4) const {
+  std::lock_guard<std::mutex> lock(mutex_);
+  int64_t n = 0;
+  throwOnError(ctx_, ls_occupancy_size(map_, which, &n), "ls_occupancy_size");
+  const size_t m = (size_t)(n > 0 ? n : 1);
+  if (keys) keys->resize(m);
+  if (log_odds) log_odds->resize(m);
+  if (centres4) centres4->resize(4 * m);
+  int64_t got = 0;
+  throwOnError(ctx_,
+               ls_occupancy_download(map_, which, keys ? keys->data() : NULL, log_odds ? log_odds->data() : NULL,
+                                     centres4 ? centres4->data() : NULL, n, &got),
+               "ls_occupancy_download");
+  if (keys) keys->resize((size_t)got);
+  if (log_odds) log_odds->resize((size_t)got);
+  if (centres4) centres4->resize(4 * (size_t)got);
+}
+
+void OccupancyMap::getOccupiedCloud(DataPoints* cloud) const {
+  if (cloud == NULL) throw std::invalid_argument("null output");
+  std::vector<float> c;
+  download(LS_OCC_OCCUPIED, NULL, NULL, &c);
+  *cloud = DataPoints::fromArrays(c.data(), NULL, c.size() / 4);
+}
+
+void OccupancyMap::getVoxels(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds) const {
+  download(which, keys, log_odds, NULL);
+}
+
+}  // namespace laser_slam
