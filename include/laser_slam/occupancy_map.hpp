@@ -1,12 +1,15 @@
 // OccupancyMap -- laser_to_octomap (reference laser_slam_tools/src/laser_to_octomap.cpp) without ROS: every scan of every
 // track of an estimator inserted at its pose into an occupancy map, over the resident map of the C ABI (ls_occupancy_*,
-// include/ls_b200.h).  The octree file format is not written; getOccupiedCloud gives what octomap_to_point_cloud exports
-// (every occupied voxel's centre at the finest resolution).  The rules are oracle/OCCUPANCY.md.
+// include/ls_b200.h).  writeBinary saves the map as octomap's pruned binary tree (.bt), the file laser_to_octomap writes;
+// getOccupiedLeafCloud gives what octomap_to_point_cloud exports from it (the occupied leaves' centres), getOccupiedCloud
+// every occupied voxel's centre at the finest resolution.  The rules are oracle/OCCUPANCY.md and, for the tree,
+// oracle/OCTREE.md.
 #ifndef LASER_SLAM_OCCUPANCY_MAP_HPP_
 #define LASER_SLAM_OCCUPANCY_MAP_HPP_
 
 #include <cstdint>
 #include <mutex>
+#include <string>
 #include <vector>
 
 #include "laser_slam/common.hpp"
@@ -44,6 +47,12 @@ class OccupancyMap {
   size_t insertLaserTracks();
   // The occupied voxels' centres, features only ({x, y, z, 1}), by ascending voxel key.
   void getOccupiedCloud(DataPoints* cloud) const;
+  // octomap's OcTree::writeBinary: the map's max-likelihood states, pruned, as a .bt file (ls_occupancy_write_octomap).
+  // Returns false when the file cannot be written.
+  bool writeBinary(const std::string& filename);
+  // The occupied leaves of the pruned tree in octomap's leaf order, features only ({x, y, z, 1}): what
+  // octomap_to_point_cloud writes from writeBinary's file.
+  void getOccupiedLeafCloud(DataPoints* cloud);
   // (new) LS_OCC_KNOWN or LS_OCC_OCCUPIED voxels: packed keys and log-odds, by ascending key.
   void getVoxels(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds) const;
 

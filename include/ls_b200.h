@@ -378,6 +378,34 @@ int ls_occupancy_size(ls_occupancy* om, int which, int64_t* n); /* voxels in LS_
 int ls_occupancy_download(ls_occupancy* om, int which, uint64_t* keys, float* log_odds, float* centres4, int64_t cap,
                           int64_t* n);
 
+/* The map as octomap's pruned binary tree, what OcTree::writeBinary saves (toMaxLikelihood, prune, writeBinaryConst) and
+ * octomap_to_point_cloud reads back (reference laser_slam_tools/src/octomap_to_point_cloud.cpp).  The rules
+ * (oracle/OCTREE.md):
+ *   states      a known voxel is occupied iff v >= L_occ, else free; a node exists iff a voxel below it is known
+ *   tree        depth 16 over the keys; child i of a node at depth d is bx | by<<1 | bz<<2, b = key bit 15-d per axis.  A node
+ *               at depth 1..15 is a leaf iff its 8 children exist, are leaves and share a state (bottom-up; the root stays)
+ *   payload     the inner nodes in pre-order (children 0..7), 2 bytes each: byte 0 covers children 0-3, byte 1 children 4-7;
+ *               bit pair (2(i%4), 2(i%4)+1) is 00 unknown, 10 free leaf, 01 occupied leaf, 11 inner
+ *   leaves      the occupied leaves in the same pre-order, centre (float)((floor((kc - 32768) / 2^s) + 0.5) * res * 2^s) per
+ *               axis in double (octomap's keyToCoord(key, depth)), s = 16 - depth, kc the node's centre key
+ * The build reads the map only and runs on its stream; an insert afterwards invalidates it, and a download then returns
+ * LS_ERR_STATE.  Legal between ls_icp_register_submap_batch_begin and _end like every ls_occupancy_* call. */
+typedef struct ls_octree_stats {
+  int64_t nodes;           /* every node, root and leaves included (the .bt file's size line); 0 for an empty map */
+  int64_t payload_bytes;   /* 2 per inner node */
+  int64_t occupied_leaves;
+  float device_ms;         /* the build on the map's stream */
+} ls_octree_stats;
+
+int ls_occupancy_build_octree(ls_occupancy* om, ls_octree_stats* stats);
+/* The last build's payload and, each when not NULL, its occupied leaves' centres {x, y, z, 1} and depths (1..16).  payload_cap:
+ * bytes payload can hold; leaf_cap: leaves centres4 and depths can hold; LS_ERR_ARG without a copy if either is too small. */
+int ls_occupancy_download_octree(ls_occupancy* om, uint8_t* payload, int64_t payload_cap, float* centres4, uint8_t* depths,
+                                 int64_t leaf_cap);
+/* The whole .bt file at `path`: octomap's three comment lines, "id OcTree", "size <nodes>", "res <resolution as %g>", "data",
+ * then the payload.  Builds the tree unless the last build is current.  stats may be NULL. */
+int ls_occupancy_write_octomap(ls_occupancy* om, const char* path, ls_octree_stats* stats);
+
 /* ---- per-scan input filters (reference laser_slam/src/laser_track.cpp:24-30 loads them from
  * LaserTrackParams::icp_input_filters_file, :81 and :146 apply them to every scan before it is stored) ----------------
  * A chain is an array of ls_point_filter records applied in order; each filter sees the cloud the previous one produced,

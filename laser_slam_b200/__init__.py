@@ -5,6 +5,7 @@ laser_slam_b200/csrc/Makefile for sm_90a).  The compute path is the CUDA library
 fallback: loading fails loudly when the shared library is missing and ls_b200_init fails when no
 CUDA device is usable.
 """
+import collections
 import ctypes
 import os
 import subprocess
@@ -94,6 +95,11 @@ class OccupancyStats(ctypes.Structure):
     _fields_ = [("rays_cast", ctypes.c_int64), ("rays_skipped", ctypes.c_int64), ("free_updates", ctypes.c_int64),
                 ("occupied_updates", ctypes.c_int64), ("known_voxels", ctypes.c_int64), ("bricks", ctypes.c_int64),
                 ("device_bytes", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
+class OctreeStats(ctypes.Structure):
+    _fields_ = [("nodes", ctypes.c_int64), ("payload_bytes", ctypes.c_int64), ("occupied_leaves", ctypes.c_int64),
+                ("device_ms", ctypes.c_float)]
 
 
 OCC_KNOWN, OCC_OCCUPIED = 1, 2
@@ -199,6 +205,9 @@ def lib():
         L.ls_occupancy_insert_scan.argtypes = [vp, vp, u64, vp, ctypes.POINTER(OccupancyStats)]
         L.ls_occupancy_size.argtypes = [vp, ci, i64p]
         L.ls_occupancy_download.argtypes = [vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
+        L.ls_occupancy_build_octree.argtypes = [vp, ctypes.POINTER(OctreeStats)]
+        L.ls_occupancy_download_octree.argtypes = [vp, vp, ctypes.c_int64, vp, vp, ctypes.c_int64]
+        L.ls_occupancy_write_octomap.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(OctreeStats)]
         _lib = L
     return _lib
 
@@ -842,6 +851,126 @@ class OccupancyMap:
         pts = self.download(OCC_OCCUPIED)[2][:, :3]
         write_point_cloud(path, pts)
         return len(pts)
+
+    def octree(self):
+        """The map as octomap's pruned tree, built on the device (ls_occupancy_build_octree): Octree(nodes, payload bytes,
+        occupied leaves' centres (n,4) float32 and depths uint8 in pre-order, device ms)."""
+        st = OctreeStats()
+        self.ctx._check(lib().ls_occupancy_build_octree(self._h, ctypes.byref(st)))
+        pay = np.empty(max(st.payload_bytes, 1), np.uint8)
+        cen = np.empty((max(st.occupied_leaves, 1), 4), np.float32)
+        dep = np.empty(max(st.occupied_leaves, 1), np.uint8)
+        self.ctx._check(lib().ls_occupancy_download_octree(self._h, pay.ctypes.data, st.payload_bytes, cen.ctypes.data,
+                                                           dep.ctypes.data, st.occupied_leaves))
+        n = st.occupied_leaves
+        return Octree(st.nodes, pay[:st.payload_bytes].tobytes(), cen[:n].copy(), dep[:n].copy(), st.device_ms)
+
+    def save_octomap(self, path):
+        """The map as an octomap binary file (.bt, OcTree::writeBinary), readable by octomap::OcTree(path).  Returns its
+        node count."""
+        st = OctreeStats()
+        self.ctx._check(lib().ls_occupancy_write_octomap(self._h, os.fsencode(path), ctypes.byref(st)))
+        return st.nodes
+
+    def save_pruned_point_cloud(self, path):
+        """The occupied leaves of the pruned tree as .pcd / .ply: what octomap_to_point_cloud writes from this map's .bt
+        file.  Returns the number of points written."""
+        ext = os.path.splitext(path)[1].lower()
+        if ext not in (".pcd", ".ply"):
+            raise ValueError(f"unsupported point cloud extension {ext!r} (.pcd or .ply)")
+        pts = self.octree().centres[:, :3]
+        write_point_cloud(path, pts)
+        return len(pts)
+
+
+Octree = collections.namedtuple("Octree", "nodes payload centres depths device_ms")
+
+_BT_FIRST_LINE = b"# Octomap OcTree binary file"
+
+
+def read_octomap(path):
+    """Parse an octomap binary file (.bt) as octomap::OcTree(path) reads it, on the CPU.  Returns a dict: resolution, nodes
+    (the header's size), payload, and every leaf in pre-order as first-voxel keys (n,3) int64, depths uint8 and states
+    uint8 (1 free, 2 occupied).  Raises ValueError on a bad header, a truncated payload or a size that does not match."""
+    data = open(path, "rb").read()
+    pos = 0
+
+    def line():
+        nonlocal pos
+        end = data.find(b"\n", pos)
+        if end < 0:
+            raise ValueError(f"{path}: header ends early")
+        s, pos = data[pos:end], end + 1
+        return s.rstrip(b"\r")
+
+    if line() != _BT_FIRST_LINE:
+        raise ValueError(f"{path}: not an octomap binary file (first line)")
+    head = {}
+    while True:
+        s = line()
+        if s.startswith(b"#") or not s.strip():
+            continue
+        if s == b"data":
+            break
+        key, _, value = s.partition(b" ")
+        head[key.decode(errors="replace")] = value.strip().decode(errors="replace")
+    if head.get("id") != "OcTree":
+        raise ValueError(f"{path}: tree type {head.get('id')!r}, expected 'OcTree'")
+    try:
+        size, res = int(head["size"]), float(head["res"])
+    except (KeyError, ValueError) as e:
+        raise ValueError(f"{path}: bad or missing size / res line") from e
+    if size < 0 or not res > 0:
+        raise ValueError(f"{path}: bad size {size} or res {res}")
+    keys, depths, states = [], [], []
+    start, nodes = pos, 0
+    # pre-order walk (children 0 ... 7): an inner node reads its two bytes when it is reached, a leaf is listed
+    stack = [(3, 0, 0, 0, 0)] if size > 0 else []  # bit pair, depth, first-voxel key
+    while stack:
+        bits, d, kx, ky, kz = stack.pop()
+        nodes += 1
+        if bits != 3:
+            keys.append((kx, ky, kz))
+            depths.append(d)
+            states.append(2 if bits == 2 else 1)
+            continue
+        if d >= 16:
+            raise ValueError(f"{path}: inner node at depth 16")
+        if pos + 2 > len(data):
+            raise ValueError(f"{path}: payload truncated")
+        m = data[pos] | (data[pos + 1] << 8)
+        pos += 2
+        sh = 15 - d
+        for i in range(7, -1, -1):
+            b = (m >> (2 * i)) & 3
+            if b:
+                stack.append((b, d + 1, kx | ((i & 1) << sh), ky | (((i >> 1) & 1) << sh), kz | (((i >> 2) & 1) << sh)))
+    if nodes != size:
+        raise ValueError(f"{path}: the header's size {size} does not match the {nodes} nodes of the payload")
+    return dict(resolution=res, nodes=size, payload=data[start:pos], keys=np.array(keys, np.int64).reshape(-1, 3),
+                depths=np.array(depths, np.uint8), states=np.array(states, np.uint8))
+
+
+def leaf_centres(keys, depths, resolution):
+    """octomap's keyToCoord(key, depth) of leaves given by their first-voxel keys (n,3): (n,3) float32."""
+    k = np.asarray(keys, np.int64).reshape(-1, 3)
+    s = (16 - np.asarray(depths, np.int64))[:, None]
+    kc = k + np.where(s > 0, np.left_shift(1, np.maximum(s - 1, 0)), 0)
+    scale = np.left_shift(1, s).astype(np.float64)
+    return ((np.floor((kc.astype(np.float64) - 32768.0) / scale) + 0.5) * (float(resolution) * scale)).astype(np.float32)
+
+
+def octomap_to_point_cloud(bt_path, out_path):
+    """The reference tool octomap_to_point_cloud without PCL: the occupied leaves' centres of a .bt file, in its leaf
+    order, written as .pcd / .ply.  Returns the number of points."""
+    ext = os.path.splitext(out_path)[1].lower()
+    if ext not in (".pcd", ".ply"):
+        raise ValueError(f"unsupported point cloud extension {ext!r} (.pcd or .ply)")
+    t = read_octomap(bt_path)
+    occ = t["states"] == 2
+    pts = leaf_centres(t["keys"][occ], t["depths"][occ], t["resolution"])
+    write_point_cloud(out_path, pts)
+    return len(pts)
 
 
 def write_point_cloud(path, xyz):

@@ -1743,7 +1743,33 @@ struct ls_occupancy {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   lso::Map map;
+  lso::Octree tree;
+  bool tree_current = false;  // the last octree build reflects every insert
+  float tree_ms = 0.f;
 };
+
+namespace {
+int build_tree(ls_occupancy* om) {
+  ls_ctx* ctx = om->ctx;
+  om->tree_current = false;
+  CU(cudaEventRecord(om->ev0, om->stream));
+  const int rc = lso::build_octree(om->map, om->prm, om->tree, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "octree export: out of device memory" : "octree export failed");
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  CU(cudaEventElapsedTime(&om->tree_ms, om->ev0, om->ev1));
+  om->tree_current = true;
+  return LS_OK;
+}
+
+void octree_stats(const ls_occupancy* om, ls_octree_stats* stats) {
+  if (!stats) return;
+  stats->nodes = om->tree.nodes;
+  stats->payload_bytes = om->tree.bytes;
+  stats->occupied_leaves = om->tree.leaves;
+  stats->device_ms = om->tree_ms;
+}
+}  // namespace
 
 extern "C" {
 
@@ -1796,6 +1822,7 @@ void ls_occupancy_destroy(ls_occupancy* om) {
   cudaSetDevice(om->ctx->device);
   if (om->stream) cudaStreamSynchronize(om->stream);
   lso::release(om->map);
+  lso::release(om->tree);
   if (om->ev0) cudaEventDestroy(om->ev0);
   if (om->ev1) cudaEventDestroy(om->ev1);
   if (om->stream) cudaStreamDestroy(om->stream);
@@ -1814,6 +1841,7 @@ int ls_occupancy_insert_scan(ls_occupancy* om, const ls_map* ring, uint64_t scan
   if (!s) return fail(ctx, LS_ERR_STATE, "scan %llu is not resident (evicted or never pushed)", (unsigned long long)scan_id);
   if (wait_slot(s, om->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
   CU(cudaEventRecord(om->ev0, om->stream));
+  om->tree_current = false;
   lso::Counters c;
   const int rc = lso::insert(om->map, om->prm, s->pts, s->n, T_w_scan, is_identity16(T_w_scan), om->stream, &c, &ctx->launches);
   if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "occupancy map growth failed" : "occupancy map insert failed");
@@ -1859,6 +1887,58 @@ int ls_occupancy_download(ls_occupancy* om, int which, uint64_t* keys, float* lo
   rc = lso::download(om->map, om->prm, which, m, keys, log_odds, centres4, om->stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "occupancy map download failed");
   *n = m;
+  return LS_OK;
+}
+
+int ls_occupancy_build_octree(ls_occupancy* om, ls_octree_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  CU(cudaSetDevice(ctx->device));
+  const int rc = build_tree(om);
+  if (rc) return rc;
+  octree_stats(om, stats);
+  return LS_OK;
+}
+
+int ls_occupancy_download_octree(ls_occupancy* om, uint8_t* payload, int64_t payload_cap, float* centres4, uint8_t* depths,
+                                 int64_t leaf_cap) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!om->tree_current) return fail(ctx, LS_ERR_STATE, "no current octree: build it after the last insert");
+  const lso::Octree& t = om->tree;
+  if ((t.bytes > 0 && !payload) || payload_cap < t.bytes)
+    return fail(ctx, LS_ERR_ARG, "a payload buffer of %lld bytes for %lld", (long long)payload_cap, t.bytes);
+  if ((centres4 || depths) && leaf_cap < t.leaves)
+    return fail(ctx, LS_ERR_ARG, "leaf buffers of %lld for %lld occupied leaves", (long long)leaf_cap, t.leaves);
+  CU(cudaSetDevice(ctx->device));
+  const int rc = lso::download_octree(t, payload, centres4, depths, om->stream);
+  if (rc) return fail(ctx, rc, "octree download failed");
+  return LS_OK;
+}
+
+int ls_occupancy_write_octomap(ls_occupancy* om, const char* path, ls_octree_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  int rc;
+  if (!om->tree_current && (rc = build_tree(om))) return rc;
+  std::vector<uint8_t> payload((size_t)om->tree.bytes);
+  if ((rc = lso::download_octree(om->tree, payload.data(), nullptr, nullptr, om->stream)))
+    return fail(ctx, rc, "octree download failed");
+  // octomap's writeBinaryConst: the resolution as a default std::ostream prints a double (%g)
+  char head[256];
+  const int n = std::snprintf(head, sizeof head,
+                              "# Octomap OcTree binary file\n# (feel free to add / change comments, but leave the first line "
+                              "as it is!)\n#\nid OcTree\nsize %lld\nres %g\ndata\n",
+                              om->tree.nodes, om->prm.res);
+  FILE* f = std::fopen(path, "wb");
+  if (!f) return fail(ctx, LS_ERR_ARG, "cannot open %s for writing", path);
+  bool ok = std::fwrite(head, 1, (size_t)n, f) == (size_t)n;
+  if (ok && !payload.empty()) ok = std::fwrite(payload.data(), 1, payload.size(), f) == payload.size();
+  ok = std::fclose(f) == 0 && ok;
+  if (!ok) return fail(ctx, LS_ERR_ARG, "writing %s failed", path);
+  octree_stats(om, stats);
   return LS_OK;
 }
 

@@ -10,6 +10,19 @@
 //                            over free), known bits set, marks cleared
 // Log-odds change only in (c).  When the pool or the hash overflows in (b) the host clears every mark, grows what filled
 // and runs (b) again, so a failed insert leaves the known voxels and their values as they were.
+//
+// Octree export (octomap's writeBinary after toMaxLikelihood and prune; rules in oracle/OCTREE.md), reading the map only:
+//   (d) oct_code_kernel      Morton code of each brick key; a CUB radix sort puts the bricks in pre-order at depth 13
+//   (e) oct_brick_kernel     one block per brick: max-likelihood states of its 512 voxels, levels 15, 14 and 13 pruned in
+//                            shared memory, the brick's state and subtree totals (nodes, payload bytes, occupied leaves)
+//   (f) oct_up_kernel        one block: levels 12 ... 0, each level's sorted list segmented by code >> 3 with a block scan,
+//                            collapse or inner per parent (the root never collapses), subtree totals summed
+//   the three totals of the root come back once and size the outputs
+//   (g) oct_down_kernel      one block: levels 0 ... 12, each inner node's two bytes, its children's offsets (its own + 2 +
+//                            the earlier siblings' totals) and the centres of occupied leaves above the bricks
+//   (h) oct_emit_kernel      one block per inner brick: (e)'s tree again, its pre-order bytes and occupied leaves written at
+//                            the offsets (g) gave it, so no per-brick staging is kept
+// A brick without a known voxel (an insert that failed after placing it leaves one) has state 0 and adds nothing.
 #include <cfloat>
 #include <cstdint>
 #include <cstring>
@@ -354,6 +367,268 @@ __global__ void occ_centres_kernel(const unsigned long long* __restrict__ keys, 
   }
 }
 
+// ---- octree export ---------------------------------------------------------------------------------------------------
+constexpr int kTreeThreads = 1024;  // (f) and (g)
+constexpr int kBrickDepth = 13;
+
+// Node states: 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner -- also the bit pair of the payload.
+// octomap's isNodeCollapsible after toMaxLikelihood: all 8 children exist, are leaves and have one state.
+__device__ __forceinline__ int parent_state(int n_free, int n_occ, int n_any, bool may_prune) {
+  if (may_prune && n_free == 8) return 1;
+  if (may_prune && n_occ == 8) return 2;
+  return n_any ? 3 : 0;
+}
+
+__device__ __forceinline__ unsigned long long spread3(unsigned v) {  // bit j to bit 3j, 13 bits
+  unsigned long long x = 0;
+  for (int j = 0; j < 13; ++j) x |= (unsigned long long)((v >> j) & 1u) << (3 * j);
+  return x;
+}
+__device__ __forceinline__ int squeeze3(unsigned long long x) {  // bit 3j to bit j
+  int v = 0;
+  for (int j = 0; j < 13; ++j) v |= (int)((x >> (3 * j)) & 1ull) << j;
+  return v;
+}
+
+// Morton index t within a brick (x, y, z bits of key bit 2, then 1, then 0) -> pool-local index x | y << 3 | z << 6
+__device__ __forceinline__ int morton_local(int t) {
+  const int x = (t & 1) | ((t >> 2) & 2) | ((t >> 4) & 4);
+  const int y = ((t >> 1) & 1) | ((t >> 3) & 2) | ((t >> 5) & 4);
+  const int z = ((t >> 2) & 1) | ((t >> 4) & 2) | ((t >> 6) & 4);
+  return x | (y << 3) | (z << 6);
+}
+
+__device__ __forceinline__ int mask8(const unsigned char* s) {
+  int m = 0;
+  for (int i = 0; i < 8; ++i) m |= (int)s[i] << (2 * i);
+  return m;
+}
+
+// octomap's keyToCoord(key, depth) of the node whose first voxel key is k0, s = 16 - depth
+__device__ __forceinline__ float leaf_coord(int k0, int s, double res) {
+  const int kc = k0 + (s > 0 ? 1 << (s - 1) : 0);
+  const double scale = (double)(1 << s);
+  return (float)((floor(((double)kc - (double)kKeyMax) / scale) + 0.5) * (res * scale));
+}
+
+__device__ __forceinline__ void put_leaf(float4* cen, unsigned char* dep, unsigned long long i, int kx, int ky, int kz,
+                                         int depth, double res) {
+  const int s = 16 - depth;
+  cen[i] = make_float4(leaf_coord(kx, s, res), leaf_coord(ky, s, res), leaf_coord(kz, s, res), 1.0f);
+  dep[i] = (unsigned char)depth;
+}
+
+struct BrickTree {
+  unsigned char s16[512], s15[64], s14[8];
+  int n15[64], l15[64], n14[8], l14[8], b14[8];
+  int st, nodes, bytes, leaves;  // the depth-13 node
+};
+
+// One block of 512 threads: thread t reads the voxel of Morton index t, then the brick's levels 15, 14 and 13.
+__device__ void brick_tree(const unsigned* __restrict__ known, const float* __restrict__ lo, int b, float l_occ, BrickTree& T) {
+  const int t = threadIdx.x;
+  const int v = morton_local(t);
+  int s = 0;
+  if ((known[(size_t)b * 16 + (v >> 5)] >> (v & 31)) & 1u) s = lo[(size_t)b * 512 + v] >= l_occ ? 2 : 1;
+  T.s16[t] = (unsigned char)s;
+  __syncthreads();
+  if (t < 64) {
+    int nf = 0, no = 0, na = 0;
+    for (int i = 0; i < 8; ++i) {
+      const int c = T.s16[8 * t + i];
+      nf += c == 1, no += c == 2, na += c != 0;
+    }
+    const int st = parent_state(nf, no, na, true);
+    T.s15[t] = (unsigned char)st;
+    T.n15[t] = st == 3 ? 1 + na : st != 0;
+    T.l15[t] = st == 3 ? no : st == 2;
+  }
+  __syncthreads();
+  if (t < 8) {
+    int nf = 0, no = 0, na = 0, n = 0, l = 0, by = 0;
+    for (int i = 0; i < 8; ++i) {
+      const int c = T.s15[8 * t + i];
+      nf += c == 1, no += c == 2, na += c != 0;
+      n += T.n15[8 * t + i], l += T.l15[8 * t + i], by += c == 3 ? 2 : 0;
+    }
+    const int st = parent_state(nf, no, na, true);
+    T.s14[t] = (unsigned char)st;
+    T.n14[t] = st == 3 ? 1 + n : st != 0;
+    T.l14[t] = st == 3 ? l : st == 2;
+    T.b14[t] = st == 3 ? 2 + by : 0;
+  }
+  __syncthreads();
+  if (t == 0) {
+    int nf = 0, no = 0, na = 0, n = 0, l = 0, by = 0;
+    for (int i = 0; i < 8; ++i) {
+      const int c = T.s14[i];
+      nf += c == 1, no += c == 2, na += c != 0;
+      n += T.n14[i], l += T.l14[i], by += T.b14[i];
+    }
+    const int st = parent_state(nf, no, na, true);
+    T.st = st;
+    T.nodes = st == 3 ? 1 + n : st != 0;
+    T.leaves = st == 3 ? l : st == 2;
+    T.bytes = st == 3 ? 2 + by : 0;
+  }
+  __syncthreads();
+}
+
+// Node records (Octree): bricks first, then each upper level.
+struct Nodes {
+  unsigned long long* code;
+  int *pool, *first, *end;
+  unsigned char* st;
+  unsigned long long *nn, *nb, *nl, *off, *loff;
+};
+
+// (d)
+__global__ void oct_code_kernel(const unsigned long long* __restrict__ bkey, int n, unsigned long long* __restrict__ code,
+                                int* __restrict__ idx) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long k = bkey[i];
+  code[i] = spread3((unsigned)(k & 0x1fff)) | (spread3((unsigned)((k >> 13) & 0x1fff)) << 1) |
+            (spread3((unsigned)((k >> 26) & 0x1fff)) << 2);
+  idx[i] = i;
+}
+
+// (e) one block per brick record, in pre-order
+__global__ void __launch_bounds__(512) oct_brick_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
+                                                        Nodes N, float l_occ) {
+  __shared__ BrickTree T;
+  const int r = blockIdx.x;
+  brick_tree(known, lo, N.pool[r], l_occ, T);
+  if (threadIdx.x == 0) {
+    N.st[r] = (unsigned char)T.st;
+    N.nn[r] = (unsigned long long)T.nodes;
+    N.nb[r] = (unsigned long long)T.bytes;
+    N.nl[r] = (unsigned long long)T.leaves;
+  }
+}
+
+// (f) levels 12 ... 0 appended after the n_b brick records; levels[2d], levels[2d + 1]: first record and count at depth d.
+// tot: nodes, payload bytes and occupied leaves of the root (all 0 when no voxel is known).
+__global__ void __launch_bounds__(kTreeThreads) oct_up_kernel(Nodes N, int n_b, int* levels, unsigned long long* tot) {
+  using Scan = cub::BlockScan<int, kTreeThreads>;
+  __shared__ typename Scan::TempStorage scan;
+  const int t = threadIdx.x;
+  int cb = 0, cn = n_b;  // the level below
+  if (t == 0) levels[2 * kBrickDepth] = 0, levels[2 * kBrickDepth + 1] = n_b;
+  for (int d = kBrickDepth - 1; d >= 0; --d) {
+    const int pb = cb + cn;
+    int pn = 0;
+    for (int c0 = 0; c0 < cn; c0 += kTreeThreads) {
+      const int i = c0 + t;
+      const int head = i < cn && (i == 0 || (N.code[cb + i] >> 3) != (N.code[cb + i - 1] >> 3));
+      int pos, total;
+      Scan(scan).ExclusiveSum(head, pos, total);
+      if (head) {
+        N.code[pb + pn + pos] = N.code[cb + i] >> 3;
+        N.first[pb + pn + pos] = cb + i;
+      }
+      pn += total;
+      __syncthreads();
+    }
+    for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
+      const int f = N.first[p], e = p + 1 < pb + pn ? N.first[p + 1] : pb;
+      int nf = 0, no = 0, na = 0;
+      unsigned long long n = 0, by = 0, l = 0;
+      for (int c = f; c < e; ++c) {
+        const int s = N.st[c];
+        nf += s == 1, no += s == 2, na += s != 0;
+        n += N.nn[c], by += N.nb[c], l += N.nl[c];
+      }
+      const int s = parent_state(nf, no, na, d > 0);  // octomap's prune() stops at depth 1: the root stays inner
+      N.st[p] = (unsigned char)s;
+      N.end[p] = e;
+      N.nn[p] = s == 3 ? n + 1 : (unsigned long long)(s != 0);
+      N.nb[p] = s == 3 ? by + 2 : 0ull;
+      N.nl[p] = s == 3 ? l : (unsigned long long)(s == 2);
+    }
+    __syncthreads();
+    if (t == 0) levels[2 * d] = pb, levels[2 * d + 1] = pn;
+    cb = pb, cn = pn;
+  }
+  if (t == 0) tot[0] = N.nn[cb], tot[1] = N.nb[cb], tot[2] = N.nl[cb];
+}
+
+// (g)
+__global__ void __launch_bounds__(kTreeThreads) oct_down_kernel(Nodes N, const int* __restrict__ levels, double res,
+                                                                unsigned char* __restrict__ payload, float4* __restrict__ cen,
+                                                                unsigned char* __restrict__ dep) {
+  const int t = threadIdx.x;
+  if (t == 0) N.off[levels[0]] = 0, N.loff[levels[0]] = 0;
+  __syncthreads();
+  for (int d = 0; d < kBrickDepth; ++d) {
+    const int pb = levels[2 * d], pn = levels[2 * d + 1];
+    for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
+      if (N.st[p] != 3) continue;  // only an inner node's children are in the tree
+      const int f = N.first[p], e = N.end[p];
+      int mask = 0;
+      for (int c = f; c < e; ++c) mask |= (int)N.st[c] << (2 * (int)(N.code[c] & 7));
+      unsigned long long o = N.off[p], l = N.loff[p];
+      payload[o] = (unsigned char)(mask & 0xff);
+      payload[o + 1] = (unsigned char)(mask >> 8);
+      o += 2;
+      for (int c = f; c < e; ++c) {
+        N.off[c] = o, N.loff[c] = l;
+        if (N.st[c] == 2) {
+          const unsigned long long k = N.code[c];
+          const int sh = 16 - (d + 1);
+          put_leaf(cen, dep, l, squeeze3(k) << sh, squeeze3(k >> 1) << sh, squeeze3(k >> 2) << sh, d + 1, res);
+        }
+        o += N.nb[c], l += N.nl[c];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// (h) one block per brick record; the inner ones write their bytes and occupied leaves
+__global__ void __launch_bounds__(512) oct_emit_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
+                                                       const unsigned long long* __restrict__ bkey, Nodes N, float l_occ,
+                                                       double res, unsigned char* __restrict__ payload,
+                                                       float4* __restrict__ cen, unsigned char* __restrict__ dep) {
+  using Scan = cub::BlockScan<int, 512>;
+  __shared__ BrickTree T;
+  __shared__ typename Scan::TempStorage scan;
+  const int r = blockIdx.x;
+  if (N.st[r] != 3) return;  // a leaf brick is written by its parent in (g)
+  const int b = N.pool[r];
+  brick_tree(known, lo, b, l_occ, T);
+  const int t = threadIdx.x;
+  if (t == 0) {  // pre-order: the brick, then each inner depth-14 node followed by its inner depth-15 nodes
+    unsigned char* p = payload + N.off[r];
+    int m = mask8(T.s14);
+    *p++ = (unsigned char)(m & 0xff), *p++ = (unsigned char)(m >> 8);
+    for (int i = 0; i < 8; ++i) {
+      if (T.s14[i] != 3) continue;
+      m = mask8(T.s15 + 8 * i);
+      *p++ = (unsigned char)(m & 0xff), *p++ = (unsigned char)(m >> 8);
+      for (int j = 0; j < 8; ++j) {
+        if (T.s15[8 * i + j] != 3) continue;
+        m = mask8(T.s16 + 64 * i + 8 * j);
+        *p++ = (unsigned char)(m & 0xff), *p++ = (unsigned char)(m >> 8);
+      }
+    }
+  }
+  // the occupied leaf whose first voxel is t, in Morton order = pre-order
+  const int s14 = T.s14[t >> 6], s15 = T.s15[t >> 3];
+  int depth = 0;
+  if (s14 != 3) depth = s14 == 2 && (t & 63) == 0 ? 14 : 0;
+  else if (s15 != 3) depth = s15 == 2 && (t & 7) == 0 ? 15 : 0;
+  else depth = T.s16[t] == 2 ? 16 : 0;
+  int idx;
+  Scan(scan).ExclusiveSum(depth != 0 ? 1 : 0, idx);
+  if (depth) {
+    const unsigned long long bk = bkey[b];
+    const int v = morton_local(t);
+    put_leaf(cen, dep, N.loff[r] + (unsigned long long)idx, (int)(bk & 0x1fff) * 8 + (v & 7),
+             (int)((bk >> 13) & 0x1fff) * 8 + ((v >> 3) & 7), (int)((bk >> 26) & 0x1fff) * 8 + (v >> 6), depth, res);
+  }
+}
+
 int code(cudaError_t e) {
   if (e == cudaSuccess) return LS_OK;
   cudaGetLastError();
@@ -518,6 +793,69 @@ int select(Map& m, const Params& P, int which, unsigned long long* keys, unsigne
   return read_counters(m, st);
 }
 
+Nodes nodes_of(const Octree& t) {
+  return Nodes{t.code, t.pool, t.first, t.end, t.st, t.n_nodes, t.n_bytes, t.n_leaves, t.off, t.loff};
+}
+
+// Records for n_b bricks and every upper node they can have: at most min(n_b, 8^d) at depth d.
+int reserve_tree(Octree& t, int n_b, cudaStream_t st) {
+  if (!t.levels) {
+    OCC_TRY(alloc(&t.levels, 2 * (kBrickDepth + 1)));
+    OCC_TRY(alloc(&t.tot_dev, 3));
+    OCC_TRY(cudaMallocHost((void**)&t.tot_host, 3 * sizeof(unsigned long long)));
+  }
+  if (n_b <= t.brick_cap) return LS_OK;
+  OCC_TRY(cudaStreamSynchronize(st));
+  free_ptr(t.code), free_ptr(t.pool), free_ptr(t.first), free_ptr(t.end), free_ptr(t.st);
+  free_ptr(t.n_nodes), free_ptr(t.n_bytes), free_ptr(t.n_leaves), free_ptr(t.off), free_ptr(t.loff);
+  free_ptr(t.sort_k), free_ptr(t.sort_v), free_ptr(t.cub_tmp);
+  t.brick_cap = 0, t.node_cap = 0, t.cub_bytes = 0;
+  const int cap = n_b + n_b / 8;
+  long long nodes = cap, level = 1;
+  for (int d = 0; d < kBrickDepth; ++d, level *= 8) nodes += level < cap ? level : cap;
+  const size_t n = (size_t)nodes;
+  OCC_TRY(alloc(&t.code, n));
+  OCC_TRY(alloc(&t.pool, (size_t)cap));
+  OCC_TRY(alloc(&t.first, n));
+  OCC_TRY(alloc(&t.end, n));
+  OCC_TRY(alloc(&t.st, n));
+  OCC_TRY(alloc(&t.n_nodes, n));
+  OCC_TRY(alloc(&t.n_bytes, n));
+  OCC_TRY(alloc(&t.n_leaves, n));
+  OCC_TRY(alloc(&t.off, n));
+  OCC_TRY(alloc(&t.loff, n));
+  OCC_TRY(alloc(&t.sort_k, (size_t)cap));
+  OCC_TRY(alloc(&t.sort_v, (size_t)cap));
+  size_t bytes = 0;
+  OCC_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, t.sort_k, t.code, t.sort_v, t.pool, cap, 0, 3 * kBrickDepth, st));
+  OCC_TRY(alloc((unsigned char**)&t.cub_tmp, bytes));
+  t.cub_bytes = bytes;
+  t.node_cap = nodes;
+  t.brick_cap = cap;
+  return LS_OK;
+}
+
+int reserve_tree_outputs(Octree& t, long long bytes, long long leaves, cudaStream_t st) {
+  if (bytes > t.pay_cap) {
+    OCC_TRY(cudaStreamSynchronize(st));
+    free_ptr(t.payload);
+    t.pay_cap = 0;
+    const long long cap = bytes + bytes / 8;
+    OCC_TRY(alloc(&t.payload, (size_t)cap));
+    t.pay_cap = cap;
+  }
+  if (leaves > t.leaf_cap) {
+    OCC_TRY(cudaStreamSynchronize(st));
+    free_ptr(t.centres), free_ptr(t.depths);
+    t.leaf_cap = 0;
+    const long long cap = leaves + leaves / 8;
+    OCC_TRY(alloc(&t.centres, (size_t)cap));
+    OCC_TRY(alloc(&t.depths, (size_t)cap));
+    t.leaf_cap = cap;
+  }
+  return LS_OK;
+}
+
 }  // namespace
 
 int init(Map& m, int initial_bricks, cudaStream_t st) {
@@ -635,6 +973,54 @@ int download(Map& m, const Params& P, int which, long long n, uint64_t* keys, fl
   if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, m.ex_v[1], (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
   return LS_OK;
+}
+
+int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches) {
+  t.nodes = t.bytes = t.leaves = 0;
+  const int n_b = m.pool_n;
+  if (n_b == 0) return LS_OK;
+  int rc;
+  if ((rc = reserve_tree(t, n_b, st))) return rc;
+  const Nodes N = nodes_of(t);
+  oct_code_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.bkey, n_b, t.sort_k, t.sort_v);
+  OCC_LAUNCHED();
+  size_t bytes = t.cub_bytes;
+  OCC_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp, bytes, t.sort_k, t.code, t.sort_v, t.pool, n_b, 0, 3 * kBrickDepth, st));
+  ++*launches;
+  oct_brick_kernel<<<n_b, 512, 0, st>>>(m.known, m.lo, N, P.l_occ);
+  OCC_LAUNCHED();
+  oct_up_kernel<<<1, kTreeThreads, 0, st>>>(N, n_b, t.levels, t.tot_dev);
+  OCC_LAUNCHED();
+  OCC_TRY(cudaMemcpyAsync(t.tot_host, t.tot_dev, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  const long long nodes = (long long)t.tot_host[0], pay = (long long)t.tot_host[1], leaves = (long long)t.tot_host[2];
+  if (nodes == 0) return LS_OK;
+  if ((rc = reserve_tree_outputs(t, pay, leaves, st))) return rc;
+  oct_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.levels, P.res, t.payload, t.centres, t.depths);
+  OCC_LAUNCHED();
+  oct_emit_kernel<<<n_b, 512, 0, st>>>(m.known, m.lo, m.bkey, N, P.l_occ, P.res, t.payload, t.centres, t.depths);
+  OCC_LAUNCHED();
+  OCC_TRY(cudaStreamSynchronize(st));
+  t.nodes = nodes, t.bytes = pay, t.leaves = leaves;
+  return LS_OK;
+}
+
+int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st) {
+  if (t.bytes > 0 && payload) OCC_TRY(cudaMemcpyAsync(payload, t.payload, (size_t)t.bytes, cudaMemcpyDeviceToHost, st));
+  if (t.leaves > 0 && centres4)
+    OCC_TRY(cudaMemcpyAsync(centres4, t.centres, (size_t)t.leaves * sizeof(float4), cudaMemcpyDeviceToHost, st));
+  if (t.leaves > 0 && depths) OCC_TRY(cudaMemcpyAsync(depths, t.depths, (size_t)t.leaves, cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  return LS_OK;
+}
+
+void release(Octree& t) {
+  free_ptr(t.levels), free_ptr(t.code), free_ptr(t.pool), free_ptr(t.first), free_ptr(t.end), free_ptr(t.st);
+  free_ptr(t.n_nodes), free_ptr(t.n_bytes), free_ptr(t.n_leaves), free_ptr(t.off), free_ptr(t.loff);
+  free_ptr(t.sort_k), free_ptr(t.sort_v), free_ptr(t.cub_tmp), free_ptr(t.tot_dev);
+  free_ptr(t.payload), free_ptr(t.centres), free_ptr(t.depths);
+  if (t.tot_host) cudaFreeHost(t.tot_host);
+  t = Octree();
 }
 
 }  // namespace lso

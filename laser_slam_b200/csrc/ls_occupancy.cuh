@@ -52,6 +52,31 @@ struct Map {
   long long n_known = 0;
 };
 
+// The map as octomap's pruned tree: depth 16 over the map's keys, each brick a depth-13 node.  Node records hold the
+// bricks by Morton code, then each upper level (12 ... 0) in turn; all scratch is O(bricks) plus the outputs.
+struct Octree {
+  int* levels = nullptr;  // per depth d = 0 ... 13: first record, count
+  long long node_cap = 0;
+  unsigned long long* code = nullptr;  // Morton code of the node at its depth
+  int* pool = nullptr;                 // bricks: pool index
+  int *first = nullptr, *end = nullptr;  // upper nodes: their children's records [first, end)
+  unsigned char* st = nullptr;         // 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner
+  unsigned long long *n_nodes = nullptr, *n_bytes = nullptr, *n_leaves = nullptr;  // subtree totals
+  unsigned long long *off = nullptr, *loff = nullptr;  // payload byte and occupied-leaf offsets in pre-order
+  int brick_cap = 0;
+  unsigned long long* sort_k = nullptr;
+  int* sort_v = nullptr;
+  void* cub_tmp = nullptr;
+  size_t cub_bytes = 0;
+  unsigned long long* tot_dev = nullptr;   // nodes, payload bytes, occupied leaves of the whole tree
+  unsigned long long* tot_host = nullptr;  // pinned
+  long long pay_cap = 0, leaf_cap = 0;
+  unsigned char* payload = nullptr;
+  float4* centres = nullptr;
+  unsigned char* depths = nullptr;
+  long long nodes = 0, bytes = 0, leaves = 0;  // of the last build
+};
+
 // All return LS_OK, LS_ERR_NOMEM or LS_ERR_CUDA (include/ls_b200.h) and count their launches in *launches.
 int init(Map& m, int initial_bricks, cudaStream_t st);
 void release(Map& m);
@@ -65,5 +90,11 @@ int count(Map& m, const Params& P, int which, long long* n, cudaStream_t st, uin
 int download(Map& m, const Params& P, int which, long long n, uint64_t* keys, float* log_odds, float* centres4, cudaStream_t st,
              uint64_t* launches);
 size_t device_bytes(const Map& m);
+// Builds the pruned tree of the map's max-likelihood states (oracle/OCTREE.md) into t: payload and occupied leaves stay
+// on the device, t.nodes / bytes / leaves hold the counts.  Reads the map only.  Synchronous.
+int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches);
+// Copies the last build's payload (t.bytes) and, each when not NULL, its t.leaves centres {x, y, z, 1} and depths.
+int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st);
+void release(Octree& t);
 
 }  // namespace lso

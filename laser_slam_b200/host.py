@@ -285,6 +285,8 @@ class OccupancyMap:
             L.lsh_occupancy_voxels.argtypes = [vp, ci, vp, vp, i64]
             L.lsh_occupancy_voxels.restype = i64
             L.lsh_occupancy_occupied_cloud.argtypes = [vp, vp, ci]
+            L.lsh_occupancy_write_binary.argtypes = [vp, ctypes.c_char_p]
+            L.lsh_occupancy_occupied_leaf_cloud.argtypes = [vp, vp, ci]
             L._occ_bound = True
         prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range], np.float64)
         err = ctypes.create_string_buffer(512)
@@ -317,4 +319,15 @@ class OccupancyMap:
         n = self._check(lib().lsh_occupancy_occupied_cloud(self._h, None, 0))
         out = np.zeros((max(n, 1), 4), np.float32)
         self._check(lib().lsh_occupancy_occupied_cloud(self._h, out.ctypes.data, n))
+        return out[:n]
+
+    def write_binary(self, path):
+        """writeBinary: the map as an octomap .bt file."""
+        self._check(lib().lsh_occupancy_write_binary(self._h, os.fsencode(path)))
+
+    def occupied_leaf_cloud(self):
+        """getOccupiedLeafCloud: the pruned tree's occupied leaves, (n,4) float32."""
+        n = self._check(lib().lsh_occupancy_occupied_leaf_cloud(self._h, None, 0))
+        out = np.zeros((max(n, 1), 4), np.float32)
+        self._check(lib().lsh_occupancy_occupied_leaf_cloud(self._h, out.ctypes.data, n))
         return out[:n]

@@ -450,4 +450,30 @@ int lsh_occupancy_occupied_cloud(void* ov, float* out4, int cap) {
     return LS_ERR_STATE;
   }
 }
+
+// writeBinary; 0 on success, LS_ERR_ARG when the file cannot be written
+int lsh_occupancy_write_binary(void* ov, const char* path) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    return h->map->writeBinary(path) ? 0 : LS_ERR_ARG;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// getOccupiedLeafCloud; returns its number of points, written when it is <= cap
+int lsh_occupancy_occupied_leaf_cloud(void* ov, float* out4, int cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    DataPoints d;
+    h->map->getOccupiedLeafCloud(&d);
+    const int n = (int)d.getNbPoints();
+    if (out4 && n <= cap) std::memcpy(out4, static_cast<const DataPoints&>(d).features.data(), sizeof(float) * 4 * (size_t)n);
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
 }  // extern "C"

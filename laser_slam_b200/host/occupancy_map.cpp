@@ -89,6 +89,27 @@ void OccupancyMap::getOccupiedCloud(DataPoints* cloud) const {
   *cloud = DataPoints::fromArrays(c.data(), NULL, c.size() / 4);
 }
 
+bool OccupancyMap::writeBinary(const std::string& filename) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  const int rc = ls_occupancy_write_octomap(map_, filename.c_str(), NULL);
+  if (rc == LS_ERR_ARG) return false;
+  throwOnError(ctx_, rc, "ls_occupancy_write_octomap");
+  return true;
+}
+
+void OccupancyMap::getOccupiedLeafCloud(DataPoints* cloud) {
+  if (cloud == NULL) throw std::invalid_argument("null output");
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_octree_stats st;
+  throwOnError(ctx_, ls_occupancy_build_octree(map_, &st), "ls_occupancy_build_octree");
+  std::vector<uint8_t> payload((size_t)(st.payload_bytes > 0 ? st.payload_bytes : 1));
+  std::vector<float> c(4 * (size_t)(st.occupied_leaves > 0 ? st.occupied_leaves : 1));
+  throwOnError(ctx_,
+               ls_occupancy_download_octree(map_, payload.data(), st.payload_bytes, c.data(), NULL, st.occupied_leaves),
+               "ls_occupancy_download_octree");
+  *cloud = DataPoints::fromArrays(c.data(), NULL, (size_t)st.occupied_leaves);
+}
+
 void OccupancyMap::getVoxels(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds) const {
   download(which, keys, log_odds, NULL);
 }

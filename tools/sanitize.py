@@ -64,4 +64,13 @@ for k in range(4):
         q, oq = lm.take_queue(), olmap.get_queued_points()
         assert len(q) == len(oq) and all(np.array_equal(a, b) for a, b in zip(q, oq))
 lm.close()
+# occupancy map and its octree export (ls_occupancy.cu): two scans, growth from 16 bricks, the pruned tree against the oracle
+from oracle import occupancy as oc, octree as oct_oracle
+om, oom = ls.OccupancyMap(ctx, resolution=0.2, max_range=10.0, initial_capacity=16), oc.OccupancyMap(resolution=0.2, max_range=10.0)
+for k in range(2):
+    om.insert_scan(mp, sid[k], truth[k].astype(np.float32))
+    oom.insert_scan(sc[k][0], truth[k].astype(np.float32))
+tr, otr = om.octree(), oct_oracle.of_map(oom)
+assert tr.nodes == otr.nodes > 0 and tr.payload == otr.payload and np.array_equal(tr.centres, otr.centres)
+om.close()
 print("sanitize workload ok:", g["stats"].iterations, "iterations;", len(batch), "batched problems;", ctx.launch_count, "launches")
