@@ -56,7 +56,34 @@ class OccupancyMap {
   // (new) LS_OCC_KNOWN or LS_OCC_OCCUPIED voxels: packed keys and log-odds, by ascending key.
   void getVoxels(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds) const;
 
+  // ---- queries: volumetric_mapping's WorldBase and octomap's castRay on the device map (ls_occupancy_cell_status /
+  // _line_status / _cast_rays; rules in oracle/QUERIES.md).  Each single query is a device call of one; the batched
+  // overloads are the intended use.
+  enum class CellStatus { kFree = LS_CELL_FREE, kOccupied = LS_CELL_OCCUPIED, kUnknown = LS_CELL_UNKNOWN };
+
+  CellStatus getCellStatusPoint(const kindr::minimal::Position& point) const;
+  // octomap's probability 1 - 1 / (1 + exp(v)) of the voxel's log-odds, -1 when unknown.
+  CellStatus getCellProbabilityPoint(const kindr::minimal::Position& point, double* probability) const;
+  CellStatus getLineStatus(const kindr::minimal::Position& start, const kindr::minimal::Position& end) const;
+  CellStatus getVisibility(const kindr::minimal::Position& view_point, const kindr::minimal::Position& voxel_to_test,
+                           bool stop_at_unknown_cell) const;
+  CellStatus getLineStatusBoundingBox(const kindr::minimal::Position& start, const kindr::minimal::Position& end,
+                                      const kindr::minimal::Position& bounding_box_size) const;
+  // octomap's castRay: true on a hit; *end (may be NULL) the centre of the voxel the ray stopped in (left alone for an
+  // invalid ray).  max_range <= 0: none.
+  bool castRay(const kindr::minimal::Position& origin, const kindr::minimal::Position& direction,
+               kindr::minimal::Position* end, bool ignore_unknown = false, double max_range = -1.0) const;
+  // Batches: one status per segment (bounding_box_size NULL: getLineStatus / getVisibility); first_keys may be NULL.
+  void getLineStatus(const std::vector<kindr::minimal::Position>& starts, const std::vector<kindr::minimal::Position>& ends,
+                     std::vector<CellStatus>* status, bool stop_at_unknown_cell = true,
+                     const kindr::minimal::Position* bounding_box_size = NULL, std::vector<uint64_t>* first_keys = NULL) const;
+  // One LS_RAY_* result and end per ray.
+  void castRays(const std::vector<kindr::minimal::Position>& origins, const std::vector<kindr::minimal::Position>& directions,
+                std::vector<int>* results, std::vector<kindr::minimal::Position>* ends, bool ignore_unknown = false,
+                double max_range = -1.0) const;
+
  private:
+  CellStatus cellStatus(const kindr::minimal::Position& point, float* log_odds) const;
   void download(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds, std::vector<float>* centres4) const;
 
   OccupancyMapParams params_;

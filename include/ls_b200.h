@@ -406,6 +406,55 @@ int ls_occupancy_download_octree(ls_occupancy* om, uint8_t* payload, int64_t pay
  * then the payload.  Builds the tree unless the last build is current.  stats may be NULL. */
 int ls_occupancy_write_octomap(ls_occupancy* om, const char* path, ls_octree_stats* stats);
 
+/* Queries of the map: volumetric_mapping's WorldBase (getCellStatusPoint, getLineStatus, getVisibility,
+ * getLineStatusBoundingBox) and octomap's castRay, batched, one device thread per query.  The rules (oracle/QUERIES.md):
+ *   cell        the key of the double point (octomap's search(x, y, z): floor(c * (1/resolution)) + 32768, no float cast);
+ *               unknown when the key is invalid (non-finite included) or the voxel is not known, occupied when known and
+ *               v >= L_occ, else free.  log_odds: v, or NaN (0x7fc00000) when unknown
+ *   line        the keys of computeRayKeys((float)start, (float)end) (as one ray of the insert: origin key first, the end
+ *               key never, none when an end key is invalid or both share a key), walked in order up to the first occupied
+ *               key or, when stop_at_unknown, the first unknown one; that key's state and packed key, else free and all
+ *               ones.  getLineStatus is stop_at_unknown = 1; getVisibility takes it as its flag.  So a segment whose ends
+ *               share a key, or whose end key is invalid, is free, and the end voxel is never checked
+ *   box         box3 = the box size (finite, >= 0 per axis).  disc = size / ceil((size + 0.001) / resolution) (1.0 if
+ *               <= 0); offsets x = -size/2; x <= size/2; x += disc, in double, y inside x and z innermost; line i runs
+ *               from start + offset_i to end + offset_i (added in double, then cast to float).  The result is that of the
+ *               first line in loop order that is not free, else free
+ *   ray         castRay(origin, direction, end, ignore_unknown, max_range) on float triples: LS_RAY_INVALID for an origin
+ *               with an invalid key or a zero direction (end NaN); an occupied origin voxel is a hit, an unknown one (not
+ *               ignored) LS_RAY_UNKNOWN, both at the origin voxel's centre; then octomap's DDA from the normalised
+ *               direction (border half step in double), stopping with LS_RAY_KEY_BOUND before a step out of [0, 65535],
+ *               LS_RAY_MAX_RANGE when max_range > 0 and the new centre is farther (sum of float squares in double > max_range^2),
+ *               LS_RAY_HIT on an occupied voxel, LS_RAY_UNKNOWN on an unknown one unless ignored.  ends3: the centre of the
+ *               voxel the result names
+ * A query reads the map only, on the map's stream, and is synchronous; only the outputs and a counter return.  Legal between
+ * ls_icp_register_submap_batch_begin and _end.  n = 0 is LS_OK without a launch.  Errors: LS_ERR_ARG for n < 0, a NULL
+ * required buffer, a negative or non-finite box size or more than 2^31 - 1 box lines in the call; LS_ERR_NOMEM when the
+ * staging cannot grow.  The map is unchanged after any call. */
+#define LS_CELL_FREE 0
+#define LS_CELL_OCCUPIED 1
+#define LS_CELL_UNKNOWN 2
+#define LS_RAY_INVALID 0
+#define LS_RAY_HIT 1
+#define LS_RAY_UNKNOWN 2
+#define LS_RAY_MAX_RANGE 3
+#define LS_RAY_KEY_BOUND 4
+
+typedef struct ls_occupancy_query_stats {
+  int64_t keys_visited; /* voxel states the kernels read */
+  float device_ms;      /* the call on the map's stream, copies included */
+} ls_occupancy_query_stats;
+
+/* points3: n double triples.  log_odds and stats may be NULL. */
+int ls_occupancy_cell_status(ls_occupancy* om, const double* points3, int n, int8_t* status, float* log_odds,
+                             ls_occupancy_query_stats* stats);
+/* starts3 / ends3: n double triples; box3: NULL for plain lines.  first_keys and stats may be NULL. */
+int ls_occupancy_line_status(ls_occupancy* om, const double* starts3, const double* ends3, int n, const double* box3,
+                             int stop_at_unknown, int8_t* status, uint64_t* first_keys, ls_occupancy_query_stats* stats);
+/* origins3 / directions3: n float triples; max_range <= 0 (or NaN): none.  ends3 and stats may be NULL. */
+int ls_occupancy_cast_rays(ls_occupancy* om, const float* origins3, const float* directions3, int n, int ignore_unknown,
+                           double max_range, int8_t* result, float* ends3, ls_occupancy_query_stats* stats);
+
 /* ---- per-scan input filters (reference laser_slam/src/laser_track.cpp:24-30 loads them from
  * LaserTrackParams::icp_input_filters_file, :81 and :146 apply them to every scan before it is stored) ----------------
  * A chain is an array of ls_point_filter records applied in order; each filter sees the cloud the previous one produced,

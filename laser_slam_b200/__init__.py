@@ -102,7 +102,13 @@ class OctreeStats(ctypes.Structure):
                 ("device_ms", ctypes.c_float)]
 
 
+class OccupancyQueryStats(ctypes.Structure):
+    _fields_ = [("keys_visited", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
 OCC_KNOWN, OCC_OCCUPIED = 1, 2
+CELL_FREE, CELL_OCCUPIED, CELL_UNKNOWN = 0, 1, 2
+RAY_INVALID, RAY_HIT, RAY_UNKNOWN, RAY_MAX_RANGE, RAY_KEY_BOUND = 0, 1, 2, 3, 4
 LS_ERR_NOMEM, LS_ERR_STATE = -3, -4
 
 
@@ -208,6 +214,10 @@ def lib():
         L.ls_occupancy_build_octree.argtypes = [vp, ctypes.POINTER(OctreeStats)]
         L.ls_occupancy_download_octree.argtypes = [vp, vp, ctypes.c_int64, vp, vp, ctypes.c_int64]
         L.ls_occupancy_write_octomap.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(OctreeStats)]
+        QS = ctypes.POINTER(OccupancyQueryStats)
+        L.ls_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp, QS]
+        L.ls_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, vp, vp, QS]
+        L.ls_occupancy_cast_rays.argtypes = [vp, vp, vp, ci, ci, ctypes.c_double, vp, vp, QS]
         _lib = L
     return _lib
 
@@ -881,6 +891,53 @@ class OccupancyMap:
         pts = self.octree().centres[:, :3]
         write_point_cloud(path, pts)
         return len(pts)
+
+    # ---- queries (ls_occupancy_cell_status / _line_status / _cast_rays); self.last_query holds the last call's stats
+    def cell_status(self, points):
+        """getCellStatusPoint per point ((n,3), taken as float64): (status int8 CELL_*, log-odds float32, NaN when
+        unknown)."""
+        p = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
+        n = len(p)
+        st = np.empty(max(n, 1), np.int8)
+        lo = np.empty(max(n, 1), np.float32)
+        self.last_query = OccupancyQueryStats()
+        self.ctx._check(lib().ls_occupancy_cell_status(self._h, p.ctypes.data, n, st.ctypes.data, lo.ctypes.data,
+                                                       ctypes.byref(self.last_query)))
+        return st[:n].copy(), lo[:n].copy()
+
+    def line_status(self, starts, ends, box=None, stop_at_unknown=True):
+        """getLineStatus (stop_at_unknown), getVisibility or, with box = its (x, y, z) size, getLineStatusBoundingBox per
+        segment ((n,3) each, taken as float64): (status int8 CELL_*, packed key uint64 that decided it, all ones when
+        free)."""
+        s = np.ascontiguousarray(np.asarray(starts, np.float64).reshape(-1, 3))
+        e = np.ascontiguousarray(np.asarray(ends, np.float64).reshape(-1, 3))
+        if len(s) != len(e):
+            raise ValueError(f"{len(s)} starts for {len(e)} ends")
+        b = None if box is None else np.ascontiguousarray(np.asarray(box, np.float64).reshape(3))
+        n = len(s)
+        st = np.empty(max(n, 1), np.int8)
+        fk = np.empty(max(n, 1), np.uint64)
+        self.last_query = OccupancyQueryStats()
+        self.ctx._check(lib().ls_occupancy_line_status(self._h, s.ctypes.data, e.ctypes.data, n,
+                                                       None if b is None else b.ctypes.data, int(bool(stop_at_unknown)),
+                                                       st.ctypes.data, fk.ctypes.data, ctypes.byref(self.last_query)))
+        return st[:n].copy(), fk[:n].copy()
+
+    def cast_rays(self, origins, directions, ignore_unknown=False, max_range=-1.0):
+        """octomap's castRay per ray ((n,3) each, taken as float32): (result int8 RAY_*, ends (n,3) float32: the centre
+        of the voxel the result names, NaN for RAY_INVALID).  max_range <= 0: none."""
+        o = np.ascontiguousarray(np.asarray(origins, np.float32).reshape(-1, 3))
+        d = np.ascontiguousarray(np.asarray(directions, np.float32).reshape(-1, 3))
+        if len(o) != len(d):
+            raise ValueError(f"{len(o)} origins for {len(d)} directions")
+        n = len(o)
+        r = np.empty(max(n, 1), np.int8)
+        ends = np.empty((max(n, 1), 3), np.float32)
+        self.last_query = OccupancyQueryStats()
+        self.ctx._check(lib().ls_occupancy_cast_rays(self._h, o.ctypes.data, d.ctypes.data, n, int(bool(ignore_unknown)),
+                                                     float(max_range), r.ctypes.data, ends.ctypes.data,
+                                                     ctypes.byref(self.last_query)))
+        return r[:n].copy(), ends[:n].copy()
 
 
 Octree = collections.namedtuple("Octree", "nodes payload centres depths device_ms")

@@ -1943,3 +1943,76 @@ int ls_occupancy_write_octomap(ls_occupancy* om, const char* path, ls_octree_sta
 }
 
 }  // extern "C"
+
+namespace {
+// The query's device time (ev0 .. ev1 around it on the map's stream) and its keys visited into *stats.
+int query_done(ls_occupancy* om, long long visited, ls_occupancy_query_stats* stats) {
+  ls_ctx* ctx = om->ctx;
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    stats->keys_visited = visited;
+    stats->device_ms = ms;
+  }
+  return LS_OK;
+}
+
+void query_none(ls_occupancy_query_stats* stats) {
+  if (stats) stats->keys_visited = 0, stats->device_ms = 0.f;
+}
+}  // namespace
+
+extern "C" {
+
+int ls_occupancy_cell_status(ls_occupancy* om, const double* points3, int n, int8_t* status, float* log_odds,
+                             ls_occupancy_query_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (n < 0 || (n > 0 && (!points3 || !status))) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (n == 0) return query_none(stats), LS_OK;
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  long long visited = 0;
+  const int rc = lso::query_cells(om->map, om->prm, points3, n, status, log_odds, &visited, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "cell query: out of device memory" : "cell query failed");
+  return query_done(om, visited, stats);
+}
+
+int ls_occupancy_line_status(ls_occupancy* om, const double* starts3, const double* ends3, int n, const double* box3,
+                             int stop_at_unknown, int8_t* status, uint64_t* first_keys, ls_occupancy_query_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (n < 0 || (n > 0 && (!starts3 || !ends3 || !status))) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (box3)
+    for (int a = 0; a < 3; ++a)
+      if (!std::isfinite(box3[a]) || box3[a] < 0.0)
+        return fail(ctx, LS_ERR_ARG, "bounding box size %g on axis %d (finite and >= 0)", box3[a], a);
+  if (n == 0) return query_none(stats), LS_OK;
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  long long visited = 0;
+  const int rc = lso::query_lines(om->map, om->prm, starts3, ends3, n, box3, stop_at_unknown, status, first_keys, &visited,
+                                  om->stream, &ctx->launches);
+  if (rc == LS_ERR_ARG) return fail(ctx, rc, "%d segments with this bounding box make more than 2^31 - 1 lines", n);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "line query: out of device memory" : "line query failed");
+  return query_done(om, visited, stats);
+}
+
+int ls_occupancy_cast_rays(ls_occupancy* om, const float* origins3, const float* directions3, int n, int ignore_unknown,
+                           double max_range, int8_t* result, float* ends3, ls_occupancy_query_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (n < 0 || (n > 0 && (!origins3 || !directions3 || !result))) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (n == 0) return query_none(stats), LS_OK;
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  long long visited = 0;
+  const int rc = lso::query_rays(om->map, om->prm, origins3, directions3, n, ignore_unknown, max_range, result, ends3, &visited,
+                                 om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "ray query: out of device memory" : "ray query failed");
+  return query_done(om, visited, stats);
+}
+
+}  // extern "C"

@@ -24,8 +24,10 @@
 //                            the offsets (g) gave it, so no per-brick staging is kept
 // A brick without a known voxel (an insert that failed after placing it leaves one) has state 0 and adds nothing.
 #include <cfloat>
+#include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <vector>
 
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
@@ -139,10 +141,13 @@ struct Cursor {
   int b = -1;
 };
 
+__device__ __forceinline__ unsigned long long brick_key(const int k[3]) {
+  return (unsigned long long)(k[0] >> 3) | ((unsigned long long)(k[1] >> 3) << 13) | ((unsigned long long)(k[2] >> 3) << 26);
+}
+
 // Set the free or occupied mark of voxel k; false when its brick could not be placed.
 __device__ __forceinline__ bool mark(const Dev& D, Counters* cnt, Cursor& cur, const int k[3], bool occ) {
-  const unsigned long long bk = (unsigned long long)(k[0] >> 3) | ((unsigned long long)(k[1] >> 3) << 13) |
-                                ((unsigned long long)(k[2] >> 3) << 26);
+  const unsigned long long bk = brick_key(k);
   if (bk != cur.bk) {
     const int b = brick_of(D, cnt, bk);
     if (b < 0) return false;
@@ -157,40 +162,55 @@ __device__ __forceinline__ bool mark(const Dev& D, Counters* cnt, Cursor& cur, c
   return true;
 }
 
-// octomap's computeRayKeys from o to e, marking every key before the end key free.
-__device__ bool walk(const Dev& D, Counters* cnt, Cursor& cur, const Params& P, const float o[3], const float e[3]) {
-  int ko[3], ke[3];
-  if (!key3(P.inv, o, ko) || !key3(P.inv, e, ke)) return true;
-  if (ko[0] == ke[0] && ko[1] == ke[1] && ko[2] == ke[2]) return true;
-  if (!mark(D, cnt, cur, ko, false)) return false;
-  float dir[3] = {e[0] - o[0], e[1] - o[1], e[2] - o[2]};
-  const float length = (float)norm3(dir);
-  for (int i = 0; i < 3; ++i) dir[i] = dir[i] / length;
-  int step[3], k[3] = {ko[0], ko[1], ko[2]};
-  double tmax[3], tdelta[3];
+// The Amanatides-Woo setup both of octomap's DDAs share, from key k at o along dir: step, tMax and tDelta per axis.  The
+// border's half step is rounded to float in computeRayKeys (kFloatHalfStep) and kept in double in castRay.
+template <bool kFloatHalfStep>
+__device__ __forceinline__ void dda_setup(const int k[3], const float o[3], const float dir[3], double res, int step[3],
+                                          double tmax[3], double tdelta[3]) {
   for (int i = 0; i < 3; ++i) {
     step[i] = dir[i] > 0.0f ? 1 : (dir[i] < 0.0f ? -1 : 0);
     if (step[i] != 0) {
-      double border = ((double)(k[i] - kKeyMax) + 0.5) * P.res;
-      border += (double)(float)((double)step[i] * P.res * 0.5);
+      double border = ((double)(k[i] - kKeyMax) + 0.5) * res;
+      const double half = (double)step[i] * res * 0.5;
+      border += kFloatHalfStep ? (double)(float)half : half;
       tmax[i] = (border - (double)o[i]) / (double)dir[i];
-      tdelta[i] = P.res / (double)fabsf(dir[i]);
+      tdelta[i] = res / (double)fabsf(dir[i]);
     } else {
       tmax[i] = DBL_MAX;
       tdelta[i] = DBL_MAX;
     }
   }
+}
+
+// The axis of the next step: the smallest tMax, ties to the later axis.
+__device__ __forceinline__ int next_axis(const double tmax[3]) {
+  if (tmax[0] < tmax[1]) return tmax[0] < tmax[2] ? 0 : 2;
+  return tmax[1] < tmax[2] ? 1 : 2;
+}
+
+// octomap's computeRayKeys from o to e: visit(k) for the origin key and every key stepped into before the end key, in
+// order.  False as soon as a visit returns false.  The insert marks each key free; the line queries read its state.
+template <class Visit>
+__device__ __forceinline__ bool walk(const Params& P, const float o[3], const float e[3], Visit&& visit) {
+  int ko[3], ke[3];
+  if (!key3(P.inv, o, ko) || !key3(P.inv, e, ke)) return true;
+  if (ko[0] == ke[0] && ko[1] == ke[1] && ko[2] == ke[2]) return true;
+  if (!visit(ko)) return false;
+  float dir[3] = {e[0] - o[0], e[1] - o[1], e[2] - o[2]};
+  const float length = (float)norm3(dir);
+  for (int i = 0; i < 3; ++i) dir[i] = dir[i] / length;
+  int step[3], k[3] = {ko[0], ko[1], ko[2]};
+  double tmax[3], tdelta[3];
+  dda_setup<true>(k, o, dir, P.res, step, tmax, tdelta);
   for (;;) {
-    int dim;
-    if (tmax[0] < tmax[1]) dim = tmax[0] < tmax[2] ? 0 : 2;
-    else dim = tmax[1] < tmax[2] ? 1 : 2;
+    const int dim = next_axis(tmax);
     k[dim] += step[dim];
     tmax[dim] += tdelta[dim];
     if (k[0] == ke[0] && k[1] == ke[1] && k[2] == ke[2]) break;
     if (k[dim] < 0 || k[dim] > 65535) break;
     const double dist = fmin(fmin(tmax[0], tmax[1]), tmax[2]);
     if (dist > (double)length) break;
-    if (!mark(D, cnt, cur, k, false)) return false;
+    if (!visit(k)) return false;
   }
   return true;
 }
@@ -274,7 +294,7 @@ __global__ void occ_cast_kernel(int n, Params P, float ox, float oy, float oz, c
   const float4 e4 = ends[i];
   const float o[3] = {ox, oy, oz}, e[3] = {e4.x, e4.y, e4.z};
   Cursor cur;
-  if (!walk(D, cnt, cur, P, o, e)) return;
+  if (!walk(P, o, e, [&](const int* k) { return mark(D, cnt, cur, k, false); })) return;
   if (c == 1 && key != kEmpty) {
     const int k[3] = {(int)(key & 0xffff), (int)((key >> 16) & 0xffff), (int)((key >> 32) & 0xffff)};
     mark(D, cnt, cur, k, true);
@@ -365,6 +385,242 @@ __global__ void occ_centres_kernel(const unsigned long long* __restrict__ keys, 
     for (int a = 0; a < 3; ++a) c[a] = (float)(((double)((int)((k >> (16 * a)) & 0xffff) - kKeyMax) + 0.5) * res);
     out[i] = make_float4(c[0], c[1], c[2], 1.0f);
   }
+}
+
+// ---- queries (volumetric_mapping's WorldBase and octomap's castRay; rules in oracle/QUERIES.md) -------------------------
+// They read tab_keys / tab_vals, the known bits and the log-odds only; no insert runs during a query.
+constexpr unsigned kNanBits = 0x7fc00000u;  // the NaN of an unknown cell's log-odds and an invalid ray's end
+
+// Pool index of brick bk, or -1 when the hash does not hold it.  Read-only: no CAS, no allocation, no wait on a pending
+// slot.  A slot whose value is negative (left by an insert whose pool filled) is absent.
+__device__ __forceinline__ int find_brick(const Dev& D, unsigned long long bk) {
+  unsigned h = hash64(bk) & D.tab_mask;
+  for (int p = 0; p < kMaxProbe; ++p, h = (h + 1u) & D.tab_mask) {
+    const unsigned long long k = D.tab_keys[h];
+    if (k == bk) {
+      const int v = D.tab_vals[h];
+      return v >= 0 ? v : -1;
+    }
+    if (k == kEmpty) return -1;
+  }
+  return -1;
+}
+
+// State of voxel k (LS_CELL_*), the brick of the last lookup cached in cur.  The known bit decides "unknown", not the
+// brick's presence: a brick placed by a failed insert holds no known voxel.  *v: the log-odds of a known voxel.
+__device__ __forceinline__ int state_of(const Dev& D, const Params& P, Cursor& cur, const int k[3], float* v) {
+  const unsigned long long bk = brick_key(k);
+  if (bk != cur.bk) {
+    cur.bk = bk;
+    cur.b = find_brick(D, bk);
+  }
+  if (cur.b < 0) return LS_CELL_UNKNOWN;
+  const int local = (k[0] & 7) | ((k[1] & 7) << 3) | ((k[2] & 7) << 6);
+  if (!((D.known[(size_t)cur.b * 16 + (local >> 5)] >> (local & 31)) & 1u)) return LS_CELL_UNKNOWN;
+  const float x = D.lo[(size_t)cur.b * 512 + local];
+  if (v) *v = x;
+  return x >= P.l_occ ? LS_CELL_OCCUPIED : LS_CELL_FREE;
+}
+
+// octomap's keyToCoord(key): (float)(((double)(k - 32768) + 0.5) * res)
+__device__ __forceinline__ float centre_of(int k, double res) { return (float)(((double)(k - kKeyMax) + 0.5) * res); }
+
+// Every lane of the warp calls it: the warp's keys_visited into cnt->n_out.
+__device__ __forceinline__ void add_visited(Counters* cnt, unsigned long long v) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0 && v) atomicAdd(&cnt->n_out, v);
+}
+
+// octomap's search(double x, double y, double z): the key of the double coordinate, valid iff in [0, 65535]
+__device__ __forceinline__ bool key_of_d(double inv, double c, int& k) {
+  const double s = floor(c * inv);
+  if (!(s >= -(double)kKeyMax && s < (double)kKeyMax)) return false;
+  k = (int)s + kKeyMax;
+  return true;
+}
+
+// getCellStatusPoint / getCellProbabilityPoint: one thread per point
+__global__ void occ_cell_kernel(const double* __restrict__ pts3, int n, Dev D, Params P, signed char* __restrict__ status,
+                                float* __restrict__ log_odds, Counters* cnt) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long visited = 0;
+  if (i < n) {
+    int k[3];
+    int s = LS_CELL_UNKNOWN;
+    float v = __uint_as_float(kNanBits);
+    if (key_of_d(P.inv, pts3[3 * (size_t)i], k[0]) && key_of_d(P.inv, pts3[3 * (size_t)i + 1], k[1]) &&
+        key_of_d(P.inv, pts3[3 * (size_t)i + 2], k[2])) {
+      Cursor cur;
+      ++visited;
+      s = state_of(D, P, cur, k, &v);
+      if (s == LS_CELL_UNKNOWN) v = __uint_as_float(kNanBits);
+    }
+    status[i] = (signed char)s;
+    log_odds[i] = v;
+  }
+  add_visited(cnt, visited);
+}
+
+// getLineStatus / getVisibility over computeRayKeys(s, e): the state of the first occupied key, or of the first unknown
+// key when stop_unknown, else free; *first its packed key (all ones when free).  cut(visited) ends the walk early (result
+// -1): the bounding-box pass drops a line once a lower line of its segment has failed.
+template <class Cut>
+__device__ __forceinline__ int line_status(const Dev& D, const Params& P, const float s[3], const float e[3], bool stop_unknown,
+                                           unsigned long long* first, unsigned long long& visited, Cut&& cut) {
+  Cursor cur;
+  int st = LS_CELL_FREE;
+  unsigned long long fk = kEmpty;
+  walk(P, s, e, [&](const int* k) {
+    if (cut(visited)) {
+      st = -1;
+      return false;
+    }
+    ++visited;
+    const int x = state_of(D, P, cur, k, nullptr);
+    if (x == LS_CELL_OCCUPIED || (x == LS_CELL_UNKNOWN && stop_unknown)) {
+      st = x;
+      fk = pack(k[0], k[1], k[2]);
+      return false;
+    }
+    return true;
+  });
+  *first = fk;
+  return st;
+}
+
+// The float ends of line `l` of a segment: each coordinate cast to float once, after the box offset is added in double
+// (kBox).  offs holds the box loop's x values, then its y values, then its z values; line l = (ix * ny + iy) * nz + iz.
+template <bool kBox>
+__device__ __forceinline__ void line_ends(const double* s3, const double* e3, int seg, const double* offs, int l, int nx, int ny,
+                                          int nz, float s[3], float e[3]) {
+  double off[3] = {0.0, 0.0, 0.0};
+  if (kBox) off[0] = offs[l / (ny * nz)], off[1] = offs[nx + (l / nz) % ny], off[2] = offs[nx + ny + l % nz];
+  for (int a = 0; a < 3; ++a) {
+    s[a] = kBox ? (float)(s3[3 * (size_t)seg + a] + off[a]) : (float)s3[3 * (size_t)seg + a];
+    e[a] = kBox ? (float)(e3[3 * (size_t)seg + a] + off[a]) : (float)e3[3 * (size_t)seg + a];
+  }
+}
+
+// Plain lines (kBox false): one thread per segment, the result written.  Bounding boxes (kBox true): one thread per
+// (segment, line); a failing line raises best[seg] to ~line with atomicMax, so best ends at the lowest failing line
+// whatever the scheduling, and a line at or above the current lowest stops (checked every 16 keys).
+template <bool kBox>
+__global__ void occ_line_kernel(const double* __restrict__ s3, const double* __restrict__ e3, long long items, int lines,
+                                const double* __restrict__ offs, int nx, int ny, int nz, int stop_unknown, Dev D, Params P,
+                                signed char* __restrict__ status, unsigned long long* __restrict__ first, unsigned* best,
+                                Counters* cnt) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long visited = 0;
+  if (i < items) {
+    const int seg = kBox ? (int)(i / lines) : (int)i;
+    const int l = kBox ? (int)(i % lines) : 0;
+    const unsigned mine = 0xffffffffu - (unsigned)l;
+    if (!kBox || *(volatile unsigned*)&best[seg] < mine) {
+      float s[3], e[3];
+      line_ends<kBox>(s3, e3, seg, offs, l, nx, ny, nz, s, e);
+      unsigned long long fk;
+      const int st = line_status(D, P, s, e, stop_unknown != 0, &fk, visited, [&](unsigned long long v) {
+        return kBox && (v & 15) == 15 && *(volatile unsigned*)&best[seg] >= mine;
+      });
+      if (!kBox) {
+        status[seg] = (signed char)st;
+        first[seg] = fk;
+      } else if (st > 0) {
+        atomicMax(&best[seg], mine);
+      }
+    }
+  }
+  add_visited(cnt, visited);
+}
+
+// The bounding box's result per segment: the lowest failing line walked again for its status and key, or free.
+__global__ void occ_box_result_kernel(const double* __restrict__ s3, const double* __restrict__ e3, int n, int lines,
+                                      const double* __restrict__ offs, int nx, int ny, int nz, int stop_unknown, Dev D, Params P,
+                                      const unsigned* __restrict__ best, signed char* __restrict__ status,
+                                      unsigned long long* __restrict__ first, Counters* cnt) {
+  const int seg = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long visited = 0;
+  if (seg < n) {
+    const unsigned b = best[seg];
+    int st = LS_CELL_FREE;
+    unsigned long long fk = kEmpty;
+    if (b != 0u) {
+      float s[3], e[3];
+      line_ends<true>(s3, e3, seg, offs, (int)(0xffffffffu - b), nx, ny, nz, s, e);
+      st = line_status(D, P, s, e, stop_unknown != 0, &fk, visited, [](unsigned long long) { return false; });
+    }
+    status[seg] = (signed char)st;
+    first[seg] = fk;
+  }
+  add_visited(cnt, visited);
+}
+
+// octomap's castRay(origin, direction, end, ignore_unknown, max_range): the result code (LS_RAY_*), end[] the centre of
+// the voxel it names (left alone for LS_RAY_INVALID).
+__device__ __forceinline__ int cast_ray(const Dev& D, const Params& P, const float o[3], const float dir_in[3], bool ignore_unknown,
+                                        double max_range, float end[3], unsigned long long& visited) {
+  int k[3];
+  if (!key3(P.inv, o, k)) return LS_RAY_INVALID;
+  Cursor cur;
+  ++visited;
+  const int s0 = state_of(D, P, cur, k, nullptr);
+  if (s0 == LS_CELL_OCCUPIED || (s0 == LS_CELL_UNKNOWN && !ignore_unknown)) {
+    for (int a = 0; a < 3; ++a) end[a] = centre_of(k[a], P.res);
+    return s0 == LS_CELL_OCCUPIED ? LS_RAY_HIT : LS_RAY_UNKNOWN;
+  }
+  float dir[3] = {dir_in[0], dir_in[1], dir_in[2]};
+  const double len = norm3(dir);  // Vector3::normalize: divided by the float length only when it is > 0
+  if (len > 0.0) {
+    const float fl = (float)len;
+    for (int a = 0; a < 3; ++a) dir[a] = dir[a] / fl;
+  }
+  int step[3];
+  double tmax[3], tdelta[3];
+  dda_setup<false>(k, o, dir, P.res, step, tmax, tdelta);
+  if (step[0] == 0 && step[1] == 0 && step[2] == 0) return LS_RAY_INVALID;
+  const bool range = max_range > 0.0;
+  const double range_sq = max_range * max_range;
+  for (;;) {
+    const int dim = next_axis(tmax);
+    if ((step[dim] < 0 && k[dim] == 0) || (step[dim] > 0 && k[dim] == 65535)) {
+      for (int a = 0; a < 3; ++a) end[a] = centre_of(k[a], P.res);
+      return LS_RAY_KEY_BOUND;
+    }
+    k[dim] += step[dim];
+    tmax[dim] += tdelta[dim];
+    for (int a = 0; a < 3; ++a) end[a] = centre_of(k[a], P.res);
+    if (range) {
+      double d = 0.0;
+      for (int a = 0; a < 3; ++a) {
+        const float x = end[a] - o[a];
+        d += (double)(x * x);
+      }
+      if (d > range_sq) return LS_RAY_MAX_RANGE;
+    }
+    ++visited;
+    const int s = state_of(D, P, cur, k, nullptr);
+    if (s == LS_CELL_OCCUPIED) return LS_RAY_HIT;
+    if (s == LS_CELL_UNKNOWN && !ignore_unknown) return LS_RAY_UNKNOWN;
+  }
+}
+
+// one thread per ray
+__global__ void occ_ray_kernel(const float* __restrict__ o3, const float* __restrict__ d3, int n, int ignore_unknown,
+                               double max_range, Dev D, Params P, signed char* __restrict__ result, float* __restrict__ ends3,
+                               Counters* cnt) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long visited = 0;
+  if (i < n) {
+    const float o[3] = {o3[3 * (size_t)i], o3[3 * (size_t)i + 1], o3[3 * (size_t)i + 2]};
+    const float d[3] = {d3[3 * (size_t)i], d3[3 * (size_t)i + 1], d3[3 * (size_t)i + 2]};
+    const float nan = __uint_as_float(kNanBits);
+    float e[3] = {nan, nan, nan};
+    const int r = cast_ray(D, P, o, d, ignore_unknown != 0, max_range, e, visited);
+    if (r == LS_RAY_INVALID) e[0] = e[1] = e[2] = nan;
+    result[i] = (signed char)r;
+    for (int a = 0; a < 3; ++a) ends3[3 * (size_t)i + a] = e[a];
+  }
+  add_visited(cnt, visited);
 }
 
 // ---- octree export ---------------------------------------------------------------------------------------------------
@@ -877,6 +1133,8 @@ void release(Map& m) {
   free_ptr(m.ends), free_ptr(m.pkey), free_ptr(m.cls), free_ptr(m.ep_keys), free_ptr(m.ep_min);
   for (int j = 0; j < 2; ++j) free_ptr(m.ex_k[j]), free_ptr(m.ex_v[j]);
   free_ptr(m.ex_c), free_ptr(m.cub_tmp), free_ptr(m.cnt_dev);
+  free_ptr(m.qbuf);
+  m.q_cap = 0;
   if (m.cnt_host) cudaFreeHost(m.cnt_host);
   m.cnt_host = nullptr;
 }
@@ -888,7 +1146,7 @@ size_t device_bytes(const Map& m) {
   const size_t pts = (size_t)m.pt_cap * (sizeof(float4) + sizeof(unsigned long long) + sizeof(int)) +
                      (size_t)m.ep_cap * (sizeof(unsigned long long) + sizeof(int));
   const size_t ex = (size_t)m.ex_cap * (2 * sizeof(unsigned long long) + 2 * sizeof(unsigned) + sizeof(float4)) + m.cub_bytes;
-  return pool + tab + pts + ex + sizeof(Counters);
+  return pool + tab + pts + ex + m.q_cap + sizeof(Counters);
 }
 
 int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16], bool identity, cudaStream_t st, Counters* out,
@@ -1012,6 +1270,157 @@ int download_octree(const Octree& t, unsigned char* payload, float* centres4, un
   if (t.leaves > 0 && depths) OCC_TRY(cudaMemcpyAsync(depths, t.depths, (size_t)t.leaves, cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
   return LS_OK;
+}
+
+namespace {
+
+// The next 256-byte aligned region of `bytes` in the query staging buffer.
+size_t take(size_t& off, size_t bytes) {
+  const size_t o = off;
+  off += (bytes + 255) & ~(size_t)255;
+  return o;
+}
+
+// Query staging of at least `bytes`, grown by doubling; the old buffer is dropped first (its contents are not needed).
+int reserve_query(Map& m, size_t bytes, cudaStream_t st) {
+  if (bytes <= m.q_cap) return LS_OK;
+  OCC_TRY(cudaStreamSynchronize(st));
+  size_t cap = m.q_cap ? 2 * m.q_cap : (size_t)1 << 16;
+  while (cap < bytes) cap *= 2;
+  free_ptr(m.qbuf);
+  m.q_cap = 0;
+  OCC_TRY(alloc(&m.qbuf, cap));
+  m.q_cap = cap;
+  return LS_OK;
+}
+
+int zero_visited(Map& m, cudaStream_t st) {
+  OCC_TRY(cudaMemsetAsync(&m.cnt_dev->n_out, 0, sizeof(unsigned long long), st));
+  return LS_OK;
+}
+
+// The outputs' copies are queued; wait for them and the keys visited.
+int finish_query(Map& m, cudaStream_t st, long long* visited) {
+  OCC_TRY(cudaMemcpyAsync(&m.cnt_host->n_out, &m.cnt_dev->n_out, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  *visited = (long long)m.cnt_host->n_out;
+  return LS_OK;
+}
+
+int blocks_of(long long n) { return (int)((n + 255) / 256); }
+
+// One axis of getLineStatusBoundingBox's offset loop (at most cap values); false when it has more.
+bool box_axis(double size, double res, long long cap, std::vector<double>* out) {
+  out->clear();
+  const double parts = std::ceil((size + 0.001) / res);
+  if (!(parts <= (double)cap + 2.0)) return false;  // the loop below runs about parts + 1 times
+  double disc = size / parts;
+  if (disc <= 0.0) disc = 1.0;
+  const double half = size * 0.5;
+  for (double x = -half; x <= half; x += disc) {
+    if ((long long)out->size() >= cap) return false;
+    out->push_back(x);
+  }
+  return true;
+}
+
+}  // namespace
+
+int query_cells(Map& m, const Params& P, const double* pts3, int n, int8_t* status, float* log_odds, long long* visited,
+                cudaStream_t st, uint64_t* launches) {
+  *visited = 0;
+  if (n <= 0) return LS_OK;
+  size_t off = 0;
+  const size_t o_in = take(off, (size_t)n * 3 * sizeof(double)), o_st = take(off, (size_t)n),
+               o_lo = take(off, (size_t)n * sizeof(float));
+  int rc;
+  if ((rc = reserve_query(m, off, st))) return rc;
+  char* q = m.qbuf;
+  OCC_TRY(cudaMemcpyAsync(q + o_in, pts3, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  if ((rc = zero_visited(m, st))) return rc;
+  occ_cell_kernel<<<blocks_of(n), 256, 0, st>>>((const double*)(q + o_in), n, dev_of(m), P, (signed char*)(q + o_st),
+                                                (float*)(q + o_lo), m.cnt_dev);
+  OCC_LAUNCHED();
+  OCC_TRY(cudaMemcpyAsync(status, q + o_st, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, q + o_lo, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  return finish_query(m, st, visited);
+}
+
+int query_lines(Map& m, const Params& P, const double* starts3, const double* ends3, int n, const double* box3,
+                int stop_at_unknown, int8_t* status, uint64_t* first_keys, long long* visited, cudaStream_t st,
+                uint64_t* launches) {
+  *visited = 0;
+  if (n <= 0) return LS_OK;
+  const long long kMaxLines = 0x7fffffffLL;
+  std::vector<double> axes[3];
+  long long lines = 1;
+  if (box3) {
+    for (int a = 0; a < 3; ++a) {
+      if (!box_axis(box3[a], P.res, kMaxLines / n, &axes[a])) return LS_ERR_ARG;
+      lines *= (long long)axes[a].size();
+      if (lines * n > kMaxLines) return LS_ERR_ARG;
+    }
+  }
+  const int nx = box3 ? (int)axes[0].size() : 1, ny = box3 ? (int)axes[1].size() : 1, nz = box3 ? (int)axes[2].size() : 1;
+  const size_t seg_bytes = (size_t)n * 3 * sizeof(double);
+  size_t off = 0;
+  const size_t o_s = take(off, seg_bytes), o_e = take(off, seg_bytes), o_off = take(off, (size_t)(nx + ny + nz) * sizeof(double)),
+               o_st = take(off, (size_t)n), o_fk = take(off, (size_t)n * sizeof(uint64_t)),
+               o_best = take(off, (size_t)n * sizeof(unsigned));
+  int rc;
+  if ((rc = reserve_query(m, off, st))) return rc;
+  char* q = m.qbuf;
+  const double* s = (const double*)(q + o_s);
+  const double* e = (const double*)(q + o_e);
+  double* offs = (double*)(q + o_off);
+  signed char* dst = (signed char*)(q + o_st);
+  unsigned long long* dfk = (unsigned long long*)(q + o_fk);
+  unsigned* best = (unsigned*)(q + o_best);
+  OCC_TRY(cudaMemcpyAsync(q + o_s, starts3, seg_bytes, cudaMemcpyHostToDevice, st));
+  OCC_TRY(cudaMemcpyAsync(q + o_e, ends3, seg_bytes, cudaMemcpyHostToDevice, st));
+  if ((rc = zero_visited(m, st))) return rc;
+  if (!box3) {
+    occ_line_kernel<false><<<blocks_of(n), 256, 0, st>>>(s, e, n, 1, nullptr, 1, 1, 1, stop_at_unknown, dev_of(m), P, dst, dfk,
+                                                         nullptr, m.cnt_dev);
+    OCC_LAUNCHED();
+  } else {
+    std::vector<double> flat;
+    for (int a = 0; a < 3; ++a) flat.insert(flat.end(), axes[a].begin(), axes[a].end());
+    OCC_TRY(cudaMemcpyAsync(offs, flat.data(), flat.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    OCC_TRY(cudaMemsetAsync(best, 0, (size_t)n * sizeof(unsigned), st));  // 0: no line failed
+    const long long items = lines * n;
+    occ_line_kernel<true><<<blocks_of(items), 256, 0, st>>>(s, e, items, (int)lines, offs, nx, ny, nz, stop_at_unknown,
+                                                            dev_of(m), P, dst, dfk, best, m.cnt_dev);
+    OCC_LAUNCHED();
+    occ_box_result_kernel<<<blocks_of(n), 256, 0, st>>>(s, e, n, (int)lines, offs, nx, ny, nz, stop_at_unknown, dev_of(m), P,
+                                                         best, dst, dfk, m.cnt_dev);
+    OCC_LAUNCHED();
+    // the pageable copy of `flat` is staged before cudaMemcpyAsync returns, so it may go out of scope here
+  }
+  OCC_TRY(cudaMemcpyAsync(status, dst, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (first_keys) OCC_TRY(cudaMemcpyAsync(first_keys, dfk, (size_t)n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  return finish_query(m, st, visited);
+}
+
+int query_rays(Map& m, const Params& P, const float* origins3, const float* directions3, int n, int ignore_unknown,
+               double max_range, int8_t* result, float* ends3, long long* visited, cudaStream_t st, uint64_t* launches) {
+  *visited = 0;
+  if (n <= 0) return LS_OK;
+  const size_t vec_bytes = (size_t)n * 3 * sizeof(float);
+  size_t off = 0;
+  const size_t o_o = take(off, vec_bytes), o_d = take(off, vec_bytes), o_r = take(off, (size_t)n), o_e = take(off, vec_bytes);
+  int rc;
+  if ((rc = reserve_query(m, off, st))) return rc;
+  char* q = m.qbuf;
+  OCC_TRY(cudaMemcpyAsync(q + o_o, origins3, vec_bytes, cudaMemcpyHostToDevice, st));
+  OCC_TRY(cudaMemcpyAsync(q + o_d, directions3, vec_bytes, cudaMemcpyHostToDevice, st));
+  if ((rc = zero_visited(m, st))) return rc;
+  occ_ray_kernel<<<blocks_of(n), 256, 0, st>>>((const float*)(q + o_o), (const float*)(q + o_d), n, ignore_unknown, max_range,
+                                               dev_of(m), P, (signed char*)(q + o_r), (float*)(q + o_e), m.cnt_dev);
+  OCC_LAUNCHED();
+  OCC_TRY(cudaMemcpyAsync(result, q + o_r, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (ends3) OCC_TRY(cudaMemcpyAsync(ends3, q + o_e, vec_bytes, cudaMemcpyDeviceToHost, st));
+  return finish_query(m, st, visited);
 }
 
 void release(Octree& t) {

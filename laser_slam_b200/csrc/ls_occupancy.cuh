@@ -47,6 +47,9 @@ struct Map {
   float4* ex_c = nullptr;
   void* cub_tmp = nullptr;
   size_t cub_bytes = 0;
+  // query staging (inputs and outputs of one call), grown by doubling
+  size_t q_cap = 0;
+  char* qbuf = nullptr;
   Counters* cnt_dev = nullptr;
   Counters* cnt_host = nullptr;  // pinned
   long long n_known = 0;
@@ -96,5 +99,20 @@ int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint
 // Copies the last build's payload (t.bytes) and, each when not NULL, its t.leaves centres {x, y, z, 1} and depths.
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st);
 void release(Octree& t);
+
+// Queries (oracle/QUERIES.md), reading the map only.  Synchronous; host inputs and outputs, *visited the voxel states the
+// kernels read.  n <= 0 launches nothing.
+// getCellStatusPoint: LS_CELL_* per point (double triples), the log-odds or NaN when unknown (log_odds may be NULL).
+int query_cells(Map& m, const Params& P, const double* pts3, int n, int8_t* status, float* log_odds, long long* visited,
+                cudaStream_t st, uint64_t* launches);
+// getLineStatus / getVisibility (box3 NULL) or getLineStatusBoundingBox (box3: the box size): LS_CELL_* per segment and the
+// packed key that decided it (all ones when free; first_keys may be NULL).  LS_ERR_ARG when the box has more than 2^31 - 1
+// lines in all.  The box size must be finite and >= 0 (checked by the caller).
+int query_lines(Map& m, const Params& P, const double* starts3, const double* ends3, int n, const double* box3,
+                int stop_at_unknown, int8_t* status, uint64_t* first_keys, long long* visited, cudaStream_t st,
+                uint64_t* launches);
+// castRay: LS_RAY_* per ray and the voxel centre it names (NaN for LS_RAY_INVALID; ends3 may be NULL).
+int query_rays(Map& m, const Params& P, const float* origins3, const float* directions3, int n, int ignore_unknown,
+               double max_range, int8_t* result, float* ends3, long long* visited, cudaStream_t st, uint64_t* launches);
 
 }  // namespace lso

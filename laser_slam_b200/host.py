@@ -287,6 +287,9 @@ class OccupancyMap:
             L.lsh_occupancy_occupied_cloud.argtypes = [vp, vp, ci]
             L.lsh_occupancy_write_binary.argtypes = [vp, ctypes.c_char_p]
             L.lsh_occupancy_occupied_leaf_cloud.argtypes = [vp, vp, ci]
+            L.lsh_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp]
+            L.lsh_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, ci, vp, vp]
+            L.lsh_occupancy_cast_rays.argtypes = [vp, vp, vp, ci, ci, ctypes.c_double, ci, vp, vp]
             L._occ_bound = True
         prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range], np.float64)
         err = ctypes.create_string_buffer(512)
@@ -331,3 +334,39 @@ class OccupancyMap:
         out = np.zeros((max(n, 1), 4), np.float32)
         self._check(lib().lsh_occupancy_occupied_leaf_cloud(self._h, out.ctypes.data, n))
         return out[:n]
+
+    def cell_probability(self, points):
+        """getCellProbabilityPoint per point (one query each): (status int8, probability float64, -1 when unknown)."""
+        p = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
+        st = np.zeros(max(len(p), 1), np.int8)
+        pr = np.zeros(max(len(p), 1), np.float64)
+        self._check(lib().lsh_occupancy_cell_status(self._h, p.ctypes.data, len(p), st.ctypes.data, pr.ctypes.data))
+        return st[:len(p)], pr[:len(p)]
+
+    def line_status(self, starts, ends, box=None, stop_at_unknown=True, single=False):
+        """The batched getLineStatus overload ((status, first keys)), or with single=True one getLineStatus /
+        getVisibility / getLineStatusBoundingBox call per segment (status only)."""
+        s = np.ascontiguousarray(np.asarray(starts, np.float64).reshape(-1, 3))
+        e = np.ascontiguousarray(np.asarray(ends, np.float64).reshape(-1, 3))
+        b = None if box is None else np.ascontiguousarray(np.asarray(box, np.float64).reshape(3))
+        n = len(s)
+        st = np.zeros(max(n, 1), np.int8)
+        fk = np.zeros(max(n, 1), np.uint64)
+        self._check(lib().lsh_occupancy_line_status(self._h, s.ctypes.data, e.ctypes.data, n,
+                                                    None if b is None else b.ctypes.data, int(bool(stop_at_unknown)),
+                                                    int(bool(single)), st.ctypes.data, fk.ctypes.data))
+        return st[:n] if single else (st[:n], fk[:n])
+
+    def cast_rays(self, origins, directions, ignore_unknown=False, max_range=-1.0, single=False, ends_in=None):
+        """castRays (LS_RAY_* results, ends (n,3) float64), or with single=True one castRay per ray (1 for a hit, else 0;
+        ends start as ends_in and are left alone where castRay leaves *end)."""
+        o = np.ascontiguousarray(np.asarray(origins, np.float64).reshape(-1, 3))
+        d = np.ascontiguousarray(np.asarray(directions, np.float64).reshape(-1, 3))
+        n = len(o)
+        r = np.zeros(max(n, 1), np.int32)
+        ends = np.zeros((max(n, 1), 3), np.float64)
+        if ends_in is not None:
+            ends[:n] = ends_in
+        self._check(lib().lsh_occupancy_cast_rays(self._h, o.ctypes.data, d.ctypes.data, n, int(bool(ignore_unknown)),
+                                                  float(max_range), int(bool(single)), r.ctypes.data, ends.ctypes.data))
+        return r[:n], ends[:n]

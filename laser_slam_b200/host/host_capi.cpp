@@ -462,6 +462,84 @@ int lsh_occupancy_write_binary(void* ov, const char* path) {
   }
 }
 
+// getCellProbabilityPoint per point (single queries): status and probability; 0 or LS_ERR_STATE
+int lsh_occupancy_cell_status(void* ov, const double* pts3, int n, int8_t* status, double* probability) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    for (int i = 0; i < n; ++i) {
+      const kindr::minimal::Position p{pts3[3 * i], pts3[3 * i + 1], pts3[3 * i + 2]};
+      status[i] = (int8_t)h->map->getCellProbabilityPoint(p, &probability[i]);
+      if (h->map->getCellStatusPoint(p) != static_cast<OccupancyMap::CellStatus>(status[i]))
+        throw std::runtime_error("getCellStatusPoint and getCellProbabilityPoint disagree");
+    }
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// Line status per segment: single = 1 calls getLineStatus (stop_at_unknown 1, no box), getVisibility or
+// getLineStatusBoundingBox (box3 set) once per segment; single = 0 the batched overload, which also gives first_keys.
+int lsh_occupancy_line_status(void* ov, const double* s3, const double* e3, int n, const double* box3, int stop_at_unknown,
+                              int single, int8_t* status, uint64_t* first_keys) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<kindr::minimal::Position> s(n), e(n);
+    for (int i = 0; i < n; ++i)
+      s[i] = {s3[3 * i], s3[3 * i + 1], s3[3 * i + 2]}, e[i] = {e3[3 * i], e3[3 * i + 1], e3[3 * i + 2]};
+    const kindr::minimal::Position box = box3 ? kindr::minimal::Position{box3[0], box3[1], box3[2]} : kindr::minimal::Position{};
+    if (single) {
+      for (int i = 0; i < n; ++i) {
+        OccupancyMap::CellStatus c;
+        if (box3) c = h->map->getLineStatusBoundingBox(s[i], e[i], box);
+        else if (stop_at_unknown) c = h->map->getLineStatus(s[i], e[i]);
+        else c = h->map->getVisibility(s[i], e[i], false);
+        status[i] = (int8_t)c;
+      }
+      return 0;
+    }
+    std::vector<OccupancyMap::CellStatus> st;
+    std::vector<uint64_t> fk;
+    h->map->getLineStatus(s, e, &st, stop_at_unknown != 0, box3 ? &box : NULL, &fk);
+    for (int i = 0; i < n; ++i) status[i] = (int8_t)st[(size_t)i], first_keys[i] = fk[(size_t)i];
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// castRay per ray (single = 1: the bool overload, results 1 for a hit and 0 otherwise) or castRays (single = 0: LS_RAY_*);
+// ends3 as the C++ layer returns them (left at the input's values where it leaves *end alone).
+int lsh_occupancy_cast_rays(void* ov, const double* o3, const double* d3, int n, int ignore_unknown, double max_range,
+                            int single, int* results, double* ends3) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<kindr::minimal::Position> o(n), d(n), e;
+    for (int i = 0; i < n; ++i)
+      o[i] = {o3[3 * i], o3[3 * i + 1], o3[3 * i + 2]}, d[i] = {d3[3 * i], d3[3 * i + 1], d3[3 * i + 2]};
+    if (single) {
+      for (int i = 0; i < n; ++i) {
+        kindr::minimal::Position end{ends3[3 * i], ends3[3 * i + 1], ends3[3 * i + 2]};
+        results[i] = h->map->castRay(o[i], d[i], &end, ignore_unknown != 0, max_range) ? 1 : 0;
+        for (int a = 0; a < 3; ++a) ends3[3 * i + a] = end[a];
+      }
+      return 0;
+    }
+    std::vector<int> r;
+    h->map->castRays(o, d, &r, &e, ignore_unknown != 0, max_range);
+    for (int i = 0; i < n; ++i) {
+      results[i] = r[(size_t)i];
+      for (int a = 0; a < 3; ++a) ends3[3 * i + a] = e[(size_t)i][a];
+    }
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
 // getOccupiedLeafCloud; returns its number of points, written when it is <= cap
 int lsh_occupancy_occupied_leaf_cloud(void* ov, float* out4, int cap) {
   OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);

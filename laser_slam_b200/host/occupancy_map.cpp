@@ -2,6 +2,7 @@
 #include "laser_slam/occupancy_map.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <stdexcept>
 #include <string>
 #include <tuple>
@@ -112,6 +113,104 @@ void OccupancyMap::getOccupiedLeafCloud(DataPoints* cloud) {
 
 void OccupancyMap::getVoxels(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds) const {
   download(which, keys, log_odds, NULL);
+}
+
+// ---- queries ------------------------------------------------------------------------------------------------------
+OccupancyMap::CellStatus OccupancyMap::cellStatus(const kindr::minimal::Position& point, float* log_odds) const {
+  std::lock_guard<std::mutex> lock(mutex_);
+  int8_t st = LS_CELL_UNKNOWN;
+  throwOnError(ctx_, ls_occupancy_cell_status(map_, point.data(), 1, &st, log_odds, NULL), "ls_occupancy_cell_status");
+  return static_cast<CellStatus>(st);
+}
+
+OccupancyMap::CellStatus OccupancyMap::getCellStatusPoint(const kindr::minimal::Position& point) const {
+  return cellStatus(point, NULL);
+}
+
+OccupancyMap::CellStatus OccupancyMap::getCellProbabilityPoint(const kindr::minimal::Position& point,
+                                                               double* probability) const {
+  float v = 0.f;
+  const CellStatus st = cellStatus(point, &v);
+  if (probability) *probability = st == CellStatus::kUnknown ? -1.0 : 1.0 - 1.0 / (1.0 + std::exp((double)v));
+  return st;
+}
+
+OccupancyMap::CellStatus OccupancyMap::getLineStatus(const kindr::minimal::Position& start,
+                                                     const kindr::minimal::Position& end) const {
+  return getVisibility(start, end, true);
+}
+
+OccupancyMap::CellStatus OccupancyMap::getVisibility(const kindr::minimal::Position& view_point,
+                                                     const kindr::minimal::Position& voxel_to_test,
+                                                     bool stop_at_unknown_cell) const {
+  std::vector<CellStatus> st;
+  getLineStatus(std::vector<kindr::minimal::Position>{view_point}, std::vector<kindr::minimal::Position>{voxel_to_test}, &st,
+                stop_at_unknown_cell);
+  return st[0];
+}
+
+OccupancyMap::CellStatus OccupancyMap::getLineStatusBoundingBox(const kindr::minimal::Position& start,
+                                                                const kindr::minimal::Position& end,
+                                                                const kindr::minimal::Position& bounding_box_size) const {
+  std::vector<CellStatus> st;
+  getLineStatus(std::vector<kindr::minimal::Position>{start}, std::vector<kindr::minimal::Position>{end}, &st, true,
+                &bounding_box_size);
+  return st[0];
+}
+
+bool OccupancyMap::castRay(const kindr::minimal::Position& origin, const kindr::minimal::Position& direction,
+                           kindr::minimal::Position* end, bool ignore_unknown, double max_range) const {
+  std::vector<int> r;
+  std::vector<kindr::minimal::Position> e;
+  castRays(std::vector<kindr::minimal::Position>{origin}, std::vector<kindr::minimal::Position>{direction}, &r, &e,
+           ignore_unknown, max_range);
+  if (end && r[0] != LS_RAY_INVALID) *end = e[0];
+  return r[0] == LS_RAY_HIT;
+}
+
+void OccupancyMap::getLineStatus(const std::vector<kindr::minimal::Position>& starts,
+                                 const std::vector<kindr::minimal::Position>& ends, std::vector<CellStatus>* status,
+                                 bool stop_at_unknown_cell, const kindr::minimal::Position* bounding_box_size,
+                                 std::vector<uint64_t>* first_keys) const {
+  if (status == NULL) throw std::invalid_argument("null output");
+  if (starts.size() != ends.size()) throw std::invalid_argument("starts and ends differ in length");
+  const size_t n = starts.size();
+  std::vector<double> s(3 * n), e(3 * n);
+  for (size_t i = 0; i < n; ++i)
+    for (int a = 0; a < 3; ++a) s[3 * i + a] = starts[i][a], e[3 * i + a] = ends[i][a];
+  std::vector<int8_t> st(n > 0 ? n : 1);
+  if (first_keys) first_keys->resize(n);
+  std::lock_guard<std::mutex> lock(mutex_);
+  throwOnError(ctx_,
+               ls_occupancy_line_status(map_, s.data(), e.data(), (int)n, bounding_box_size ? bounding_box_size->data() : NULL,
+                                        stop_at_unknown_cell ? 1 : 0, st.data(), first_keys ? first_keys->data() : NULL, NULL),
+               "ls_occupancy_line_status");
+  status->resize(n);
+  for (size_t i = 0; i < n; ++i) (*status)[i] = static_cast<CellStatus>(st[i]);
+}
+
+void OccupancyMap::castRays(const std::vector<kindr::minimal::Position>& origins,
+                            const std::vector<kindr::minimal::Position>& directions, std::vector<int>* results,
+                            std::vector<kindr::minimal::Position>* ends, bool ignore_unknown, double max_range) const {
+  if (results == NULL) throw std::invalid_argument("null output");
+  if (origins.size() != directions.size()) throw std::invalid_argument("origins and directions differ in length");
+  const size_t n = origins.size();
+  std::vector<float> o(3 * n), d(3 * n), e(3 * (n > 0 ? n : 1));
+  for (size_t i = 0; i < n; ++i)
+    for (int a = 0; a < 3; ++a) o[3 * i + a] = (float)origins[i][a], d[3 * i + a] = (float)directions[i][a];
+  std::vector<int8_t> r(n > 0 ? n : 1);
+  {
+    std::lock_guard<std::mutex> lock(mutex_);
+    throwOnError(ctx_,
+                 ls_occupancy_cast_rays(map_, o.data(), d.data(), (int)n, ignore_unknown ? 1 : 0, max_range, r.data(), e.data(),
+                                        NULL),
+                 "ls_occupancy_cast_rays");
+  }
+  results->assign(r.begin(), r.begin() + (std::ptrdiff_t)n);
+  if (ends) {
+    ends->resize(n);
+    for (size_t i = 0; i < n; ++i) (*ends)[i] = kindr::minimal::Position{e[3 * i], e[3 * i + 1], e[3 * i + 2]};
+  }
 }
 
 }  // namespace laser_slam

@@ -72,5 +72,18 @@ for k in range(2):
     oom.insert_scan(sc[k][0], truth[k].astype(np.float32))
 tr, otr = om.octree(), oct_oracle.of_map(oom)
 assert tr.nodes == otr.nodes > 0 and tr.payload == otr.payload and np.array_equal(tr.centres, otr.centres)
+# queries of that map (cells, lines, a bounding box, rays) against the query oracle
+from oracle import queries as occ_queries
+qo = occ_queries.KnownVoxels(*oom.download(), resolution=0.2, max_range=10.0)
+rng = np.random.default_rng(5)
+qs = truth[0][:3, 3] + rng.uniform(-4.0, 4.0, (256, 3))
+qe = qs + rng.uniform(-4.0, 4.0, (256, 3))
+qd = rng.normal(size=(256, 3)).astype(np.float32)
+qorg = np.repeat(truth[1][:3, 3][None], 256, axis=0).astype(np.float32)
+for got, want in ((om.cell_status(qs), qo.cell_status(qs)), (om.line_status(qs, qe), qo.line_status(qs, qe)),
+                  (om.line_status(qs[:32], qe[:32], box=(0.6, 0.6, 0.3)), qo.line_status(qs[:32], qe[:32], box=(0.6, 0.6, 0.3))),
+                  (om.cast_rays(qorg, qd, False, 10.0), qo.cast_rays(qorg, qd, False, 10.0)),
+                  (om.cast_rays(qorg, qd, True, 10.0), qo.cast_rays(qorg, qd, True, 10.0))):
+    assert np.array_equal(got[0], want[0]) and np.array_equal(np.asarray(got[1]).view(np.uint8), np.asarray(want[1]).view(np.uint8))
 om.close()
 print("sanitize workload ok:", g["stats"].iterations, "iterations;", len(batch), "batched problems;", ctx.launch_count, "launches")
