@@ -37,8 +37,6 @@ struct Workspace {
   float* T_hist = nullptr;
   BuildJob* job_host = nullptr;  // pinned; this workspace's slot of the context's job array
   BuildJob* job_dev = nullptr;
-  IcpWork* h_work = nullptr;  // pinned host mirrors of the small results
-  Grid* h_grid = nullptr;
   IcpProblem hp;              // host copy of this problem's descriptor
   bool stream_dirty = false;  // work (allocation-time clears) was enqueued on this workspace's own stream
 };
@@ -56,6 +54,8 @@ struct ls_ctx {
   BuildJob* jobs_dev = nullptr;      // [kMaxBatch]: workspace b stages its build in slot b
   BuildJob* jobs_host = nullptr;     // pinned
   IcpWork* work_pool = nullptr;      // [kMaxBatch] contiguous, so one memset clears a whole batch
+  IcpResult* results_dev = nullptr;  // [kMaxBatch]: launch_icp gathers every problem's results here ...
+  IcpResult* results_host = nullptr; // ... and copies them back in one piece (pinned)
   // staging of the entry points that take host clouds (used on workspace 0's stream; ensure_staging)
   float4* reading = nullptr;                               // raw reading
   float4 *ref_stage = nullptr, *ref_nrm_stage = nullptr;  // reference points and normals (scan frame)
@@ -297,19 +297,22 @@ int launch_build(ls_ctx* ctx, const BuildJob* jobs_dev, int batch, int m_max, co
   LAUNCH_CHECK();
   tables_kernel<<<dim3(cap, B), 256, 0, st>>>(jobs_dev);
   LAUNCH_CHECK();
-  scatter_kernel<<<dim3(pb, B), 256, 0, st>>>(jobs_dev);
+  // Many CTAs per job (one point per thread up to 16 CTAs per SM): the CTAs start in job order, more of them than fit on
+  // the device at once, so about one job's scatter is in flight at a time and its sorted
+  // arrays (32 B per point) stay in L2 until the scattered 16-byte writes have filled their sectors.  Grid-striding
+  // every job over 2 CTAs per SM instead keeps several jobs' arrays open at once, more than L2 holds.
+  scatter_kernel<<<dim3(blocks_for(m_max, 256, ctx->sm_count * 16), B), 256, 0, st>>>(jobs_dev);
   LAUNCH_CHECK();
   return LS_OK;
 }
 
-// R' = T_refMean_dataIn * R for every staged job, then the readings are ordered by their map's cell keys (q_count_kernel).
+// R' = T_refMean_dataIn * R for every staged job, and the readings ordered by their map's cell keys (q_count_kernel
+// does both in one pass).
 int launch_reading_sort(ls_ctx* ctx, const BuildJob* jobs_dev, int batch, int n_max, const Resolved& r, cudaStream_t st) {
   const unsigned int B = (unsigned int)batch;
   const int cap = batch > 1 ? ctx->sm_count * 2 : ctx->sm_count * 8;
   const int qb = blocks_for(n_max, 256, cap);
   const int scan_tiles = (r.max_cells + kScanTile - 1) / kScanTile;
-  reading_kernel<<<dim3(qb, B), 256, 0, st>>>(jobs_dev);
-  LAUNCH_CHECK();
   q_count_kernel<<<dim3(qb, B), 256, 0, st>>>(jobs_dev);
   LAUNCH_CHECK();
   q_tables_kernel<<<dim3(cap, B), 256, 0, st>>>(jobs_dev);
@@ -431,21 +434,29 @@ int launch_icp(ls_ctx* ctx, const ls_icp_params* prm, int batch, int n_max, bool
   CU(cudaLaunchCooperativeKernel((void*)icp_kernel, dim3(ctas * batch), dim3(kIcpThreads), args, kIcpPairBytes, w0->stream));
   ++ctx->launches;
   CU(cudaEventRecord(w0->ev2, w0->stream));
-  for (int b = 0; b < batch; ++b) {
-    Workspace* w = ctx->ws[b];
-    // only the results at the tail of the scratch come back (not the 48 KB of histograms in front of them)
-    constexpr size_t off = offsetof(IcpWork, T_out);
-    CU(cudaMemcpyAsync(reinterpret_cast<char*>(w->h_work) + off, reinterpret_cast<const char*>(w->work) + off,
-                       sizeof(IcpWork) - off, cudaMemcpyDeviceToHost, w0->stream));
-    CU(cudaMemcpyAsync(w->h_grid, &w->bs->grid, sizeof(Grid), cudaMemcpyDeviceToHost, w0->stream));
-  }
+  // one gather and one copy for the whole batch (a pair of small copies per problem costs more than the kernel)
+  collect_results_kernel<<<batch, 32, 0, w0->stream>>>(ctx->probs_dev, ctx->results_dev);
+  LAUNCH_CHECK();
+  CU(cudaMemcpyAsync(ctx->results_host, ctx->results_dev, sizeof(IcpResult) * (size_t)batch, cudaMemcpyDeviceToHost,
+                     w0->stream));
   return LS_OK;
 }
 
-// After launch_icp + a synchronise of workspace 0's stream: unpack one problem's results.
-int fetch_icp(ls_ctx* ctx, Workspace* w, int n, const float T0[16], float T_out[16], ls_icp_stats* stats,
-              bool batch_timing = false) {
-  const IcpWork& wk = *w->h_work;
+// Device times of the last launch, recorded on workspace 0 (a batch is staged, built and launched as one, so its problems
+// share them): staging .. end of the ICP launch, staging .. end of the build, the ICP launch.
+void launch_times(ls_ctx* ctx, float t[3]) {
+  const Workspace* w = ctx->ws[0];
+  t[0] = t[1] = t[2] = 0.f;
+  cudaEventElapsedTime(&t[0], w->ev0, w->ev2);
+  cudaEventElapsedTime(&t[1], w->ev0, w->ev1);
+  cudaEventElapsedTime(&t[2], w->ev_launch, w->ev2);
+}
+
+// After launch_icp + a synchronise of workspace 0's stream: unpack the results of problem k (workspace k).  `times`:
+// launch_times of the launch, when the caller already has them.
+int fetch_icp(ls_ctx* ctx, int k, int n, const float T0[16], float T_out[16], ls_icp_stats* stats,
+              const float* times = nullptr) {
+  const IcpResult& wk = ctx->results_host[k];
   std::memcpy(T_out, wk.T_out, 16 * sizeof(float));
   if (stats) {
     std::memset(stats, 0, sizeof(*stats));
@@ -455,17 +466,17 @@ int fetch_icp(ls_ctx* ctx, Workspace* w, int n, const float T0[16], float T_out[
     stats->last_kept = wk.last_kept;
     stats->last_limit = wk.last_limit;
     stats->used_ratio = n > 0 ? (float)wk.last_kept / (float)n : 0.f;
-    float ms = 0.f, bms = 0.f, kms = 0.f;
-    const Workspace* tw = batch_timing ? ctx->ws[0] : w;  // a batch is staged and built as one: its timing is shared
-    cudaEventElapsedTime(&ms, tw->ev0, ctx->ws[0]->ev2);  // staging .. end of the (shared) ICP launch
-    cudaEventElapsedTime(&bms, tw->ev0, tw->ev1);
-    cudaEventElapsedTime(&kms, ctx->ws[0]->ev_launch, ctx->ws[0]->ev2);
-    stats->device_ms = ms;
-    stats->build_ms = bms;
-    stats->icp_ms = kms;
-    stats->grid_cells = w->h_grid->n_cells0;
-    stats->grid_tables = w->h_grid->n_tab1;
-    stats->grid_overflow = w->h_grid->overflow;
+    float own[3];
+    if (!times) {
+      launch_times(ctx, own);
+      times = own;
+    }
+    stats->device_ms = times[0];
+    stats->build_ms = times[1];
+    stats->icp_ms = times[2];
+    stats->grid_cells = wk.n_cells0;
+    stats->grid_tables = wk.n_tab1;
+    stats->grid_overflow = wk.overflow;
   }
   if (wk.status != 0) {
     std::memcpy(T_out, T0, 16 * sizeof(float));
@@ -487,7 +498,7 @@ int run_icp(ls_ctx* ctx, const ls_icp_params* prm, const float4* reading_dev, in
     CU(cudaMemcpyAsync(opt_T_hist, w->T_hist, (size_t)prm->max_iterations * 16 * sizeof(float), cudaMemcpyDeviceToHost,
                        w->stream));
   CU(cudaStreamSynchronize(w->stream));
-  return fetch_icp(ctx, w, n, T0, T_out, stats);
+  return fetch_icp(ctx, 0, n, T0, T_out, stats);
 }
 
 bool is_identity16(const float* T) {
@@ -546,9 +557,7 @@ Workspace* new_workspace(ls_ctx* ctx, int index) {
   bool ok = cudaStreamCreateWithFlags(&w->stream, cudaStreamNonBlocking) == cudaSuccess &&
             cudaEventCreate(&w->ev0) == cudaSuccess && cudaEventCreate(&w->ev1) == cudaSuccess &&
             cudaEventCreate(&w->ev2) == cudaSuccess && cudaEventCreate(&w->ev_launch) == cudaSuccess &&
-            cudaMalloc((void**)&w->bs, sizeof(BuildState)) == cudaSuccess &&
-            cudaMallocHost((void**)&w->h_work, sizeof(IcpWork)) == cudaSuccess &&
-            cudaMallocHost((void**)&w->h_grid, sizeof(Grid)) == cudaSuccess;
+            cudaMalloc((void**)&w->bs, sizeof(BuildState)) == cudaSuccess;
   if (!ok) return nullptr;  // partially built workspace is leaked only on an out-of-memory init failure
   return w;
 }
@@ -561,8 +570,6 @@ void free_workspace(Workspace* w) {
                   w->A.qtab_local, w->A.qtab_total, w->A.qtop_start};
   for (void* b : bufs)
     if (b) cudaFree(b);
-  if (w->h_work) cudaFreeHost(w->h_work);
-  if (w->h_grid) cudaFreeHost(w->h_grid);
   if (w->ev0) cudaEventDestroy(w->ev0);
   if (w->ev1) cudaEventDestroy(w->ev1);
   if (w->ev2) cudaEventDestroy(w->ev2);
@@ -607,6 +614,8 @@ int ls_b200_init(int device, ls_ctx** out) {
   if (cudaMalloc((void**)&ctx->jobs_dev, sizeof(BuildJob) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (cudaMallocHost((void**)&ctx->jobs_host, sizeof(BuildJob) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (cudaMalloc((void**)&ctx->work_pool, sizeof(IcpWork) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (cudaMalloc((void**)&ctx->results_dev, sizeof(IcpResult) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (cudaMallocHost((void**)&ctx->results_host, sizeof(IcpResult) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (cudaMalloc((void**)&ctx->T0_dev, 16 * sizeof(float)) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (ensure_workspaces(ctx, 1) != LS_OK) return bail(LS_ERR_NOMEM);
   *out = ctx;
@@ -622,6 +631,8 @@ void ls_b200_destroy(ls_ctx* ctx) {
   if (ctx->jobs_dev) cudaFree(ctx->jobs_dev);
   if (ctx->jobs_host) cudaFreeHost(ctx->jobs_host);
   if (ctx->work_pool) cudaFree(ctx->work_pool);
+  if (ctx->results_dev) cudaFree(ctx->results_dev);
+  if (ctx->results_host) cudaFreeHost(ctx->results_host);
   void* stage[] = {ctx->reading, ctx->ref_stage, ctx->ref_nrm_stage, ctx->nrm_raw, ctx->T0_dev};
   for (void* b : stage)
     if (b) cudaFree(b);
@@ -1274,8 +1285,8 @@ int ls_icp_register_submap_sharded(ls_ctx* ctx, const ls_icp_params* prm, const 
   // every shard runs the full co-resident grid (the exchange needs a CTA per peer, and all shards the same shape)
   if ((rc = launch_icp(ctx, prm, 1, 1 << 30, shard_count > 1))) return rc;
   CU(cudaStreamSynchronize(w->stream));
-  ctx->xflag_base += w->h_work->xsignals;
-  return fetch_icp(ctx, w, n, T0, T_out, stats);
+  ctx->xflag_base += ctx->results_host[0].xsignals;
+  return fetch_icp(ctx, 0, n, T0, T_out, stats);
 }
 
 // Sub-map <-> sub-map registration with both clouds assembled on the device (SURVEY.md 8 f2: the loop-closure ICP of
@@ -1410,6 +1421,8 @@ int ls_icp_register_submap_batch_end(ls_ctx* ctx, float* T_outs, ls_icp_stats* s
   std::memcpy(T_outs, ctx->pending_T0.data(), 16 * sizeof(float) * (size_t)batch);
   CU(cudaSetDevice(ctx->device));
   CU(cudaStreamSynchronize(ctx->ws[0]->stream));
+  float times[3] = {0.f, 0.f, 0.f};
+  if (stats && !ctx->pending_n.empty()) launch_times(ctx, times);  // nothing was launched: no events to read
   for (int b = 0; b < batch; ++b) {
     const int k = ctx->pending_ws[b];
     if (k < 0) {  // not launched: T_out is already T0
@@ -1417,8 +1430,8 @@ int ls_icp_register_submap_batch_end(ls_ctx* ctx, float* T_outs, ls_icp_stats* s
       statuses[b] = fail(ctx, LS_ERR_CONVERGENCE, "empty reading or reference");
       continue;
     }
-    const int st = fetch_icp(ctx, ctx->ws[k], ctx->pending_n[k], ctx->pending_T0.data() + 16 * b, T_outs + 16 * b,
-                             stats ? stats + b : nullptr, true);
+    const int st = fetch_icp(ctx, k, ctx->pending_n[k], ctx->pending_T0.data() + 16 * b, T_outs + 16 * b,
+                             stats ? stats + b : nullptr, times);
     if (st < 0) return st;
     statuses[b] = st;
   }

@@ -26,6 +26,10 @@ constexpr int kIcpThreads = 512;
 constexpr int kIcpCtasPerSm = 1024 / kIcpThreads;
 constexpr int kMaxSmooth = 15;
 constexpr uint32_t kTag1 = 1u << 31, kKeyMask = (1u << 31) - 1u;  // pkey: tag | key (fine keys < 2^31)
+// Untagged pkey between count0 and scatter: the fine sub-index (< LS_FB3 = 2^9) above the level-0 cell (< 2^22: the
+// device caps max_cells there).
+constexpr int kSubShift = 22;
+constexpr uint32_t kCellMask = (1u << kSubShift) - 1u;
 
 struct Parts {
   int n_parts;
@@ -45,7 +49,7 @@ struct BuildState {
 };
 
 struct BuildArrays {
-  float4* sub_pts;   // assembled (then centred) sub-map, original order
+  float4* sub_pts;   // assembled sub-map, original order (not centred: scatter_kernel centres the sorted copy)
   float4* sub_nrm;
   float4* srt_pts;   // sorted {x,y,z,idx}
   float4* srt_nrm;
@@ -104,6 +108,16 @@ struct alignas(16) IcpWork {
   double dbg_A[6], dbg_x[6];
 };
 
+// What the host reads back of one registration: the results at the tail of its IcpWork and its grid's statistics.  A
+// launch gathers them for all its problems into one array (collect_results_kernel), which comes back in one copy.
+struct IcpResult {
+  float T_out[16];
+  int status, iterations, converged, max_iter_reached, last_kept;
+  float last_limit;
+  unsigned int xsignals;
+  int n_cells0, n_tab1, overflow;
+};
+
 // Query-sharded registration: how one GPU reaches the others.  Every GPU owns an array of `shard_count` IcpWork
 // "slots" plus an arrival counter.  Slot [self] is where the GPU's own CTAs accumulate (L2 atomics, as in the unsharded
 // kernel); slot [r] receives, by plain stores over NVLink, the sections of shard r's slot [r] that the next step reads.
@@ -158,6 +172,26 @@ __device__ __forceinline__ long long warp_sum_ll(long long v) {
   mid = __reduce_add_sync(0xffffffffu, mid);
   hi = __reduce_add_sync(0xffffffffu, hi);
   return ((long long)hi << 42) + ((long long)mid << 21) + (long long)lo;
+}
+
+// Histogram counters of the build.  Consecutive points of a lidar ring fall into the same cell, so the 32 lanes of a
+// warp often carry one or two distinct keys: the lanes with equal keys (`active` = the lanes taking part) form a group
+// whose leader does one atomic for all of them.  Every lane of `active` must make the call with the key (tagged
+// pkey/qkey or level-0 cell) that names its counter `ctr` uniquely.
+__device__ __forceinline__ void warp_count(uint32_t* ctr, uint32_t key, unsigned int active) {
+  const unsigned int peers = __match_any_sync(active, key);
+  if ((threadIdx.x & 31) == (unsigned int)(__ffs(peers) - 1)) atomicAdd(ctr, (unsigned int)__popc(peers));
+}
+// Scatter cursor: takes one slot per lane from *ctr (counting down) and returns the lane's slot; the group of lanes
+// with equal keys takes its slots with one atomicSub.  The counter ends at zero once every point is placed.
+__device__ __forceinline__ uint32_t warp_take(uint32_t* ctr, uint32_t key, unsigned int active) {
+  const unsigned int peers = __match_any_sync(active, key);
+  const int leader = __ffs(peers) - 1;
+  const unsigned int lane = threadIdx.x & 31;
+  uint32_t old = 0;
+  if (lane == (unsigned int)leader) old = atomicSub(ctr, (unsigned int)__popc(peers));
+  old = __shfl_sync(peers, old, leader);
+  return old - 1u - (uint32_t)__popc(peers & ((1u << lane) - 1u));
 }
 
 // ---- K0: assemble + statistics -------------------------------------------------------------------
@@ -265,7 +299,11 @@ __global__ void setup_kernel(const BuildJob* __restrict__ jobs, float cell_size,
   for (int a = 0; a < 3; ++a) bs->T_pre[12 + a] = T0[12 + a] - mu[a];
 }
 
-// ---- K1b: centre + level-0 histogram --------------------------------------------------------------
+// ---- K1b: level-0 histogram, and each point's level-0 cell and fine sub-index ----------------------------------
+// The sub-map stays as assembled (the scatter centres it); the cell expressions take the centred coordinates, so
+// membership is exactly what the queries assume.
+// The point loops of the build run a whole warp per step (the warp-aggregated counters need all its lanes there): a
+// warp takes 32 consecutive points, `active` holds the lanes that have one.
 __global__ void __launch_bounds__(256) count0_kernel(const BuildJob* __restrict__ jobs) {
   const BuildJob& J = jobs[blockIdx.y];
   const BuildState* __restrict__ bs = J.bs;
@@ -274,15 +312,17 @@ __global__ void __launch_bounds__(256) count0_kernel(const BuildJob* __restrict_
   __shared__ Grid g;
   if (threadIdx.x == 0) g = bs->grid;
   __syncthreads();
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
-    float4 p = A.sub_pts[i];
-    p.x = p.x - g.mu[0];
-    p.y = p.y - g.mu[1];
-    p.z = p.z - g.mu[2];
-    A.sub_pts[i] = p;
-    const int c0 = top_index(g, p.x, p.y, p.z);
-    atomicAdd(&A.cnt0[c0], 1u);
-    A.pkey[i] = (uint32_t)c0;
+  const int lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i - lane < m; i += gridDim.x * blockDim.x) {
+    const unsigned int active = __ballot_sync(0xffffffffu, i < m);
+    if (i >= m) break;
+    const float4 p = A.sub_pts[i];
+    const float x = p.x - g.mu[0], y = p.y - g.mu[1], z = p.z - g.mu[2];
+    const int c0 = top_index(g, x, y, z);
+    float lx, ly, lz;
+    top_origin(g, c0, lx, ly, lz);
+    warp_count(A.cnt0 + c0, (uint32_t)c0, active);
+    A.pkey[i] = ((uint32_t)sub_index(x, y, z, lx, ly, lz, g.inv1) << kSubShift) | (uint32_t)c0;
   }
 }
 
@@ -429,23 +469,18 @@ __global__ void __launch_bounds__(1024) pyramid_up_kernel(const BuildJob* __rest
   }
 }
 
-// ---- K1d: level-1 histogram -------------------------------------------------------------------------
+// ---- K1d: level-1 histogram (from the keys count0 left: the points are not read again) ----------------------
 __global__ void __launch_bounds__(256) count1_kernel(const BuildJob* __restrict__ jobs) {
-  const BuildState* __restrict__ bs = jobs[blockIdx.y].bs;
   const BuildArrays A = jobs[blockIdx.y].A;
   const int m = jobs[blockIdx.y].m;
-  __shared__ Grid g;
-  if (threadIdx.x == 0) g = bs->grid;
-  __syncthreads();
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
-    const uint32_t c0 = A.pkey[i];
-    const Entry e = A.top[c0];
-    if (e.meta >= 0) continue;
-    const float4 p = A.sub_pts[i];
-    float lx, ly, lz;
-    top_origin(g, (int)c0, lx, ly, lz);
-    const uint32_t key = (uint32_t)(~e.meta) * (uint32_t)LS_FB3 + (uint32_t)sub_index(p.x, p.y, p.z, lx, ly, lz, g.inv1);
-    atomicAdd(&A.cnt1[key], 1u);
+  const int lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i - lane < m; i += gridDim.x * blockDim.x) {
+    const uint32_t k = i < m ? A.pkey[i] : 0u;
+    const int meta = i < m ? A.top[k & kCellMask].meta : 0;
+    const unsigned int active = __ballot_sync(0xffffffffu, meta < 0);
+    if (meta >= 0) continue;
+    const uint32_t key = (uint32_t)(~meta) * (uint32_t)LS_FB3 + (k >> kSubShift);
+    warp_count(A.cnt1 + key, key, active);
     A.pkey[i] = kTag1 | key;
   }
 }
@@ -504,17 +539,26 @@ __global__ void __launch_bounds__(256) tables_kernel(const BuildJob* __restrict_
   }
 }
 
-// ---- K1f: scatter into sorted order (the leaf histograms double as cursors and end at zero) ---------
+// ---- K1f: centre and scatter into sorted order (the leaf histograms double as cursors and end at zero) -----------
 __global__ void __launch_bounds__(256) scatter_kernel(const BuildJob* __restrict__ jobs) {
   const BuildArrays A = jobs[blockIdx.y].A;
   const int m = jobs[blockIdx.y].m;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+  const float* mu = jobs[blockIdx.y].bs->grid.mu;
+  const float mx = mu[0], my = mu[1], mz = mu[2];
+  const int lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i - lane < m; i += gridDim.x * blockDim.x) {
+    const unsigned int active = __ballot_sync(0xffffffffu, i < m);
+    if (i >= m) break;
     const uint32_t k = A.pkey[i];
-    const uint32_t tag = k & ~kKeyMask, key = k & kKeyMask;
-    uint32_t pos;
-    if (tag == kTag1) pos = A.tab1[key].start + atomicSub(&A.cnt1[key], 1u) - 1u;
-    else pos = A.top[key].start + atomicSub(&A.cnt0[key], 1u) - 1u;
+    const bool fine = (k & kTag1) != 0u;
+    const uint32_t key = fine ? k : (k & kCellMask);  // tagged: never equal to a level-0 cell
+    const Entry* e = fine ? A.tab1 + (key & kKeyMask) : A.top + key;
+    uint32_t* ctr = fine ? A.cnt1 + (key & kKeyMask) : A.cnt0 + key;
+    const uint32_t pos = e->start + warp_take(ctr, key, active);
     float4 p = A.sub_pts[i];
+    p.x = p.x - mx;
+    p.y = p.y - my;
+    p.z = p.z - mz;
     p.w = __int_as_float(i);
     A.srt_pts[pos] = p;
     A.srt_nrm[pos] = A.sub_nrm[i];
@@ -527,29 +571,42 @@ __global__ void __launch_bounds__(256) scatter_kernel(const BuildJob* __restrict
 // lidar ring.  It is a counting sort that borrows the map's histogram arrays -- they are all zero again once the
 // map's scatter has run, and the cursors below return them to zero.  Results do not depend on the order: every
 // reduction of the ICP kernel is an exact integer sum.
+// q_count_kernel also pre-transforms the reading, R' = T_refMean_dataIn * R, into `rd` (reading_kernel's arithmetic).
 __global__ void __launch_bounds__(256) q_count_kernel(const BuildJob* __restrict__ jobs) {
   const BuildState* __restrict__ bs = jobs[blockIdx.y].bs;
   const BuildArrays A = jobs[blockIdx.y].A;
-  const float4* __restrict__ rd = jobs[blockIdx.y].rd;
+  const float4* __restrict__ in = jobs[blockIdx.y].reading;
+  float4* __restrict__ rd = jobs[blockIdx.y].rd;
   const int n = jobs[blockIdx.y].n;
   __shared__ Grid g;
+  __shared__ float T[16];
   if (threadIdx.x == 0) g = bs->grid;
+  if (threadIdx.x < 16) T[threadIdx.x] = bs->T_pre[threadIdx.x];
   __syncthreads();
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 p = __ldg(rd + i);
+  const int lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i - lane < n; i += gridDim.x * blockDim.x) {
+    const unsigned int active = __ballot_sync(0xffffffffu, i < n);
+    if (i >= n) break;
+    const float4 a = __ldg(in + i);
+    float4 p;
+    xform_point(T, a.x, a.y, a.z, p.x, p.y, p.z);
+    p.w = a.w;
+    rd[i] = p;
     const int c0 = top_index(g, p.x, p.y, p.z);
     const Entry e = A.top[c0];
     uint32_t key;
+    uint32_t* ctr;
     if (e.meta < 0) {
       float lx, ly, lz;
       top_origin(g, c0, lx, ly, lz);
       key = (uint32_t)(~e.meta) * (uint32_t)LS_FB3 + (uint32_t)sub_index(p.x, p.y, p.z, lx, ly, lz, g.inv1);
-      atomicAdd(&A.cnt1[key], 1u);
+      ctr = A.cnt1 + key;
       key |= kTag1;
     } else {
       key = (uint32_t)c0;
-      atomicAdd(&A.cnt0[c0], 1u);
+      ctr = A.cnt0 + c0;
     }
+    warp_count(ctr, key, active);
     A.qkey[i] = key;
   }
 }
@@ -669,15 +726,22 @@ __global__ void __launch_bounds__(256) q_scatter_kernel(const BuildJob* __restri
   const BuildArrays A = jobs[blockIdx.y].A;
   const float4* __restrict__ rd = jobs[blockIdx.y].rd;
   const int n = jobs[blockIdx.y].n;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+  const int lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i - lane < n; i += gridDim.x * blockDim.x) {
+    const unsigned int active = __ballot_sync(0xffffffffu, i < n);
+    if (i >= n) break;
     const uint32_t k = A.qkey[i];
-    uint32_t rank;
+    uint32_t start;
+    uint32_t* ctr;
     if (k & kTag1) {
       const uint32_t key = k & kKeyMask;
-      rank = A.qtop_start[A.tab1_cell[key / (uint32_t)LS_FB3]] + A.qtab_local[key] + atomicSub(&A.cnt1[key], 1u) - 1u;
+      start = A.qtop_start[A.tab1_cell[key / (uint32_t)LS_FB3]] + A.qtab_local[key];
+      ctr = A.cnt1 + key;
     } else {
-      rank = A.qtop_start[k] + atomicSub(&A.cnt0[k], 1u) - 1u;
+      start = A.qtop_start[k];
+      ctr = A.cnt0 + k;
     }
+    const uint32_t rank = start + warp_take(ctr, k, active);
     A.rd_s[rank] = __ldg(rd + i);
     A.qperm[rank] = (uint32_t)i;
   }
@@ -711,6 +775,26 @@ __global__ void shard_slice_kernel(IcpProblem* P, const BuildJob* __restrict__ j
   P->lists.vq += q0;
   P->lists.vpts += q0;  // the candidate slots keep their stride (lists.n = the whole reading)
   P->n = q1 - q0;
+}
+
+// one CTA per problem of an ICP launch, after it: results -> out[problem]
+__global__ void collect_results_kernel(const IcpProblem* __restrict__ probs, IcpResult* __restrict__ out) {
+  const IcpProblem& P = probs[blockIdx.x];
+  const IcpWork* W = P.work;
+  IcpResult& r = out[blockIdx.x];
+  if (threadIdx.x < 16) r.T_out[threadIdx.x] = W->T_out[threadIdx.x];
+  if (threadIdx.x == 0) {
+    r.status = W->status;
+    r.iterations = W->iterations;
+    r.converged = W->converged;
+    r.max_iter_reached = W->max_iter_reached;
+    r.last_kept = W->last_kept;
+    r.last_limit = W->last_limit;
+    r.xsignals = W->xsignals;
+    r.n_cells0 = P.bs->grid.n_cells0;
+    r.n_tab1 = P.bs->grid.n_tab1;
+    r.overflow = P.bs->grid.overflow;
+  }
 }
 
 // ---- reading pre-transform: R' = T_refMean_dataIn * R ----------------------------------------------
@@ -764,8 +848,6 @@ __global__ void pack_normals_kernel(const float4* __restrict__ in, int n, float*
   }
 }
 
-// un-centre an assembled sub-map is never needed: ls_map_assemble downloads before centring.
-
 // ---- matcher-only kernel (ls_nn_query): cold exact NN for every pre-transformed reading point -------
 __global__ void __launch_bounds__(256) nn_query_kernel(const BuildState* __restrict__ bs, GridView view,
                                                        const float4* __restrict__ rd, int n, int* __restrict__ ids,
@@ -788,20 +870,28 @@ __global__ void __launch_bounds__(256) nn_query_kernel(const BuildState* __restr
 // accumulated in double in (d2, index) order, eigenvector of the smallest eigenvalue, flipped towards the sensor
 // (the origin of the scan frame).  Deterministic; bit-comparable with the CPU restatement in oracle/.
 __global__ void __launch_bounds__(128) knn_normals_kernel(const BuildState* __restrict__ bs, GridView view,
-                                                           const float4* __restrict__ pts_c /* centred, original order */,
+                                                           const float4* __restrict__ pts /* assembled, original order */,
                                                            int n, int k, float4* __restrict__ out) {
   __shared__ Grid g;
   if (threadIdx.x == 0) g = bs->grid;
   __syncthreads();
+  // the centred coordinates, as scatter_kernel computes them for the hash
+  auto centred = [&](int j) {
+    float4 p = __ldg(pts + j);
+    p.x = p.x - g.mu[0];
+    p.y = p.y - g.mu[1];
+    p.z = p.z - g.mu[2];
+    return p;
+  };
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 q = __ldg(pts_c + i);
+    const float4 q = centred(i);
     TopK t;
     knn_search(g, view, q.x, q.y, q.z, k, t);
     int cnt = 0;
     double mx = 0.0, my = 0.0, mz = 0.0;
     for (int j = 0; j < k; ++j) {
       if (t.id[j] == INT_MAX) break;
-      const float4 p = __ldg(pts_c + t.id[j]);
+      const float4 p = centred(t.id[j]);
       mx = mx + (double)p.x;
       my = my + (double)p.y;
       mz = mz + (double)p.z;
@@ -813,7 +903,7 @@ __global__ void __launch_bounds__(128) knn_normals_kernel(const BuildState* __re
       mx = mx * inv; my = my * inv; mz = mz * inv;
       double C[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
       for (int j = 0; j < cnt; ++j) {
-        const float4 p = __ldg(pts_c + t.id[j]);
+        const float4 p = centred(t.id[j]);
         const double dx = (double)p.x - mx, dy = (double)p.y - my, dz = (double)p.z - mz;
         C[0] = C[0] + dx * dx; C[1] = C[1] + dx * dy; C[2] = C[2] + dx * dz;
         C[4] = C[4] + dy * dy; C[5] = C[5] + dy * dz; C[8] = C[8] + dz * dz;
