@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/ls_b200.h"
+#include "ls_buffer.cuh"
 #include "ls_filters.cuh"
 #include "ls_kernels.cuh"
 #include "ls_occupancy.cuh"
@@ -21,20 +22,32 @@ using namespace ls;
 
 // Everything one registration needs on the device.  A context owns one workspace per concurrently
 // running problem (ls_icp_register_submap_batch); single-problem entry points use workspace 0.
+// The arrays come in groups that grow together (ensure_capacity); the first array of a group tells its capacity.
 struct Workspace {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev_launch = nullptr;
-  int n_cap = 0, m_cap = 0, cells_cap = 0, tab_cap = 0, hist_cap = 0;
-  BuildArrays A{};
-  BuildState* bs = nullptr;
-  float4* rd = nullptr;  // pre-transformed reading
-  int* pos = nullptr;
-  float4 *vq = nullptr, *vpts = nullptr;                   // certified candidate lists (ls_grid.cuh VLists)
-  float* d2 = nullptr;
-  int* ids = nullptr;
-  float* d2_out = nullptr;
+  Buffer<BuildState> bs;
+  // per reading point
+  Buffer<float4> rd;  // pre-transformed reading
+  Buffer<int> pos;
+  Buffer<float> d2;
+  Buffer<float4> vq, vpts;  // certified candidate lists (ls_grid.cuh VLists)
+  Buffer<int> ids;
+  Buffer<float> d2_out;
+  Buffer<uint32_t> qkey, qperm;
+  Buffer<float4> rd_s;
+  // per sub-map point, and the fine tables (BuildArrays)
+  Buffer<float4> sub_pts, sub_nrm, srt_pts, srt_nrm;
+  Buffer<uint32_t> pkey;
+  Buffer<Entry> tab1;
+  Buffer<uint32_t> cnt1, tab1_cell, qtab_local, qtab_total;
+  // per level-0 cell
+  Buffer<Entry> top;
+  Buffer<uint32_t> cnt0;
+  Buffer<unsigned long long> pyr, topmask;
+  Buffer<uint32_t> qtop_start;
+  Buffer<float> T_hist;  // per iteration
   IcpWork* work = nullptr;
-  float* T_hist = nullptr;
   BuildJob* job_host = nullptr;  // pinned; this workspace's slot of the context's job array
   BuildJob* job_dev = nullptr;
   IcpProblem hp;              // host copy of this problem's descriptor
@@ -49,20 +62,18 @@ struct ls_ctx {
   std::string err;
   uint64_t launches = 0;
   std::vector<Workspace*> ws;
-  IcpProblem* probs_dev = nullptr;   // [kMaxBatch]
-  IcpProblem* probs_host = nullptr;  // pinned
-  BuildJob* jobs_dev = nullptr;      // [kMaxBatch]: workspace b stages its build in slot b
-  BuildJob* jobs_host = nullptr;     // pinned
-  IcpWork* work_pool = nullptr;      // [kMaxBatch] contiguous, so one memset clears a whole batch
-  IcpResult* results_dev = nullptr;  // [kMaxBatch]: launch_icp gathers every problem's results here ...
-  IcpResult* results_host = nullptr; // ... and copies them back in one piece (pinned)
+  Buffer<IcpProblem> probs_dev;          // [kMaxBatch]
+  PinnedBuffer<IcpProblem> probs_host;
+  Buffer<BuildJob> jobs_dev;             // [kMaxBatch]: workspace b stages its build in slot b
+  PinnedBuffer<BuildJob> jobs_host;
+  Buffer<IcpWork> work_pool;             // [kMaxBatch] contiguous, so one memset clears a whole batch
+  Buffer<IcpResult> results_dev;         // [kMaxBatch]: launch_icp gathers every problem's results here ...
+  PinnedBuffer<IcpResult> results_host;  // ... and copies them back in one piece
   // staging of the entry points that take host clouds (used on workspace 0's stream; ensure_staging)
-  float4* reading = nullptr;                               // raw reading
-  float4 *ref_stage = nullptr, *ref_nrm_stage = nullptr;  // reference points and normals (scan frame)
-  int reading_cap = 0, ref_cap = 0;
-  float* nrm_raw = nullptr;                                // raw normals (upload_normals)
-  size_t nrm_raw_cap = 0;
-  float* T0_dev = nullptr;                                 // 16 floats: ls_transform_cloud's transformation
+  Buffer<float4> reading;                 // raw reading
+  Buffer<float4> ref_stage, ref_nrm_stage;  // reference points and normals (scan frame)
+  Buffer<float> nrm_raw;                  // raw normals (upload_normals)
+  Buffer<float> T0_dev;                   // 16 floats: ls_transform_cloud's transformation
   // query-sharded registration: this GPU's exchange buffer (shard_count slots + the arrival counter) and the peers'
   unsigned char* xbuf = nullptr;
   unsigned char* xpeer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -83,8 +94,7 @@ struct ls_ctx {
 constexpr int kMaxBatch = 160;
 
 struct ls_scan_slot {
-  float4* pts = nullptr;
-  float4* nrm = nullptr;
+  Buffer<float4> pts, nrm;
   int n = 0;
   uint64_t id = 0;
   bool used = false;
@@ -100,13 +110,11 @@ struct ls_map {
   std::vector<ls_scan_slot> slots;
   // asynchronous uploads (ls_map_push_scan_async): own stream, a small ring of raw-normals staging buffers
   cudaStream_t up_stream = nullptr;
-  float* stage[kStageRing] = {};
-  size_t stage_cap[kStageRing] = {};
+  Buffer<float> stage[kStageRing];
   cudaEvent_t stage_free[kStageRing] = {};
   uint64_t n_async = 0;
   // pinned host staging of ls_map_push_scan (pageable caller memory is copied here, the DMA then runs behind the call)
-  float* host_stage[kStageRing] = {};
-  size_t host_stage_cap[kStageRing] = {};
+  PinnedBuffer<float> host_stage[kStageRing];
 };
 
 namespace {
@@ -142,92 +150,98 @@ int fail(ls_ctx* ctx, int code, const char* fmt, ...) {
     if (e_ != cudaSuccess) return fail(ctx, LS_ERR_CUDA, "kernel launch: %s", cudaGetErrorString(e_)); \
   } while (0)
 
-template <typename T>
-int dev_alloc(ls_ctx* ctx, T** p, size_t count) {
-  if (*p) cudaFree(*p);
-  *p = nullptr;
-  CU(cudaMalloc((void**)p, count * sizeof(T)));
-  return LS_OK;
-}
-
 inline int blocks_for(int n, int threads, int cap) {
   int b = (n + threads - 1) / threads;
   if (b < 1) b = 1;
   return b > cap ? cap : b;
 }
 
+// A group of arrays that failed to grow (and was emptied), reported as CU reports a failed call.
+int grow_failed(ls_ctx* ctx, cudaError_t e, const char* group) {
+  return fail(ctx, e == cudaErrorMemoryAllocation ? LS_ERR_NOMEM : LS_ERR_CUDA, "%s: %s", group, cudaGetErrorString(e));
+}
+
+// Each group grows all or nothing: when one array fails, the whole group is emptied, so a later call regrows all of it.
 int ensure_capacity(ls_ctx* ctx, Workspace* w, int n, int m, int max_cells, int max_iter) {
-  if (n > w->n_cap) {
-    const int cap = n + n / 8 + 1024;
-    int rc;
-    if ((rc = dev_alloc(ctx, &w->rd, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->pos, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->d2, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->vq, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->vpts, (size_t)cap * LS_VK))) return rc;
-    if ((rc = dev_alloc(ctx, &w->ids, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->d2_out, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.qkey, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.qperm, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.rd_s, (size_t)cap))) return rc;
-    w->n_cap = cap;
+  cudaError_t e;
+  if ((size_t)n > w->rd.capacity()) {
+    const size_t c = (size_t)(n + n / 8 + 1024), cv = c * LS_VK;
+    if ((e = w->rd.reserve(c, c)) || (e = w->pos.reserve(c, c)) || (e = w->d2.reserve(c, c)) || (e = w->vq.reserve(c, c)) ||
+        (e = w->vpts.reserve(cv, cv)) || (e = w->ids.reserve(c, c)) || (e = w->d2_out.reserve(c, c)) ||
+        (e = w->qkey.reserve(c, c)) || (e = w->qperm.reserve(c, c)) || (e = w->rd_s.reserve(c, c))) {
+      w->rd.reset(), w->pos.reset(), w->d2.reset(), w->vq.reset(), w->vpts.reset(), w->ids.reset(), w->d2_out.reset();
+      w->qkey.reset(), w->qperm.reset(), w->rd_s.reset();
+      return grow_failed(ctx, e, "reading arrays");
+    }
   }
-  if (m > w->m_cap) {
+  if ((size_t)m > w->sub_pts.capacity()) {
     const int cap = m + m / 8 + 1024;
-    int rc;
-    if ((rc = dev_alloc(ctx, &w->A.sub_pts, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.sub_nrm, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.srt_pts, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.srt_nrm, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.pkey, (size_t)cap))) return rc;
     // a fine table exists only for a level-0 cell with > leaf_split (>= 16) points; the pool is also capped at
     // ~1.5 GB (cells beyond the pool stay leaves: slower, still exact, flagged in stats.grid_overflow)
     int tcap = cap / 17 + 1024;
     const int tmax = (int)((size_t)1536 * 1024 * 1024 / ((size_t)LS_FB3 * 12));
     if (tcap > tmax) tcap = tmax;
-    if ((rc = dev_alloc(ctx, &w->A.tab1, (size_t)tcap * LS_FB3))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.cnt1, (size_t)tcap * LS_FB3))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.tab1_cell, (size_t)tcap))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.qtab_local, (size_t)tcap * LS_FB3))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.qtab_total, (size_t)tcap))) return rc;
-    CU(cudaMemsetAsync(w->A.cnt1, 0, (size_t)tcap * LS_FB3 * sizeof(uint32_t), w->stream));
+    const size_t c = (size_t)cap, t = (size_t)tcap, tf = t * LS_FB3;
+    if ((e = w->sub_pts.reserve(c, c)) || (e = w->sub_nrm.reserve(c, c)) || (e = w->srt_pts.reserve(c, c)) ||
+        (e = w->srt_nrm.reserve(c, c)) || (e = w->pkey.reserve(c, c)) || (e = w->tab1.reserve(tf, tf)) ||
+        (e = w->cnt1.reserve(tf, tf)) || (e = w->tab1_cell.reserve(t, t)) || (e = w->qtab_local.reserve(tf, tf)) ||
+        (e = w->qtab_total.reserve(t, t))) {
+      w->sub_pts.reset(), w->sub_nrm.reset(), w->srt_pts.reset(), w->srt_nrm.reset(), w->pkey.reset(), w->tab1.reset();
+      w->cnt1.reset(), w->tab1_cell.reset(), w->qtab_local.reset(), w->qtab_total.reset();
+      return grow_failed(ctx, e, "sub-map arrays");
+    }
+    CU(cudaMemsetAsync(w->cnt1.get(), 0, tf * sizeof(uint32_t), w->stream));
     w->stream_dirty = true;
-    w->A.tab_cap = tcap;
-    w->tab_cap = tcap;
-    w->m_cap = cap;
   }
-  if (max_cells > w->cells_cap) {
-    int rc;
-    if ((rc = dev_alloc(ctx, &w->A.top, (size_t)max_cells + 1))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.cnt0, (size_t)max_cells + 1))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.pyr, (size_t)max_cells / 2 + 4096))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.topmask, (size_t)max_cells + 1))) return rc;
-    if ((rc = dev_alloc(ctx, &w->A.qtop_start, (size_t)max_cells + 1))) return rc;
-    CU(cudaMemsetAsync(w->A.cnt0, 0, ((size_t)max_cells + 1) * sizeof(uint32_t), w->stream));
+  if ((size_t)max_cells + 1 > w->top.capacity()) {
+    const size_t c = (size_t)max_cells + 1, cp = (size_t)max_cells / 2 + 4096;
+    if ((e = w->top.reserve(c, c)) || (e = w->cnt0.reserve(c, c)) || (e = w->pyr.reserve(cp, cp)) ||
+        (e = w->topmask.reserve(c, c)) || (e = w->qtop_start.reserve(c, c))) {
+      w->top.reset(), w->cnt0.reset(), w->pyr.reset(), w->topmask.reset(), w->qtop_start.reset();
+      return grow_failed(ctx, e, "cell arrays");
+    }
+    CU(cudaMemsetAsync(w->cnt0.get(), 0, c * sizeof(uint32_t), w->stream));
     w->stream_dirty = true;
-    w->cells_cap = max_cells;
   }
-  if (max_iter > w->hist_cap) {
-    int rc;
-    if ((rc = dev_alloc(ctx, &w->T_hist, (size_t)max_iter * 16))) return rc;
-    w->hist_cap = max_iter;
-  }
+  CU(w->T_hist.reserve((size_t)max_iter * 16, (size_t)max_iter * 16));
   return LS_OK;
+}
+
+// The kernels' view of workspace w's arrays.
+BuildArrays arrays(const Workspace* w) {
+  BuildArrays A;
+  A.sub_pts = w->sub_pts.get();
+  A.sub_nrm = w->sub_nrm.get();
+  A.srt_pts = w->srt_pts.get();
+  A.srt_nrm = w->srt_nrm.get();
+  A.pkey = w->pkey.get();
+  A.top = w->top.get();
+  A.cnt0 = w->cnt0.get();
+  A.tab1 = w->tab1.get();
+  A.cnt1 = w->cnt1.get();
+  A.tab1_cell = w->tab1_cell.get();
+  A.tab_cap = (int)w->tab1_cell.capacity();
+  A.pyr = w->pyr.get();
+  A.topmask = w->topmask.get();
+  A.qkey = w->qkey.get();
+  A.qtop_start = w->qtop_start.get();
+  A.qtab_local = w->qtab_local.get();
+  A.qtab_total = w->qtab_total.get();
+  A.qperm = w->qperm.get();
+  A.rd_s = w->rd_s.get();
+  return A;
 }
 
 // The context's staging for a host reading of n points and a host reference of m points, grown like the workspaces.
 int ensure_staging(ls_ctx* ctx, int n, int m) {
-  int rc;
-  if (n > ctx->reading_cap) {
-    const int cap = n + n / 8 + 1024;
-    if ((rc = dev_alloc(ctx, &ctx->reading, (size_t)cap))) return rc;
-    ctx->reading_cap = cap;
-  }
-  if (m > ctx->ref_cap) {
-    const int cap = m + m / 8 + 1024;
-    if ((rc = dev_alloc(ctx, &ctx->ref_stage, (size_t)cap))) return rc;
-    if ((rc = dev_alloc(ctx, &ctx->ref_nrm_stage, (size_t)cap))) return rc;
-    ctx->ref_cap = cap;
+  const size_t cn = (size_t)(n + n / 8 + 1024), cm = (size_t)(m + m / 8 + 1024);
+  CU(ctx->reading.reserve((size_t)n, cn));
+  if ((size_t)m > ctx->ref_stage.capacity()) {
+    cudaError_t e;
+    if ((e = ctx->ref_stage.reserve(cm, cm)) || (e = ctx->ref_nrm_stage.reserve(cm, cm))) {
+      ctx->ref_stage.reset(), ctx->ref_nrm_stage.reset();
+      return grow_failed(ctx, e, "reference staging");
+    }
   }
   return LS_OK;
 }
@@ -261,12 +275,12 @@ int check_params(ls_ctx* ctx, const ls_icp_params* p) {
 void fill_job(Workspace* w, const Parts& parts, const float* T0_host, const float4* reading_dev, int n) {
   BuildJob& J = *w->job_host;
   J.parts = parts;
-  J.bs = w->bs;
-  J.A = w->A;
+  J.bs = w->bs.get();
+  J.A = arrays(w);
   J.m = parts.offset[parts.n_parts];
   J.n = n;
   J.reading = reading_dev;
-  J.rd = w->rd;
+  J.rd = w->rd.get();
   std::memcpy(J.T0, T0_host, sizeof(J.T0));
 }
 
@@ -337,20 +351,16 @@ int upload_normals(ls_ctx* ctx, Workspace* w, const float* normals, int stride, 
   // the descriptor block may be addressed at a row offset (normals = descriptors.data() + row, stride = D): the last
   // point's normal ends (n-1)*stride + 3 floats after `normals`, and nothing beyond that may be read
   const size_t need = n > 0 ? (stride <= 8 ? (size_t)(n - 1) * (size_t)stride + 3 : (size_t)n * 3) : 0;
-  if (need > ctx->nrm_raw_cap) {
-    int rc;
-    if ((rc = dev_alloc(ctx, &ctx->nrm_raw, need + 4096))) return rc;
-    ctx->nrm_raw_cap = need + 4096;
-  }
+  CU(ctx->nrm_raw.reserve(need, need + 4096));
   int dstride = stride;
   if (stride <= 8) {
-    CU(cudaMemcpyAsync(ctx->nrm_raw, normals, need * sizeof(float), cudaMemcpyHostToDevice, w->stream));
+    CU(cudaMemcpyAsync(ctx->nrm_raw.get(), normals, need * sizeof(float), cudaMemcpyHostToDevice, w->stream));
   } else {
-    CU(cudaMemcpy2DAsync(ctx->nrm_raw, 3 * sizeof(float), normals, (size_t)stride * sizeof(float), 3 * sizeof(float),
+    CU(cudaMemcpy2DAsync(ctx->nrm_raw.get(), 3 * sizeof(float), normals, (size_t)stride * sizeof(float), 3 * sizeof(float),
                          (size_t)n, cudaMemcpyHostToDevice, w->stream));
     dstride = 3;
   }
-  expand_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->nrm_raw, dstride, n, dst);
+  expand_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->nrm_raw.get(), dstride, n, dst);
   LAUNCH_CHECK();
   return LS_OK;
 }
@@ -359,30 +369,30 @@ int upload_normals(ls_ctx* ctx, Workspace* w, const float* normals, int stride, 
 int fill_problem(ls_ctx* ctx, Workspace* w, const ls_icp_params* prm, int n, const float T0[16], bool want_matches,
                  bool want_hist) {
   IcpProblem& hp = w->hp;
-  hp.bs = w->bs;
-  hp.view.top = w->A.top;
-  hp.view.tab1 = w->A.tab1;
-  hp.view.pts = w->A.srt_pts;
-  hp.view.pyr = w->A.pyr;
-  hp.view.topmask = w->A.topmask;
-  hp.nrm = w->A.srt_nrm;
-  hp.rd = w->A.rd_s;
+  hp.bs = w->bs.get();
+  hp.view.top = w->top.get();
+  hp.view.tab1 = w->tab1.get();
+  hp.view.pts = w->srt_pts.get();
+  hp.view.pyr = w->pyr.get();
+  hp.view.topmask = w->topmask.get();
+  hp.nrm = w->srt_nrm.get();
+  hp.rd = w->rd_s.get();
   hp.n = n;
-  hp.pos = w->pos;
-  hp.d2 = w->d2;
-  hp.ids = w->ids;
-  hp.d2_out = w->d2_out;
-  hp.qperm = w->A.qperm;
-  hp.lists.vq = w->vq;
-  hp.lists.vpts = w->vpts;
+  hp.pos = w->pos.get();
+  hp.d2 = w->d2.get();
+  hp.ids = w->ids.get();
+  hp.d2_out = w->d2_out.get();
+  hp.qperm = w->qperm.get();
+  hp.lists.vq = w->vq.get();
+  hp.lists.vpts = w->vpts.get();
   hp.lists.n = n;
   hp.work = w->work;
   hp.shard_rank = 0;
   hp.shard_count = 1;
   std::memset(&hp.link, 0, sizeof(hp.link));
-  hp.T_hist = want_hist ? w->T_hist : nullptr;
+  hp.T_hist = want_hist ? w->T_hist.get() : nullptr;
   if (want_hist) {  // entries past the executed iterations read as zeros, not as stale device memory
-    CU(cudaMemsetAsync(w->T_hist, 0, (size_t)prm->max_iterations * 16 * sizeof(float), w->stream));
+    CU(cudaMemsetAsync(w->T_hist.get(), 0, (size_t)prm->max_iterations * 16 * sizeof(float), w->stream));
     w->stream_dirty = true;
   }
   hp.want_matches = want_matches ? 1 : 0;
@@ -410,8 +420,9 @@ int prep_icp(ls_ctx* ctx, Workspace* w, const ls_icp_params* prm, const float4* 
 // staging has finished; on return the results are on the host (pinned mirrors).
 int launch_icp(ls_ctx* ctx, const ls_icp_params* prm, int batch, int n_max, bool sharded = false) {
   Workspace* w0 = ctx->ws[0];
-  for (int b = 0; b < batch; ++b) ctx->probs_host[b] = ctx->ws[b]->hp;
-  CU(cudaMemcpyAsync(ctx->probs_dev, ctx->probs_host, sizeof(IcpProblem) * (size_t)batch, cudaMemcpyHostToDevice, w0->stream));
+  for (int b = 0; b < batch; ++b) ctx->probs_host.get()[b] = ctx->ws[b]->hp;
+  CU(cudaMemcpyAsync(ctx->probs_dev.get(), ctx->probs_host.get(), sizeof(IcpProblem) * (size_t)batch, cudaMemcpyHostToDevice,
+                     w0->stream));
   IcpParamsDev dp;
   dp.max_iterations = prm->max_iterations;
   dp.trim_ratio = prm->trim_ratio;
@@ -423,11 +434,11 @@ int launch_icp(ls_ctx* ctx, const ls_icp_params* prm, int batch, int n_max, bool
   const int need = (n_max + 31) / 32;
   if (ctas > need) ctas = need;
   if (ctas < 1) ctas = 1;
-  const IcpProblem* probs = ctx->probs_dev;
+  const IcpProblem* probs = ctx->probs_dev.get();
   int dynamic = batch > 1 ? 1 : 0;  // several problems: warps pull work from per-problem counters
   void* args[] = {(void*)&probs, (void*)&ctas, (void*)&dp, (void*)&dynamic};
   if (sharded) {  // narrow the staged problem to this shard's queries (cuts at cell starts, computed on the device)
-    shard_slice_kernel<<<1, 32, 0, w0->stream>>>(ctx->probs_dev, w0->job_dev, w0->hp.shard_rank, w0->hp.shard_count);
+    shard_slice_kernel<<<1, 32, 0, w0->stream>>>(ctx->probs_dev.get(), w0->job_dev, w0->hp.shard_rank, w0->hp.shard_count);
     LAUNCH_CHECK();
   }
   CU(cudaEventRecord(w0->ev_launch, w0->stream));
@@ -435,9 +446,9 @@ int launch_icp(ls_ctx* ctx, const ls_icp_params* prm, int batch, int n_max, bool
   ++ctx->launches;
   CU(cudaEventRecord(w0->ev2, w0->stream));
   // one gather and one copy for the whole batch (a pair of small copies per problem costs more than the kernel)
-  collect_results_kernel<<<batch, 32, 0, w0->stream>>>(ctx->probs_dev, ctx->results_dev);
+  collect_results_kernel<<<batch, 32, 0, w0->stream>>>(ctx->probs_dev.get(), ctx->results_dev.get());
   LAUNCH_CHECK();
-  CU(cudaMemcpyAsync(ctx->results_host, ctx->results_dev, sizeof(IcpResult) * (size_t)batch, cudaMemcpyDeviceToHost,
+  CU(cudaMemcpyAsync(ctx->results_host.get(), ctx->results_dev.get(), sizeof(IcpResult) * (size_t)batch, cudaMemcpyDeviceToHost,
                      w0->stream));
   return LS_OK;
 }
@@ -456,7 +467,7 @@ void launch_times(ls_ctx* ctx, float t[3]) {
 // launch_times of the launch, when the caller already has them.
 int fetch_icp(ls_ctx* ctx, int k, int n, const float T0[16], float T_out[16], ls_icp_stats* stats,
               const float* times = nullptr) {
-  const IcpResult& wk = ctx->results_host[k];
+  const IcpResult& wk = ctx->results_host.get()[k];
   std::memcpy(T_out, wk.T_out, 16 * sizeof(float));
   if (stats) {
     std::memset(stats, 0, sizeof(*stats));
@@ -492,10 +503,10 @@ int run_icp(ls_ctx* ctx, const ls_icp_params* prm, const float4* reading_dev, in
   int rc;
   if ((rc = prep_icp(ctx, w, prm, reading_dev, n, T0, opt_ids || opt_d2, opt_T_hist != nullptr))) return rc;
   if ((rc = launch_icp(ctx, prm, 1, n))) return rc;
-  if (opt_ids) CU(cudaMemcpyAsync(opt_ids, w->ids, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, w->stream));
-  if (opt_d2) CU(cudaMemcpyAsync(opt_d2, w->d2_out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
+  if (opt_ids) CU(cudaMemcpyAsync(opt_ids, w->ids.get(), (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, w->stream));
+  if (opt_d2) CU(cudaMemcpyAsync(opt_d2, w->d2_out.get(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
   if (opt_T_hist)
-    CU(cudaMemcpyAsync(opt_T_hist, w->T_hist, (size_t)prm->max_iterations * 16 * sizeof(float), cudaMemcpyDeviceToHost,
+    CU(cudaMemcpyAsync(opt_T_hist, w->T_hist.get(), (size_t)prm->max_iterations * 16 * sizeof(float), cudaMemcpyDeviceToHost,
                        w->stream));
   CU(cudaStreamSynchronize(w->stream));
   return fetch_icp(ctx, 0, n, T0, T_out, stats);
@@ -531,8 +542,8 @@ int make_parts(ls_ctx* ctx, const ls_map* map, int n_parts, const uint64_t* part
                         (unsigned long long)part_ids[p]);
     if (wait_slot(s, consumer) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
     parts.offset[p] = (int)off;
-    parts.pts[p] = s->pts;
-    parts.nrm[p] = s->nrm;
+    parts.pts[p] = s->pts.get();
+    parts.nrm[p] = s->nrm.get();
     std::memcpy(parts.T[p], T_parts + 16 * p, 16 * sizeof(float));
     parts.identity[p] = is_identity16(T_parts + 16 * p) ? 1 : 0;
     off += s->n;
@@ -551,25 +562,19 @@ int ls_b200_version(void) { return LS_VERSION; }
 namespace {
 Workspace* new_workspace(ls_ctx* ctx, int index) {
   Workspace* w = new Workspace();
-  w->work = ctx->work_pool + index;
-  w->job_dev = ctx->jobs_dev + index;
-  w->job_host = ctx->jobs_host + index;
+  w->work = ctx->work_pool.get() + index;
+  w->job_dev = ctx->jobs_dev.get() + index;
+  w->job_host = ctx->jobs_host.get() + index;
   bool ok = cudaStreamCreateWithFlags(&w->stream, cudaStreamNonBlocking) == cudaSuccess &&
             cudaEventCreate(&w->ev0) == cudaSuccess && cudaEventCreate(&w->ev1) == cudaSuccess &&
             cudaEventCreate(&w->ev2) == cudaSuccess && cudaEventCreate(&w->ev_launch) == cudaSuccess &&
-            cudaMalloc((void**)&w->bs, sizeof(BuildState)) == cudaSuccess;
+            w->bs.reserve(1, 1) == cudaSuccess;
   if (!ok) return nullptr;  // partially built workspace is leaked only on an out-of-memory init failure
   return w;
 }
 void free_workspace(Workspace* w) {
   if (!w) return;
   if (w->stream) cudaStreamSynchronize(w->stream);
-  void* bufs[] = {w->A.sub_pts, w->A.sub_nrm, w->A.srt_pts, w->A.srt_nrm, w->A.pkey, w->A.top, w->A.cnt0, w->A.tab1, w->A.cnt1,
-                  w->A.tab1_cell, w->A.pyr, w->A.topmask, w->bs, w->rd, w->pos, w->d2,
-                  w->ids, w->vq, w->vpts, w->T_hist, w->d2_out, w->A.qkey, w->A.qperm, w->A.rd_s,
-                  w->A.qtab_local, w->A.qtab_total, w->A.qtop_start};
-  for (void* b : bufs)
-    if (b) cudaFree(b);
   if (w->ev0) cudaEventDestroy(w->ev0);
   if (w->ev1) cudaEventDestroy(w->ev1);
   if (w->ev2) cudaEventDestroy(w->ev2);
@@ -609,14 +614,14 @@ int ls_b200_init(int device, ls_ctx** out) {
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, icp_kernel, kIcpThreads, kIcpPairBytes) != cudaSuccess || occ < 1)
     return bail(LS_ERR_CUDA);
   ctx->icp_ctas = ctx->icp_ctas_max = occ * ctx->sm_count;
-  if (cudaMalloc((void**)&ctx->probs_dev, sizeof(IcpProblem) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
-  if (cudaMallocHost((void**)&ctx->probs_host, sizeof(IcpProblem) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
-  if (cudaMalloc((void**)&ctx->jobs_dev, sizeof(BuildJob) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
-  if (cudaMallocHost((void**)&ctx->jobs_host, sizeof(BuildJob) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
-  if (cudaMalloc((void**)&ctx->work_pool, sizeof(IcpWork) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
-  if (cudaMalloc((void**)&ctx->results_dev, sizeof(IcpResult) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
-  if (cudaMallocHost((void**)&ctx->results_host, sizeof(IcpResult) * kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
-  if (cudaMalloc((void**)&ctx->T0_dev, 16 * sizeof(float)) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->probs_dev.reserve(kMaxBatch, kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->probs_host.reserve(kMaxBatch, kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->jobs_dev.reserve(kMaxBatch, kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->jobs_host.reserve(kMaxBatch, kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->work_pool.reserve(kMaxBatch, kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->results_dev.reserve(kMaxBatch, kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->results_host.reserve(kMaxBatch, kMaxBatch) != cudaSuccess) return bail(LS_ERR_NOMEM);
+  if (ctx->T0_dev.reserve(16, 16) != cudaSuccess) return bail(LS_ERR_NOMEM);
   if (ensure_workspaces(ctx, 1) != LS_OK) return bail(LS_ERR_NOMEM);
   *out = ctx;
   return LS_OK;
@@ -626,17 +631,6 @@ void ls_b200_destroy(ls_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   for (Workspace* w : ctx->ws) free_workspace(w);
-  if (ctx->probs_dev) cudaFree(ctx->probs_dev);
-  if (ctx->probs_host) cudaFreeHost(ctx->probs_host);
-  if (ctx->jobs_dev) cudaFree(ctx->jobs_dev);
-  if (ctx->jobs_host) cudaFreeHost(ctx->jobs_host);
-  if (ctx->work_pool) cudaFree(ctx->work_pool);
-  if (ctx->results_dev) cudaFree(ctx->results_dev);
-  if (ctx->results_host) cudaFreeHost(ctx->results_host);
-  void* stage[] = {ctx->reading, ctx->ref_stage, ctx->ref_nrm_stage, ctx->nrm_raw, ctx->T0_dev};
-  for (void* b : stage)
-    if (b) cudaFree(b);
-  lsf::release(ctx->chain);
   ls_shard_exchange_close(ctx);
   delete ctx;
 }
@@ -689,19 +683,19 @@ int ls_icp_register(ls_ctx* ctx, const ls_icp_params* prm, const float* reading4
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
   if ((rc = ensure_staging(ctx, n, m))) return rc;
   CU(cudaEventRecord(w->ev0, w->stream));
-  CU(cudaMemcpyAsync(ctx->reading, reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemcpyAsync(ctx->ref_stage, ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  if ((rc = upload_normals(ctx, w, ref_normals, normals_stride, m, ctx->ref_nrm_stage))) return rc;
+  CU(cudaMemcpyAsync(ctx->reading.get(), reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemcpyAsync(ctx->ref_stage.get(), ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if ((rc = upload_normals(ctx, w, ref_normals, normals_stride, m, ctx->ref_nrm_stage.get()))) return rc;
   Parts parts;
   std::memset(&parts, 0, sizeof(parts));
   parts.n_parts = 1;
   parts.offset[0] = 0;
   parts.offset[1] = m;
-  parts.pts[0] = ctx->ref_stage;
-  parts.nrm[0] = ctx->ref_nrm_stage;
+  parts.pts[0] = ctx->ref_stage.get();
+  parts.nrm[0] = ctx->ref_nrm_stage.get();
   parts.identity[0] = 1;
   if ((rc = enqueue_build(ctx, w, parts, r, T0))) return rc;
-  return run_icp(ctx, prm, ctx->reading, n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist);
+  return run_icp(ctx, prm, ctx->reading.get(), n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist);
 }
 
 int ls_nn_query(ls_ctx* ctx, const ls_icp_params* prm, const float* reading4, int n, const float* ref4, int m,
@@ -721,27 +715,28 @@ int ls_nn_query(ls_ctx* ctx, const ls_icp_params* prm, const float* reading4, in
   const Resolved r = resolve(prm);
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, 1))) return rc;
   if ((rc = ensure_staging(ctx, n, m))) return rc;
-  CU(cudaMemcpyAsync(ctx->reading, reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemcpyAsync(ctx->ref_stage, ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemsetAsync(ctx->ref_nrm_stage, 0, (size_t)m * sizeof(float4), w->stream));
+  CU(cudaMemcpyAsync(ctx->reading.get(), reading4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemcpyAsync(ctx->ref_stage.get(), ref4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemsetAsync(ctx->ref_nrm_stage.get(), 0, (size_t)m * sizeof(float4), w->stream));
   Parts parts;
   std::memset(&parts, 0, sizeof(parts));
   parts.n_parts = 1;
   parts.offset[1] = m;
-  parts.pts[0] = ctx->ref_stage;
-  parts.nrm[0] = ctx->ref_nrm_stage;
+  parts.pts[0] = ctx->ref_stage.get();
+  parts.nrm[0] = ctx->ref_nrm_stage.get();
   parts.identity[0] = 1;
   if ((rc = enqueue_build(ctx, w, parts, r, T0))) return rc;
-  w->job_host->reading = ctx->reading;
+  w->job_host->reading = ctx->reading.get();
   w->job_host->n = n;
   CU(cudaMemcpyAsync(w->job_dev, w->job_host, sizeof(BuildJob), cudaMemcpyHostToDevice, w->stream));
   reading_kernel<<<dim3(blocks_for(n, 256, ctx->sm_count * 8), 1), 256, 0, w->stream>>>(w->job_dev);
   LAUNCH_CHECK();
-  GridView v{w->A.top, w->A.tab1, w->A.srt_pts, w->A.pyr, w->A.topmask};
-  nn_query_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->bs, v, w->rd, n, w->ids, w->d2);
+  GridView v{w->top.get(), w->tab1.get(), w->srt_pts.get(), w->pyr.get(), w->topmask.get()};
+  nn_query_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->bs.get(), v, w->rd.get(), n, w->ids.get(),
+                                                                                w->d2.get());
   LAUNCH_CHECK();
-  CU(cudaMemcpyAsync(ids, w->ids, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, w->stream));
-  CU(cudaMemcpyAsync(d2, w->d2, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
+  CU(cudaMemcpyAsync(ids, w->ids.get(), (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, w->stream));
+  CU(cudaMemcpyAsync(d2, w->d2.get(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
   CU(cudaStreamSynchronize(w->stream));
   return LS_OK;
 }
@@ -758,18 +753,18 @@ int ls_transform_cloud(ls_ctx* ctx, const float T[16], const float* in4, const f
   int rc;
   if ((rc = ensure_capacity(ctx, w, n, n, 64, 1))) return rc;
   if ((rc = ensure_staging(ctx, n, n))) return rc;
-  CU(cudaMemcpyAsync(ctx->T0_dev, T, 16 * sizeof(float), cudaMemcpyHostToDevice, w->stream));
-  CU(cudaMemcpyAsync(ctx->reading, in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  if (normals && (rc = upload_normals(ctx, w, normals, normals_stride, n, ctx->ref_nrm_stage))) return rc;
+  CU(cudaMemcpyAsync(ctx->T0_dev.get(), T, 16 * sizeof(float), cudaMemcpyHostToDevice, w->stream));
+  CU(cudaMemcpyAsync(ctx->reading.get(), in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if (normals && (rc = upload_normals(ctx, w, normals, normals_stride, n, ctx->ref_nrm_stage.get()))) return rc;
   transform_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(
-      ctx->T0_dev, ctx->reading, normals ? ctx->ref_nrm_stage : nullptr, n, w->rd, w->A.sub_nrm);
+      ctx->T0_dev.get(), ctx->reading.get(), normals ? ctx->ref_nrm_stage.get() : nullptr, n, w->rd.get(), w->sub_nrm.get());
   LAUNCH_CHECK();
-  CU(cudaMemcpyAsync(out4, w->rd, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
+  CU(cudaMemcpyAsync(out4, w->rd.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
   if (normals) {
-    pack_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->A.sub_nrm, n,
-                                                                                         (float*)w->A.srt_nrm);
+    pack_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->sub_nrm.get(), n,
+                                                                                         (float*)w->srt_nrm.get());
     LAUNCH_CHECK();
-    CU(cudaMemcpyAsync(out_normals3, w->A.srt_nrm, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
+    CU(cudaMemcpyAsync(out_normals3, w->srt_nrm.get(), (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
   }
   CU(cudaStreamSynchronize(w->stream));
   return LS_OK;
@@ -792,8 +787,8 @@ int ls_map_create(ls_ctx* ctx, int capacity_scans, int max_pts_per_scan, ls_map*
     return fail(ctx, LS_ERR_CUDA, "stream creation failed");
   }
   for (auto& s : map->slots) {
-    if (cudaMalloc((void**)&s.pts, (size_t)max_pts_per_scan * sizeof(float4)) != cudaSuccess ||
-        cudaMalloc((void**)&s.nrm, (size_t)max_pts_per_scan * sizeof(float4)) != cudaSuccess ||
+    const size_t c = (size_t)max_pts_per_scan;
+    if (s.pts.reserve(c, c) != cudaSuccess || s.nrm.reserve(c, c) != cudaSuccess ||
         cudaEventCreateWithFlags(&s.ready, cudaEventDisableTiming) != cudaSuccess) {
       ls_map_destroy(map);
       return fail(ctx, LS_ERR_NOMEM, "map allocation failed");
@@ -810,16 +805,10 @@ void ls_map_destroy(ls_map* map) {
     for (Workspace* w : map->ctx->ws) cudaStreamSynchronize(w->stream);
   }
   if (map->up_stream) cudaStreamSynchronize(map->up_stream);
-  for (auto& s : map->slots) {
-    if (s.pts) cudaFree(s.pts);
-    if (s.nrm) cudaFree(s.nrm);
+  for (auto& s : map->slots)
     if (s.ready) cudaEventDestroy(s.ready);
-  }
-  for (int k = 0; k < kStageRing; ++k) {
-    if (map->host_stage[k]) cudaFreeHost(map->host_stage[k]);
-    if (map->stage[k]) cudaFree(map->stage[k]);
+  for (int k = 0; k < kStageRing; ++k)
     if (map->stage_free[k]) cudaEventDestroy(map->stage_free[k]);
-  }
   if (map->up_stream) cudaStreamDestroy(map->up_stream);
   delete map;
 }
@@ -841,15 +830,9 @@ int ls_map_push_scan(ls_map* map, const float* features4, const float* normals, 
   if (map->stage_free[k]) CU(cudaEventSynchronize(map->stage_free[k]));  // the upload that used this staging slot last
   const int stride = normals_stride <= 8 ? normals_stride : 3;
   const size_t nf = (size_t)n * 4, nn = (size_t)(n - 1) * (size_t)stride + 3;
-  if (nf + nn > map->host_stage_cap[k]) {
-    if (map->host_stage[k]) CU(cudaFreeHost(map->host_stage[k]));
-    map->host_stage[k] = nullptr;
-    map->host_stage_cap[k] = 0;
-    if (cudaMallocHost((void**)&map->host_stage[k], (nf + nn + 1024) * sizeof(float)) != cudaSuccess)
-      return fail(ctx, LS_ERR_NOMEM, "pinned staging allocation failed");
-    map->host_stage_cap[k] = nf + nn + 1024;
-  }
-  float* hf = map->host_stage[k];
+  if (map->host_stage[k].reserve(nf + nn, nf + nn + 1024) != cudaSuccess)
+    return fail(ctx, LS_ERR_NOMEM, "pinned staging allocation failed");
+  float* hf = map->host_stage[k].get();
   float* hn = hf + nf;
   std::memcpy(hf, features4, nf * sizeof(float));
   if (normals_stride <= 8) {
@@ -891,17 +874,11 @@ int ls_map_push_scan_async(ls_map* map, const float* features4, const float* nor
     const size_t need = (size_t)(n - 1) * (size_t)normals_stride + 3;  // never read past the last normal
     if (!map->stage_free[k]) CU(cudaEventCreateWithFlags(&map->stage_free[k], cudaEventDisableTiming));
     else CU(cudaEventSynchronize(map->stage_free[k]));  // the upload that used this staging buffer 16 pushes ago
-    if (need > map->stage_cap[k]) {
-      if (map->stage[k]) CU(cudaFree(map->stage[k]));
-      map->stage[k] = nullptr;
-      map->stage_cap[k] = 0;
-      if (cudaMalloc((void**)&map->stage[k], (need + 1024) * sizeof(float)) != cudaSuccess)
-        return fail(ctx, LS_ERR_NOMEM, "staging allocation failed");
-      map->stage_cap[k] = need + 1024;
-    }
-    CU(cudaMemcpyAsync(s.pts, features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, map->up_stream));
-    CU(cudaMemcpyAsync(map->stage[k], normals, need * sizeof(float), cudaMemcpyHostToDevice, map->up_stream));
-    expand_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, map->up_stream>>>(map->stage[k], normals_stride, n, s.nrm);
+    if (map->stage[k].reserve(need, need + 1024) != cudaSuccess) return fail(ctx, LS_ERR_NOMEM, "staging allocation failed");
+    CU(cudaMemcpyAsync(s.pts.get(), features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, map->up_stream));
+    CU(cudaMemcpyAsync(map->stage[k].get(), normals, need * sizeof(float), cudaMemcpyHostToDevice, map->up_stream));
+    expand_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, map->up_stream>>>(map->stage[k].get(), normals_stride,
+        n, s.nrm.get());
     LAUNCH_CHECK();
     CU(cudaEventRecord(map->stage_free[k], map->up_stream));
   }
@@ -950,8 +927,9 @@ int enqueue_normals(ls_ctx* ctx, Workspace* w, const float4* pts_dev, int n, int
   parts.identity[0] = 1;
   const float I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
   if ((rc = enqueue_build(ctx, w, parts, r, I))) return rc;
-  GridView v{w->A.top, w->A.tab1, w->A.srt_pts, w->A.pyr, w->A.topmask};
-  knn_normals_kernel<<<blocks_for(n, 128, ctx->sm_count * 16), 128, 0, w->stream>>>(w->bs, v, w->A.sub_pts, n, knn, nrm_out);
+  GridView v{w->top.get(), w->tab1.get(), w->srt_pts.get(), w->pyr.get(), w->topmask.get()};
+  knn_normals_kernel<<<blocks_for(n, 128, ctx->sm_count * 16), 128, 0, w->stream>>>(w->bs.get(), v, w->sub_pts.get(), n, knn,
+                                                                                    nrm_out);
   LAUNCH_CHECK();
   return LS_OK;
 }
@@ -967,11 +945,12 @@ int ls_estimate_normals(ls_ctx* ctx, const float* features4, int n, int knn, flo
   int rc;
   if ((rc = ensure_capacity(ctx, w, n, n, 64, 1))) return rc;
   if ((rc = ensure_staging(ctx, n, n))) return rc;
-  CU(cudaMemcpyAsync(ctx->reading, features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  if ((rc = enqueue_normals(ctx, w, ctx->reading, n, knn, ctx->ref_nrm_stage))) return rc;
-  pack_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->ref_nrm_stage, n, (float*)w->A.srt_nrm);
+  CU(cudaMemcpyAsync(ctx->reading.get(), features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if ((rc = enqueue_normals(ctx, w, ctx->reading.get(), n, knn, ctx->ref_nrm_stage.get()))) return rc;
+  pack_normals_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->ref_nrm_stage.get(), n,
+                                                                                    (float*)w->srt_nrm.get());
   LAUNCH_CHECK();
-  CU(cudaMemcpyAsync(out_normals3, w->A.srt_nrm, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
+  CU(cudaMemcpyAsync(out_normals3, w->srt_nrm.get(), (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
   CU(cudaStreamSynchronize(w->stream));
   return LS_OK;
 }
@@ -992,8 +971,8 @@ int ls_map_push_scan_estimate_normals(ls_map* map, const float* features4, int n
     s.async = false;
   }
   if (n > 0) {
-    CU(cudaMemcpyAsync(s.pts, features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-    int rc = enqueue_normals(ctx, w, s.pts, n, knn, s.nrm);
+    CU(cudaMemcpyAsync(s.pts.get(), features4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+    int rc = enqueue_normals(ctx, w, s.pts.get(), n, knn, s.nrm.get());
     if (rc) return rc;
     CU(cudaStreamSynchronize(w->stream));
   }
@@ -1019,7 +998,7 @@ bool chain_makes_normals(const ls_point_filter* f, int n_filters) {
 }
 
 // Upload a host cloud (and its normals) into the chain buffers and run the chain on workspace 0's stream.  On return the
-// result is in ctx->chain.pts[*cur] / nrm[*cur] (normals valid iff *has_nrm), *n_out points; nothing has been copied back
+// result is in ctx->chain.pts[*cur].get() / nrm[*cur] (normals valid iff *has_nrm), *n_out points; nothing has been copied back
 // but counts.  Runs of mask filters are one flag launch per point-wise run / sampler plus one compaction; the voxel grid
 // and the normals work on the device buffers in place of ls_voxel_grid / ls_estimate_normals' host round trips.
 int run_chain(ls_ctx* ctx, const ls_point_filter* f, int n_filters, const float* in4, const float* normals, int normals_stride,
@@ -1032,22 +1011,24 @@ int run_chain(ls_ctx* ctx, const ls_point_filter* f, int n_filters, const float*
   *n_out = n;
   if (n == 0) return LS_OK;
   int rc;
-  CU(cudaMemcpyAsync(b.pts[0], in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
-  if (normals && (rc = upload_normals(ctx, w, normals, normals_stride, n, b.nrm[0]))) return rc;
+  CU(cudaMemcpyAsync(b.pts[0].get(), in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, w->stream));
+  if (normals && (rc = upload_normals(ctx, w, normals, normals_stride, n, b.nrm[0].get()))) return rc;
   int k = 0, m = n, c = 0;
   while (k < n_filters && m > 0) {
     const ls_point_filter& fk = f[k];
     if (lsf::is_mask_filter(fk.type)) {
       int used = 0;
-      CU(lsf::enqueue_mask_run(f + k, n_filters - k, b.pts[c], *has_nrm ? b.nrm[c] : nullptr, m, b.pts[1 - c], b.nrm[1 - c], b,
+      CU(lsf::enqueue_mask_run(f + k, n_filters - k, b.pts[c].get(), *has_nrm ? b.nrm[c].get() : nullptr, m, b.pts[1 - c].get(),
+                               b.nrm[1 - c].get(), b,
                                w->stream, &used, &ctx->launches));
-      CU(cudaMemcpyAsync(&m, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, w->stream));
+      CU(cudaMemcpyAsync(&m, b.small.get() + 6, sizeof(int), cudaMemcpyDeviceToHost, w->stream));
       CU(cudaStreamSynchronize(w->stream));
       c = 1 - c;
       k += used;
     } else if (fk.type == LS_PF_VOXEL_GRID) {
       int v = 0;
-      rc = lsf::enqueue_voxel_grid(b.pts[c], *has_nrm ? b.nrm[c] : nullptr, m, fk.leaf, b.pts[1 - c], b.nrm[1 - c], 0,
+      rc = lsf::enqueue_voxel_grid(b.pts[c].get(), *has_nrm ? b.nrm[c].get() : nullptr, m, fk.leaf, b.pts[1 - c].get(),
+                                   b.nrm[1 - c].get(), 0,
                                    lsf::voxel_buffers(b), w->stream, &v, &ctx->launches);
       if (rc == LS_ERR_ARG) return fail(ctx, rc, "filter %d: voxel leaf too small for the cloud's extent", k);
       if (rc) return fail(ctx, rc, "filter %d: voxel grid: %s", k, cudaGetErrorString(cudaGetLastError()));
@@ -1056,13 +1037,14 @@ int run_chain(ls_ctx* ctx, const ls_point_filter* f, int n_filters, const float*
       ++k;
     } else {  // (Sampling)SurfaceNormal: exact k-NN normals of the current cloud, then the sampling of the Sampling variant
       const int knn = fk.knn < 3 ? 3 : (fk.knn > LS_KNN_MAX ? LS_KNN_MAX : fk.knn);
-      if ((rc = enqueue_normals(ctx, w, b.pts[c], m, knn, b.nrm[c]))) return rc;
+      if ((rc = enqueue_normals(ctx, w, b.pts[c].get(), m, knn, b.nrm[c].get()))) return rc;
       *has_nrm = true;
       if (fk.type == LS_PF_SAMPLING_SURFACE_NORMAL && fk.prob < 1.0f) {
         int used = 0;
-        CU(lsf::enqueue_mask_run(&fk, 1, b.pts[c], b.nrm[c], m, b.pts[1 - c], b.nrm[1 - c], b, w->stream, &used,
+        CU(lsf::enqueue_mask_run(&fk, 1, b.pts[c].get(), b.nrm[c].get(), m, b.pts[1 - c].get(), b.nrm[1 - c].get(), b, w->stream,
+                                 &used,
                                  &ctx->launches));
-        CU(cudaMemcpyAsync(&m, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, w->stream));
+        CU(cudaMemcpyAsync(&m, b.small.get() + 6, sizeof(int), cudaMemcpyDeviceToHost, w->stream));
         CU(cudaStreamSynchronize(w->stream));
         c = 1 - c;
       }
@@ -1092,12 +1074,13 @@ int ls_filter_cloud(ls_ctx* ctx, const ls_point_filter* filters, int n_filters, 
   bool has_nrm = false;
   if ((rc = run_chain(ctx, filters, n_filters, in4, normals, normals_stride, n, &cur, &has_nrm, &m))) return rc;
   if (m > 0) {
-    CU(cudaMemcpyAsync(out4, ctx->chain.pts[cur], (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
+    CU(cudaMemcpyAsync(out4, ctx->chain.pts[cur].get(), (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
     if (out_normals3) {
-      pack_normals_kernel<<<blocks_for(m, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->chain.nrm[cur], m,
-                                                                                           (float*)ctx->chain.nrm[1 - cur]);
+      pack_normals_kernel<<<blocks_for(m, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(ctx->chain.nrm[cur].get(), m,
+                                                                                           (float*)ctx->chain.nrm[1 - cur].get());
       LAUNCH_CHECK();
-      CU(cudaMemcpyAsync(out_normals3, ctx->chain.nrm[1 - cur], (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
+      CU(cudaMemcpyAsync(out_normals3, ctx->chain.nrm[1 - cur].get(), (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost,
+                         w->stream));
     }
     CU(cudaStreamSynchronize(w->stream));
   }
@@ -1130,8 +1113,8 @@ int ls_map_push_scan_filtered(ls_map* map, const ls_point_filter* filters, int n
     s.async = false;
   }
   if (m > 0) {
-    CU(cudaMemcpyAsync(s.pts, ctx->chain.pts[cur], (size_t)m * sizeof(float4), cudaMemcpyDeviceToDevice, w->stream));
-    CU(cudaMemcpyAsync(s.nrm, ctx->chain.nrm[cur], (size_t)m * sizeof(float4), cudaMemcpyDeviceToDevice, w->stream));
+    CU(cudaMemcpyAsync(s.pts.get(), ctx->chain.pts[cur].get(), (size_t)m * sizeof(float4), cudaMemcpyDeviceToDevice, w->stream));
+    CU(cudaMemcpyAsync(s.nrm.get(), ctx->chain.nrm[cur].get(), (size_t)m * sizeof(float4), cudaMemcpyDeviceToDevice, w->stream));
     CU(cudaStreamSynchronize(w->stream));
   }
   s.n = m;
@@ -1171,7 +1154,7 @@ int ls_icp_register_submap(ls_ctx* ctx, const ls_icp_params* prm, const ls_map* 
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
   CU(cudaEventRecord(w->ev0, w->stream));
   if ((rc = enqueue_build(ctx, w, parts, r, T0))) return rc;
-  return run_icp(ctx, prm, rs->pts, n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist);
+  return run_icp(ctx, prm, rs->pts.get(), n, T0, T_out, stats, opt_ids, opt_d2, opt_T_iter_hist);
 }
 
 // ---- query-sharded registration (SURVEY.md 8 e-2) -------------------------------------------------------------
@@ -1265,7 +1248,7 @@ int ls_icp_register_submap_sharded(ls_ctx* ctx, const ls_icp_params* prm, const 
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
   CU(cudaEventRecord(w->ev0, w->stream));
   if ((rc = enqueue_build(ctx, w, parts, r, T0))) return rc;
-  if ((rc = prep_icp(ctx, w, prm, rs->pts, n, T0, false, false))) return rc;
+  if ((rc = prep_icp(ctx, w, prm, rs->pts.get(), n, T0, false, false))) return rc;
   IcpProblem& hp = w->hp;
   hp.shard_rank = shard_rank;
   hp.shard_count = shard_count;
@@ -1285,7 +1268,7 @@ int ls_icp_register_submap_sharded(ls_ctx* ctx, const ls_icp_params* prm, const 
   // every shard runs the full co-resident grid (the exchange needs a CTA per peer, and all shards the same shape)
   if ((rc = launch_icp(ctx, prm, 1, 1 << 30, shard_count > 1))) return rc;
   CU(cudaStreamSynchronize(w->stream));
-  ctx->xflag_base += ctx->results_host[0].xsignals;
+  ctx->xflag_base += ctx->results_host.get()[0].xsignals;
   return fetch_icp(ctx, 0, n, T0, T_out, stats);
 }
 
@@ -1317,10 +1300,10 @@ int ls_icp_register_submaps(ls_ctx* ctx, const ls_icp_params* prm, const ls_map*
   if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
   if ((rc = ensure_staging(ctx, n, 0))) return rc;
   CU(cudaEventRecord(w->ev0, w->stream));
-  assemble_points_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(rd, ctx->reading);
+  assemble_points_kernel<<<blocks_for(n, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(rd, ctx->reading.get());
   LAUNCH_CHECK();
   if ((rc = enqueue_build(ctx, w, ref, r, T0))) return rc;
-  return run_icp(ctx, prm, ctx->reading, n, T0, T_out, stats, nullptr, nullptr, nullptr);
+  return run_icp(ctx, prm, ctx->reading.get(), n, T0, T_out, stats, nullptr, nullptr, nullptr);
 }
 
 // Several independent scan -> sub-map registrations in ONE cooperative launch (the multi-robot case: the
@@ -1391,7 +1374,7 @@ int ls_icp_register_submap_batch_begin(ls_ctx* ctx, const ls_icp_params* prm, co
     n_max = n > n_max ? n : n_max;
     m_max = m > m_max ? m : m_max;
     if ((rc = ensure_capacity(ctx, w, n, m, r.max_cells, prm->max_iterations))) return rc;
-    fill_job(w, parts, T0, rs->pts, n);
+    fill_job(w, parts, T0, rs->pts.get(), n);
     if ((rc = fill_problem(ctx, w, prm, n, T0, false, false))) return rc;
   }
   for (int k = 1; k < launched; ++k) {  // allocation-time clears a workspace enqueued on its own stream come first
@@ -1401,11 +1384,12 @@ int ls_icp_register_submap_batch_begin(ls_ctx* ctx, const ls_icp_params* prm, co
     ctx->ws[k]->stream_dirty = false;
   }
   CU(cudaEventRecord(w0->ev0, w0->stream));
-  CU(cudaMemcpyAsync(ctx->jobs_dev, ctx->jobs_host, sizeof(BuildJob) * (size_t)launched, cudaMemcpyHostToDevice, w0->stream));
-  if ((rc = launch_build(ctx, ctx->jobs_dev, launched, m_max, r, w0->stream))) return rc;
-  if ((rc = launch_reading_sort(ctx, ctx->jobs_dev, launched, n_max, r, w0->stream))) return rc;
+  CU(cudaMemcpyAsync(ctx->jobs_dev.get(), ctx->jobs_host.get(), sizeof(BuildJob) * (size_t)launched, cudaMemcpyHostToDevice,
+                     w0->stream));
+  if ((rc = launch_build(ctx, ctx->jobs_dev.get(), launched, m_max, r, w0->stream))) return rc;
+  if ((rc = launch_reading_sort(ctx, ctx->jobs_dev.get(), launched, n_max, r, w0->stream))) return rc;
   CU(cudaEventRecord(w0->ev1, w0->stream));
-  CU(cudaMemsetAsync(ctx->work_pool, 0, sizeof(IcpWork) * (size_t)launched, w0->stream));
+  CU(cudaMemsetAsync(ctx->work_pool.get(), 0, sizeof(IcpWork) * (size_t)launched, w0->stream));
   if ((rc = launch_icp(ctx, prm, launched, n_max))) return rc;
   ctx->pending = true;
   return LS_OK;
@@ -1470,12 +1454,12 @@ int ls_map_assemble(ls_ctx* ctx, const ls_map* map, int n_parts, const uint64_t*
   LAUNCH_CHECK();
   assemble_kernel<<<dim3(blocks_for(m, 256, ctx->sm_count * 8), 1), 256, 0, w->stream>>>(w->job_dev);
   LAUNCH_CHECK();
-  CU(cudaMemcpyAsync(out4, w->A.sub_pts, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
+  CU(cudaMemcpyAsync(out4, w->sub_pts.get(), (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, w->stream));
   if (out_normals3) {
-    pack_normals_kernel<<<blocks_for(m, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->A.sub_nrm, m,
-                                                                                         (float*)w->A.srt_nrm);
+    pack_normals_kernel<<<blocks_for(m, 256, ctx->sm_count * 8), 256, 0, w->stream>>>(w->sub_nrm.get(), m,
+                                                                                         (float*)w->srt_nrm.get());
     LAUNCH_CHECK();
-    CU(cudaMemcpyAsync(out_normals3, w->A.srt_nrm, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
+    CU(cudaMemcpyAsync(out_normals3, w->srt_nrm.get(), (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, w->stream));
   }
   CU(cudaStreamSynchronize(w->stream));
   return LS_OK;
@@ -1492,70 +1476,62 @@ struct ls_local_map {
   ls_local_map_params prm{};
   int initial_cap = 0;
   cudaStream_t stream = nullptr;
-  float4* local[2] = {nullptr, nullptr};
-  int local_cap[2] = {0, 0};
+  Buffer<float4> local[2];
   int cur = 0, n_local = 0;
-  float4* filt = nullptr;  // local_map_filtered_
-  int filt_cap = 0, n_filt = 0;
-  float4* dist = nullptr;  // distant_map_
-  int dist_cap = 0, n_dist = 0;
-  float4* queue = nullptr;  // local_map_queue_, clouds back to back
-  int queue_cap = 0, n_queue = 0;
+  Buffer<float4> filt;  // local_map_filtered_
+  int n_filt = 0;
+  Buffer<float4> dist;  // distant_map_
+  int n_dist = 0;
+  Buffer<float4> queue;  // local_map_queue_, clouds back to back
+  int n_queue = 0;
   std::vector<int> queue_sizes;
-  float4* result = nullptr;  // the last filter's result (separate distant map only)
-  int result_cap = 0, n_result = 0;
+  Buffer<float4> result;  // the last filter's result (separate distant map only)
+  int n_result = 0;
   lsf::ChainBuffers scratch;  // per-call flags, scans and voxel arrays, sized for the largest cloud seen
 };
 
 namespace {
 // Grows a persistent cloud to hold `need` points (doubling), keeping its first `keep` points.  If the allocation fails the
 // old buffer is left as it was.
-int grow_cloud(ls_local_map* lm, float4** p, int* cap, long long need, int keep) {
+int grow_cloud(ls_local_map* lm, Buffer<float4>& p, long long need, int keep) {
   ls_ctx* ctx = lm->ctx;
-  if (need <= *cap) return LS_OK;
+  const long long cap = (long long)p.capacity();
+  if (need <= cap) return LS_OK;
   if (need > 0x7fffffffLL) return fail(ctx, LS_ERR_NOMEM, "local map cloud of %lld points", need);
-  long long c = *cap > lm->initial_cap ? *cap : lm->initial_cap;
+  long long c = cap > lm->initial_cap ? cap : lm->initial_cap;
   while (c < need) c *= 2;
   if (c > 0x7fffffffLL) c = 0x7fffffffLL;
-  float4* q = nullptr;
-  if (cudaMalloc((void**)&q, (size_t)c * sizeof(float4)) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(ctx, LS_ERR_NOMEM, "local map growth to %lld points failed", c);
-  }
-  if (keep > 0 && cudaMemcpyAsync(q, *p, (size_t)keep * sizeof(float4), cudaMemcpyDeviceToDevice, lm->stream) != cudaSuccess) {
-    cudaFree(q);
+  Buffer<float4> q;
+  if (q.reserve((size_t)c, (size_t)c) != cudaSuccess) return fail(ctx, LS_ERR_NOMEM, "local map growth to %lld points failed", c);
+  if (keep > 0 &&
+      cudaMemcpyAsync(q.get(), p.get(), (size_t)keep * sizeof(float4), cudaMemcpyDeviceToDevice, lm->stream) != cudaSuccess)
     return fail(ctx, LS_ERR_CUDA, "local map growth copy failed");
-  }
   CU(cudaStreamSynchronize(lm->stream));
-  if (*p) cudaFree(*p);
-  *p = q;
-  *cap = (int)c;
+  p = std::move(q);
   return LS_OK;
 }
 
 int reserve_scratch(ls_local_map* lm, int n) {
   ls_ctx* ctx = lm->ctx;
   const int want = n > lm->initial_cap ? n : lm->initial_cap;
-  if (want <= lm->scratch.cap && lm->scratch.pts[0]) return LS_OK;
+  if (lm->scratch.pts[0].get() && (size_t)want <= lm->scratch.pts[0].capacity()) return LS_OK;
   CU(cudaStreamSynchronize(lm->stream));
-  if (lsf::reserve(lm->scratch, want) != cudaSuccess) {
-    cudaGetLastError();
+  if (lsf::reserve(lm->scratch, want) != cudaSuccess)
     return fail(lm->ctx, LS_ERR_NOMEM, "local map scratch for %d points failed", want);
-  }
   return LS_OK;
 }
 
 // LS_LM_* -> (device pointer, points)
 bool lm_cloud(const ls_local_map* lm, int which, const float4** p, int* n) {
   switch (which) {
-    case LS_LM_LOCAL: *p = lm->local[lm->cur]; *n = lm->n_local; return true;
-    case LS_LM_LOCAL_FILTERED: *p = lm->filt; *n = lm->n_filt; return true;
-    case LS_LM_DISTANT: *p = lm->dist; *n = lm->n_dist; return true;
+    case LS_LM_LOCAL: *p = lm->local[lm->cur].get(); *n = lm->n_local; return true;
+    case LS_LM_LOCAL_FILTERED: *p = lm->filt.get(); *n = lm->n_filt; return true;
+    case LS_LM_DISTANT: *p = lm->dist.get(); *n = lm->n_dist; return true;
     case LS_LM_FILTERED_MAP:
-      *p = lm->prm.separate_distant_map ? lm->result : lm->local[1 - lm->cur];
+      *p = lm->prm.separate_distant_map ? lm->result.get() : lm->local[1 - lm->cur].get();
       *n = lm->n_result;
       return true;
-    case LS_LM_QUEUE: *p = lm->queue; *n = lm->n_queue; return true;
+    case LS_LM_QUEUE: *p = lm->queue.get(); *n = lm->n_queue; return true;
     default: return false;
   }
 }
@@ -1589,10 +1565,6 @@ void ls_local_map_destroy(ls_local_map* lm) {
   if (!lm) return;
   cudaSetDevice(lm->ctx->device);
   if (lm->stream) cudaStreamSynchronize(lm->stream);
-  void* bufs[] = {lm->local[0], lm->local[1], lm->filt, lm->dist, lm->queue, lm->result};
-  for (void* b : bufs)
-    if (b) cudaFree(b);
-  lsf::release(lm->scratch);
   if (lm->stream) cudaStreamDestroy(lm->stream);
   delete lm;
 }
@@ -1612,15 +1584,15 @@ int ls_local_map_add_scan(ls_local_map* lm, const ls_map* ring, uint64_t scan_id
   if (n == 0) return LS_OK;
   int rc;
   const int c = lm->cur;
-  if ((rc = grow_cloud(lm, &lm->local[c], &lm->local_cap[c], (long long)lm->n_local + n, lm->n_local))) return rc;
-  if ((rc = grow_cloud(lm, &lm->queue, &lm->queue_cap, (long long)lm->n_queue + n, lm->n_queue))) return rc;
+  if ((rc = grow_cloud(lm, lm->local[c], (long long)lm->n_local + n, lm->n_local))) return rc;
+  if ((rc = grow_cloud(lm, lm->queue, (long long)lm->n_queue + n, lm->n_queue))) return rc;
   if ((rc = reserve_scratch(lm, n))) return rc;
   if (wait_slot(s, lm->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
   int kept = 0;
   const double z_min = robot_z - lm->prm.ground_distance_to_robot_center_m;
-  rc = lsf::enqueue_local_map_append(s->pts, n, T_w_scan, is_identity16(T_w_scan), lm->prm.remove_ground_from_local_map != 0,
-                                     z_min, lm->local[c] + lm->n_local, lm->queue + lm->n_queue, lm->scratch, lm->stream, &kept,
-                                     &ctx->launches);
+  rc = lsf::enqueue_local_map_append(s->pts.get(), n, T_w_scan, is_identity16(T_w_scan),
+                                     lm->prm.remove_ground_from_local_map != 0, z_min, lm->local[c].get() + lm->n_local,
+                                     lm->queue.get() + lm->n_queue, lm->scratch, lm->stream, &kept, &ctx->launches);
   if (rc) return fail(ctx, rc, "local map append failed");
   if (kept > 0) {
     lm->n_local += kept;
@@ -1639,18 +1611,19 @@ int ls_local_map_filter(ls_local_map* lm, const double center[3], int* n_filtere
   const bool separate = lm->prm.separate_distant_map != 0;
   const double radius = lm->prm.distance_to_consider_fixed, height = 40.0;  // the reference hard-codes the height
   const int c = lm->cur, n = lm->n_local;
-  const float4* snap = lm->local[c];
+  const float4* snap = lm->local[c].get();
   int rc;
   // every buffer this call can write, before anything changes (the previous result is kept until the new one exists)
-  if ((rc = grow_cloud(lm, &lm->local[1 - c], &lm->local_cap[1 - c], n, separate ? 0 : lm->n_result))) return rc;
+  if ((rc = grow_cloud(lm, lm->local[1 - c], n, separate ? 0 : lm->n_result))) return rc;
   if ((rc = reserve_scratch(lm, n))) return rc;
   if (separate) {
-    if ((rc = grow_cloud(lm, &lm->filt, &lm->filt_cap, n, lm->n_filt))) return rc;
-    if ((rc = grow_cloud(lm, &lm->dist, &lm->dist_cap, (long long)lm->n_dist + n, lm->n_dist))) return rc;
-    if ((rc = grow_cloud(lm, &lm->result, &lm->result_cap, (long long)lm->n_dist + 2LL * n, lm->n_result))) return rc;
+    if ((rc = grow_cloud(lm, lm->filt, n, lm->n_filt))) return rc;
+    if ((rc = grow_cloud(lm, lm->dist, (long long)lm->n_dist + n, lm->n_dist))) return rc;
+    if ((rc = grow_cloud(lm, lm->result, (long long)lm->n_dist + 2LL * n, lm->n_result))) return rc;
   }
   int n_cropped = 0;
-  if ((rc = lsf::enqueue_cylinder_crop(snap, n, center, radius, height, lm->local[1 - c], lm->scratch, lm->stream, &n_cropped,
+  if ((rc = lsf::enqueue_cylinder_crop(snap, n, center, radius, height, lm->local[1 - c].get(), lm->scratch, lm->stream,
+                                       &n_cropped,
                                        &ctx->launches)))
     return fail(ctx, rc, "local map crop failed");
   if (!separate) {  // the result is the snapshot itself, uncropped and not voxelised
@@ -1662,23 +1635,26 @@ int ls_local_map_filter(ls_local_map* lm, const double center[3], int* n_filtere
   }
   const float leaf[3] = {(float)lm->prm.voxel_size_m, (float)lm->prm.voxel_size_m, (float)lm->prm.voxel_size_m};
   lsf::VoxelBuffers vb = lsf::voxel_buffers(lm->scratch);
-  vb.cent = lm->scratch.nrm[0];
-  float4* vox = lm->scratch.pts[1];
+  vb.cent = lm->scratch.nrm[0].get();
+  float4* vox = lm->scratch.pts[1].get();
   int m = 0;
   if ((rc = lsf::enqueue_voxel_grid(snap, nullptr, n, leaf, vox, nullptr, lm->prm.minimum_point_number_per_voxel, vb, lm->stream,
                                     &m, &ctx->launches)))
     return fail(ctx, rc, rc == LS_ERR_ARG ? "leaf too small for the local map's extent" : "local map voxel grid failed");
   int n_in = 0, n_out = 0;
-  if ((rc = lsf::enqueue_cylinder_split(vox, m, center, radius, height, lm->filt, lm->dist + lm->n_dist, lm->scratch, lm->stream,
+  if ((rc = lsf::enqueue_cylinder_split(vox, m, center, radius, height, lm->filt.get(), lm->dist.get() + lm->n_dist, lm->scratch,
+                                        lm->stream,
                                         &n_in, &n_out, &ctx->launches)))
     return fail(ctx, rc, "local map split failed");
   lm->cur = 1 - c;
   lm->n_local = n_cropped;
   lm->n_filt = n_in;
   lm->n_dist += n_out;
-  if (n_in > 0) CU(cudaMemcpyAsync(lm->result, lm->filt, (size_t)n_in * sizeof(float4), cudaMemcpyDeviceToDevice, lm->stream));
+  if (n_in > 0) CU(cudaMemcpyAsync(lm->result.get(), lm->filt.get(), (size_t)n_in * sizeof(float4), cudaMemcpyDeviceToDevice,
+                                   lm->stream));
   if (lm->n_dist > 0)
-    CU(cudaMemcpyAsync(lm->result + n_in, lm->dist, (size_t)lm->n_dist * sizeof(float4), cudaMemcpyDeviceToDevice, lm->stream));
+    CU(cudaMemcpyAsync(lm->result.get() + n_in, lm->dist.get(), (size_t)lm->n_dist * sizeof(float4), cudaMemcpyDeviceToDevice,
+                       lm->stream));
   CU(cudaStreamSynchronize(lm->stream));
   lm->n_result = n_in + lm->n_dist;
   *n_filtered_map = lm->n_result;
@@ -1715,7 +1691,7 @@ int ls_local_map_take_queue(ls_local_map* lm, float* out4, int cap_points, int* 
     return fail(ctx, LS_ERR_ARG, "buffers of %d points / %d clouds for a queue of %d / %d", cap_points, cap_clouds, lm->n_queue, k);
   CU(cudaSetDevice(ctx->device));
   if (lm->n_queue > 0)
-    CU(cudaMemcpyAsync(out4, lm->queue, (size_t)lm->n_queue * sizeof(float4), cudaMemcpyDeviceToHost, lm->stream));
+    CU(cudaMemcpyAsync(out4, lm->queue.get(), (size_t)lm->n_queue * sizeof(float4), cudaMemcpyDeviceToHost, lm->stream));
   CU(cudaStreamSynchronize(lm->stream));
   cloud_offsets[0] = 0;
   for (int j = 0; j < k; ++j) cloud_offsets[j + 1] = cloud_offsets[j] + lm->queue_sizes[j];
@@ -1730,7 +1706,7 @@ int ls_local_map_transform(ls_local_map* lm, const float T[16]) {
   ls_ctx* ctx = lm->ctx;
   if (!T) return fail(ctx, LS_ERR_ARG, "bad argument");
   CU(cudaSetDevice(ctx->device));
-  float4* clouds[2] = {lm->local[lm->cur], lm->filt};
+  float4* clouds[2] = {lm->local[lm->cur].get(), lm->filt.get()};
   const int counts[2] = {lm->n_local, lm->n_filt};
   for (int k = 0; k < 2; ++k) {
     const int rc = lsf::enqueue_transform_in_place(clouds[k], counts[k], T, lm->stream, &ctx->launches);
@@ -1834,8 +1810,6 @@ void ls_occupancy_destroy(ls_occupancy* om) {
   if (!om) return;
   cudaSetDevice(om->ctx->device);
   if (om->stream) cudaStreamSynchronize(om->stream);
-  lso::release(om->map);
-  lso::release(om->tree);
   if (om->ev0) cudaEventDestroy(om->ev0);
   if (om->ev1) cudaEventDestroy(om->ev1);
   if (om->stream) cudaStreamDestroy(om->stream);
@@ -1856,7 +1830,8 @@ int ls_occupancy_insert_scan(ls_occupancy* om, const ls_map* ring, uint64_t scan
   CU(cudaEventRecord(om->ev0, om->stream));
   om->tree_current = false;
   lso::Counters c;
-  const int rc = lso::insert(om->map, om->prm, s->pts, s->n, T_w_scan, is_identity16(T_w_scan), om->stream, &c, &ctx->launches);
+  const int rc = lso::insert(om->map, om->prm, s->pts.get(), s->n, T_w_scan, is_identity16(T_w_scan), om->stream, &c,
+                             &ctx->launches);
   if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "occupancy map growth failed" : "occupancy map insert failed");
   CU(cudaEventRecord(om->ev1, om->stream));
   CU(cudaEventSynchronize(om->ev1));

@@ -17,6 +17,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/ls_b200.h"
+#include "ls_buffer.cuh"
 
 namespace {
 
@@ -62,9 +63,9 @@ struct ls_comm {
   int device = 0, rank = 0, nranks = 1;
   NcclComm comm = nullptr;
   cudaStream_t stream = nullptr;
-  ls_pose_record* d_send = nullptr;
-  ls_pose_record* d_recv = nullptr;
-  ls_pose_record* h_pinned = nullptr;  // [1 + nranks]
+  ls::Buffer<ls_pose_record> d_send;
+  ls::Buffer<ls_pose_record> d_recv;
+  ls::PinnedBuffer<ls_pose_record> h_pinned;  // [1 + nranks]
   bool pending = false;                // a begin() without its end()
   std::string err;
 };
@@ -94,9 +95,8 @@ int ls_comm_init(int device, int rank, int nranks, const void* id128, ls_comm** 
   NcclUniqueId id;
   std::memcpy(&id, id128, sizeof(id));
   if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaMalloc((void**)&c->d_send, sizeof(ls_pose_record)) != cudaSuccess ||
-      cudaMalloc((void**)&c->d_recv, sizeof(ls_pose_record) * (size_t)nranks) != cudaSuccess ||
-      cudaMallocHost((void**)&c->h_pinned, sizeof(ls_pose_record) * (size_t)(nranks + 1)) != cudaSuccess) {
+      c->d_send.reserve(1, 1) != cudaSuccess || c->d_recv.reserve((size_t)nranks, (size_t)nranks) != cudaSuccess ||
+      c->h_pinned.reserve((size_t)nranks + 1, (size_t)nranks + 1) != cudaSuccess) {
     ls_comm_destroy(c);
     return LS_ERR_CUDA;
   }
@@ -114,9 +114,6 @@ void ls_comm_destroy(ls_comm* c) {
   cudaSetDevice(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
   if (c->comm && api().ok) api().comm_destroy(c->comm);
-  if (c->d_send) cudaFree(c->d_send);
-  if (c->d_recv) cudaFree(c->d_recv);
-  if (c->h_pinned) cudaFreeHost(c->h_pinned);
   if (c->stream) cudaStreamDestroy(c->stream);
   delete c;
 }
@@ -127,15 +124,17 @@ int ls_comm_allgather_pose_records_begin(ls_comm* c, const ls_pose_record* mine)
   if (!c || !mine) return LS_ERR_ARG;
   if (c->pending) return LS_ERR_STATE;
   if (cudaSetDevice(c->device) != cudaSuccess) return LS_ERR_CUDA;
-  c->h_pinned[0] = *mine;
-  if (cudaMemcpyAsync(c->d_send, &c->h_pinned[0], sizeof(ls_pose_record), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+  c->h_pinned.get()[0] = *mine;
+  if (cudaMemcpyAsync(c->d_send.get(), c->h_pinned.get(), sizeof(ls_pose_record), cudaMemcpyHostToDevice,
+                      c->stream) != cudaSuccess)
     return LS_ERR_CUDA;
-  const int rc = api().all_gather(c->d_send, c->d_recv, sizeof(ls_pose_record), 0 /* ncclInt8 */, c->comm, c->stream);
+  const int rc = api().all_gather(c->d_send.get(), c->d_recv.get(), sizeof(ls_pose_record), 0 /* ncclInt8 */, c->comm, c->stream);
   if (rc != 0) {
     c->err = api().get_error_string ? api().get_error_string(rc) : "ncclAllGather failed";
     return LS_ERR_NCCL;
   }
-  if (cudaMemcpyAsync(&c->h_pinned[1], c->d_recv, sizeof(ls_pose_record) * (size_t)c->nranks, cudaMemcpyDeviceToHost, c->stream) !=
+  if (cudaMemcpyAsync(c->h_pinned.get() + 1, c->d_recv.get(), sizeof(ls_pose_record) * (size_t)c->nranks, cudaMemcpyDeviceToHost,
+                      c->stream) !=
       cudaSuccess)
     return LS_ERR_CUDA;
   c->pending = true;
@@ -148,7 +147,7 @@ int ls_comm_allgather_pose_records_end(ls_comm* c, ls_pose_record* all) {
   if (cudaSetDevice(c->device) != cudaSuccess) return LS_ERR_CUDA;
   c->pending = false;
   if (cudaStreamSynchronize(c->stream) != cudaSuccess) return LS_ERR_CUDA;
-  std::memcpy(all, &c->h_pinned[1], sizeof(ls_pose_record) * (size_t)c->nranks);
+  std::memcpy(all, c->h_pinned.get() + 1, sizeof(ls_pose_record) * (size_t)c->nranks);
   return LS_OK;
 }
 

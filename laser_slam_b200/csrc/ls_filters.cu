@@ -313,20 +313,6 @@ __global__ void split_scatter_kernel(const float4* __restrict__ in, const unsign
   }
 }
 
-struct Scratch {  // freed on every exit path
-  void* p[12] = {};
-  int n = 0;
-  template <typename T>
-  cudaError_t alloc(T** out, size_t count) {
-    cudaError_t e = cudaMalloc((void**)out, (count ? count : 1) * sizeof(T));
-    if (e == cudaSuccess) p[n++] = *out;
-    return e;
-  }
-  ~Scratch() {
-    for (int i = 0; i < n; ++i) cudaFree(p[i]);
-  }
-};
-
 // grid-stride kernels: at most 8 CTAs of 256 threads per SM of the current device (set by every entry point)
 inline int blocks(int n) {
   int dev = 0, sms = 1;
@@ -354,14 +340,14 @@ int ls_ingest_pointcloud2(int device, const void* data, int point_step, int off_
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return LS_ERR_CUDA;  // no CPU fallback
   FCU(cudaSetDevice(device));
-  Scratch s;
-  unsigned char* d_in;
-  float4* d_out;
-  FCU(s.alloc(&d_in, (size_t)n * point_step));
-  FCU(s.alloc(&d_out, (size_t)n));
-  FCU(cudaMemcpy(d_in, data, (size_t)n * point_step, cudaMemcpyHostToDevice));
-  ingest_kernel<<<blocks(n), 256>>>(d_in, point_step, off_x, off_y, off_z, n, d_out);
-  FCU(cudaMemcpy(out4, d_out, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost));
+  const size_t bytes = (size_t)n * point_step;
+  ls::Buffer<unsigned char> d_in;
+  ls::Buffer<float4> d_out;
+  FCU(d_in.reserve(bytes, bytes));
+  FCU(d_out.reserve(n, n));
+  FCU(cudaMemcpy(d_in.get(), data, bytes, cudaMemcpyHostToDevice));
+  ingest_kernel<<<blocks(n), 256>>>(d_in.get(), point_step, off_x, off_y, off_z, n, d_out.get());
+  FCU(cudaMemcpy(out4, d_out.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost));
   return LS_OK;
 }
 
@@ -373,27 +359,26 @@ int ls_filter_cylinder(int device, const float* in4, int n, const double center[
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return LS_ERR_CUDA;
   FCU(cudaSetDevice(device));
-  Scratch s;
-  float4 *d_in, *d_out;
-  int *d_keep, *d_pos;
-  FCU(s.alloc(&d_in, (size_t)n));
-  FCU(s.alloc(&d_out, (size_t)n));
-  FCU(s.alloc(&d_keep, (size_t)n));
-  FCU(s.alloc(&d_pos, (size_t)n));
-  FCU(cudaMemcpy(d_in, in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice));
-  cylinder_flag_kernel<<<blocks(n), 256>>>(d_in, n, center[0], center[1], center[2], radius_m * radius_m, height_m / 2.0,
-                                          remove_points_inside, d_keep);
+  ls::Buffer<float4> d_in, d_out;
+  ls::Buffer<int> d_keep, d_pos;
+  FCU(d_in.reserve(n, n));
+  FCU(d_out.reserve(n, n));
+  FCU(d_keep.reserve(n, n));
+  FCU(d_pos.reserve(n, n));
+  FCU(cudaMemcpy(d_in.get(), in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice));
+  cylinder_flag_kernel<<<blocks(n), 256>>>(d_in.get(), n, center[0], center[1], center[2], radius_m * radius_m, height_m / 2.0,
+                                          remove_points_inside, d_keep.get());
   size_t tmp_bytes = 0;
-  FCU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_keep, d_pos, n));
-  void* d_tmp;
-  FCU(s.alloc((unsigned char**)&d_tmp, tmp_bytes));
-  FCU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_keep, d_pos, n));
-  compact_kernel<<<blocks(n), 256>>>(d_in, nullptr, d_keep, d_pos, n, d_out, nullptr, nullptr);
+  FCU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_keep.get(), d_pos.get(), n));
+  ls::Buffer<unsigned char> d_tmp;
+  FCU(d_tmp.reserve(tmp_bytes, tmp_bytes));
+  FCU(cub::DeviceScan::ExclusiveSum(d_tmp.get(), tmp_bytes, d_keep.get(), d_pos.get(), n));
+  compact_kernel<<<blocks(n), 256>>>(d_in.get(), nullptr, d_keep.get(), d_pos.get(), n, d_out.get(), nullptr, nullptr);
   int last_pos = 0, last_keep = 0;
-  FCU(cudaMemcpy(&last_pos, d_pos + (n - 1), sizeof(int), cudaMemcpyDeviceToHost));
-  FCU(cudaMemcpy(&last_keep, d_keep + (n - 1), sizeof(int), cudaMemcpyDeviceToHost));
+  FCU(cudaMemcpy(&last_pos, d_pos.get() + (n - 1), sizeof(int), cudaMemcpyDeviceToHost));
+  FCU(cudaMemcpy(&last_keep, d_keep.get() + (n - 1), sizeof(int), cudaMemcpyDeviceToHost));
   *n_out = last_pos + last_keep;
-  FCU(cudaMemcpy(out4, d_out, (size_t)*n_out * sizeof(float4), cudaMemcpyDeviceToHost));
+  FCU(cudaMemcpy(out4, d_out.get(), (size_t)*n_out * sizeof(float4), cudaMemcpyDeviceToHost));
   return LS_OK;
 }
 
@@ -409,21 +394,21 @@ int ls_deskew_revolution(int device, const float* points4, const int* packet_off
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return LS_ERR_CUDA;
   FCU(cudaSetDevice(device));
-  Scratch s;
-  float4 *d_in, *d_out;
-  int* d_offs;
-  float* d_T;
-  FCU(s.alloc(&d_in, (size_t)m));
-  FCU(s.alloc(&d_out, (size_t)m));
-  FCU(s.alloc(&d_offs, (size_t)n_packets + 1));
-  FCU(s.alloc(&d_T, 16 * ((size_t)n_packets + 1)));
-  FCU(cudaMemcpy(d_in, points4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice));
-  FCU(cudaMemcpy(d_offs, packet_offsets, ((size_t)n_packets + 1) * sizeof(int), cudaMemcpyHostToDevice));
-  FCU(cudaMemcpy(d_T, T_packets, 16 * (size_t)n_packets * sizeof(float), cudaMemcpyHostToDevice));
-  FCU(cudaMemcpy(d_T + 16 * (size_t)n_packets, T_final, 16 * sizeof(float), cudaMemcpyHostToDevice));
-  deskew_kernel<<<blocks(m), 256>>>(d_in, m, d_offs, n_packets, d_T, d_T + 16 * (size_t)n_packets, d_out);
+  const size_t np = (size_t)n_packets;
+  ls::Buffer<float4> d_in, d_out;
+  ls::Buffer<int> d_offs;
+  ls::Buffer<float> d_T;
+  FCU(d_in.reserve(m, m));
+  FCU(d_out.reserve(m, m));
+  FCU(d_offs.reserve(np + 1, np + 1));
+  FCU(d_T.reserve(16 * (np + 1), 16 * (np + 1)));
+  FCU(cudaMemcpy(d_in.get(), points4, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice));
+  FCU(cudaMemcpy(d_offs.get(), packet_offsets, (np + 1) * sizeof(int), cudaMemcpyHostToDevice));
+  FCU(cudaMemcpy(d_T.get(), T_packets, 16 * np * sizeof(float), cudaMemcpyHostToDevice));
+  FCU(cudaMemcpy(d_T.get() + 16 * np, T_final, 16 * sizeof(float), cudaMemcpyHostToDevice));
+  deskew_kernel<<<blocks(m), 256>>>(d_in.get(), m, d_offs.get(), n_packets, d_T.get(), d_T.get() + 16 * np, d_out.get());
   FCU(cudaGetLastError());
-  FCU(cudaMemcpy(out4, d_out, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost));
+  FCU(cudaMemcpy(out4, d_out.get(), (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost));
   return LS_OK;
 }
 
@@ -435,27 +420,39 @@ int ls_voxel_grid(int device, const float* in4, int n, const float leaf_size[3],
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return LS_ERR_CUDA;
   FCU(cudaSetDevice(device));
-  Scratch s;
-  float4 *d_in, *d_out;
+  const size_t tmp_bytes = lsf::voxel_temp_bytes(n);
+  ls::Buffer<float4> d_in, d_out;
+  ls::Buffer<int> mm, idx, idx2, head, slot;
+  ls::Buffer<unsigned long long> key, key2, sums;
+  ls::Buffer<unsigned char> tmp;
+  FCU(d_in.reserve(n, n));
+  FCU(d_out.reserve(n, n));
+  FCU(mm.reserve(6, 6));
+  FCU(idx.reserve(n, n));
+  FCU(idx2.reserve(n, n));
+  FCU(head.reserve(n, n));
+  FCU(slot.reserve(n, n));
+  FCU(key.reserve(n, n));
+  FCU(key2.reserve(n, n));
+  FCU(sums.reserve((size_t)n * 4, (size_t)n * 4));
+  FCU(tmp.reserve(tmp_bytes, tmp_bytes));
   lsf::VoxelBuffers vb;
-  FCU(s.alloc(&d_in, (size_t)n));
-  FCU(s.alloc(&d_out, (size_t)n));
-  FCU(s.alloc(&vb.mm, 6));
-  FCU(s.alloc(&vb.idx, (size_t)n));
-  FCU(s.alloc(&vb.idx2, (size_t)n));
-  FCU(s.alloc(&vb.head, (size_t)n));
-  FCU(s.alloc(&vb.slot, (size_t)n));
-  FCU(s.alloc(&vb.key, (size_t)n));
-  FCU(s.alloc(&vb.key2, (size_t)n));
-  FCU(s.alloc(&vb.sums, (size_t)n * 4));
-  vb.tmp_bytes = lsf::voxel_temp_bytes(n);
-  FCU(s.alloc((unsigned char**)&vb.tmp, vb.tmp_bytes));
-  FCU(cudaMemcpy(d_in, in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice));
+  vb.mm = mm.get();
+  vb.key = key.get();
+  vb.key2 = key2.get();
+  vb.sums = sums.get();
+  vb.idx = idx.get();
+  vb.idx2 = idx2.get();
+  vb.head = head.get();
+  vb.slot = slot.get();
+  vb.tmp = tmp.get();
+  vb.tmp_bytes = tmp_bytes;
+  FCU(cudaMemcpy(d_in.get(), in4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice));
   uint64_t launches = 0;
   int m = 0;
-  const int rc = lsf::enqueue_voxel_grid(d_in, nullptr, n, leaf_size, d_out, nullptr, 0, vb, 0, &m, &launches);
+  const int rc = lsf::enqueue_voxel_grid(d_in.get(), nullptr, n, leaf_size, d_out.get(), nullptr, 0, vb, 0, &m, &launches);
   if (rc != LS_OK) return rc;
-  if (m > 0) FCU(cudaMemcpy(out4, d_out, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost));
+  if (m > 0) FCU(cudaMemcpy(out4, d_out.get(), (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost));
   *n_out = m;
   return LS_OK;
 }
@@ -477,10 +474,6 @@ size_t scan_temp_bytes(int n) {
   a = a > b ? a : b;
   return a > c ? a : c;
 }
-template <typename T>
-cudaError_t grow(T** p, size_t count) {
-  return cudaMalloc((void**)p, (count ? count : 1) * sizeof(T));
-}
 }  // namespace
 
 bool is_mask_filter(int type) {
@@ -495,46 +488,35 @@ size_t voxel_temp_bytes(int n) {
   return sort > scan ? sort : scan;
 }
 
-void release(ChainBuffers& b) {
-  void* all[] = {b.pts[0], b.pts[1], b.nrm[0], b.nrm[1], b.keep, b.pos, b.small, b.key, b.key2, b.idx, b.idx2, b.head, b.slot, b.sums, b.tmp};
-  for (void* p : all)
-    if (p) cudaFree(p);
-  b = ChainBuffers();
-}
-
 cudaError_t reserve(ChainBuffers& b, int n) {
-  if (n <= b.cap && b.pts[0]) return cudaSuccess;
-  release(b);
+  if (b.pts[0].get() && (size_t)n <= b.pts[0].capacity()) return cudaSuccess;
+  b = ChainBuffers();  // the old arrays go before the new ones are allocated
   const int cap = n + n / 8 + 1024;
-  const size_t c = (size_t)cap;
+  const size_t c = (size_t)cap, tmp_bytes = voxel_temp_bytes(cap);
   cudaError_t e;
-  if ((e = grow(&b.pts[0], c)) || (e = grow(&b.pts[1], c)) || (e = grow(&b.nrm[0], c)) || (e = grow(&b.nrm[1], c)) ||
-      (e = grow(&b.keep, c)) || (e = grow(&b.pos, c)) || (e = grow(&b.small, 8)) || (e = grow(&b.key, c)) ||
-      (e = grow(&b.key2, c)) || (e = grow(&b.idx, c)) || (e = grow(&b.idx2, c)) || (e = grow(&b.head, c)) ||
-      (e = grow(&b.slot, c)) || (e = grow(&b.sums, 7 * c))) {
-    release(b);
+  if ((e = b.pts[0].reserve(c, c)) || (e = b.pts[1].reserve(c, c)) || (e = b.nrm[0].reserve(c, c)) ||
+      (e = b.nrm[1].reserve(c, c)) || (e = b.keep.reserve(c, c)) || (e = b.pos.reserve(c, c)) || (e = b.small.reserve(8, 8)) ||
+      (e = b.key.reserve(c, c)) || (e = b.key2.reserve(c, c)) || (e = b.idx.reserve(c, c)) || (e = b.idx2.reserve(c, c)) ||
+      (e = b.head.reserve(c, c)) || (e = b.slot.reserve(c, c)) || (e = b.sums.reserve(7 * c, 7 * c)) ||
+      (e = b.tmp.reserve(tmp_bytes, tmp_bytes))) {
+    b = ChainBuffers();
     return e;
   }
-  b.tmp_bytes = voxel_temp_bytes(cap);
-  if ((e = grow((unsigned char**)&b.tmp, b.tmp_bytes))) {
-    release(b);
-    return e;
-  }
-  b.cap = cap;
+  b.tmp_bytes = tmp_bytes;
   return cudaSuccess;
 }
 
 VoxelBuffers voxel_buffers(const ChainBuffers& b) {
   VoxelBuffers v;
-  v.mm = b.small;
-  v.key = b.key;
-  v.key2 = b.key2;
-  v.sums = b.sums;
-  v.idx = b.idx;
-  v.idx2 = b.idx2;
-  v.head = b.head;
-  v.slot = b.slot;
-  v.tmp = b.tmp;
+  v.mm = b.small.get();
+  v.key = b.key.get();
+  v.key2 = b.key2.get();
+  v.sums = b.sums.get();
+  v.idx = b.idx.get();
+  v.idx2 = b.idx2.get();
+  v.head = b.head.get();
+  v.slot = b.slot.get();
+  v.tmp = b.tmp.get();
   v.tmp_bytes = b.tmp_bytes;
   return v;
 }
@@ -551,8 +533,8 @@ cudaError_t enqueue_mask_run(const ls_point_filter* filters, int n_filters, cons
     const int t = filters[j].type;
     if (!is_pointwise(t)) {  // a sampler: rank of every point in the cloud entering it = exclusive scan of the flags so far
       if (have_keep) {
-        if ((e = cub::DeviceScan::ExclusiveSum(b.tmp, b.tmp_bytes, b.keep, b.pos, n, st))) return e;
-        rank = b.pos;
+        if ((e = cub::DeviceScan::ExclusiveSum(b.tmp.get(), b.tmp_bytes, b.keep.get(), b.pos.get(), n, st))) return e;
+        rank = b.pos.get();
       }
       s.sampler = t;
       s.prob = filters[j].prob;
@@ -569,14 +551,14 @@ cudaError_t enqueue_mask_run(const ls_point_filter* filters, int n_filters, cons
       o.dist = f.dist;
       for (int a = 0; a < 6; ++a) o.box[a] = f.box[a];
     }
-    mask_kernel<<<blocks(n), 256, 0, st>>>(pts, n, have_keep ? b.keep : nullptr, rank, s, b.keep);
+    mask_kernel<<<blocks(n), 256, 0, st>>>(pts, n, have_keep ? b.keep.get() : nullptr, rank, s, b.keep.get());
     ++*launches;
     if ((e = cudaGetLastError())) return e;
     have_keep = true;
   }
   *used = j;
-  if ((e = cub::DeviceScan::ExclusiveSum(b.tmp, b.tmp_bytes, b.keep, b.pos, n, st))) return e;
-  compact_kernel<<<blocks(n), 256, 0, st>>>(pts, nrm, b.keep, b.pos, n, out, out_nrm, b.small + 6);
+  if ((e = cub::DeviceScan::ExclusiveSum(b.tmp.get(), b.tmp_bytes, b.keep.get(), b.pos.get(), n, st))) return e;
+  compact_kernel<<<blocks(n), 256, 0, st>>>(pts, nrm, b.keep.get(), b.pos.get(), n, out, out_nrm, b.small.get() + 6);
   ++*launches;
   return cudaGetLastError();
 }
@@ -638,14 +620,16 @@ int enqueue_local_map_append(const float4* scan, int n, const float T[16], bool 
   if (n == 0) return LS_OK;
   Xform16 x;
   memcpy(x.T, T, sizeof(x.T));
-  local_map_append_kernel<<<blocks(n), 256, 0, st>>>(scan, n, x, identity ? 1 : 0, remove_ground ? 1 : 0, z_min, b.pts[0], b.keep);
+  local_map_append_kernel<<<blocks(n), 256, 0, st>>>(scan, n, x, identity ? 1 : 0, remove_ground ? 1 : 0, z_min, b.pts[0].get(),
+                                                     b.keep.get());
   size_t bytes = b.tmp_bytes;
-  FCU(cub::DeviceScan::ExclusiveSum(b.tmp, bytes, b.keep, b.pos, n, st));
+  FCU(cub::DeviceScan::ExclusiveSum(b.tmp.get(), bytes, b.keep.get(), b.pos.get(), n, st));
   // one compaction fills both: the local map's tail as the points, the queue's tail as the "normals" of the same points
-  compact_kernel<<<blocks(n), 256, 0, st>>>(b.pts[0], b.pts[0], b.keep, b.pos, n, local_tail, queue_tail, b.small + 6);
+  compact_kernel<<<blocks(n), 256, 0, st>>>(b.pts[0].get(), b.pts[0].get(), b.keep.get(), b.pos.get(), n, local_tail, queue_tail,
+                                            b.small.get() + 6);
   *launches += 2;
   FCU(cudaGetLastError());
-  FCU(cudaMemcpyAsync(kept, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+  FCU(cudaMemcpyAsync(kept, b.small.get() + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
   FCU(cudaStreamSynchronize(st));
   return LS_OK;
 }
@@ -665,13 +649,13 @@ int enqueue_cylinder_crop(const float4* in, int n, const double center[3], doubl
   *kept = 0;
   if (n == 0) return LS_OK;
   cylinder_flag_kernel<<<blocks(n), 256, 0, st>>>(in, n, center[0], center[1], center[2], radius_m * radius_m, height_m / 2.0, 0,
-                                                  b.keep);
+                                                  b.keep.get());
   size_t bytes = b.tmp_bytes;
-  FCU(cub::DeviceScan::ExclusiveSum(b.tmp, bytes, b.keep, b.pos, n, st));
-  compact_kernel<<<blocks(n), 256, 0, st>>>(in, nullptr, b.keep, b.pos, n, out, nullptr, b.small + 6);
+  FCU(cub::DeviceScan::ExclusiveSum(b.tmp.get(), bytes, b.keep.get(), b.pos.get(), n, st));
+  compact_kernel<<<blocks(n), 256, 0, st>>>(in, nullptr, b.keep.get(), b.pos.get(), n, out, nullptr, b.small.get() + 6);
   *launches += 2;
   FCU(cudaGetLastError());
-  FCU(cudaMemcpyAsync(kept, b.small + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+  FCU(cudaMemcpyAsync(kept, b.small.get() + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
   FCU(cudaStreamSynchronize(st));
   return LS_OK;
 }
@@ -680,14 +664,15 @@ int enqueue_cylinder_split(const float4* in, int n, const double center[3], doub
                            float4* outside, ChainBuffers& b, cudaStream_t st, int* n_inside, int* n_outside, uint64_t* launches) {
   *n_inside = *n_outside = 0;
   if (n == 0) return LS_OK;
-  split_flag_kernel<<<blocks(n), 256, 0, st>>>(in, n, center[0], center[1], center[2], radius_m * radius_m, height_m / 2.0, b.key);
+  split_flag_kernel<<<blocks(n), 256, 0, st>>>(in, n, center[0], center[1], center[2], radius_m * radius_m, height_m / 2.0,
+                                               b.key.get());
   size_t bytes = b.tmp_bytes;
-  FCU(cub::DeviceScan::ExclusiveSum(b.tmp, bytes, b.key, b.key2, n, st));
-  split_scatter_kernel<<<blocks(n), 256, 0, st>>>(in, b.key, b.key2, n, inside, outside, b.small + 6);
+  FCU(cub::DeviceScan::ExclusiveSum(b.tmp.get(), bytes, b.key.get(), b.key2.get(), n, st));
+  split_scatter_kernel<<<blocks(n), 256, 0, st>>>(in, b.key.get(), b.key2.get(), n, inside, outside, b.small.get() + 6);
   *launches += 2;
   FCU(cudaGetLastError());
   int c[2];
-  FCU(cudaMemcpyAsync(c, b.small + 6, sizeof(c), cudaMemcpyDeviceToHost, st));
+  FCU(cudaMemcpyAsync(c, b.small.get() + 6, sizeof(c), cudaMemcpyDeviceToHost, st));
   FCU(cudaStreamSynchronize(st));
   *n_inside = c[0];
   *n_outside = c[1];

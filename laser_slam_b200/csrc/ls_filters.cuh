@@ -9,25 +9,24 @@
 #include <cuda_runtime.h>
 
 #include "../../include/ls_b200.h"
+#include "ls_buffer.cuh"
 
 namespace lsf {
 
-// Device scratch of one chain run, grown to the largest cloud seen (reserve()).  The chain ping-pongs between
-// pts[0]/nrm[0] and pts[1]/nrm[1].
+// Device scratch of one chain run, grown to the largest cloud seen (reserve()); pts[0]'s capacity is the group's.  The
+// chain ping-pongs between pts[0]/nrm[0] and pts[1]/nrm[1].
 struct ChainBuffers {
-  int cap = 0;
-  float4* pts[2] = {nullptr, nullptr};
-  float4* nrm[2] = {nullptr, nullptr};
-  int *keep = nullptr, *pos = nullptr;  // per-point flags and their exclusive scan
-  int* small = nullptr;                 // 8 ints: voxel cell bounds (6), kept count
-  unsigned long long *key = nullptr, *key2 = nullptr;
-  int *idx = nullptr, *idx2 = nullptr, *head = nullptr, *slot = nullptr;
-  unsigned long long* sums = nullptr;   // 7 per voxel: x, y, z, count, nx, ny, nz (fixed point)
-  void* tmp = nullptr;                  // CUB temporary storage
+  ls::Buffer<float4> pts[2], nrm[2];
+  ls::Buffer<int> keep, pos;  // per-point flags and their exclusive scan
+  ls::Buffer<int> small;      // 8 ints: voxel cell bounds (6), kept count
+  ls::Buffer<unsigned long long> key, key2;
+  ls::Buffer<int> idx, idx2, head, slot;
+  ls::Buffer<unsigned long long> sums;  // 7 per voxel: x, y, z, count, nx, ny, nz (fixed point)
+  ls::Buffer<unsigned char> tmp;        // CUB temporary storage
   size_t tmp_bytes = 0;
 };
+// All or nothing: on a failure every array is freed and the error returned.
 cudaError_t reserve(ChainBuffers& b, int n);
-void release(ChainBuffers& b);
 
 // Flag / compact one run of mask filters (point-wise tests and index samplers) that starts at filters[0].  `n` points in
 // pts/nrm (nrm may be NULL).  Writes the survivors to out/out_nrm and their number to b.small[6]; the caller reads it

@@ -27,6 +27,7 @@
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <utility>
 #include <vector>
 
 #include <cub/cub.cuh>
@@ -70,8 +71,8 @@ struct Dev {
 };
 
 Dev dev_of(const Map& m) {
-  return Dev{m.tab_keys, m.tab_vals, (unsigned)m.tab_cap - 1u, m.pool_cap, m.lo, m.known, m.mfree, m.mocc, m.bkey, m.touched,
-             m.tlist};
+  return Dev{m.tab_keys.get(), m.tab_vals.get(), (unsigned)m.tab_cap() - 1u, m.pool_cap(), m.lo.get(), m.known.get(),
+             m.mfree.get(), m.mocc.get(), m.bkey.get(), m.touched.get(), m.tlist.get()};
 }
 
 __device__ __forceinline__ unsigned hash64(unsigned long long k) {
@@ -903,27 +904,15 @@ int code(cudaError_t e) {
     OCC_TRY(cudaGetLastError());              \
   } while (0)
 
-template <typename T>
-cudaError_t alloc(T** p, size_t count) {
-  *p = nullptr;
-  return cudaMalloc((void**)p, (count ? count : 1) * sizeof(T));
-}
-
-template <typename T>
-void free_ptr(T*& p) {
-  if (p) cudaFree(p);
-  p = nullptr;
-}
-
 int upload_counters(Map& m, cudaStream_t st) {
-  std::memset(m.cnt_host, 0, sizeof(Counters));
-  m.cnt_host->pool_n = m.pool_n;
-  OCC_TRY(cudaMemcpyAsync(m.cnt_dev, m.cnt_host, sizeof(Counters), cudaMemcpyHostToDevice, st));
+  std::memset(m.cnt_host.get(), 0, sizeof(Counters));
+  m.cnt_host.get()->pool_n = m.pool_n;
+  OCC_TRY(cudaMemcpyAsync(m.cnt_dev.get(), m.cnt_host.get(), sizeof(Counters), cudaMemcpyHostToDevice, st));
   return LS_OK;
 }
 
 int read_counters(Map& m, cudaStream_t st) {
-  OCC_TRY(cudaMemcpyAsync(m.cnt_host, m.cnt_dev, sizeof(Counters), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaMemcpyAsync(m.cnt_host.get(), m.cnt_dev.get(), sizeof(Counters), cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
@@ -933,29 +922,29 @@ int read_counters(Map& m, cudaStream_t st) {
 int grow_pool(Map& m, int cap, cudaStream_t st) {
   Map q;
   const size_t c = (size_t)cap;
-  cudaError_t e = alloc(&q.lo, c * 512);
-  if (e == cudaSuccess) e = alloc(&q.known, c * 16);
-  if (e == cudaSuccess) e = alloc(&q.mfree, c * 16);
-  if (e == cudaSuccess) e = alloc(&q.mocc, c * 16);
-  if (e == cudaSuccess) e = alloc(&q.bkey, c);
-  if (e == cudaSuccess) e = alloc(&q.touched, c);
-  if (e == cudaSuccess) e = alloc(&q.tlist, c);
+  cudaError_t e = q.lo.reserve(c * 512, c * 512);
+  if (e == cudaSuccess) e = q.known.reserve(c * 16, c * 16);
+  if (e == cudaSuccess) e = q.mfree.reserve(c * 16, c * 16);
+  if (e == cudaSuccess) e = q.mocc.reserve(c * 16, c * 16);
+  if (e == cudaSuccess) e = q.bkey.reserve(c, c);
+  if (e == cudaSuccess) e = q.touched.reserve(c, c);
+  if (e == cudaSuccess) e = q.tlist.reserve(c, c);
   const size_t n = (size_t)m.pool_n;
-  if (e == cudaSuccess) e = cudaMemsetAsync(q.lo + n * 512, 0, (c - n) * 512 * sizeof(float), st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(q.known + n * 16, 0, (c - n) * 16 * sizeof(unsigned), st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(q.mfree, 0, c * 16 * sizeof(unsigned), st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(q.mocc, 0, c * 16 * sizeof(unsigned), st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(q.touched, 0, c * sizeof(unsigned), st);
-  if (e == cudaSuccess && n > 0) e = cudaMemcpyAsync(q.lo, m.lo, n * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess && n > 0) e = cudaMemcpyAsync(q.known, m.known, n * 16 * sizeof(unsigned), cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess && n > 0) e = cudaMemcpyAsync(q.bkey, m.bkey, n * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(q.lo.get() + n * 512, 0, (c - n) * 512 * sizeof(float), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(q.known.get() + n * 16, 0, (c - n) * 16 * sizeof(unsigned), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(q.mfree.get(), 0, c * 16 * sizeof(unsigned), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(q.mocc.get(), 0, c * 16 * sizeof(unsigned), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(q.touched.get(), 0, c * sizeof(unsigned), st);
+  if (e == cudaSuccess && n > 0) e = cudaMemcpyAsync(q.lo.get(), m.lo.get(), n * 512 * sizeof(float), cudaMemcpyDeviceToDevice,
+                                                     st);
+  if (e == cudaSuccess && n > 0)
+    e = cudaMemcpyAsync(q.known.get(), m.known.get(), n * 16 * sizeof(unsigned), cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess && n > 0)
+    e = cudaMemcpyAsync(q.bkey.get(), m.bkey.get(), n * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  Map& drop = e == cudaSuccess ? m : q;
-  free_ptr(drop.lo), free_ptr(drop.known), free_ptr(drop.mfree), free_ptr(drop.mocc), free_ptr(drop.bkey);
-  free_ptr(drop.touched), free_ptr(drop.tlist);
   if (e != cudaSuccess) return code(e);
-  m.lo = q.lo, m.known = q.known, m.mfree = q.mfree, m.mocc = q.mocc, m.bkey = q.bkey, m.touched = q.touched, m.tlist = q.tlist;
-  m.pool_cap = cap;
+  m.lo = std::move(q.lo), m.known = std::move(q.known), m.mfree = std::move(q.mfree), m.mocc = std::move(q.mocc);
+  m.bkey = std::move(q.bkey), m.touched = std::move(q.touched), m.tlist = std::move(q.tlist);
   return LS_OK;
 }
 
@@ -963,75 +952,70 @@ int grow_pool(Map& m, int cap, cudaStream_t st) {
 // table stays when an allocation fails.
 int rebuild_table(Map& m, int cap, cudaStream_t st, uint64_t* launches) {
   for (;; cap *= 2) {
-    unsigned long long* keys = nullptr;
-    int* vals = nullptr;
-    cudaError_t e = alloc(&keys, (size_t)cap);
-    if (e == cudaSuccess) e = alloc(&vals, (size_t)cap);
-    if (e == cudaSuccess) e = cudaMemsetAsync(keys, 0xff, (size_t)cap * sizeof(unsigned long long), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(vals, 0xff, (size_t)cap * sizeof(int), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(&m.cnt_dev->overflow, 0, sizeof(int), st);
+    const size_t c = (size_t)cap;
+    ls::Buffer<unsigned long long> keys;
+    ls::Buffer<int> vals;
+    cudaError_t e = keys.reserve(c, c);
+    if (e == cudaSuccess) e = vals.reserve(c, c);
+    if (e == cudaSuccess) e = cudaMemsetAsync(keys.get(), 0xff, c * sizeof(unsigned long long), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(vals.get(), 0xff, c * sizeof(int), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(&m.cnt_dev.get()->overflow, 0, sizeof(int), st);
     if (e == cudaSuccess && m.pool_n > 0) {
-      occ_rehash_kernel<<<(m.pool_n + 255) / 256, 256, 0, st>>>(m.bkey, m.pool_n, keys, vals, (unsigned)cap - 1u, m.cnt_dev);
+      occ_rehash_kernel<<<(m.pool_n + 255) / 256, 256, 0, st>>>(m.bkey.get(), m.pool_n, keys.get(), vals.get(),
+                                                                (unsigned)cap - 1u,
+                                                                m.cnt_dev.get());
       ++*launches;
       e = cudaGetLastError();
     }
     int overflow = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&overflow, &m.cnt_dev->overflow, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&overflow, &m.cnt_dev.get()->overflow, sizeof(int), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess || overflow) {
-      free_ptr(keys), free_ptr(vals);
-      if (e != cudaSuccess) return code(e);
-      continue;
-    }
-    free_ptr(m.tab_keys), free_ptr(m.tab_vals);
-    m.tab_keys = keys, m.tab_vals = vals, m.tab_cap = cap;
+    if (e != cudaSuccess) return code(e);
+    if (overflow) continue;
+    m.tab_keys = std::move(keys), m.tab_vals = std::move(vals);
     return LS_OK;
   }
 }
 
 int reserve_points(Map& m, int n, cudaStream_t st) {
-  if (n > m.pt_cap) {
+  cudaError_t e;
+  if ((size_t)n > m.ends.capacity()) {
     OCC_TRY(cudaStreamSynchronize(st));
-    const int cap = n + n / 8;
-    free_ptr(m.ends), free_ptr(m.pkey), free_ptr(m.cls);
-    m.pt_cap = 0;
-    OCC_TRY(alloc(&m.ends, (size_t)cap));
-    OCC_TRY(alloc(&m.pkey, (size_t)cap));
-    OCC_TRY(alloc(&m.cls, (size_t)cap));
-    m.pt_cap = cap;
+    const size_t cap = (size_t)(n + n / 8);
+    if ((e = m.ends.reserve(cap, cap)) || (e = m.pkey.reserve(cap, cap)) || (e = m.cls.reserve(cap, cap))) {
+      m.ends.reset(), m.pkey.reset(), m.cls.reset();
+      return code(e);
+    }
   }
-  int ep = 1024;
-  while (ep < 2 * n) ep *= 2;
-  if (ep > m.ep_cap) {
+  size_t ep = 1024;
+  while (ep < 2 * (size_t)n) ep *= 2;
+  if (ep > m.ep_keys.capacity()) {
     OCC_TRY(cudaStreamSynchronize(st));
-    free_ptr(m.ep_keys), free_ptr(m.ep_min);
-    m.ep_cap = 0;
-    OCC_TRY(alloc(&m.ep_keys, (size_t)ep));
-    OCC_TRY(alloc(&m.ep_min, (size_t)ep));
-    m.ep_cap = ep;
+    if ((e = m.ep_keys.reserve(ep, ep)) || (e = m.ep_min.reserve(ep, ep))) {
+      m.ep_keys.reset(), m.ep_min.reset();
+      return code(e);
+    }
   }
   return LS_OK;
 }
 
 int reserve_export(Map& m, long long n, cudaStream_t st) {
-  if (n <= m.ex_cap && m.ex_c) return LS_OK;
+  if ((size_t)n <= m.ex_c.capacity()) return LS_OK;
   OCC_TRY(cudaStreamSynchronize(st));
-  for (int j = 0; j < 2; ++j) free_ptr(m.ex_k[j]), free_ptr(m.ex_v[j]);
-  free_ptr(m.ex_c);
-  free_ptr(m.cub_tmp);
-  m.ex_cap = 0;
-  m.cub_bytes = 0;
   const long long cap = n + n / 8 + 1024;
-  for (int j = 0; j < 2; ++j) {
-    OCC_TRY(alloc(&m.ex_k[j], (size_t)cap));
-    OCC_TRY(alloc(&m.ex_v[j], (size_t)cap));
-  }
-  OCC_TRY(alloc(&m.ex_c, (size_t)cap));
+  const size_t c = (size_t)cap;
   size_t bytes = 0;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, m.ex_k[0], m.ex_k[1], m.ex_v[0], m.ex_v[1], (int)cap, 0, 48, st));
-  OCC_TRY(alloc((unsigned char**)&m.cub_tmp, bytes));
+  cudaError_t e;
+  if ((e = m.ex_c.reserve(c, c)) || (e = m.ex_k[0].reserve(c, c)) || (e = m.ex_v[0].reserve(c, c)) ||
+      (e = m.ex_k[1].reserve(c, c)) || (e = m.ex_v[1].reserve(c, c)) ||
+      (e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, m.ex_k[0].get(), m.ex_k[1].get(), m.ex_v[0].get(), m.ex_v[1].get(),
+                                           (int)cap, 0, 48, st)) ||
+      (e = m.cub_tmp.reserve(bytes, bytes))) {
+    m.ex_c.reset(), m.ex_k[0].reset(), m.ex_v[0].reset(), m.ex_k[1].reset(), m.ex_v[1].reset(), m.cub_tmp.reset();
+    m.cub_bytes = 0;
+    return code(e);
+  }
   m.cub_bytes = bytes;
-  m.ex_cap = cap;
   return LS_OK;
 }
 
@@ -1043,71 +1027,59 @@ int select(Map& m, const Params& P, int which, unsigned long long* keys, unsigne
   if (nvox > 0) {
     long long blocks = (nvox + 255) / 256;
     if (blocks > 65536) blocks = 65536;
-    occ_select_kernel<<<(int)blocks, 256, 0, st>>>(dev_of(m), P, which, nvox, keys, vals, m.cnt_dev);
+    occ_select_kernel<<<(int)blocks, 256, 0, st>>>(dev_of(m), P, which, nvox, keys, vals, m.cnt_dev.get());
     OCC_LAUNCHED();
   }
   return read_counters(m, st);
 }
 
 Nodes nodes_of(const Octree& t) {
-  return Nodes{t.code, t.pool, t.first, t.end, t.st, t.n_nodes, t.n_bytes, t.n_leaves, t.off, t.loff};
+  return Nodes{t.code.get(), t.pool.get(), t.first.get(), t.end.get(), t.st.get(),
+               t.n_nodes.get(), t.n_bytes.get(), t.n_leaves.get(), t.off.get(), t.loff.get()};
 }
 
 // Records for n_b bricks and every upper node they can have: at most min(n_b, 8^d) at depth d.
 int reserve_tree(Octree& t, int n_b, cudaStream_t st) {
-  if (!t.levels) {
-    OCC_TRY(alloc(&t.levels, 2 * (kBrickDepth + 1)));
-    OCC_TRY(alloc(&t.tot_dev, 3));
-    OCC_TRY(cudaMallocHost((void**)&t.tot_host, 3 * sizeof(unsigned long long)));
-  }
-  if (n_b <= t.brick_cap) return LS_OK;
+  OCC_TRY(t.levels.reserve(2 * (kBrickDepth + 1), 2 * (kBrickDepth + 1)));
+  OCC_TRY(t.tot_dev.reserve(3, 3));
+  OCC_TRY(t.tot_host.reserve(3, 3));
+  if ((size_t)n_b <= t.pool.capacity()) return LS_OK;
   OCC_TRY(cudaStreamSynchronize(st));
-  free_ptr(t.code), free_ptr(t.pool), free_ptr(t.first), free_ptr(t.end), free_ptr(t.st);
-  free_ptr(t.n_nodes), free_ptr(t.n_bytes), free_ptr(t.n_leaves), free_ptr(t.off), free_ptr(t.loff);
-  free_ptr(t.sort_k), free_ptr(t.sort_v), free_ptr(t.cub_tmp);
-  t.brick_cap = 0, t.node_cap = 0, t.cub_bytes = 0;
   const int cap = n_b + n_b / 8;
   long long nodes = cap, level = 1;
   for (int d = 0; d < kBrickDepth; ++d, level *= 8) nodes += level < cap ? level : cap;
-  const size_t n = (size_t)nodes;
-  OCC_TRY(alloc(&t.code, n));
-  OCC_TRY(alloc(&t.pool, (size_t)cap));
-  OCC_TRY(alloc(&t.first, n));
-  OCC_TRY(alloc(&t.end, n));
-  OCC_TRY(alloc(&t.st, n));
-  OCC_TRY(alloc(&t.n_nodes, n));
-  OCC_TRY(alloc(&t.n_bytes, n));
-  OCC_TRY(alloc(&t.n_leaves, n));
-  OCC_TRY(alloc(&t.off, n));
-  OCC_TRY(alloc(&t.loff, n));
-  OCC_TRY(alloc(&t.sort_k, (size_t)cap));
-  OCC_TRY(alloc(&t.sort_v, (size_t)cap));
+  const size_t n = (size_t)nodes, c = (size_t)cap;
   size_t bytes = 0;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, t.sort_k, t.code, t.sort_v, t.pool, cap, 0, 3 * kBrickDepth, st));
-  OCC_TRY(alloc((unsigned char**)&t.cub_tmp, bytes));
+  cudaError_t e;
+  if ((e = t.pool.reserve(c, c)) || (e = t.code.reserve(n, n)) || (e = t.first.reserve(n, n)) || (e = t.end.reserve(n, n)) ||
+      (e = t.st.reserve(n, n)) || (e = t.n_nodes.reserve(n, n)) || (e = t.n_bytes.reserve(n, n)) ||
+      (e = t.n_leaves.reserve(n, n)) || (e = t.off.reserve(n, n)) || (e = t.loff.reserve(n, n)) ||
+      (e = t.sort_k.reserve(c, c)) || (e = t.sort_v.reserve(c, c)) ||
+      (e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, t.sort_k.get(), t.code.get(), t.sort_v.get(), t.pool.get(), cap, 0,
+                                           3 * kBrickDepth, st)) ||
+      (e = t.cub_tmp.reserve(bytes, bytes))) {
+    t.pool.reset(), t.code.reset(), t.first.reset(), t.end.reset(), t.st.reset(), t.n_nodes.reset(), t.n_bytes.reset();
+    t.n_leaves.reset(), t.off.reset(), t.loff.reset(), t.sort_k.reset(), t.sort_v.reset(), t.cub_tmp.reset();
+    t.cub_bytes = 0;
+    return code(e);
+  }
   t.cub_bytes = bytes;
-  t.node_cap = nodes;
-  t.brick_cap = cap;
   return LS_OK;
 }
 
 int reserve_tree_outputs(Octree& t, long long bytes, long long leaves, cudaStream_t st) {
-  if (bytes > t.pay_cap) {
+  if ((size_t)bytes > t.payload.capacity()) {
     OCC_TRY(cudaStreamSynchronize(st));
-    free_ptr(t.payload);
-    t.pay_cap = 0;
-    const long long cap = bytes + bytes / 8;
-    OCC_TRY(alloc(&t.payload, (size_t)cap));
-    t.pay_cap = cap;
+    OCC_TRY(t.payload.reserve((size_t)bytes, (size_t)(bytes + bytes / 8)));
   }
-  if (leaves > t.leaf_cap) {
+  if ((size_t)leaves > t.centres.capacity()) {
     OCC_TRY(cudaStreamSynchronize(st));
-    free_ptr(t.centres), free_ptr(t.depths);
-    t.leaf_cap = 0;
-    const long long cap = leaves + leaves / 8;
-    OCC_TRY(alloc(&t.centres, (size_t)cap));
-    OCC_TRY(alloc(&t.depths, (size_t)cap));
-    t.leaf_cap = cap;
+    const size_t cap = (size_t)(leaves + leaves / 8);
+    cudaError_t e;
+    if ((e = t.centres.reserve(cap, cap)) || (e = t.depths.reserve(cap, cap))) {
+      t.centres.reset(), t.depths.reset();
+      return code(e);
+    }
   }
   return LS_OK;
 }
@@ -1116,8 +1088,8 @@ int reserve_tree_outputs(Octree& t, long long bytes, long long leaves, cudaStrea
 
 int init(Map& m, int initial_bricks, cudaStream_t st) {
   m = Map();
-  OCC_TRY(cudaMalloc((void**)&m.cnt_dev, sizeof(Counters)));
-  OCC_TRY(cudaMallocHost((void**)&m.cnt_host, sizeof(Counters)));
+  OCC_TRY(m.cnt_dev.reserve(1, 1));
+  OCC_TRY(m.cnt_host.reserve(1, 1));
   int rc;
   if ((rc = grow_pool(m, initial_bricks, st))) return rc;
   int cap = 1024;
@@ -1126,27 +1098,14 @@ int init(Map& m, int initial_bricks, cudaStream_t st) {
   return rebuild_table(m, cap, st, &launches);
 }
 
-void release(Map& m) {
-  free_ptr(m.tab_keys), free_ptr(m.tab_vals);
-  free_ptr(m.lo), free_ptr(m.known), free_ptr(m.mfree), free_ptr(m.mocc), free_ptr(m.bkey), free_ptr(m.touched);
-  free_ptr(m.tlist);
-  free_ptr(m.ends), free_ptr(m.pkey), free_ptr(m.cls), free_ptr(m.ep_keys), free_ptr(m.ep_min);
-  for (int j = 0; j < 2; ++j) free_ptr(m.ex_k[j]), free_ptr(m.ex_v[j]);
-  free_ptr(m.ex_c), free_ptr(m.cub_tmp), free_ptr(m.cnt_dev);
-  free_ptr(m.qbuf);
-  m.q_cap = 0;
-  if (m.cnt_host) cudaFreeHost(m.cnt_host);
-  m.cnt_host = nullptr;
-}
-
 size_t device_bytes(const Map& m) {
-  const size_t pool = (size_t)m.pool_cap * (512 * sizeof(float) + 48 * sizeof(unsigned) + sizeof(unsigned long long) +
-                                            sizeof(unsigned) + sizeof(int));
-  const size_t tab = (size_t)m.tab_cap * (sizeof(unsigned long long) + sizeof(int));
-  const size_t pts = (size_t)m.pt_cap * (sizeof(float4) + sizeof(unsigned long long) + sizeof(int)) +
-                     (size_t)m.ep_cap * (sizeof(unsigned long long) + sizeof(int));
-  const size_t ex = (size_t)m.ex_cap * (2 * sizeof(unsigned long long) + 2 * sizeof(unsigned) + sizeof(float4)) + m.cub_bytes;
-  return pool + tab + pts + ex + m.q_cap + sizeof(Counters);
+  const size_t pool = (size_t)m.pool_cap() * (512 * sizeof(float) + 48 * sizeof(unsigned) + sizeof(unsigned long long) +
+                                              sizeof(unsigned) + sizeof(int));
+  const size_t tab = (size_t)m.tab_cap() * (sizeof(unsigned long long) + sizeof(int));
+  const size_t pts = m.ends.capacity() * (sizeof(float4) + sizeof(unsigned long long) + sizeof(int)) +
+                     m.ep_keys.capacity() * (sizeof(unsigned long long) + sizeof(int));
+  const size_t ex = m.ex_c.capacity() * (2 * sizeof(unsigned long long) + 2 * sizeof(unsigned) + sizeof(float4)) + m.cub_bytes;
+  return pool + tab + pts + ex + m.qbuf.capacity() + sizeof(Counters);
 }
 
 int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16], bool identity, cudaStream_t st, Counters* out,
@@ -1154,47 +1113,49 @@ int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16],
   int rc;
   std::memset(out, 0, sizeof(Counters));
   if ((rc = reserve_points(m, n, st))) return rc;
-  if (2LL * m.pool_n > m.tab_cap && (rc = rebuild_table(m, m.tab_cap * 2, st, launches))) return rc;
+  if (2LL * m.pool_n > m.tab_cap() && (rc = rebuild_table(m, m.tab_cap() * 2, st, launches))) return rc;
   if ((rc = upload_counters(m, st))) return rc;
-  OCC_TRY(cudaMemsetAsync(m.ep_keys, 0xff, (size_t)m.ep_cap * sizeof(unsigned long long), st));
-  OCC_TRY(cudaMemsetAsync(m.ep_min, 0x7f, (size_t)m.ep_cap * sizeof(int), st));  // 0x7f7f7f7f: above any point index
+  OCC_TRY(cudaMemsetAsync(m.ep_keys.get(), 0xff, m.ep_keys.capacity() * sizeof(unsigned long long), st));
+  OCC_TRY(cudaMemsetAsync(m.ep_min.get(), 0x7f, m.ep_keys.capacity() * sizeof(int), st));  // 0x7f7f7f7f: above any point index
   Xform16 x;
   std::memcpy(x.T, T, sizeof(x.T));
   const int blocks = (n + 255) / 256;
   if (n > 0) {
-    occ_classify_kernel<<<blocks, 256, 0, st>>>(pts, n, x, identity ? 1 : 0, P, m.ends, m.pkey, m.cls, m.ep_keys, m.ep_min,
-                                                 (unsigned)m.ep_cap - 1u);
+    occ_classify_kernel<<<blocks, 256, 0, st>>>(pts, n, x, identity ? 1 : 0, P, m.ends.get(), m.pkey.get(), m.cls.get(),
+                                                m.ep_keys.get(), m.ep_min.get(),
+                                                 (unsigned)m.ep_keys.capacity() - 1u);
     OCC_LAUNCHED();
   }
   for (;;) {
     if (n > 0) {
-      occ_cast_kernel<<<blocks, 256, 0, st>>>(n, P, T[12], T[13], T[14], m.ends, m.pkey, m.cls, m.ep_keys, m.ep_min,
-                                              (unsigned)m.ep_cap - 1u, dev_of(m), m.cnt_dev);
+      occ_cast_kernel<<<blocks, 256, 0, st>>>(n, P, T[12], T[13], T[14], m.ends.get(), m.pkey.get(), m.cls.get(), m.ep_keys.get(),
+                                              m.ep_min.get(),
+                                              (unsigned)m.ep_keys.capacity() - 1u, dev_of(m), m.cnt_dev.get());
       OCC_LAUNCHED();
     }
     if ((rc = read_counters(m, st))) return rc;
-    const Counters c = *m.cnt_host;
+    const Counters c = *m.cnt_host.get();
     if (!c.overflow) break;
     // Undo the marking: clear every mark and touched flag, keep the bricks that got a pool index, drop the rest from the
     // hash, grow what filled and mark again.
-    m.pool_n = c.pool_n < m.pool_cap ? c.pool_n : m.pool_cap;
-    OCC_TRY(cudaMemsetAsync(m.mfree, 0, (size_t)m.pool_cap * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mocc, 0, (size_t)m.pool_cap * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.touched, 0, (size_t)m.pool_cap * sizeof(unsigned), st));
-    int tab = m.tab_cap;
+    m.pool_n = c.pool_n < m.pool_cap() ? c.pool_n : m.pool_cap();
+    OCC_TRY(cudaMemsetAsync(m.mfree.get(), 0, (size_t)m.pool_cap() * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.mocc.get(), 0, (size_t)m.pool_cap() * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.touched.get(), 0, (size_t)m.pool_cap() * sizeof(unsigned), st));
+    int tab = m.tab_cap();
     if ((c.overflow & kOverflowTable) || 2LL * m.pool_n > tab) tab *= 2;
     if ((rc = rebuild_table(m, tab, st, launches))) return rc;
-    if ((c.overflow & kOverflowPool) && (rc = grow_pool(m, m.pool_cap * 2, st))) return rc;
+    if ((c.overflow & kOverflowPool) && (rc = grow_pool(m, m.pool_cap() * 2, st))) return rc;
     if ((rc = upload_counters(m, st))) return rc;
   }
-  m.pool_n = m.cnt_host->pool_n;
-  if (m.cnt_host->n_touched > 0) {
-    occ_update_kernel<<<m.cnt_host->n_touched, 512, 0, st>>>(dev_of(m), P, m.cnt_dev);
+  m.pool_n = m.cnt_host.get()->pool_n;
+  if (m.cnt_host.get()->n_touched > 0) {
+    occ_update_kernel<<<m.cnt_host.get()->n_touched, 512, 0, st>>>(dev_of(m), P, m.cnt_dev.get());
     OCC_LAUNCHED();
     if ((rc = read_counters(m, st))) return rc;
   }
-  m.n_known += (long long)m.cnt_host->new_known;
-  *out = *m.cnt_host;
+  m.n_known += (long long)m.cnt_host.get()->new_known;
+  *out = *m.cnt_host.get();
   return LS_OK;
 }
 
@@ -1205,7 +1166,7 @@ int count(Map& m, const Params& P, int which, long long* n, cudaStream_t st, uin
   }
   int rc;
   if ((rc = select(m, P, which, nullptr, nullptr, st, launches))) return rc;
-  *n = (long long)m.cnt_host->n_out;
+  *n = (long long)m.cnt_host.get()->n_out;
   return LS_OK;
 }
 
@@ -1215,20 +1176,21 @@ int download(Map& m, const Params& P, int which, long long n, uint64_t* keys, fl
   if (n > 0x7fffffffLL) return LS_ERR_NOMEM;
   int rc;
   if ((rc = reserve_export(m, n, st))) return rc;
-  if ((rc = select(m, P, which, m.ex_k[0], m.ex_v[0], st, launches))) return rc;
-  if ((long long)m.cnt_host->n_out != n) return LS_ERR_CUDA;
+  if ((rc = select(m, P, which, m.ex_k[0].get(), m.ex_v[0].get(), st, launches))) return rc;
+  if ((long long)m.cnt_host.get()->n_out != n) return LS_ERR_CUDA;
   size_t bytes = m.cub_bytes;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(m.cub_tmp, bytes, m.ex_k[0], m.ex_k[1], m.ex_v[0], m.ex_v[1], (int)n, 0, 48, st));
+  OCC_TRY(cub::DeviceRadixSort::SortPairs(m.cub_tmp.get(), bytes, m.ex_k[0].get(), m.ex_k[1].get(), m.ex_v[0].get(),
+                                          m.ex_v[1].get(), (int)n, 0, 48, st));
   ++*launches;
   if (centres4) {
     long long blocks = (n + 255) / 256;
     if (blocks > 65536) blocks = 65536;
-    occ_centres_kernel<<<(int)blocks, 256, 0, st>>>(m.ex_k[1], n, P.res, m.ex_c);
+    occ_centres_kernel<<<(int)blocks, 256, 0, st>>>(m.ex_k[1].get(), n, P.res, m.ex_c.get());
     OCC_LAUNCHED();
-    OCC_TRY(cudaMemcpyAsync(centres4, m.ex_c, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    OCC_TRY(cudaMemcpyAsync(centres4, m.ex_c.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, st));
   }
-  if (keys) OCC_TRY(cudaMemcpyAsync(keys, m.ex_k[1], (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, m.ex_v[1], (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (keys) OCC_TRY(cudaMemcpyAsync(keys, m.ex_k[1].get(), (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, m.ex_v[1].get(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
@@ -1240,23 +1202,26 @@ int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint
   int rc;
   if ((rc = reserve_tree(t, n_b, st))) return rc;
   const Nodes N = nodes_of(t);
-  oct_code_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.bkey, n_b, t.sort_k, t.sort_v);
+  oct_code_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.bkey.get(), n_b, t.sort_k.get(), t.sort_v.get());
   OCC_LAUNCHED();
   size_t bytes = t.cub_bytes;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp, bytes, t.sort_k, t.code, t.sort_v, t.pool, n_b, 0, 3 * kBrickDepth, st));
+  OCC_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp.get(), bytes, t.sort_k.get(), t.code.get(), t.sort_v.get(), t.pool.get(), n_b,
+                                          0, 3 * kBrickDepth, st));
   ++*launches;
-  oct_brick_kernel<<<n_b, 512, 0, st>>>(m.known, m.lo, N, P.l_occ);
+  oct_brick_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, P.l_occ);
   OCC_LAUNCHED();
-  oct_up_kernel<<<1, kTreeThreads, 0, st>>>(N, n_b, t.levels, t.tot_dev);
+  oct_up_kernel<<<1, kTreeThreads, 0, st>>>(N, n_b, t.levels.get(), t.tot_dev.get());
   OCC_LAUNCHED();
-  OCC_TRY(cudaMemcpyAsync(t.tot_host, t.tot_dev, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaMemcpyAsync(t.tot_host.get(), t.tot_dev.get(), 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
-  const long long nodes = (long long)t.tot_host[0], pay = (long long)t.tot_host[1], leaves = (long long)t.tot_host[2];
+  const unsigned long long* tot = t.tot_host.get();
+  const long long nodes = (long long)tot[0], pay = (long long)tot[1], leaves = (long long)tot[2];
   if (nodes == 0) return LS_OK;
   if ((rc = reserve_tree_outputs(t, pay, leaves, st))) return rc;
-  oct_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.levels, P.res, t.payload, t.centres, t.depths);
+  oct_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), P.res, t.payload.get(), t.centres.get(), t.depths.get());
   OCC_LAUNCHED();
-  oct_emit_kernel<<<n_b, 512, 0, st>>>(m.known, m.lo, m.bkey, N, P.l_occ, P.res, t.payload, t.centres, t.depths);
+  oct_emit_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, P.res, t.payload.get(),
+                                       t.centres.get(), t.depths.get());
   OCC_LAUNCHED();
   OCC_TRY(cudaStreamSynchronize(st));
   t.nodes = nodes, t.bytes = pay, t.leaves = leaves;
@@ -1264,10 +1229,10 @@ int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint
 }
 
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st) {
-  if (t.bytes > 0 && payload) OCC_TRY(cudaMemcpyAsync(payload, t.payload, (size_t)t.bytes, cudaMemcpyDeviceToHost, st));
+  if (t.bytes > 0 && payload) OCC_TRY(cudaMemcpyAsync(payload, t.payload.get(), (size_t)t.bytes, cudaMemcpyDeviceToHost, st));
   if (t.leaves > 0 && centres4)
-    OCC_TRY(cudaMemcpyAsync(centres4, t.centres, (size_t)t.leaves * sizeof(float4), cudaMemcpyDeviceToHost, st));
-  if (t.leaves > 0 && depths) OCC_TRY(cudaMemcpyAsync(depths, t.depths, (size_t)t.leaves, cudaMemcpyDeviceToHost, st));
+    OCC_TRY(cudaMemcpyAsync(centres4, t.centres.get(), (size_t)t.leaves * sizeof(float4), cudaMemcpyDeviceToHost, st));
+  if (t.leaves > 0 && depths) OCC_TRY(cudaMemcpyAsync(depths, t.depths.get(), (size_t)t.leaves, cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
@@ -1283,27 +1248,25 @@ size_t take(size_t& off, size_t bytes) {
 
 // Query staging of at least `bytes`, grown by doubling; the old buffer is dropped first (its contents are not needed).
 int reserve_query(Map& m, size_t bytes, cudaStream_t st) {
-  if (bytes <= m.q_cap) return LS_OK;
+  if (bytes <= m.qbuf.capacity()) return LS_OK;
   OCC_TRY(cudaStreamSynchronize(st));
-  size_t cap = m.q_cap ? 2 * m.q_cap : (size_t)1 << 16;
+  size_t cap = m.qbuf.capacity() ? 2 * m.qbuf.capacity() : (size_t)1 << 16;
   while (cap < bytes) cap *= 2;
-  free_ptr(m.qbuf);
-  m.q_cap = 0;
-  OCC_TRY(alloc(&m.qbuf, cap));
-  m.q_cap = cap;
+  OCC_TRY(m.qbuf.reserve(bytes, cap));
   return LS_OK;
 }
 
 int zero_visited(Map& m, cudaStream_t st) {
-  OCC_TRY(cudaMemsetAsync(&m.cnt_dev->n_out, 0, sizeof(unsigned long long), st));
+  OCC_TRY(cudaMemsetAsync(&m.cnt_dev.get()->n_out, 0, sizeof(unsigned long long), st));
   return LS_OK;
 }
 
 // The outputs' copies are queued; wait for them and the keys visited.
 int finish_query(Map& m, cudaStream_t st, long long* visited) {
-  OCC_TRY(cudaMemcpyAsync(&m.cnt_host->n_out, &m.cnt_dev->n_out, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaMemcpyAsync(&m.cnt_host.get()->n_out, &m.cnt_dev.get()->n_out, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                          st));
   OCC_TRY(cudaStreamSynchronize(st));
-  *visited = (long long)m.cnt_host->n_out;
+  *visited = (long long)m.cnt_host.get()->n_out;
   return LS_OK;
 }
 
@@ -1335,11 +1298,11 @@ int query_cells(Map& m, const Params& P, const double* pts3, int n, int8_t* stat
                o_lo = take(off, (size_t)n * sizeof(float));
   int rc;
   if ((rc = reserve_query(m, off, st))) return rc;
-  char* q = m.qbuf;
+  char* q = m.qbuf.get();
   OCC_TRY(cudaMemcpyAsync(q + o_in, pts3, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
   if ((rc = zero_visited(m, st))) return rc;
   occ_cell_kernel<<<blocks_of(n), 256, 0, st>>>((const double*)(q + o_in), n, dev_of(m), P, (signed char*)(q + o_st),
-                                                (float*)(q + o_lo), m.cnt_dev);
+                                                (float*)(q + o_lo), m.cnt_dev.get());
   OCC_LAUNCHED();
   OCC_TRY(cudaMemcpyAsync(status, q + o_st, (size_t)n, cudaMemcpyDeviceToHost, st));
   if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, q + o_lo, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -1369,7 +1332,7 @@ int query_lines(Map& m, const Params& P, const double* starts3, const double* en
                o_best = take(off, (size_t)n * sizeof(unsigned));
   int rc;
   if ((rc = reserve_query(m, off, st))) return rc;
-  char* q = m.qbuf;
+  char* q = m.qbuf.get();
   const double* s = (const double*)(q + o_s);
   const double* e = (const double*)(q + o_e);
   double* offs = (double*)(q + o_off);
@@ -1381,7 +1344,7 @@ int query_lines(Map& m, const Params& P, const double* starts3, const double* en
   if ((rc = zero_visited(m, st))) return rc;
   if (!box3) {
     occ_line_kernel<false><<<blocks_of(n), 256, 0, st>>>(s, e, n, 1, nullptr, 1, 1, 1, stop_at_unknown, dev_of(m), P, dst, dfk,
-                                                         nullptr, m.cnt_dev);
+                                                         nullptr, m.cnt_dev.get());
     OCC_LAUNCHED();
   } else {
     std::vector<double> flat;
@@ -1390,10 +1353,10 @@ int query_lines(Map& m, const Params& P, const double* starts3, const double* en
     OCC_TRY(cudaMemsetAsync(best, 0, (size_t)n * sizeof(unsigned), st));  // 0: no line failed
     const long long items = lines * n;
     occ_line_kernel<true><<<blocks_of(items), 256, 0, st>>>(s, e, items, (int)lines, offs, nx, ny, nz, stop_at_unknown,
-                                                            dev_of(m), P, dst, dfk, best, m.cnt_dev);
+                                                            dev_of(m), P, dst, dfk, best, m.cnt_dev.get());
     OCC_LAUNCHED();
     occ_box_result_kernel<<<blocks_of(n), 256, 0, st>>>(s, e, n, (int)lines, offs, nx, ny, nz, stop_at_unknown, dev_of(m), P,
-                                                         best, dst, dfk, m.cnt_dev);
+                                                         best, dst, dfk, m.cnt_dev.get());
     OCC_LAUNCHED();
     // the pageable copy of `flat` is staged before cudaMemcpyAsync returns, so it may go out of scope here
   }
@@ -1411,25 +1374,16 @@ int query_rays(Map& m, const Params& P, const float* origins3, const float* dire
   const size_t o_o = take(off, vec_bytes), o_d = take(off, vec_bytes), o_r = take(off, (size_t)n), o_e = take(off, vec_bytes);
   int rc;
   if ((rc = reserve_query(m, off, st))) return rc;
-  char* q = m.qbuf;
+  char* q = m.qbuf.get();
   OCC_TRY(cudaMemcpyAsync(q + o_o, origins3, vec_bytes, cudaMemcpyHostToDevice, st));
   OCC_TRY(cudaMemcpyAsync(q + o_d, directions3, vec_bytes, cudaMemcpyHostToDevice, st));
   if ((rc = zero_visited(m, st))) return rc;
   occ_ray_kernel<<<blocks_of(n), 256, 0, st>>>((const float*)(q + o_o), (const float*)(q + o_d), n, ignore_unknown, max_range,
-                                               dev_of(m), P, (signed char*)(q + o_r), (float*)(q + o_e), m.cnt_dev);
+                                               dev_of(m), P, (signed char*)(q + o_r), (float*)(q + o_e), m.cnt_dev.get());
   OCC_LAUNCHED();
   OCC_TRY(cudaMemcpyAsync(result, q + o_r, (size_t)n, cudaMemcpyDeviceToHost, st));
   if (ends3) OCC_TRY(cudaMemcpyAsync(ends3, q + o_e, vec_bytes, cudaMemcpyDeviceToHost, st));
   return finish_query(m, st, visited);
-}
-
-void release(Octree& t) {
-  free_ptr(t.levels), free_ptr(t.code), free_ptr(t.pool), free_ptr(t.first), free_ptr(t.end), free_ptr(t.st);
-  free_ptr(t.n_nodes), free_ptr(t.n_bytes), free_ptr(t.n_leaves), free_ptr(t.off), free_ptr(t.loff);
-  free_ptr(t.sort_k), free_ptr(t.sort_v), free_ptr(t.cub_tmp), free_ptr(t.tot_dev);
-  free_ptr(t.payload), free_ptr(t.centres), free_ptr(t.depths);
-  if (t.tot_host) cudaFreeHost(t.tot_host);
-  t = Octree();
 }
 
 }  // namespace lso

@@ -6,6 +6,8 @@
 
 #include <cuda_runtime.h>
 
+#include "ls_buffer.cuh"
+
 namespace lso {
 
 // The rules' constants: log-odds computed on the host in double and rounded to float once.
@@ -22,67 +24,62 @@ struct Counters {
 
 // Bricks of 8x8x8 voxels.  The hash maps a brick key (13 bits per axis) to a pool index; per brick the pool holds 512
 // float log-odds, 16 words of known bits and 16 + 16 words of per-scan free / occupied marks.
+// Each group of arrays grows all or nothing; its first array tells its capacity.
 struct Map {
-  int tab_cap = 0;  // power of two
-  unsigned long long* tab_keys = nullptr;
-  int* tab_vals = nullptr;
-  int pool_cap = 0, pool_n = 0;
-  float* lo = nullptr;
-  unsigned *known = nullptr, *mfree = nullptr, *mocc = nullptr;
-  unsigned long long* bkey = nullptr;  // brick key of each pool brick
-  unsigned* touched = nullptr;         // per brick: marked in this scan
-  int* tlist = nullptr;                // bricks marked in this scan
+  ls::Buffer<unsigned long long> tab_keys;  // power-of-two slots
+  ls::Buffer<int> tab_vals;
+  int pool_n = 0;
+  ls::Buffer<int> tlist;  // per pool brick: bricks marked in this scan
+  ls::Buffer<float> lo;
+  ls::Buffer<unsigned> known, mfree, mocc;
+  ls::Buffer<unsigned long long> bkey;  // brick key of each pool brick
+  ls::Buffer<unsigned> touched;         // per brick: marked in this scan
   // per-scan scratch: ray ends, endpoint keys and classes; the endpoint-key -> first point index table
-  int pt_cap = 0;
-  float4* ends = nullptr;
-  unsigned long long* pkey = nullptr;
-  int* cls = nullptr;
-  int ep_cap = 0;
-  unsigned long long* ep_keys = nullptr;
-  int* ep_min = nullptr;
+  ls::Buffer<float4> ends;
+  ls::Buffer<unsigned long long> pkey;
+  ls::Buffer<int> cls;
+  ls::Buffer<unsigned long long> ep_keys;
+  ls::Buffer<int> ep_min;
   // export scratch
-  long long ex_cap = 0;
-  unsigned long long* ex_k[2] = {nullptr, nullptr};
-  unsigned* ex_v[2] = {nullptr, nullptr};
-  float4* ex_c = nullptr;
-  void* cub_tmp = nullptr;
+  ls::Buffer<float4> ex_c;
+  ls::Buffer<unsigned long long> ex_k[2];
+  ls::Buffer<unsigned> ex_v[2];
+  ls::Buffer<unsigned char> cub_tmp;
   size_t cub_bytes = 0;
   // query staging (inputs and outputs of one call), grown by doubling
-  size_t q_cap = 0;
-  char* qbuf = nullptr;
-  Counters* cnt_dev = nullptr;
-  Counters* cnt_host = nullptr;  // pinned
+  ls::Buffer<char> qbuf;
+  ls::Buffer<Counters> cnt_dev;
+  ls::PinnedBuffer<Counters> cnt_host;
   long long n_known = 0;
+
+  int tab_cap() const { return (int)tab_keys.capacity(); }
+  int pool_cap() const { return (int)tlist.capacity(); }
 };
 
 // The map as octomap's pruned tree: depth 16 over the map's keys, each brick a depth-13 node.  Node records hold the
 // bricks by Morton code, then each upper level (12 ... 0) in turn; all scratch is O(bricks) plus the outputs.
 struct Octree {
-  int* levels = nullptr;  // per depth d = 0 ... 13: first record, count
-  long long node_cap = 0;
-  unsigned long long* code = nullptr;  // Morton code of the node at its depth
-  int* pool = nullptr;                 // bricks: pool index
-  int *first = nullptr, *end = nullptr;  // upper nodes: their children's records [first, end)
-  unsigned char* st = nullptr;         // 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner
-  unsigned long long *n_nodes = nullptr, *n_bytes = nullptr, *n_leaves = nullptr;  // subtree totals
-  unsigned long long *off = nullptr, *loff = nullptr;  // payload byte and occupied-leaf offsets in pre-order
-  int brick_cap = 0;
-  unsigned long long* sort_k = nullptr;
-  int* sort_v = nullptr;
-  void* cub_tmp = nullptr;
+  ls::Buffer<int> levels;  // per depth d = 0 ... 13: first record, count
+  ls::Buffer<int> pool;    // bricks: pool index (its capacity is the group's, in bricks)
+  ls::Buffer<unsigned long long> code;  // Morton code of the node at its depth
+  ls::Buffer<int> first, end;           // upper nodes: their children's records [first, end)
+  ls::Buffer<unsigned char> st;         // 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner
+  ls::Buffer<unsigned long long> n_nodes, n_bytes, n_leaves;  // subtree totals
+  ls::Buffer<unsigned long long> off, loff;  // payload byte and occupied-leaf offsets in pre-order
+  ls::Buffer<unsigned long long> sort_k;
+  ls::Buffer<int> sort_v;
+  ls::Buffer<unsigned char> cub_tmp;
   size_t cub_bytes = 0;
-  unsigned long long* tot_dev = nullptr;   // nodes, payload bytes, occupied leaves of the whole tree
-  unsigned long long* tot_host = nullptr;  // pinned
-  long long pay_cap = 0, leaf_cap = 0;
-  unsigned char* payload = nullptr;
-  float4* centres = nullptr;
-  unsigned char* depths = nullptr;
+  ls::Buffer<unsigned long long> tot_dev;    // nodes, payload bytes, occupied leaves of the whole tree
+  ls::PinnedBuffer<unsigned long long> tot_host;
+  ls::Buffer<unsigned char> payload;
+  ls::Buffer<float4> centres;  // with depths
+  ls::Buffer<unsigned char> depths;
   long long nodes = 0, bytes = 0, leaves = 0;  // of the last build
 };
 
 // All return LS_OK, LS_ERR_NOMEM or LS_ERR_CUDA (include/ls_b200.h) and count their launches in *launches.
 int init(Map& m, int initial_bricks, cudaStream_t st);
-void release(Map& m);
 // One scan of n points (device, float4) moved by T (column-major float32; identity: copied).  Synchronous; *out holds the
 // scan's counters.  On an error the known voxels and their log-odds are unchanged.
 int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16], bool identity, cudaStream_t st, Counters* out,
@@ -98,7 +95,6 @@ size_t device_bytes(const Map& m);
 int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches);
 // Copies the last build's payload (t.bytes) and, each when not NULL, its t.leaves centres {x, y, z, 1} and depths.
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st);
-void release(Octree& t);
 
 // Queries (oracle/QUERIES.md), reading the map only.  Synchronous; host inputs and outputs, *visited the voxel states the
 // kernels read.  n <= 0 launches nothing.

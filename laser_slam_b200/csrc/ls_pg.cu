@@ -26,6 +26,9 @@
 #include <cuda_runtime.h>
 
 #include "../../include/ls_b200.h"
+#include "ls_buffer.cuh"
+
+using ls::Buffer;
 
 namespace {
 
@@ -629,20 +632,21 @@ struct ls_pg {
   std::unordered_map<uint64_t, int> key_index;
   std::vector<HostFactor> factors;
   uint64_t launches = 0;
-  // device buffers (grown on demand)
-  size_t capF = 0, capP = 0, capZ = 0, capS = 0, capInc = 0, capE = 0;
-  FactorDev* d_fac = nullptr;
-  double *d_poses = nullptr, *d_Ja = nullptr, *d_Jb = nullptr, *d_r = nullptr, *d_D = nullptr, *d_B = nullptr,
-         *d_g = nullptr, *d_Z = nullptr, *d_S = nullptr, *d_rhs = nullptr, *d_cost = nullptr;
-  int *d_inc_ptr = nullptr, *d_inc_fac = nullptr, *d_extra = nullptr, *d_track_begin = nullptr, *d_fail = nullptr,
-      *d_damp = nullptr;
-  unsigned long long* d_dmax = nullptr;
+  // device buffers, grown on demand in groups (solve); the first array of a group tells its capacity
+  Buffer<FactorDev> d_fac;  // per factor
+  Buffer<double> d_Ja, d_Jb, d_r;
+  Buffer<double> d_poses, d_D, d_B, d_g;  // per pose
+  Buffer<int> d_inc_ptr, d_track_begin, d_damp;
+  Buffer<double> d_Dc, d_Di, d_Ll;  // cyclic reduction: current diagonals, inverses, per-level couplings
+  Buffer<int> d_inc_fac, d_extra;
+  Buffer<double> d_Z, d_S, d_rhs;
+  Buffer<double> d_cost;
+  Buffer<int> d_fail;
+  Buffer<unsigned long long> d_dmax;
   // marginals scratch
-  size_t capX = 0, capW = 0, capQ = 0;
-  double *d_X = nullptr, *d_W = nullptr, *d_cov = nullptr;
-  double *d_Dc = nullptr, *d_Di = nullptr, *d_Ll = nullptr;  // cyclic reduction: current diagonals, inverses, per-level couplings
-  size_t capCR = 0;
-  int *d_qpos = nullptr, *d_qtb = nullptr, *d_qte = nullptr;
+  Buffer<double> d_X, d_W;
+  Buffer<int> d_qpos, d_qtb, d_qte;  // per marginal, with d_cov
+  Buffer<double> d_cov;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
 
@@ -659,14 +663,6 @@ int pg_fail(ls_pg* pg, int code, const char* msg) {
     if (e_ != cudaSuccess) return pg_fail(pg, LS_ERR_CUDA, cudaGetErrorString(e_)); \
   } while (0)
 
-template <typename T>
-int grow(ls_pg* pg, T** p, size_t count) {
-  if (*p) cudaFree(*p);
-  *p = nullptr;
-  PGCU(cudaMalloc((void**)p, count * sizeof(T)));
-  return LS_OK;
-}
-
 }  // namespace
 
 extern "C" {
@@ -681,8 +677,8 @@ int ls_pg_create(int device, ls_pg** out) {
   pg->device = device;
   cudaSetDevice(device);
   if (cudaStreamCreateWithFlags(&pg->stream, cudaStreamNonBlocking) != cudaSuccess) { delete pg; return LS_ERR_CUDA; }
-  if (cudaMalloc((void**)&pg->d_cost, sizeof(double)) != cudaSuccess || cudaMalloc((void**)&pg->d_fail, sizeof(int)) != cudaSuccess ||
-      cudaMalloc((void**)&pg->d_dmax, sizeof(unsigned long long)) != cudaSuccess || cudaEventCreate(&pg->e0) != cudaSuccess ||
+  if (pg->d_cost.reserve(1, 1) != cudaSuccess || pg->d_fail.reserve(1, 1) != cudaSuccess ||
+      pg->d_dmax.reserve(1, 1) != cudaSuccess || cudaEventCreate(&pg->e0) != cudaSuccess ||
       cudaEventCreate(&pg->e1) != cudaSuccess) {
     ls_pg_destroy(pg);
     return LS_ERR_NOMEM;
@@ -695,11 +691,6 @@ void ls_pg_destroy(ls_pg* pg) {
   if (!pg) return;
   cudaSetDevice(pg->device);
   if (pg->stream) cudaStreamSynchronize(pg->stream);
-  void* bufs[] = {pg->d_fac, pg->d_poses, pg->d_Ja, pg->d_Jb, pg->d_r, pg->d_D, pg->d_B, pg->d_g, pg->d_Z,
-                  pg->d_S, pg->d_rhs, pg->d_cost, pg->d_inc_ptr, pg->d_inc_fac, pg->d_extra, pg->d_track_begin, pg->d_fail,
-                  pg->d_dmax, pg->d_damp, pg->d_X, pg->d_W, pg->d_cov, pg->d_qpos, pg->d_qtb, pg->d_qte, pg->d_Dc, pg->d_Di, pg->d_Ll};
-  for (void* b : bufs)
-    if (b) cudaFree(b);
   if (pg->e0) cudaEventDestroy(pg->e0);
   if (pg->e1) cudaEventDestroy(pg->e1);
   if (pg->stream) cudaStreamDestroy(pg->stream);
@@ -883,22 +874,26 @@ int pg_run(ls_pg* pg, int gn_iters, ls_pg_stats* stats, const uint64_t* mkeys, i
   std::vector<double> hp(7 * (size_t)P);
   for (int k = 0; k < P; ++k) std::memcpy(&hp[7 * (size_t)k], &pg->poses[7 * (size_t)order[k]], 7 * sizeof(double));
   // ---- device buffers
-  int rc;
-  if ((size_t)F > pg->capF) {
+  // each group grows all or nothing: when one array fails the group is emptied, so a later call regrows all of it
+  cudaError_t e;
+  if ((size_t)F > pg->d_fac.capacity()) {
     const size_t cap = (size_t)F + F / 4 + 64;
-    if ((rc = grow(pg, &pg->d_fac, cap)) || (rc = grow(pg, &pg->d_Ja, cap * 36)) || (rc = grow(pg, &pg->d_Jb, cap * 36)) ||
-        (rc = grow(pg, &pg->d_r, cap * 6)))
-      return rc;
-    pg->capF = cap;
+    if ((e = pg->d_fac.reserve(cap, cap)) || (e = pg->d_Ja.reserve(cap * 36, cap * 36)) ||
+        (e = pg->d_Jb.reserve(cap * 36, cap * 36)) || (e = pg->d_r.reserve(cap * 6, cap * 6))) {
+      pg->d_fac.reset(), pg->d_Ja.reset(), pg->d_Jb.reset(), pg->d_r.reset();
+      PGCU(e);
+    }
   }
-  if ((size_t)P > pg->capP) {
+  if ((size_t)P > pg->d_poses.capacity() / 7) {
     const size_t cap = (size_t)P + P / 4 + 64;
-    if ((rc = grow(pg, &pg->d_poses, cap * 7)) || (rc = grow(pg, &pg->d_D, cap * 36)) || (rc = grow(pg, &pg->d_B, cap * 36)) ||
-        (rc = grow(pg, &pg->d_g, cap * 6)) ||
-        (rc = grow(pg, &pg->d_inc_ptr, cap + 1)) || (rc = grow(pg, &pg->d_track_begin, cap + 1)) ||
-        (rc = grow(pg, &pg->d_damp, cap + 1)))
-      return rc;
-    pg->capP = cap;
+    if ((e = pg->d_poses.reserve(cap * 7, cap * 7)) || (e = pg->d_D.reserve(cap * 36, cap * 36)) ||
+        (e = pg->d_B.reserve(cap * 36, cap * 36)) || (e = pg->d_g.reserve(cap * 6, cap * 6)) ||
+        (e = pg->d_inc_ptr.reserve(cap + 1, cap + 1)) || (e = pg->d_track_begin.reserve(cap + 1, cap + 1)) ||
+        (e = pg->d_damp.reserve(cap + 1, cap + 1))) {
+      pg->d_poses.reset(), pg->d_D.reset(), pg->d_B.reset(), pg->d_g.reset(), pg->d_inc_ptr.reset(), pg->d_track_begin.reset();
+      pg->d_damp.reset();
+      PGCU(e);
+    }
   }
   // cyclic-reduction levels: level l holds one coupling per node m = j << l, j = 1 .. P >> l
   std::vector<size_t> lvl_off;
@@ -911,38 +906,36 @@ int pg_run(ls_pg* pg, int gn_iters, ls_pg_stats* stats, const uint64_t* mkeys, i
   }
   lvl_off.push_back(lvl_total);
   lvl_total += 2;  // the "next level" slot the top level's (empty) reduction would write
-  if (lvl_total > pg->capCR || (size_t)P > pg->capCR) {
-    const size_t cap = lvl_total + lvl_total / 4 + 64;
-    if ((rc = grow(pg, &pg->d_Dc, cap * 36)) || (rc = grow(pg, &pg->d_Di, cap * 36)) || (rc = grow(pg, &pg->d_Ll, cap * 36))) return rc;
-    pg->capCR = cap;
+  const size_t capCR = pg->d_Dc.capacity() / 36;
+  if (lvl_total > capCR || (size_t)P > capCR) {
+    const size_t cap = (lvl_total + lvl_total / 4 + 64) * 36;
+    if ((e = pg->d_Dc.reserve(cap, cap)) || (e = pg->d_Di.reserve(cap, cap)) || (e = pg->d_Ll.reserve(cap, cap))) {
+      pg->d_Dc.reset(), pg->d_Di.reset(), pg->d_Ll.reset();
+      PGCU(e);
+    }
   }
-  if (inc_fac.size() > pg->capInc) {
-    if ((rc = grow(pg, &pg->d_inc_fac, inc_fac.size() * 2 + 64))) return rc;
-    pg->capInc = inc_fac.size() * 2 + 64;
-  }
-  if ((size_t)E + 1 > pg->capE) {
-    if ((rc = grow(pg, &pg->d_extra, (size_t)E * 2 + 64))) return rc;
-    pg->capE = (size_t)E * 2 + 64;
-  }
+  PGCU(pg->d_inc_fac.reserve(inc_fac.size(), inc_fac.size() * 2 + 64));
+  PGCU(pg->d_extra.reserve((size_t)E + 1, (size_t)E * 2 + 64));
   const size_t needZ = (size_t)P * 6 * ncol;
-  if (needZ > pg->capZ) {
-    if ((rc = grow(pg, &pg->d_Z, needZ + needZ / 4))) return rc;
-    pg->capZ = needZ + needZ / 4;
-  }
+  PGCU(pg->d_Z.reserve(needZ, needZ + needZ / 4));
   const size_t needS = (size_t)n16 * n16 + n16 + 16;
-  if (needS > pg->capS) {
-    if ((rc = grow(pg, &pg->d_S, needS * 2)) || (rc = grow(pg, &pg->d_rhs, (size_t)n16 * 2 + 64))) return rc;
-    pg->capS = needS * 2;
+  if (needS > pg->d_S.capacity()) {
+    const size_t capR = (size_t)n16 * 2 + 64;
+    if ((e = pg->d_S.reserve(needS * 2, needS * 2)) || (e = pg->d_rhs.reserve(capR, capR))) {
+      pg->d_S.reset(), pg->d_rhs.reset();
+      PGCU(e);
+    }
   }
   cudaStream_t st = pg->stream;
-  PGCU(cudaMemcpyAsync(pg->d_fac, fd.data(), (size_t)F * sizeof(FactorDev), cudaMemcpyHostToDevice, st));
-  PGCU(cudaMemcpyAsync(pg->d_poses, hp.data(), hp.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-  PGCU(cudaMemcpyAsync(pg->d_inc_ptr, inc_ptr.data(), inc_ptr.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  PGCU(cudaMemcpyAsync(pg->d_inc_fac, inc_fac.data(), inc_fac.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  if (E) PGCU(cudaMemcpyAsync(pg->d_extra, extra_fac.data(), (size_t)E * sizeof(int), cudaMemcpyHostToDevice, st));
-  PGCU(cudaMemcpyAsync(pg->d_track_begin, track_begin.data(), track_begin.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  PGCU(cudaMemcpyAsync(pg->d_damp, damp.data(), (size_t)P * sizeof(int), cudaMemcpyHostToDevice, st));
-  PGCU(cudaMemsetAsync(pg->d_fail, 0, sizeof(int), st));
+  PGCU(cudaMemcpyAsync(pg->d_fac.get(), fd.data(), (size_t)F * sizeof(FactorDev), cudaMemcpyHostToDevice, st));
+  PGCU(cudaMemcpyAsync(pg->d_poses.get(), hp.data(), hp.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  PGCU(cudaMemcpyAsync(pg->d_inc_ptr.get(), inc_ptr.data(), inc_ptr.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  PGCU(cudaMemcpyAsync(pg->d_inc_fac.get(), inc_fac.data(), inc_fac.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (E) PGCU(cudaMemcpyAsync(pg->d_extra.get(), extra_fac.data(), (size_t)E * sizeof(int), cudaMemcpyHostToDevice, st));
+  PGCU(cudaMemcpyAsync(pg->d_track_begin.get(), track_begin.data(), track_begin.size() * sizeof(int), cudaMemcpyHostToDevice,
+                       st));
+  PGCU(cudaMemcpyAsync(pg->d_damp.get(), damp.data(), (size_t)P * sizeof(int), cudaMemcpyHostToDevice, st));
+  PGCU(cudaMemsetAsync(pg->d_fail.get(), 0, sizeof(int), st));
   cudaEvent_t e0 = pg->e0, e1 = pg->e1;
   cudaEventRecord(e0, st);
   double cost_first = 0.0, cost_last = 0.0, dmax_last = 0.0;
@@ -952,71 +945,82 @@ int pg_run(ls_pg* pg, int gn_iters, ls_pg_stats* stats, const uint64_t* mkeys, i
       const long long sl = 1ll << l;
       const int n_elim = (int)((P - sl) / (2 * sl)) + 1, n_keep = (int)(P / (2 * sl));
       if (n_elim > kMaxGridY)
-        cr_fwd_elim_kernel<true><<<dim3((ncols + 127) / 128, kMaxGridY), 128, 0, st>>>(P, (int)sl, ncols, pg->d_Di, buf);
+        cr_fwd_elim_kernel<true><<<dim3((ncols + 127) / 128, kMaxGridY), 128, 0, st>>>(P, (int)sl, ncols, pg->d_Di.get(), buf);
       else
-        cr_fwd_elim_kernel<false><<<dim3((ncols + 127) / 128, n_elim), 128, 0, st>>>(P, (int)sl, ncols, pg->d_Di, buf);
+        cr_fwd_elim_kernel<false><<<dim3((ncols + 127) / 128, n_elim), 128, 0, st>>>(P, (int)sl, ncols, pg->d_Di.get(), buf);
       if (n_keep > kMaxGridY)
-        cr_fwd_keep_kernel<true><<<dim3((ncols + 127) / 128, kMaxGridY), 128, 0, st>>>(P, (int)sl, l, ncols, pg->d_Ll + 36 * lvl_off[l], buf);
+        cr_fwd_keep_kernel<true><<<dim3((ncols + 127) / 128, kMaxGridY), 128, 0, st>>>(P, (int)sl, l, ncols,
+                                                                                       pg->d_Ll.get() + 36 * lvl_off[l], buf);
       else if (n_keep > 0)
-        cr_fwd_keep_kernel<false><<<dim3((ncols + 127) / 128, n_keep), 128, 0, st>>>(P, (int)sl, l, ncols, pg->d_Ll + 36 * lvl_off[l], buf);
+        cr_fwd_keep_kernel<false><<<dim3((ncols + 127) / 128, n_keep), 128, 0, st>>>(P, (int)sl, l, ncols,
+                                                                                     pg->d_Ll.get() + 36 * lvl_off[l], buf);
       pg->launches += n_keep > 0 ? 2 : 1;
     }
     for (int l = n_levels - 1; l >= 0; --l) {
       const long long sl = 1ll << l;
       const int n_elim = (int)((P - sl) / (2 * sl)) + 1;
       if (n_elim > kMaxGridY)
-        cr_bwd_kernel<true><<<dim3((ncols + 127) / 128, kMaxGridY), 128, 0, st>>>(P, (int)sl, l, ncols, pg->d_Di, pg->d_Ll + 36 * lvl_off[l], buf);
+        cr_bwd_kernel<true><<<dim3((ncols + 127) / 128, kMaxGridY), 128, 0, st>>>(P, (int)sl, l, ncols, pg->d_Di.get(),
+                                                                                  pg->d_Ll.get() + 36 * lvl_off[l], buf);
       else
-        cr_bwd_kernel<false><<<dim3((ncols + 127) / 128, n_elim), 128, 0, st>>>(P, (int)sl, l, ncols, pg->d_Di, pg->d_Ll + 36 * lvl_off[l], buf);
+        cr_bwd_kernel<false><<<dim3((ncols + 127) / 128, n_elim), 128, 0, st>>>(P, (int)sl, l, ncols, pg->d_Di.get(),
+                                                                                pg->d_Ll.get() + 36 * lvl_off[l], buf);
       ++pg->launches;
     }
   };
   const int n_pass = gn_iters + (n_mk > 0 ? 1 : 0);  // the last pass of a marginals request only linearises and factors
   for (int it = 0; it < n_pass; ++it) {
     const bool update = it < gn_iters;
-    PGCU(cudaMemsetAsync(pg->d_cost, 0, sizeof(double), st));
-    PGCU(cudaMemsetAsync(pg->d_dmax, 0, sizeof(unsigned long long), st));
-    pg_linearize_kernel<<<(F + 127) / 128, 128, 0, st>>>(F, pg->d_fac, pg->d_poses, pg->d_Ja, pg->d_Jb, pg->d_r, pg->d_cost);
-    pg_assemble_kernel<<<(P + 127) / 128, 128, 0, st>>>(P, pg->d_inc_ptr, pg->d_inc_fac, pg->d_fac, pg->d_Ja, pg->d_Jb, pg->d_r,
-                                                        pg->d_damp, pg->d_D, pg->d_B, pg->d_g);
+    PGCU(cudaMemsetAsync(pg->d_cost.get(), 0, sizeof(double), st));
+    PGCU(cudaMemsetAsync(pg->d_dmax.get(), 0, sizeof(unsigned long long), st));
+    pg_linearize_kernel<<<(F + 127) / 128, 128, 0, st>>>(F, pg->d_fac.get(), pg->d_poses.get(), pg->d_Ja.get(), pg->d_Jb.get(),
+                                                         pg->d_r.get(), pg->d_cost.get());
+    pg_assemble_kernel<<<(P + 127) / 128, 128, 0, st>>>(P, pg->d_inc_ptr.get(), pg->d_inc_fac.get(), pg->d_fac.get(),
+                                                        pg->d_Ja.get(), pg->d_Jb.get(), pg->d_r.get(),
+                                                        pg->d_damp.get(), pg->d_D.get(), pg->d_B.get(), pg->d_g.get());
     // H_c^-1 [ -g | U^T ] by block cyclic reduction (K6a'): factor the levels, then every right-hand side through them
-    cr_init_kernel<<<(P + 127) / 128, 128, 0, st>>>(P, pg->d_D, pg->d_B, pg->d_Dc, pg->d_Ll + 36 * lvl_off[0]);
+    cr_init_kernel<<<(P + 127) / 128, 128, 0, st>>>(P, pg->d_D.get(), pg->d_B.get(), pg->d_Dc.get(),
+                                                    pg->d_Ll.get() + 36 * lvl_off[0]);
     for (int l = 0; l < n_levels; ++l) {
       const long long sl = 1ll << l;
       const int n_elim = (int)((P - sl) / (2 * sl)) + 1, n_keep = (int)(P / (2 * sl));
-      cr_invert_kernel<<<(n_elim + 63) / 64, 64, 0, st>>>(P, (int)sl, pg->d_Dc, pg->d_Di, pg->d_fail);
+      cr_invert_kernel<<<(n_elim + 63) / 64, 64, 0, st>>>(P, (int)sl, pg->d_Dc.get(), pg->d_Di.get(), pg->d_fail.get());
       if (n_keep > 0)
-        cr_reduce_kernel<<<(n_keep + 63) / 64, 64, 0, st>>>(P, (int)sl, l, pg->d_Dc, pg->d_Di, pg->d_Ll + 36 * lvl_off[l],
-                                                            pg->d_Ll + 36 * lvl_off[l + 1]);
+        cr_reduce_kernel<<<(n_keep + 63) / 64, 64, 0, st>>>(P, (int)sl, l, pg->d_Dc.get(), pg->d_Di.get(),
+                                                            pg->d_Ll.get() + 36 * lvl_off[l],
+                                                            pg->d_Ll.get() + 36 * lvl_off[l + 1]);
       pg->launches += n_keep > 0 ? 2 : 1;
     }
-    PGCU(cudaMemsetAsync(pg->d_Z, 0, (size_t)P * 6 * ncol * sizeof(double), st));
-    cr_rhs_kernel<<<dim3((ncol + 127) / 128, 256), 128, 0, st>>>(P, ncol, pg->d_fac, pg->d_extra, pg->d_Ja, pg->d_Jb, pg->d_g, pg->d_Z);
-    cr_solve(pg->d_Z, ncol);
+    PGCU(cudaMemsetAsync(pg->d_Z.get(), 0, (size_t)P * 6 * ncol * sizeof(double), st));
+    cr_rhs_kernel<<<dim3((ncol + 127) / 128, 256), 128, 0, st>>>(P, ncol, pg->d_fac.get(), pg->d_extra.get(), pg->d_Ja.get(),
+                                                                 pg->d_Jb.get(), pg->d_g.get(), pg->d_Z.get());
+    cr_solve(pg->d_Z.get(), ncol);
     pg->launches += 4;
     if (E) {
-      pg_border_kernel<<<dim3((n16 + 1 + 127) / 128, n16), 128, 0, st>>>(n, n16, ncol, pg->d_fac, pg->d_extra, pg->d_Ja, pg->d_Jb,
-                                                                        pg->d_Z, pg->d_S, pg->d_rhs);
+      pg_border_kernel<<<dim3((n16 + 1 + 127) / 128, n16), 128, 0, st>>>(n, n16, ncol, pg->d_fac.get(), pg->d_extra.get(),
+                                                                         pg->d_Ja.get(), pg->d_Jb.get(),
+                                                                        pg->d_Z.get(), pg->d_S.get(), pg->d_rhs.get());
       ++pg->launches;
       for (int p = 0; p < n16; p += NB) {
-        dense_panel_kernel<<<1, 256, 0, st>>>(n16, p, pg->d_S);
+        dense_panel_kernel<<<1, 256, 0, st>>>(n16, p, pg->d_S.get());
         const int rem = (n16 - p - NB) / NB;
-        if (rem > 0) dense_update_kernel<<<dim3(rem, rem), dim3(NB, NB), 0, st>>>(n16, p, pg->d_S);
+        if (rem > 0) dense_update_kernel<<<dim3(rem, rem), dim3(NB, NB), 0, st>>>(n16, p, pg->d_S.get());
         pg->launches += rem > 0 ? 2 : 1;
       }
       if (update) {
-        dense_solve_kernel<<<1, 1024, 0, st>>>(n16, pg->d_S, pg->d_rhs);
+        dense_solve_kernel<<<1, 1024, 0, st>>>(n16, pg->d_S.get(), pg->d_rhs.get());
         ++pg->launches;
       }
     }
     if (!update) break;
-    pg_update_kernel<<<(P * 32 + 255) / 256, 256, 0, st>>>(P, ncol, pg->d_Z, pg->d_rhs, pg->d_poses, pg->d_dmax);
+    pg_update_kernel<<<(P * 32 + 255) / 256, 256, 0, st>>>(P, ncol, pg->d_Z.get(), pg->d_rhs.get(), pg->d_poses.get(),
+                                                           pg->d_dmax.get());
     ++pg->launches;
     if (it == 0 || it == gn_iters - 1) {
       double c;
       unsigned long long dm;
-      PGCU(cudaMemcpyAsync(&c, pg->d_cost, sizeof(double), cudaMemcpyDeviceToHost, st));
-      PGCU(cudaMemcpyAsync(&dm, pg->d_dmax, sizeof(dm), cudaMemcpyDeviceToHost, st));
+      PGCU(cudaMemcpyAsync(&c, pg->d_cost.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
+      PGCU(cudaMemcpyAsync(&dm, pg->d_dmax.get(), sizeof(dm), cudaMemcpyDeviceToHost, st));
       PGCU(cudaStreamSynchronize(st));
       if (it == 0) cost_first = c;
       cost_last = c;
@@ -1036,40 +1040,43 @@ int pg_run(ls_pg* pg, int gn_iters, ls_pg_stats* stats, const uint64_t* mkeys, i
     }
     const int ncm = 6 * kChunk;
     const size_t needX = (size_t)P * 6 * ncm, needW = (size_t)(n16 > 0 ? n16 : 1) * ncm;
-    if (needX > pg->capX) { if ((rc = grow(pg, &pg->d_X, needX))) return rc; pg->capX = needX; }
-    if (needW > pg->capW) { if ((rc = grow(pg, &pg->d_W, needW))) return rc; pg->capW = needW; }
-    if ((size_t)n_mk > pg->capQ) {
+    PGCU(pg->d_X.reserve(needX, needX));
+    PGCU(pg->d_W.reserve(needW, needW));
+    if ((size_t)n_mk > pg->d_qpos.capacity()) {
       const size_t cap = (size_t)n_mk + 64;
-      if ((rc = grow(pg, &pg->d_qpos, cap)) || (rc = grow(pg, &pg->d_qtb, cap)) || (rc = grow(pg, &pg->d_qte, cap)) ||
-          (rc = grow(pg, &pg->d_cov, cap * 36)))
-        return rc;
-      pg->capQ = cap;
+      if ((e = pg->d_qpos.reserve(cap, cap)) || (e = pg->d_qtb.reserve(cap, cap)) || (e = pg->d_qte.reserve(cap, cap)) ||
+          (e = pg->d_cov.reserve(cap * 36, cap * 36))) {
+        pg->d_qpos.reset(), pg->d_qtb.reset(), pg->d_qte.reset(), pg->d_cov.reset();
+        PGCU(e);
+      }
     }
-    PGCU(cudaMemcpyAsync(pg->d_qpos, qpos.data(), (size_t)n_mk * sizeof(int), cudaMemcpyHostToDevice, st));
-    PGCU(cudaMemcpyAsync(pg->d_qtb, qtb.data(), (size_t)n_mk * sizeof(int), cudaMemcpyHostToDevice, st));
-    PGCU(cudaMemcpyAsync(pg->d_qte, qte.data(), (size_t)n_mk * sizeof(int), cudaMemcpyHostToDevice, st));
+    PGCU(cudaMemcpyAsync(pg->d_qpos.get(), qpos.data(), (size_t)n_mk * sizeof(int), cudaMemcpyHostToDevice, st));
+    PGCU(cudaMemcpyAsync(pg->d_qtb.get(), qtb.data(), (size_t)n_mk * sizeof(int), cudaMemcpyHostToDevice, st));
+    PGCU(cudaMemcpyAsync(pg->d_qte.get(), qte.data(), (size_t)n_mk * sizeof(int), cudaMemcpyHostToDevice, st));
     for (int q0 = 0; q0 < n_mk; q0 += kChunk) {
       const int nq = n_mk - q0 < kChunk ? n_mk - q0 : kChunk, nc = 6 * nq;
-      PGCU(cudaMemsetAsync(pg->d_X, 0, (size_t)P * 6 * nc * sizeof(double), st));
-      cr_unit_rhs_kernel<<<(nc + 127) / 128, 128, 0, st>>>(nc, pg->d_qpos + q0, pg->d_X);
+      PGCU(cudaMemsetAsync(pg->d_X.get(), 0, (size_t)P * 6 * nc * sizeof(double), st));
+      cr_unit_rhs_kernel<<<(nc + 127) / 128, 128, 0, st>>>(nc, pg->d_qpos.get() + q0, pg->d_X.get());
       ++pg->launches;
-      cr_solve(pg->d_X, nc);
+      cr_solve(pg->d_X.get(), nc);
       if (E) {
-        pg_border_rhs_kernel<<<dim3((nc + 127) / 128, n16), 128, 0, st>>>(n, n16, nc, pg->d_fac, pg->d_extra, pg->d_Ja, pg->d_Jb,
-                                                                          pg->d_qtb + q0, pg->d_qte + q0, pg->d_X, pg->d_W);
-        dense_solve_multi_kernel<<<(nc + 63) / 64, 64, 0, st>>>(n16, nc, pg->d_S, pg->d_W);
+        pg_border_rhs_kernel<<<dim3((nc + 127) / 128, n16), 128, 0, st>>>(n, n16, nc, pg->d_fac.get(), pg->d_extra.get(),
+                                                                          pg->d_Ja.get(), pg->d_Jb.get(), pg->d_qtb.get() + q0,
+                                                                          pg->d_qte.get() + q0, pg->d_X.get(), pg->d_W.get());
+        dense_solve_multi_kernel<<<(nc + 63) / 64, 64, 0, st>>>(n16, nc, pg->d_S.get(), pg->d_W.get());
         pg->launches += 2;
       }
-      pg_marginal_block_kernel<<<(nq * 36 + 127) / 128, 128, 0, st>>>(nq, nc, E ? n : 0, ncol, pg->d_qpos + q0, pg->d_X, pg->d_Z,
-                                                                      pg->d_W, pg->d_cov + 36 * (size_t)q0);
+      pg_marginal_block_kernel<<<(nq * 36 + 127) / 128, 128, 0, st>>>(nq, nc, E ? n : 0, ncol, pg->d_qpos.get() + q0,
+                                                                      pg->d_X.get(), pg->d_Z.get(),
+                                                                      pg->d_W.get(), pg->d_cov.get() + 36 * (size_t)q0);
       ++pg->launches;
     }
-    PGCU(cudaMemcpyAsync(cov_out, pg->d_cov, (size_t)n_mk * 36 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    PGCU(cudaMemcpyAsync(cov_out, pg->d_cov.get(), (size_t)n_mk * 36 * sizeof(double), cudaMemcpyDeviceToHost, st));
   }
   cudaEventRecord(e1, st);
   int fail = 0;
-  PGCU(cudaMemcpyAsync(&fail, pg->d_fail, sizeof(int), cudaMemcpyDeviceToHost, st));
-  PGCU(cudaMemcpyAsync(hp.data(), pg->d_poses, hp.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  PGCU(cudaMemcpyAsync(&fail, pg->d_fail.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
+  PGCU(cudaMemcpyAsync(hp.data(), pg->d_poses.get(), hp.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
   PGCU(cudaStreamSynchronize(st));
   PGCU(cudaGetLastError());
   float ms = 0.f;

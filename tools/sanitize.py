@@ -86,4 +86,9 @@ for got, want in ((om.cell_status(qs), qo.cell_status(qs)), (om.line_status(qs, 
                   (om.cast_rays(qorg, qd, True, 10.0), qo.cast_rays(qorg, qd, True, 10.0))):
     assert np.array_equal(got[0], want[0]) and np.array_equal(np.asarray(got[1]).view(np.uint8), np.asarray(want[1]).view(np.uint8))
 om.close()
-print("sanitize workload ok:", g["stats"].iterations, "iterations;", len(batch), "batched problems;", ctx.launch_count, "launches")
+launches = ctx.launch_count
+# every handle closed, so a leak check sees only what the library failed to free
+mp.close()
+ctx.close()
+G.close()
+print("sanitize workload ok:", g["stats"].iterations, "iterations;", len(batch), "batched problems;", launches, "launches")
