@@ -50,6 +50,10 @@ class OccupancyMap {
   // octomap's OcTree::writeBinary: the map's max-likelihood states, pruned, as a .bt file (ls_occupancy_write_octomap).
   // Returns false when the file cannot be written.
   bool writeBinary(const std::string& filename);
+  // octomap's OcTree::readBinary: the .bt file replaces the map, its resolution becomes the map's, free leaves load as
+  // clamping_thres_min and occupied ones as clamping_thres_max (ls_occupancy_read_octomap).  Returns false, with the map
+  // unchanged, when the file cannot be read, is malformed or covers more than the map can hold.
+  bool readBinary(const std::string& filename);
   // The occupied leaves of the pruned tree in octomap's leaf order, features only ({x, y, z, 1}): what
   // octomap_to_point_cloud writes from writeBinary's file.
   void getOccupiedLeafCloud(DataPoints* cloud);

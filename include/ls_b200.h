@@ -406,6 +406,29 @@ int ls_occupancy_download_octree(ls_occupancy* om, uint8_t* payload, int64_t pay
  * then the payload.  Builds the tree unless the last build is current.  stats may be NULL. */
 int ls_occupancy_write_octomap(ls_occupancy* om, const char* path, ls_octree_stats* stats);
 
+/* octomap's OcTree::readBinary into the map (DESIGN.md §4b'''''').  A read replaces the map: the file's
+ * resolution becomes the map's (hit, miss, clamps, threshold and max range stay), and every voxel below a free leaf becomes
+ * known with L_min (the clamp_min log-odds), below an occupied leaf with L_max; the rest is unknown.  Unpruned files and
+ * inner nodes without children are accepted.  With clamp_min < occupancy_threshold <= clamp_max (the defaults) writing the
+ * loaded map gives the file's bytes again.  The parse and the expansion run on the device, on the map's stream; the call
+ * is synchronous, invalidates the last octree build on success and is legal between ls_icp_register_submap_batch_begin and
+ * _end.  Errors: LS_ERR_ARG for a bad header, a truncated payload, an inner node at depth 16, a size that does not count
+ * the payload's nodes or a resolution that is not finite and > 0 (bytes after the tree are ignored); LS_ERR_NOMEM, before
+ * the map grows, when the file covers more bricks than the map can index (2^29), or when it cannot grow.  The map, its
+ * resolution and a current octree build are unchanged after any error. */
+typedef struct ls_octomap_read_stats {
+  int64_t nodes, inner_nodes, free_leaves, occupied_leaves;
+  int64_t known_voxels, bricks; /* of the map after the read */
+  double resolution;            /* the map's resolution after the read */
+  float device_ms;              /* the read on the map's stream, the payload's upload included */
+} ls_octomap_read_stats;
+/* payload: the bytes after "data\n" (payload_bytes of them; NULL when 0); nodes: the header's size (>= 0).  stats may be
+ * NULL. */
+int ls_occupancy_read_octree(ls_occupancy* om, const uint8_t* payload, int64_t payload_bytes, int64_t nodes,
+                             double resolution, ls_octomap_read_stats* stats);
+/* The whole .bt file at `path`: its header is parsed on the host as laser_slam_b200.read_octomap parses it, then as above. */
+int ls_occupancy_read_octomap(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats);
+
 /* Queries of the map: volumetric_mapping's WorldBase (getCellStatusPoint, getLineStatus, getVisibility,
  * getLineStatusBoundingBox) and octomap's castRay, batched, one device thread per query.  The rules (oracle/QUERIES.md):
  *   cell        the key of the double point (octomap's search(x, y, z): floor(c * (1/resolution)) + 32768, no float cast);

@@ -102,6 +102,13 @@ class OctreeStats(ctypes.Structure):
                 ("device_ms", ctypes.c_float)]
 
 
+class OctomapReadStats(ctypes.Structure):
+    """ls_octomap_read_stats: the file's node counts, the map's known voxels, bricks and resolution after the read."""
+    _fields_ = [("nodes", ctypes.c_int64), ("inner_nodes", ctypes.c_int64), ("free_leaves", ctypes.c_int64),
+                ("occupied_leaves", ctypes.c_int64), ("known_voxels", ctypes.c_int64), ("bricks", ctypes.c_int64),
+                ("resolution", ctypes.c_double), ("device_ms", ctypes.c_float)]
+
+
 class OccupancyQueryStats(ctypes.Structure):
     _fields_ = [("keys_visited", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
@@ -214,6 +221,9 @@ def lib():
         L.ls_occupancy_build_octree.argtypes = [vp, ctypes.POINTER(OctreeStats)]
         L.ls_occupancy_download_octree.argtypes = [vp, vp, ctypes.c_int64, vp, vp, ctypes.c_int64]
         L.ls_occupancy_write_octomap.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(OctreeStats)]
+        L.ls_occupancy_read_octree.argtypes = [vp, vp, ctypes.c_int64, ctypes.c_int64, ctypes.c_double,
+                                               ctypes.POINTER(OctomapReadStats)]
+        L.ls_occupancy_read_octomap.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(OctomapReadStats)]
         QS = ctypes.POINTER(OccupancyQueryStats)
         L.ls_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp, QS]
         L.ls_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, vp, vp, QS]
@@ -891,6 +901,25 @@ class OccupancyMap:
         pts = self.octree().centres[:, :3]
         write_point_cloud(path, pts)
         return len(pts)
+
+    def read_octomap(self, path):
+        """octomap's readBinary of a .bt file into this map, replacing it (ls_occupancy_read_octomap): free leaves load as
+        clamp_min, occupied ones as clamp_max, and the file's resolution becomes the map's (self.params.resolution).
+        Returns OctomapReadStats; on an error the map is unchanged."""
+        st = OctomapReadStats()
+        self.ctx._check(lib().ls_occupancy_read_octomap(self._h, os.fsencode(path), ctypes.byref(st)))
+        self.params.resolution = st.resolution
+        return st
+
+    def read_octree(self, payload, nodes, resolution):
+        """As read_octomap, from a payload in memory (the bytes after "data\\n", as an octomap_msgs binary message carries
+        them), the node count of its size line and its resolution."""
+        buf = np.frombuffer(bytes(payload), np.uint8)
+        st = OctomapReadStats()
+        self.ctx._check(lib().ls_occupancy_read_octree(self._h, buf.ctypes.data if len(buf) else None, len(buf), int(nodes),
+                                                       float(resolution), ctypes.byref(st)))
+        self.params.resolution = st.resolution
+        return st
 
     # ---- queries (ls_occupancy_cell_status / _line_status / _cast_rays); self.last_query holds the last call's stats
     def cell_status(self, points):

@@ -1,5 +1,6 @@
 // C-ABI implementation (include/ls_b200.h): context, device memory, kernel launches.
 // There is no CPU fallback anywhere in this file: every entry point needs a live CUDA device.
+#include <cerrno>
 #include <cmath>
 #include <cstdarg>
 #include <cstddef>
@@ -1758,6 +1759,53 @@ void octree_stats(const ls_occupancy* om, ls_octree_stats* stats) {
   stats->occupied_leaves = om->tree.leaves;
   stats->device_ms = om->tree_ms;
 }
+
+// A .bt header as laser_slam_b200.read_octomap parses it: the first line exactly (a trailing \r dropped), then "#" and
+// blank lines skipped, "key value" lines, up to "data"; id OcTree, an integer size >= 0 and a res.  *off: the payload's
+// first byte.  NULL when it is valid, else why not.
+const char* parse_bt_header(const std::vector<uint8_t>& d, size_t* off, long long* nodes, double* res) {
+  size_t pos = 0;
+  std::string line;
+  auto next = [&]() {
+    const uint8_t* nl = static_cast<const uint8_t*>(std::memchr(d.data() + pos, '\n', d.size() - pos));
+    if (!nl) return false;
+    const size_t end = (size_t)(nl - d.data());
+    line.assign(reinterpret_cast<const char*>(d.data()) + pos, end - pos);
+    pos = end + 1;
+    while (!line.empty() && line.back() == '\r') line.pop_back();
+    return true;
+  };
+  auto strip = [](const std::string& s) {
+    const char* ws = " \t\n\r\v\f";
+    const size_t a = s.find_first_not_of(ws);
+    return a == std::string::npos ? std::string() : s.substr(a, s.find_last_not_of(ws) + 1 - a);
+  };
+  if (d.empty() || !next()) return "header ends early";
+  if (line != "# Octomap OcTree binary file") return "not an octomap binary file (first line)";
+  std::string id, size, resolution;
+  bool have_id = false, have_size = false, have_res = false;
+  for (;;) {
+    if (!next()) return "header ends early";
+    if ((!line.empty() && line[0] == '#') || strip(line).empty()) continue;
+    if (line == "data") break;
+    const size_t sp = line.find(' ');
+    const std::string key = line.substr(0, sp), value = sp == std::string::npos ? std::string() : strip(line.substr(sp + 1));
+    if (key == "id") id = value, have_id = true;
+    if (key == "size") size = value, have_size = true;
+    if (key == "res") resolution = value, have_res = true;
+  }
+  if (!have_id || id != "OcTree") return "tree type is not OcTree";
+  if (!have_size || !have_res || size.empty() || resolution.empty()) return "bad or missing size / res line";
+  char* e = nullptr;
+  errno = 0;
+  const long long n = std::strtoll(size.c_str(), &e, 10);
+  if (*e != '\0' || errno == ERANGE) return "bad or missing size / res line";
+  const double r = std::strtod(resolution.c_str(), &e);
+  if (*e != '\0') return "bad or missing size / res line";
+  if (n < 0) return "negative size";
+  *off = pos, *nodes = n, *res = r;
+  return nullptr;
+}
 }  // namespace
 
 extern "C" {
@@ -1928,6 +1976,64 @@ int ls_occupancy_write_octomap(ls_occupancy* om, const char* path, ls_octree_sta
   if (!ok) return fail(ctx, LS_ERR_ARG, "writing %s failed", path);
   octree_stats(om, stats);
   return LS_OK;
+}
+
+int ls_occupancy_read_octree(ls_occupancy* om, const uint8_t* payload, int64_t payload_bytes, int64_t nodes,
+                             double resolution, ls_octomap_read_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (nodes < 0 || payload_bytes < 0 || (payload_bytes > 0 && !payload)) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!(resolution > 0.0) || !std::isfinite(resolution))
+    return fail(ctx, LS_ERR_ARG, "octomap resolution %g (finite and > 0)", resolution);
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  lso::Params P = om->prm;
+  P.res = resolution;
+  P.inv = 1.0 / resolution;
+  lso::ReadCounters c;
+  const char* why = "";
+  const int rc = lso::read_octree(om->map, P, payload, payload_bytes, nodes, &c, &why, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "octomap read refused, the map is unchanged: %s", why);
+  om->prm = P;
+  om->tree_current = false;
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    stats->nodes = (int64_t)c.nodes;
+    stats->inner_nodes = (int64_t)c.inner;
+    stats->free_leaves = (int64_t)c.free_leaves;
+    stats->occupied_leaves = (int64_t)c.occ_leaves;
+    stats->known_voxels = om->map.n_known;
+    stats->bricks = om->map.pool_n;
+    stats->resolution = P.res;
+    stats->device_ms = ms;
+  }
+  return LS_OK;
+}
+
+int ls_occupancy_read_octomap(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
+  std::vector<uint8_t> data;
+  {
+    FILE* f = std::fopen(path, "rb");
+    if (!f) return fail(ctx, LS_ERR_ARG, "cannot open %s", path);
+    uint8_t buf[1 << 16];
+    size_t got;
+    while ((got = std::fread(buf, 1, sizeof buf, f)) > 0) data.insert(data.end(), buf, buf + got);
+    const bool err = std::ferror(f) != 0;
+    std::fclose(f);
+    if (err) return fail(ctx, LS_ERR_ARG, "reading %s failed", path);
+  }
+  size_t off = 0;
+  long long nodes = 0;
+  double res = 0.0;
+  const char* why = parse_bt_header(data, &off, &nodes, &res);
+  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
+  return ls_occupancy_read_octree(om, data.data() + off, (int64_t)(data.size() - off), nodes, res, stats);
 }
 
 }  // extern "C"

@@ -23,7 +23,23 @@
 //   (h) oct_emit_kernel      one block per inner brick: (e)'s tree again, its pre-order bytes and occupied leaves written at
 //                            the offsets (g) gave it, so no per-brick staging is kept
 // A brick without a known voxel (an insert that failed after placing it leaves one) has state 0 and adds nothing.
+//
+// .bt read (octomap's readBinary; DESIGN.md §4b''''''), replacing the map.  The payload is uploaded once and
+// parsed without a walk, one thread per pair (= inner node):
+//   (r1) rd_excess_kernel + a CUB scan   the excess E_i of each pair: inner nodes found but not yet read
+//   (r2) rd_end_kernel                   the tree's end (the first E_i = 0) and each block's least excess
+//   (r3) rd_parent_kernel                each inner node's parent (the last earlier pair with E <= its own) and slot
+//   (r4) rd_node_kernel                  depth and first key (at most 15 parents up), the depth-13 ancestor, and the
+//                                        counts: nodes, leaves, known voxels and bricks; a CUB scan gives each inner node
+//                                        its first brick, so the bricks are numbered in pre-order with no deduplication
+//   one readback validates the stream, checks the size line and the brick bound, and sizes the pool
+//   (r5) rd_brick_kernel                 each new brick's key and state (uniform free / occupied, or mixed)
+//   the hash is built from those keys beside the old one, so a failure up to here leaves the map as it was
+//   (r6) rd_fill_kernel                  one block per brick: uniform bricks written whole, mixed ones cleared
+//   (r7) rd_leaf_kernel                  the voxels of each leaf at depth 14 ... 16, each written once
+#include <algorithm>
 #include <cfloat>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -886,6 +902,221 @@ __global__ void __launch_bounds__(512) oct_emit_kernel(const unsigned* __restric
   }
 }
 
+// ---- .bt read (octomap's readBinary; DESIGN.md §4b'''''') ------------------------------------------------
+// Pair i of the payload is the i-th inner node in pre-order.  With c_i its inner children, the excess E_0 = 1,
+// E_{i+1} = E_i + c_i - 1 counts the inner nodes found but not yet read; the tree ends at the first i >= 1 with E_i = 0.
+constexpr int kReadThreads = 256;
+constexpr int kMaxInnerExcess = 8 + 7 * 14;      // the largest excess of a tree whose inner nodes lie at depth <= 15
+constexpr long long kMaxReadBricks = 1LL << 29;  // a hash of at most 2^30 slots at load <= 1/2
+constexpr long long kMaxReadPairs = 1LL << 30;
+constexpr int kBadDepth = 1;
+
+struct MinOp {
+  __device__ __forceinline__ int operator()(int a, int b) const { return a < b ? a : b; }
+};
+
+__device__ __forceinline__ int pair_mask(const unsigned char* pay, int i) {
+  return (int)pay[2 * (size_t)i] | ((int)pay[2 * (size_t)i + 1] << 8);
+}
+__device__ __forceinline__ int inner_children(int mask) {
+  int c = 0;
+  for (int s = 0; s < 8; ++s) c += ((mask >> (2 * s)) & 3) == 3;
+  return c;
+}
+
+// (r1) in[0] = 1 and in[i + 1] = c_i - 1: an inclusive sum gives E_0 ... E_n
+__global__ void rd_excess_kernel(const unsigned char* __restrict__ pay, int n, int* __restrict__ in) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) in[0] = 1;
+  if (i < n) in[i + 1] = inner_children(pair_mask(pay, i)) - 1;
+}
+
+// (r2) the tree's end and, per block of kReadThreads pairs, the least excess (r3) skips blocks by
+__global__ void __launch_bounds__(kReadThreads) rd_end_kernel(const int* __restrict__ ex, int n, int* __restrict__ bmin,
+                                                             ReadCounters* cnt) {
+  using Reduce = cub::BlockReduce<int, kReadThreads>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int e = i <= n ? ex[i] : INT_MAX;
+  if (i >= 1 && i <= n && e == 0) atomicMin(&cnt->end, i);
+  const int m = Reduce(tmp).Reduce(e, MinOp());
+  if (threadIdx.x == 0) bmin[blockIdx.x] = m;
+}
+
+// (r3) per inner node j >= 1 of the tree: its parent, the last i < j with E_i <= E_j, and its slot, the child index of the
+// (E_p + c_p - 1 - E_j)-th inner child of p.  An excess above kMaxInnerExcess proves an inner node at depth 16.
+__global__ void rd_parent_kernel(const unsigned char* __restrict__ pay, const int* __restrict__ ex,
+                                 const int* __restrict__ bmin, int n, int* __restrict__ par, unsigned char* __restrict__ slot,
+                                 ReadCounters* cnt) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n || j >= cnt->end) return;
+  const int e = ex[j];
+  if (e > kMaxInnerExcess) {
+    atomicOr(&cnt->bad, kBadDepth);
+    return;
+  }
+  if (j == 0) {
+    par[0] = -1, slot[0] = 0;
+    return;
+  }
+  const int b0 = j / kReadThreads * kReadThreads;
+  int p = j - 1;
+  while (p >= b0 && ex[p] > e) --p;
+  if (p < b0) {  // E_0 = 1 <= e: some earlier block holds the parent
+    int b = j / kReadThreads - 1;
+    while (bmin[b] > e) --b;
+    p = b * kReadThreads + kReadThreads - 1;
+    while (ex[p] > e) --p;
+  }
+  const int m = pair_mask(pay, p);
+  int rank = ex[p] + inner_children(m) - 1 - e, s = 0;
+  for (; s < 8; ++s)
+    if (((m >> (2 * s)) & 3) == 3 && rank-- == 0) break;
+  par[j] = p;
+  slot[j] = (unsigned char)s;
+}
+
+// (r4) per inner node j of the tree: depth and first key from at most 15 parents (more: an inner node at depth 16), its
+// depth-13 ancestor, and its children's counts: nodes, leaves, known voxels 8^(16-d) and bricks 8^(13-d) per leaf at depth
+// d (d <= 13), one brick for the node itself at depth 13.  nb[j] = its bricks (0 past the tree, nb[n] = 0).
+__global__ void __launch_bounds__(kReadThreads) rd_node_kernel(const unsigned char* __restrict__ pay,
+                                                              const int* __restrict__ par,
+                                                              const unsigned char* __restrict__ slot, int n,
+                                                              unsigned char* __restrict__ depth,
+                                                              unsigned long long* __restrict__ key, int* __restrict__ anc,
+                                                              long long* __restrict__ nb, ReadCounters* cnt) {
+  using Reduce = cub::BlockReduce<unsigned long long, kReadThreads>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long v[4] = {0, 0, 0, 0};  // child nodes, free leaves, occupied leaves, known voxels
+  long long bricks = 0;
+  if (j < n && j < cnt->end && !cnt->bad) {
+    // step i visits the ancestor at depth d - i: its slot is key bit 16 - d + i; the depth-13 one is among steps 0 ... 2
+    int d = 0, x = j, a1 = j, a2 = j;
+    unsigned long long slots = 0;
+    while (x != 0 && d < 15) {
+      if (d == 1) a1 = x;
+      if (d == 2) a2 = x;
+      slots |= (unsigned long long)slot[x] << (3 * d);
+      ++d;
+      x = par[x];
+    }
+    if (x != 0) {
+      atomicOr(&cnt->bad, kBadDepth);
+    } else {
+      unsigned kx = 0, ky = 0, kz = 0;
+      for (int i = 0; i < d; ++i) {
+        const unsigned s = (unsigned)(slots >> (3 * i)) & 7u, b = (unsigned)(16 - d + i);
+        kx |= (s & 1u) << b, ky |= ((s >> 1) & 1u) << b, kz |= ((s >> 2) & 1u) << b;
+      }
+      depth[j] = (unsigned char)d;
+      key[j] = pack((int)kx, (int)ky, (int)kz);
+      anc[j] = d == kBrickDepth ? j : d == kBrickDepth + 1 ? a1 : d == kBrickDepth + 2 ? a2 : -1;
+      const int m = pair_mask(pay, j);
+      for (int s = 0; s < 8; ++s) {
+        const int b = (m >> (2 * s)) & 3;
+        if (!b) continue;
+        ++v[0];
+        if (b == 3) continue;
+        ++v[b];
+        v[3] += 1ull << (3 * (15 - d));
+        if (d + 1 <= kBrickDepth) bricks += 1LL << (3 * (kBrickDepth - 1 - d));
+      }
+      if (d == kBrickDepth) bricks += 1;
+    }
+  }
+  if (j <= n) nb[j] = bricks;
+  for (int k = 0; k < 4; ++k) {
+    const unsigned long long t = Reduce(tmp).Sum(v[k]);
+    if (threadIdx.x == 0 && t) atomicAdd(k == 0 ? &cnt->nodes : k == 1 ? &cnt->free_leaves : k == 2 ? &cnt->occ_leaves
+                                                                                                     : &cnt->known, t);
+    __syncthreads();
+  }
+}
+
+// (r5) per new brick, in pre-order: its key and state (1 free, 2 occupied: under a leaf at depth <= 13; 3: below an inner
+// node at depth 13).  Its inner node is the last j with boff[j] <= b; a leaf's bricks are in Morton order.
+__global__ void rd_brick_kernel(const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
+                                const unsigned long long* __restrict__ key, const long long* __restrict__ boff, int end,
+                                int n_b, unsigned long long* __restrict__ bkey, unsigned char* __restrict__ bst) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= n_b) return;
+  int lo = 0, hi = end - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (boff[mid] <= b) lo = mid;
+    else hi = mid - 1;
+  }
+  const int j = lo, d = depth[j];
+  const unsigned long long k0 = key[j];
+  int kx = (int)(k0 & 0xffff), ky = (int)((k0 >> 16) & 0xffff), kz = (int)((k0 >> 32) & 0xffff), st = 3;
+  if (d != kBrickDepth) {
+    const int m = pair_mask(pay, j), sh = 15 - d;
+    long long r = b - boff[j];
+    for (int s = 0; s < 8; ++s) {
+      const int bits = (m >> (2 * s)) & 3;
+      if (bits == 0 || bits == 3) continue;
+      const long long c = 1LL << (3 * (kBrickDepth - 1 - d));
+      if (r >= c) {
+        r -= c;
+        continue;
+      }
+      st = bits;
+      kx += ((s & 1) << sh) + (squeeze3((unsigned long long)r) << 3);
+      ky += (((s >> 1) & 1) << sh) + (squeeze3((unsigned long long)r >> 1) << 3);
+      kz += (((s >> 2) & 1) << sh) + (squeeze3((unsigned long long)r >> 2) << 3);
+      break;
+    }
+  }
+  const int k[3] = {kx, ky, kz};
+  bkey[b] = brick_key(k);
+  bst[b] = (unsigned char)st;
+}
+
+// (r6) one block of 512 threads per new brick: a uniform brick holds L_min or L_max and is all known, a mixed one starts
+// empty; marks and touched flags clear
+__global__ void __launch_bounds__(512) rd_fill_kernel(Dev D, Params P, const unsigned long long* __restrict__ bkey,
+                                                      const unsigned char* __restrict__ bst) {
+  const int b = blockIdx.x, t = threadIdx.x, st = bst[b];
+  D.lo[(size_t)b * 512 + t] = st == 1 ? P.l_min : st == 2 ? P.l_max : 0.0f;
+  if (t < 16) {
+    D.known[(size_t)b * 16 + t] = st == 3 ? 0u : ~0u;
+    D.mfree[(size_t)b * 16 + t] = 0u;
+    D.mocc[(size_t)b * 16 + t] = 0u;
+  }
+  if (t == 0) D.touched[b] = 0u, D.bkey[b] = bkey[b];
+}
+
+// (r7) per inner node at depth 13 ... 15: the 64, 8 or 1 voxels of each of its leaves, in its depth-13 ancestor's brick
+__global__ void rd_leaf_kernel(Dev D, Params P, const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
+                               const unsigned long long* __restrict__ key, const int* __restrict__ anc,
+                               const long long* __restrict__ boff, int end) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= end) return;
+  const int d = depth[j];
+  if (d < kBrickDepth) return;
+  const size_t b = (size_t)boff[anc[j]];
+  const unsigned long long k0 = key[j];
+  const int m = pair_mask(pay, j), sh = 15 - d, side = 1 << sh;
+  for (int s = 0; s < 8; ++s) {
+    const int bits = (m >> (2 * s)) & 3;
+    if (bits == 0 || bits == 3) continue;
+    const float v = bits == 1 ? P.l_min : P.l_max;
+    const int x0 = ((int)(k0 & 7)) | ((s & 1) << sh), y0 = ((int)((k0 >> 16) & 7)) | (((s >> 1) & 1) << sh),
+              z0 = ((int)((k0 >> 32) & 7)) | (((s >> 2) & 1) << sh);
+    for (int z = z0; z < z0 + side; ++z)
+      for (int y = y0; y < y0 + side; ++y) {
+        unsigned bitsw = 0;
+        const int row = (y << 3) | (z << 6);  // side <= 4 voxels of one row share a known word
+        for (int x = x0; x < x0 + side; ++x) {
+          D.lo[b * 512 + row + x] = v;
+          bitsw |= 1u << ((row + x) & 31);
+        }
+        atomicOr(&D.known[b * 16 + (row >> 5)], bitsw);
+      }
+  }
+}
+
 int code(cudaError_t e) {
   if (e == cudaSuccess) return LS_OK;
   cudaGetLastError();
@@ -948,33 +1179,71 @@ int grow_pool(Map& m, int cap, cudaStream_t st) {
   return LS_OK;
 }
 
-// A hash of at least `cap` slots (power of two) holding every pool brick; doubles until the probe bound holds.  The old
-// table stays when an allocation fails.
-int rebuild_table(Map& m, int cap, cudaStream_t st, uint64_t* launches) {
+// A hash of at least `cap` slots (power of two) holding the n bricks of bkey (pool index = position) into keys / vals;
+// doubles until the probe bound holds.  The map's own table is not touched.
+int build_table(Map& m, const unsigned long long* bkey, int n, int cap, ls::Buffer<unsigned long long>& keys,
+                ls::Buffer<int>& vals, cudaStream_t st, uint64_t* launches) {
   for (;; cap *= 2) {
     const size_t c = (size_t)cap;
-    ls::Buffer<unsigned long long> keys;
-    ls::Buffer<int> vals;
+    keys.reset(), vals.reset();
     cudaError_t e = keys.reserve(c, c);
     if (e == cudaSuccess) e = vals.reserve(c, c);
     if (e == cudaSuccess) e = cudaMemsetAsync(keys.get(), 0xff, c * sizeof(unsigned long long), st);
     if (e == cudaSuccess) e = cudaMemsetAsync(vals.get(), 0xff, c * sizeof(int), st);
     if (e == cudaSuccess) e = cudaMemsetAsync(&m.cnt_dev.get()->overflow, 0, sizeof(int), st);
-    if (e == cudaSuccess && m.pool_n > 0) {
-      occ_rehash_kernel<<<(m.pool_n + 255) / 256, 256, 0, st>>>(m.bkey.get(), m.pool_n, keys.get(), vals.get(),
-                                                                (unsigned)cap - 1u,
-                                                                m.cnt_dev.get());
+    if (e == cudaSuccess && n > 0) {
+      occ_rehash_kernel<<<(n + 255) / 256, 256, 0, st>>>(bkey, n, keys.get(), vals.get(), (unsigned)cap - 1u, m.cnt_dev.get());
       ++*launches;
       e = cudaGetLastError();
     }
     int overflow = 0;
     if (e == cudaSuccess) e = cudaMemcpyAsync(&overflow, &m.cnt_dev.get()->overflow, sizeof(int), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return code(e);
-    if (overflow) continue;
-    m.tab_keys = std::move(keys), m.tab_vals = std::move(vals);
-    return LS_OK;
+    if (e != cudaSuccess) {
+      keys.reset(), vals.reset();
+      return code(e);
+    }
+    if (!overflow) return LS_OK;
   }
+}
+
+// A hash of at least `cap` slots holding every pool brick.  The old table stays when an allocation fails.
+int rebuild_table(Map& m, int cap, cudaStream_t st, uint64_t* launches) {
+  ls::Buffer<unsigned long long> keys;
+  ls::Buffer<int> vals;
+  const int rc = build_table(m, m.bkey.get(), m.pool_n, cap, keys, vals, st, launches);
+  if (rc) return rc;
+  m.tab_keys = std::move(keys), m.tab_vals = std::move(vals);
+  return LS_OK;
+}
+
+// The read's per-pair scratch for n pairs of `bytes` payload bytes, grown all or nothing.
+int reserve_read(Map& m, int n, size_t bytes, cudaStream_t st) {
+  OCC_TRY(m.rd_cnt_dev.reserve(1, 1));
+  OCC_TRY(m.rd_cnt_host.reserve(1, 1));
+  if (bytes > m.rd_pay.capacity()) {
+    OCC_TRY(cudaStreamSynchronize(st));
+    OCC_TRY(m.rd_pay.reserve(bytes, bytes + bytes / 8));
+  }
+  if ((size_t)n + 1 <= m.rd_ex.capacity()) return LS_OK;
+  OCC_TRY(cudaStreamSynchronize(st));
+  const size_t c = (size_t)n + n / 8 + 1, blocks = c / kReadThreads + 1;
+  size_t b1 = 0, b2 = 0;
+  cudaError_t e;
+  if ((e = m.rd_ex.reserve(c, c)) || (e = m.rd_tmp.reserve(c, c)) || (e = m.rd_par.reserve(c, c)) ||
+      (e = m.rd_anc.reserve(c, c)) || (e = m.rd_bmin.reserve(blocks, blocks)) || (e = m.rd_slot.reserve(c, c)) ||
+      (e = m.rd_depth.reserve(c, c)) || (e = m.rd_key.reserve(c, c)) || (e = m.rd_nb.reserve(c, c)) ||
+      (e = m.rd_boff.reserve(c, c)) ||
+      (e = cub::DeviceScan::InclusiveSum(nullptr, b1, m.rd_tmp.get(), m.rd_ex.get(), (int)c, st)) ||
+      (e = cub::DeviceScan::ExclusiveSum(nullptr, b2, m.rd_nb.get(), m.rd_boff.get(), (int)c, st)) ||
+      (e = m.rd_cub.reserve(std::max(b1, b2), std::max(b1, b2)))) {
+    m.rd_ex.reset(), m.rd_tmp.reset(), m.rd_par.reset(), m.rd_anc.reset(), m.rd_bmin.reset(), m.rd_slot.reset();
+    m.rd_depth.reset(), m.rd_key.reset(), m.rd_nb.reset(), m.rd_boff.reset(), m.rd_cub.reset();
+    m.rd_cub_bytes = 0;
+    return code(e);
+  }
+  m.rd_cub_bytes = std::max(b1, b2);
+  return LS_OK;
 }
 
 int reserve_points(Map& m, int n, cudaStream_t st) {
@@ -1105,7 +1374,11 @@ size_t device_bytes(const Map& m) {
   const size_t pts = m.ends.capacity() * (sizeof(float4) + sizeof(unsigned long long) + sizeof(int)) +
                      m.ep_keys.capacity() * (sizeof(unsigned long long) + sizeof(int));
   const size_t ex = m.ex_c.capacity() * (2 * sizeof(unsigned long long) + 2 * sizeof(unsigned) + sizeof(float4)) + m.cub_bytes;
-  return pool + tab + pts + ex + m.qbuf.capacity() + sizeof(Counters);
+  const size_t rd = m.rd_pay.capacity() + m.rd_ex.capacity() * (4 * sizeof(int) + 2 + sizeof(unsigned long long) +
+                                                                2 * sizeof(long long)) +
+                    m.rd_bmin.capacity() * sizeof(int) + m.rd_cub.capacity() +
+                    m.rd_bkey.capacity() * (sizeof(unsigned long long) + 1) + m.rd_cnt_dev.capacity() * sizeof(ReadCounters);
+  return pool + tab + pts + ex + m.qbuf.capacity() + sizeof(Counters) + rd;
 }
 
 int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16], bool identity, cudaStream_t st, Counters* out,
@@ -1234,6 +1507,102 @@ int download_octree(const Octree& t, unsigned char* payload, float* centres4, un
     OCC_TRY(cudaMemcpyAsync(centres4, t.centres.get(), (size_t)t.leaves * sizeof(float4), cudaMemcpyDeviceToHost, st));
   if (t.leaves > 0 && depths) OCC_TRY(cudaMemcpyAsync(depths, t.depths.get(), (size_t)t.leaves, cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
+  return LS_OK;
+}
+
+int read_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes, ReadCounters* out,
+                const char** why, cudaStream_t st, uint64_t* launches) {
+  std::memset(out, 0, sizeof(ReadCounters));
+  *why = "";
+  int rc, n_b = 0, end = 0;
+  // A valid tree has at most `nodes` inner nodes, so later pairs cannot belong to it.
+  const long long pairs = nodes > 0 ? std::min(bytes / 2, nodes) : 0;
+  if (nodes > 0 && pairs == 0) return *why = "the payload is truncated", LS_ERR_ARG;
+  if (pairs > kMaxReadPairs) return *why = "more than 2^30 inner nodes", LS_ERR_NOMEM;
+  if (pairs > 0) {
+    const int n = (int)pairs;
+    if ((rc = reserve_read(m, n, 2 * (size_t)n, st))) return *why = "out of device memory for the parse", rc;
+    ReadCounters* cnt = m.rd_cnt_dev.get();
+    ReadCounters init{};
+    init.end = INT_MAX;
+    *m.rd_cnt_host.get() = init;
+    OCC_TRY(cudaMemcpyAsync(cnt, m.rd_cnt_host.get(), sizeof(ReadCounters), cudaMemcpyHostToDevice, st));
+    OCC_TRY(cudaMemcpyAsync(m.rd_pay.get(), payload, 2 * (size_t)n, cudaMemcpyHostToDevice, st));
+    const int blocks = (n + kReadThreads) / kReadThreads;  // n + 1 items
+    rd_excess_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), n, m.rd_tmp.get());
+    OCC_LAUNCHED();
+    size_t tb = m.rd_cub_bytes;
+    OCC_TRY(cub::DeviceScan::InclusiveSum(m.rd_cub.get(), tb, m.rd_tmp.get(), m.rd_ex.get(), n + 1, st));
+    ++*launches;
+    rd_end_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_ex.get(), n, m.rd_bmin.get(), cnt);
+    OCC_LAUNCHED();
+    rd_parent_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_ex.get(), m.rd_bmin.get(), n, m.rd_par.get(),
+                                                      m.rd_slot.get(), cnt);
+    OCC_LAUNCHED();
+    rd_node_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_par.get(), m.rd_slot.get(), n, m.rd_depth.get(),
+                                                    m.rd_key.get(), m.rd_anc.get(), m.rd_nb.get(), cnt);
+    OCC_LAUNCHED();
+    tb = m.rd_cub_bytes;
+    OCC_TRY(cub::DeviceScan::ExclusiveSum(m.rd_cub.get(), tb, m.rd_nb.get(), m.rd_boff.get(), n + 1, st));
+    ++*launches;
+    OCC_TRY(cudaMemcpyAsync(&cnt->bricks, m.rd_boff.get() + n, sizeof(long long), cudaMemcpyDeviceToDevice, st));
+    OCC_TRY(cudaMemcpyAsync(m.rd_cnt_host.get(), cnt, sizeof(ReadCounters), cudaMemcpyDeviceToHost, st));
+    OCC_TRY(cudaStreamSynchronize(st));
+    const ReadCounters c = *m.rd_cnt_host.get();
+    if (c.end == INT_MAX) return *why = "the payload is truncated", LS_ERR_ARG;
+    if (c.bad) return *why = "an inner node at depth 16", LS_ERR_ARG;
+    if ((long long)c.nodes + 1 != nodes) return *why = "the header's size does not count the payload's nodes", LS_ERR_ARG;
+    if (c.bricks > kMaxReadBricks) return *why = "the file covers more bricks than the map can index", LS_ERR_NOMEM;
+    *out = c;
+    out->nodes = c.nodes + 1;
+    out->inner = (unsigned long long)c.end;
+    end = c.end;
+    n_b = (int)c.bricks;
+  }
+  // The file is valid: grow, then build the new hash beside the old one; the map is still unchanged if either fails.
+  const char* nomem = "the map cannot grow";
+  if (n_b > 0) {
+    cudaError_t e = m.rd_bkey.capacity() >= (size_t)n_b ? cudaSuccess : m.rd_bkey.reserve(n_b, n_b + n_b / 8);
+    if (e == cudaSuccess && m.rd_bst.capacity() < (size_t)n_b) e = m.rd_bst.reserve(n_b, n_b + n_b / 8);
+    if (e != cudaSuccess) {
+      m.rd_bkey.reset(), m.rd_bst.reset();
+      return *why = nomem, code(e);
+    }
+    rd_brick_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_boff.get(), end,
+                                                       n_b, m.rd_bkey.get(), m.rd_bst.get());
+    OCC_LAUNCHED();
+  }
+  if (n_b > m.pool_cap()) {
+    long long cap = m.pool_cap() > 0 ? m.pool_cap() : 1;
+    while (cap < n_b) cap *= 2;
+    if ((rc = grow_pool(m, (int)cap, st))) return *why = nomem, rc;
+  }
+  int tab = 1024;
+  while (tab < 2 * n_b) tab *= 2;
+  ls::Buffer<unsigned long long> keys;
+  ls::Buffer<int> vals;
+  if ((rc = build_table(m, m.rd_bkey.get(), n_b, tab, keys, vals, st, launches))) return *why = nomem, rc;
+  // Only now is the map written.
+  const Dev D = dev_of(m);
+  if (n_b > 0) {
+    rd_fill_kernel<<<n_b, 512, 0, st>>>(D, P, m.rd_bkey.get(), m.rd_bst.get());
+    OCC_LAUNCHED();
+    rd_leaf_kernel<<<(end + 255) / 256, 256, 0, st>>>(D, P, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(),
+                                                      m.rd_boff.get(), end);
+    OCC_LAUNCHED();
+  }
+  if (m.pool_n > n_b) {  // bricks past the new pool start empty, as a grown pool's do
+    const size_t a = (size_t)n_b, k = (size_t)(m.pool_n - n_b);
+    OCC_TRY(cudaMemsetAsync(m.lo.get() + a * 512, 0, k * 512 * sizeof(float), st));
+    OCC_TRY(cudaMemsetAsync(m.known.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.mfree.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.mocc.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.touched.get() + a, 0, k * sizeof(unsigned), st));
+  }
+  OCC_TRY(cudaStreamSynchronize(st));
+  m.tab_keys = std::move(keys), m.tab_vals = std::move(vals);
+  m.pool_n = n_b;
+  m.n_known = (long long)out->known;
   return LS_OK;
 }
 

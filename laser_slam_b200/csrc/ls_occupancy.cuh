@@ -22,6 +22,14 @@ struct Counters {
   int pool_n, n_touched, overflow, rays_cast, rays_skipped, pad[3];
 };
 
+// Device counters of one .bt read, copied back once after the parse: the node counts, the pair after the tree (INT_MAX
+// while none is found), the known voxels and bricks the file covers, and why it is malformed (0 when it is not).
+struct ReadCounters {
+  unsigned long long nodes, inner, free_leaves, occ_leaves, known;
+  long long bricks;
+  int end, bad, pad[2];
+};
+
 // Bricks of 8x8x8 voxels.  The hash maps a brick key (13 bits per axis) to a pool index; per brick the pool holds 512
 // float log-odds, 16 words of known bits and 16 + 16 words of per-scan free / occupied marks.
 // Each group of arrays grows all or nothing; its first array tells its capacity.
@@ -48,6 +56,18 @@ struct Map {
   size_t cub_bytes = 0;
   // query staging (inputs and outputs of one call), grown by doubling
   ls::Buffer<char> qbuf;
+  // .bt read scratch: per payload pair (the excess, parent, depth, first key, bricks) and per new brick (key, state)
+  ls::Buffer<unsigned char> rd_pay;
+  ls::Buffer<int> rd_ex, rd_tmp, rd_par, rd_anc, rd_bmin;
+  ls::Buffer<unsigned char> rd_slot, rd_depth;
+  ls::Buffer<unsigned long long> rd_key;
+  ls::Buffer<long long> rd_nb, rd_boff;
+  ls::Buffer<unsigned char> rd_cub;
+  size_t rd_cub_bytes = 0;
+  ls::Buffer<unsigned long long> rd_bkey;
+  ls::Buffer<unsigned char> rd_bst;
+  ls::Buffer<ReadCounters> rd_cnt_dev;
+  ls::PinnedBuffer<ReadCounters> rd_cnt_host;
   ls::Buffer<Counters> cnt_dev;
   ls::PinnedBuffer<Counters> cnt_host;
   long long n_known = 0;
@@ -95,6 +115,14 @@ size_t device_bytes(const Map& m);
 int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches);
 // Copies the last build's payload (t.bytes) and, each when not NULL, its t.leaves centres {x, y, z, 1} and depths.
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st);
+
+// octomap's readBinary of a .bt payload (`bytes` bytes after "data\n", `nodes` the header's size) into the map, replacing
+// it (DESIGN.md §4b'''''').  P: the map's parameters at the file's resolution.  Synchronous.  Validates the
+// whole stream and the brick count before it grows or writes anything: LS_ERR_ARG for a malformed payload, LS_ERR_NOMEM
+// for more bricks than the map can index or a failed growth, and the map is unchanged after any error (*why then says
+// why).  *out: the counts.
+int read_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes, ReadCounters* out,
+                const char** why, cudaStream_t st, uint64_t* launches);
 
 // Queries (oracle/QUERIES.md), reading the map only.  Synchronous; host inputs and outputs, *visited the voxel states the
 // kernels read.  n <= 0 launches nothing.

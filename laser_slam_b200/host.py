@@ -286,6 +286,7 @@ class OccupancyMap:
             L.lsh_occupancy_voxels.restype = i64
             L.lsh_occupancy_occupied_cloud.argtypes = [vp, vp, ci]
             L.lsh_occupancy_write_binary.argtypes = [vp, ctypes.c_char_p]
+            L.lsh_occupancy_read_binary.argtypes = [vp, ctypes.c_char_p]
             L.lsh_occupancy_occupied_leaf_cloud.argtypes = [vp, vp, ci]
             L.lsh_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp]
             L.lsh_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, ci, vp, vp]
@@ -327,6 +328,14 @@ class OccupancyMap:
     def write_binary(self, path):
         """writeBinary: the map as an octomap .bt file."""
         self._check(lib().lsh_occupancy_write_binary(self._h, os.fsencode(path)))
+
+    def read_binary(self, path):
+        """readBinary: the .bt file replaces the map.  False, with the map unchanged, when the file is refused."""
+        rc = lib().lsh_occupancy_read_binary(self._h, os.fsencode(path))
+        if rc == -1:  # LS_ERR_ARG
+            return False
+        self._check(rc)
+        return True
 
     def occupied_leaf_cloud(self):
         """getOccupiedLeafCloud: the pruned tree's occupied leaves, (n,4) float32."""

@@ -462,6 +462,17 @@ int lsh_occupancy_write_binary(void* ov, const char* path) {
   }
 }
 
+// readBinary; 0 on success, LS_ERR_ARG when it returns false
+int lsh_occupancy_read_binary(void* ov, const char* path) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    return h->map->readBinary(path) ? 0 : LS_ERR_ARG;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
 // getCellProbabilityPoint per point (single queries): status and probability; 0 or LS_ERR_STATE
 int lsh_occupancy_cell_status(void* ov, const double* pts3, int n, int8_t* status, double* probability) {
   OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);

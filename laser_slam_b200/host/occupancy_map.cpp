@@ -98,6 +98,16 @@ bool OccupancyMap::writeBinary(const std::string& filename) {
   return true;
 }
 
+bool OccupancyMap::readBinary(const std::string& filename) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_octomap_read_stats stats;
+  const int rc = ls_occupancy_read_octomap(map_, filename.c_str(), &stats);
+  if (rc == LS_ERR_ARG || rc == LS_ERR_NOMEM) return false;
+  throwOnError(ctx_, rc, "ls_occupancy_read_octomap");
+  params_.resolution = stats.resolution;
+  return true;
+}
+
 void OccupancyMap::getOccupiedLeafCloud(DataPoints* cloud) {
   if (cloud == NULL) throw std::invalid_argument("null output");
   std::lock_guard<std::mutex> lock(mutex_);

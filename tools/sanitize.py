@@ -85,6 +85,19 @@ for got, want in ((om.cell_status(qs), qo.cell_status(qs)), (om.line_status(qs, 
                   (om.cast_rays(qorg, qd, False, 10.0), qo.cast_rays(qorg, qd, False, 10.0)),
                   (om.cast_rays(qorg, qd, True, 10.0), qo.cast_rays(qorg, qd, True, 10.0))):
     assert np.array_equal(got[0], want[0]) and np.array_equal(np.asarray(got[1]).view(np.uint8), np.asarray(want[1]).view(np.uint8))
+# that map's .bt file read back into a map of 16 bricks (parse, growth, expansion) against the reference expansion
+import tempfile
+sys.path.insert(1, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+import octomap_read_ref as rr
+with tempfile.TemporaryDirectory() as tmp:
+    bt = os.path.join(tmp, "map.bt")
+    om.save_octomap(bt)
+    rm = ls.OccupancyMap(ctx, resolution=0.05, max_range=10.0, initial_capacity=16)
+    rm.read_octomap(bt)
+    rk, rv, _ = rm.download(ls.OCC_KNOWN)
+    wk, wv = rr.expand(ls.read_octomap(bt), *rr.clamps())
+    assert np.array_equal(rk, wk) and np.array_equal(rv.view(np.uint32), wv.view(np.uint32)) and len(rk) > 0
+    rm.close()
 om.close()
 launches = ctx.launch_count
 # every handle closed, so a leak check sees only what the library failed to free
