@@ -54,6 +54,18 @@ class OccupancyMap {
   // clamping_thres_min and occupied ones as clamping_thres_max (ls_occupancy_read_octomap).  Returns false, with the map
   // unchanged, when the file cannot be read, is malformed or covers more than the map can hold.
   bool readBinary(const std::string& filename);
+  // octomap's OcTree::write: every node's float log-odds, pruned by value, as a .ot file (ls_occupancy_write_octomap_full),
+  // so a saved map resumes mapping exactly.  Returns false when the file cannot be written.
+  bool write(const std::string& filename);
+  // octomap's AbstractOcTree::read of a .ot file: it replaces the map, its resolution becomes the map's and every leaf's
+  // voxels take its value verbatim (ls_occupancy_read_octomap_full).  Returns false, with the map unchanged, when the file
+  // cannot be read, is malformed or covers more than the map can hold.
+  bool read(const std::string& filename);
+  // The full tree's payload (what getOctomapFullMsg carries as data) and its node count.
+  void writeData(std::vector<uint8_t>* payload, int64_t* nodes);
+  // setOctomapFromFullMsg: a full-tree payload of `nodes` nodes at `resolution` replaces the map, as read().  Returns false,
+  // with the map unchanged, when it is refused.
+  bool readData(const std::vector<uint8_t>& payload, int64_t nodes, double resolution);
   // The occupied leaves of the pruned tree in octomap's leaf order, features only ({x, y, z, 1}): what
   // octomap_to_point_cloud writes from writeBinary's file.
   void getOccupiedLeafCloud(DataPoints* cloud);

@@ -429,6 +429,49 @@ int ls_occupancy_read_octree(ls_occupancy* om, const uint8_t* payload, int64_t p
 /* The whole .bt file at `path`: its header is parsed on the host as laser_slam_b200.read_octomap parses it, then as above. */
 int ls_occupancy_read_octomap(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats);
 
+/* The map as octomap's full tree, what OcTree::write saves (the .ot file) and the data of a full octomap message
+ * (getOctomapFullMsg): every node's float log-odds, so a saved map resumes mapping exactly (DESIGN.md §4b').  Rules:
+ *   tree        as the .bt tree (depth 16, child i = bx | by<<1 | bz<<2); a node exists iff a known voxel lies below it
+ *   pruning     a node at depth 1..15 is a leaf iff its 8 children exist, are leaves and their log-odds compare equal as
+ *               floats (+0.0 == -0.0); bottom-up and maximal, the root stays.  The collapsed leaf keeps child 0's bits
+ *   inner       an inner node holds its largest child's value (a strict > scan over children 0..7: the earliest wins ties)
+ *   payload     every node in pre-order (children 0..7), 5 bytes each: its value as float32 little-endian, then a byte whose
+ *               bit i is set iff child i exists
+ * The build reads the map only, runs on its stream and is cached apart from the .bt build: neither build invalidates the
+ * other; an insert or a successful read invalidates both, and a download then returns LS_ERR_STATE.  Legal between
+ * ls_icp_register_submap_batch_begin and _end like every ls_occupancy_* call. */
+typedef struct ls_full_octree_stats {
+  int64_t nodes;          /* every node, root and leaves included (the .ot file's size line); 0 for an empty map */
+  int64_t leaves;
+  int64_t payload_bytes;  /* 5 per node */
+  float device_ms;        /* the build on the map's stream */
+} ls_full_octree_stats;
+
+int ls_occupancy_build_full_octree(ls_occupancy* om, ls_full_octree_stats* stats);
+/* The last full build's payload; LS_ERR_ARG without a copy when payload_cap is below its size. */
+int ls_occupancy_download_full_octree(ls_occupancy* om, uint8_t* payload, int64_t payload_cap);
+/* The whole .ot file at `path`: "# Octomap OcTree file", octomap's two further comment lines, "id OcTree", "size <nodes>",
+ * "res <resolution as %g>", "data", then the payload.  Builds the full tree unless the last full build is current.  stats may
+ * be NULL. */
+int ls_occupancy_write_octomap_full(ls_occupancy* om, const char* path, ls_full_octree_stats* stats);
+
+/* octomap's readData of a full tree into the map (setOctomapFromFullMsg; AbstractOcTree::read for a file).  A read
+ * replaces the map: the file's resolution becomes the map's, and every voxel below a leaf becomes known with the leaf's
+ * value verbatim (no clamp: the next insert clamps as usual); stored inner values are not used.  Unpruned files are
+ * accepted.  Read then write gives the bytes of any file this library wrote, and the map's .bt equals the original's.  The
+ * parse and the expansion run on the device, on the map's stream; the call is synchronous and legal between
+ * ls_icp_register_submap_batch_begin and _end.  Errors: LS_ERR_ARG for a bad header (first line, id other than OcTree), a
+ * truncated payload, a node at depth 16 with children, a size other than the nodes parsed, a leaf value that is NaN or
+ * infinite, or a resolution that is not finite and > 0 (bytes after the tree are ignored); LS_ERR_NOMEM, before the map
+ * grows, when the file covers more than 2^29 bricks or the map cannot grow.  After any error the map, its resolution and
+ * both cached builds are unchanged.  stats (may be NULL): nodes, inner_nodes = nodes with children, free and occupied
+ * leaves classified by the map's occupancy threshold. */
+int ls_occupancy_read_full_octree(ls_occupancy* om, const uint8_t* payload, int64_t payload_bytes, int64_t nodes,
+                                  double resolution, ls_octomap_read_stats* stats);
+/* The whole .ot file at `path`: its header is parsed on the host as laser_slam_b200.read_octomap_full parses it, then as
+ * above. */
+int ls_occupancy_read_octomap_full(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats);
+
 /* Queries of the map: volumetric_mapping's WorldBase (getCellStatusPoint, getLineStatus, getVisibility,
  * getLineStatusBoundingBox) and octomap's castRay, batched, one device thread per query.  The rules (oracle/QUERIES.md):
  *   cell        the key of the double point (octomap's search(x, y, z): floor(c * (1/resolution)) + 32768, no float cast);

@@ -7,7 +7,9 @@ CUDA device is usable.
 """
 import collections
 import ctypes
+import math
 import os
+import struct
 import subprocess
 
 import numpy as np
@@ -99,6 +101,11 @@ class OccupancyStats(ctypes.Structure):
 
 class OctreeStats(ctypes.Structure):
     _fields_ = [("nodes", ctypes.c_int64), ("payload_bytes", ctypes.c_int64), ("occupied_leaves", ctypes.c_int64),
+                ("device_ms", ctypes.c_float)]
+
+
+class FullOctreeStats(ctypes.Structure):
+    _fields_ = [("nodes", ctypes.c_int64), ("leaves", ctypes.c_int64), ("payload_bytes", ctypes.c_int64),
                 ("device_ms", ctypes.c_float)]
 
 
@@ -224,6 +231,12 @@ def lib():
         L.ls_occupancy_read_octree.argtypes = [vp, vp, ctypes.c_int64, ctypes.c_int64, ctypes.c_double,
                                                ctypes.POINTER(OctomapReadStats)]
         L.ls_occupancy_read_octomap.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(OctomapReadStats)]
+        L.ls_occupancy_build_full_octree.argtypes = [vp, ctypes.POINTER(FullOctreeStats)]
+        L.ls_occupancy_download_full_octree.argtypes = [vp, vp, ctypes.c_int64]
+        L.ls_occupancy_write_octomap_full.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(FullOctreeStats)]
+        L.ls_occupancy_read_full_octree.argtypes = [vp, vp, ctypes.c_int64, ctypes.c_int64, ctypes.c_double,
+                                                    ctypes.POINTER(OctomapReadStats)]
+        L.ls_occupancy_read_octomap_full.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(OctomapReadStats)]
         QS = ctypes.POINTER(OccupancyQueryStats)
         L.ls_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp, QS]
         L.ls_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, vp, vp, QS]
@@ -921,6 +934,42 @@ class OccupancyMap:
         self.params.resolution = st.resolution
         return st
 
+    def full_octree(self):
+        """The map as octomap's full tree (every node's log-odds, pruned by value), built on the device
+        (ls_occupancy_build_full_octree): FullOctree(nodes, payload bytes, device ms)."""
+        st = FullOctreeStats()
+        self.ctx._check(lib().ls_occupancy_build_full_octree(self._h, ctypes.byref(st)))
+        pay = np.empty(max(st.payload_bytes, 1), np.uint8)
+        self.ctx._check(lib().ls_occupancy_download_full_octree(self._h, pay.ctypes.data, st.payload_bytes))
+        return FullOctree(st.nodes, pay[:st.payload_bytes].tobytes(), st.device_ms)
+
+    def save_octomap_full(self, path):
+        """The map as an octomap full tree file (.ot, OcTree::write), readable by octomap's AbstractOcTree::read(path).
+        Unlike the .bt file it keeps every voxel's log-odds, so a map read back maps on exactly as this one would.  Returns
+        its node count."""
+        st = FullOctreeStats()
+        self.ctx._check(lib().ls_occupancy_write_octomap_full(self._h, os.fsencode(path), ctypes.byref(st)))
+        return st.nodes
+
+    def read_octomap_full(self, path):
+        """octomap's read of a .ot file into this map, replacing it (ls_occupancy_read_octomap_full): every leaf's voxels
+        take its log-odds verbatim, and the file's resolution becomes the map's (self.params.resolution).  Returns
+        OctomapReadStats; on an error the map is unchanged."""
+        st = OctomapReadStats()
+        self.ctx._check(lib().ls_occupancy_read_octomap_full(self._h, os.fsencode(path), ctypes.byref(st)))
+        self.params.resolution = st.resolution
+        return st
+
+    def read_full_octree(self, payload, nodes, resolution):
+        """As read_octomap_full, from a payload in memory (the bytes after "data\\n", as a full octomap message carries
+        them), the node count of its size line and its resolution."""
+        buf = np.frombuffer(bytes(payload), np.uint8)
+        st = OctomapReadStats()
+        self.ctx._check(lib().ls_occupancy_read_full_octree(self._h, buf.ctypes.data if len(buf) else None, len(buf),
+                                                            int(nodes), float(resolution), ctypes.byref(st)))
+        self.params.resolution = st.resolution
+        return st
+
     # ---- queries (ls_occupancy_cell_status / _line_status / _cast_rays); self.last_query holds the last call's stats
     def cell_status(self, points):
         """getCellStatusPoint per point ((n,3), taken as float64): (status int8 CELL_*, log-odds float32, NaN when
@@ -970,15 +1019,14 @@ class OccupancyMap:
 
 
 Octree = collections.namedtuple("Octree", "nodes payload centres depths device_ms")
+FullOctree = collections.namedtuple("FullOctree", "nodes payload device_ms")
 
 _BT_FIRST_LINE = b"# Octomap OcTree binary file"
+_OT_FIRST_LINE = b"# Octomap OcTree file"
 
 
-def read_octomap(path):
-    """Parse an octomap binary file (.bt) as octomap::OcTree(path) reads it, on the CPU.  Returns a dict: resolution, nodes
-    (the header's size), payload, and every leaf in pre-order as first-voxel keys (n,3) int64, depths uint8 and states
-    uint8 (1 free, 2 occupied).  Raises ValueError on a bad header, a truncated payload or a size that does not match."""
-    data = open(path, "rb").read()
+def _read_header(path, data, first_line, what):
+    """(size, res, payload offset) of an octomap file's header."""
     pos = 0
 
     def line():
@@ -989,8 +1037,8 @@ def read_octomap(path):
         s, pos = data[pos:end], end + 1
         return s.rstrip(b"\r")
 
-    if line() != _BT_FIRST_LINE:
-        raise ValueError(f"{path}: not an octomap binary file (first line)")
+    if line() != first_line:
+        raise ValueError(f"{path}: not an octomap {what} file (first line)")
     head = {}
     while True:
         s = line()
@@ -1008,6 +1056,15 @@ def read_octomap(path):
         raise ValueError(f"{path}: bad or missing size / res line") from e
     if size < 0 or not res > 0:
         raise ValueError(f"{path}: bad size {size} or res {res}")
+    return size, res, pos
+
+
+def read_octomap(path):
+    """Parse an octomap binary file (.bt) as octomap::OcTree(path) reads it, on the CPU.  Returns a dict: resolution, nodes
+    (the header's size), payload, and every leaf in pre-order as first-voxel keys (n,3) int64, depths uint8 and states
+    uint8 (1 free, 2 occupied).  Raises ValueError on a bad header, a truncated payload or a size that does not match."""
+    data = open(path, "rb").read()
+    size, res, pos = _read_header(path, data, _BT_FIRST_LINE, "binary")
     keys, depths, states = [], [], []
     start, nodes = pos, 0
     # pre-order walk (children 0 ... 7): an inner node reads its two bytes when it is reached, a leaf is listed
@@ -1035,6 +1092,46 @@ def read_octomap(path):
         raise ValueError(f"{path}: the header's size {size} does not match the {nodes} nodes of the payload")
     return dict(resolution=res, nodes=size, payload=data[start:pos], keys=np.array(keys, np.int64).reshape(-1, 3),
                 depths=np.array(depths, np.uint8), states=np.array(states, np.uint8))
+
+
+def read_octomap_full(path):
+    """Parse an octomap full tree file (.ot, OcTree::write) as AbstractOcTree::read reads it, on the CPU.  Returns a dict:
+    resolution, nodes (the header's size), payload, and every leaf in pre-order as first-voxel keys (n,3) int64, depths
+    uint8 and log-odds float32.  Raises ValueError on a bad header or tree type, a resolution that is not finite and > 0, a
+    truncated payload, a node at depth 16 with children, a leaf value that is NaN or infinite, or a size that does not
+    match the nodes parsed."""
+    data = open(path, "rb").read()
+    size, res, pos = _read_header(path, data, _OT_FIRST_LINE, "full tree")
+    if not math.isfinite(res):
+        raise ValueError(f"{path}: res {res} is not finite")
+    keys, depths, values = [], [], []
+    start, nodes = pos, 0
+    unpack = struct.Struct("<fB").unpack_from
+    stack = [(0, 0, 0, 0)] if size > 0 else []  # depth, first-voxel key; children pushed 7 ... 0, so read in pre-order
+    while stack:
+        d, kx, ky, kz = stack.pop()
+        if pos + 5 > len(data):
+            raise ValueError(f"{path}: payload truncated")
+        v, m = unpack(data, pos)
+        pos += 5
+        nodes += 1
+        if not m:
+            if not math.isfinite(v):
+                raise ValueError(f"{path}: leaf value {v} is not finite")
+            keys.append((kx, ky, kz))
+            depths.append(d)
+            values.append(v)
+            continue
+        if d >= 16:
+            raise ValueError(f"{path}: node at depth 16 with children")
+        sh = 15 - d
+        for i in range(7, -1, -1):
+            if (m >> i) & 1:
+                stack.append((d + 1, kx | ((i & 1) << sh), ky | (((i >> 1) & 1) << sh), kz | (((i >> 2) & 1) << sh)))
+    if nodes != size:
+        raise ValueError(f"{path}: the header's size {size} does not match the {nodes} nodes of the payload")
+    return dict(resolution=res, nodes=size, payload=data[start:pos], keys=np.array(keys, np.int64).reshape(-1, 3),
+                depths=np.array(depths, np.uint8), values=np.array(values, np.float32))
 
 
 def leaf_centres(keys, depths, resolution):

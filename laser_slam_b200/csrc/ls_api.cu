@@ -1736,6 +1736,9 @@ struct ls_occupancy {
   lso::Octree tree;
   bool tree_current = false;  // the last octree build reflects every insert
   float tree_ms = 0.f;
+  lso::Octree full;           // the full tree (.ot), cached apart from the .bt build
+  bool full_current = false;
+  float full_ms = 0.f;
 };
 
 namespace {
@@ -1752,6 +1755,39 @@ int build_tree(ls_occupancy* om) {
   return LS_OK;
 }
 
+int build_full(ls_occupancy* om) {
+  ls_ctx* ctx = om->ctx;
+  om->full_current = false;
+  CU(cudaEventRecord(om->ev0, om->stream));
+  const int rc = lso::build_full_octree(om->map, om->full, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "full octree export: out of device memory" : "full octree export failed");
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  CU(cudaEventElapsedTime(&om->full_ms, om->ev0, om->ev1));
+  om->full_current = true;
+  return LS_OK;
+}
+
+void full_stats(const ls_occupancy* om, ls_full_octree_stats* stats) {
+  if (!stats) return;
+  stats->nodes = om->full.nodes;
+  stats->leaves = om->full.leaves;
+  stats->payload_bytes = om->full.bytes;
+  stats->device_ms = om->full_ms;
+}
+
+// The file at `path`, whole.  NULL on success, else why not.
+const char* read_file(const char* path, std::vector<uint8_t>* data) {
+  FILE* f = std::fopen(path, "rb");
+  if (!f) return "cannot open the file";
+  uint8_t buf[1 << 16];
+  size_t got;
+  while ((got = std::fread(buf, 1, sizeof buf, f)) > 0) data->insert(data->end(), buf, buf + got);
+  const bool err = std::ferror(f) != 0;
+  std::fclose(f);
+  return err ? "reading the file failed" : nullptr;
+}
+
 void octree_stats(const ls_occupancy* om, ls_octree_stats* stats) {
   if (!stats) return;
   stats->nodes = om->tree.nodes;
@@ -1760,10 +1796,10 @@ void octree_stats(const ls_occupancy* om, ls_octree_stats* stats) {
   stats->device_ms = om->tree_ms;
 }
 
-// A .bt header as laser_slam_b200.read_octomap parses it: the first line exactly (a trailing \r dropped), then "#" and
-// blank lines skipped, "key value" lines, up to "data"; id OcTree, an integer size >= 0 and a res.  *off: the payload's
-// first byte.  NULL when it is valid, else why not.
-const char* parse_bt_header(const std::vector<uint8_t>& d, size_t* off, long long* nodes, double* res) {
+// A .bt header (with `full`, a .ot header) as laser_slam_b200.read_octomap (read_octomap_full) parses it: the first line
+// exactly (a trailing \r dropped), then "#" and blank lines skipped, "key value" lines, up to "data"; id OcTree, an integer
+// size >= 0 and a res.  *off: the payload's first byte.  NULL when it is valid, else why not.
+const char* parse_bt_header(const std::vector<uint8_t>& d, size_t* off, long long* nodes, double* res, bool full = false) {
   size_t pos = 0;
   std::string line;
   auto next = [&]() {
@@ -1781,7 +1817,8 @@ const char* parse_bt_header(const std::vector<uint8_t>& d, size_t* off, long lon
     return a == std::string::npos ? std::string() : s.substr(a, s.find_last_not_of(ws) + 1 - a);
   };
   if (d.empty() || !next()) return "header ends early";
-  if (line != "# Octomap OcTree binary file") return "not an octomap binary file (first line)";
+  if (line != (full ? "# Octomap OcTree file" : "# Octomap OcTree binary file"))
+    return full ? "not an octomap full tree file (first line)" : "not an octomap binary file (first line)";
   std::string id, size, resolution;
   bool have_id = false, have_size = false, have_res = false;
   for (;;) {
@@ -1877,6 +1914,7 @@ int ls_occupancy_insert_scan(ls_occupancy* om, const ls_map* ring, uint64_t scan
   if (wait_slot(s, om->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
   CU(cudaEventRecord(om->ev0, om->stream));
   om->tree_current = false;
+  om->full_current = false;
   lso::Counters c;
   const int rc = lso::insert(om->map, om->prm, s->pts.get(), s->n, T_w_scan, is_identity16(T_w_scan), om->stream, &c,
                              &ctx->launches);
@@ -1996,6 +2034,7 @@ int ls_occupancy_read_octree(ls_occupancy* om, const uint8_t* payload, int64_t p
   if (rc) return fail(ctx, rc, "octomap read refused, the map is unchanged: %s", why);
   om->prm = P;
   om->tree_current = false;
+  om->full_current = false;
   CU(cudaEventRecord(om->ev1, om->stream));
   CU(cudaEventSynchronize(om->ev1));
   if (stats) {
@@ -2018,22 +2057,114 @@ int ls_occupancy_read_octomap(ls_occupancy* om, const char* path, ls_octomap_rea
   ls_ctx* ctx = om->ctx;
   if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
   std::vector<uint8_t> data;
-  {
-    FILE* f = std::fopen(path, "rb");
-    if (!f) return fail(ctx, LS_ERR_ARG, "cannot open %s", path);
-    uint8_t buf[1 << 16];
-    size_t got;
-    while ((got = std::fread(buf, 1, sizeof buf, f)) > 0) data.insert(data.end(), buf, buf + got);
-    const bool err = std::ferror(f) != 0;
-    std::fclose(f);
-    if (err) return fail(ctx, LS_ERR_ARG, "reading %s failed", path);
-  }
+  const char* why = read_file(path, &data);
+  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
   size_t off = 0;
   long long nodes = 0;
   double res = 0.0;
-  const char* why = parse_bt_header(data, &off, &nodes, &res);
+  why = parse_bt_header(data, &off, &nodes, &res);
   if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
   return ls_occupancy_read_octree(om, data.data() + off, (int64_t)(data.size() - off), nodes, res, stats);
+}
+
+int ls_occupancy_build_full_octree(ls_occupancy* om, ls_full_octree_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  CU(cudaSetDevice(ctx->device));
+  const int rc = build_full(om);
+  if (rc) return rc;
+  full_stats(om, stats);
+  return LS_OK;
+}
+
+int ls_occupancy_download_full_octree(ls_occupancy* om, uint8_t* payload, int64_t payload_cap) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!om->full_current) return fail(ctx, LS_ERR_STATE, "no current full octree: build it after the last insert or read");
+  const lso::Octree& t = om->full;
+  if ((t.bytes > 0 && !payload) || payload_cap < t.bytes)
+    return fail(ctx, LS_ERR_ARG, "a payload buffer of %lld bytes for %lld", (long long)payload_cap, t.bytes);
+  CU(cudaSetDevice(ctx->device));
+  const int rc = lso::download_octree(t, payload, nullptr, nullptr, om->stream);
+  if (rc) return fail(ctx, rc, "full octree download failed");
+  return LS_OK;
+}
+
+int ls_occupancy_write_octomap_full(ls_occupancy* om, const char* path, ls_full_octree_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  int rc;
+  if (!om->full_current && (rc = build_full(om))) return rc;
+  std::vector<uint8_t> payload((size_t)om->full.bytes);
+  if ((rc = lso::download_octree(om->full, payload.data(), nullptr, nullptr, om->stream)))
+    return fail(ctx, rc, "full octree download failed");
+  // octomap's AbstractOcTree::write: the resolution as a default std::ostream prints a double (%g)
+  char head[256];
+  const int n = std::snprintf(head, sizeof head,
+                              "# Octomap OcTree file\n# (feel free to add / change comments, but leave the first line as it "
+                              "is!)\n#\nid OcTree\nsize %lld\nres %g\ndata\n",
+                              om->full.nodes, om->prm.res);
+  FILE* f = std::fopen(path, "wb");
+  if (!f) return fail(ctx, LS_ERR_ARG, "cannot open %s for writing", path);
+  bool ok = std::fwrite(head, 1, (size_t)n, f) == (size_t)n;
+  if (ok && !payload.empty()) ok = std::fwrite(payload.data(), 1, payload.size(), f) == payload.size();
+  ok = std::fclose(f) == 0 && ok;
+  if (!ok) return fail(ctx, LS_ERR_ARG, "writing %s failed", path);
+  full_stats(om, stats);
+  return LS_OK;
+}
+
+int ls_occupancy_read_full_octree(ls_occupancy* om, const uint8_t* payload, int64_t payload_bytes, int64_t nodes,
+                                  double resolution, ls_octomap_read_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (nodes < 0 || payload_bytes < 0 || (payload_bytes > 0 && !payload)) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!(resolution > 0.0) || !std::isfinite(resolution))
+    return fail(ctx, LS_ERR_ARG, "octomap resolution %g (finite and > 0)", resolution);
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  lso::Params P = om->prm;
+  P.res = resolution;
+  P.inv = 1.0 / resolution;
+  lso::ReadCounters c;
+  const char* why = "";
+  const int rc = lso::read_full_octree(om->map, P, payload, payload_bytes, nodes, &c, &why, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "octomap full tree read refused, the map is unchanged: %s", why);
+  om->prm = P;
+  om->tree_current = false;
+  om->full_current = false;
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    stats->nodes = (int64_t)c.nodes;
+    stats->inner_nodes = (int64_t)c.inner;
+    stats->free_leaves = (int64_t)c.free_leaves;
+    stats->occupied_leaves = (int64_t)c.occ_leaves;
+    stats->known_voxels = om->map.n_known;
+    stats->bricks = om->map.pool_n;
+    stats->resolution = P.res;
+    stats->device_ms = ms;
+  }
+  return LS_OK;
+}
+
+int ls_occupancy_read_octomap_full(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
+  std::vector<uint8_t> data;
+  const char* why = read_file(path, &data);
+  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
+  size_t off = 0;
+  long long nodes = 0;
+  double res = 0.0;
+  why = parse_bt_header(data, &off, &nodes, &res, true);
+  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
+  return ls_occupancy_read_full_octree(om, data.data() + off, (int64_t)(data.size() - off), nodes, res, stats);
 }
 
 }  // extern "C"

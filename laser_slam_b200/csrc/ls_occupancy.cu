@@ -37,12 +37,22 @@
 //   the hash is built from those keys beside the old one, so a failure up to here leaves the map as it was
 //   (r6) rd_fill_kernel                  one block per brick: uniform bricks written whole, mixed ones cleared
 //   (r7) rd_leaf_kernel                  the voxels of each leaf at depth 14 ... 16, each written once
+//
+// Full tree export (octomap's OcTree::write, the .ot payload; DESIGN.md §4b'), reading the map only: (d) and its
+// sort, then (e') ful_brick_kernel, (f') ful_up_kernel, (g') ful_down_kernel and (h') ful_emit_kernel as (e) ... (h) with
+// every node's float value in place of its state (value-equality pruning, inner nodes holding their largest child) and
+// 5 payload bytes per node; (h') places a brick's up to 585 nodes in parallel with a block scan.
+// Full tree read (octomap's readData; DESIGN.md §4b'), replacing the map: (s1) fr_excess_kernel over every node
+// (c_i = the popcount of its child mask), (r2), (s3) fr_parent_kernel, (s4) fr_node_kernel (depth up to 16, the leaf
+// checks and counts), one readback, then the tail the .bt read shares (replace_map) with (s5) fr_brick_kernel, (s6)
+// fr_fill_kernel and (s7) fr_leaf_kernel writing each leaf's own value.
 #include <algorithm>
 #include <cfloat>
 #include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <functional>
 #include <utility>
 #include <vector>
 
@@ -902,6 +912,219 @@ __global__ void __launch_bounds__(512) oct_emit_kernel(const unsigned* __restric
   }
 }
 
+// ---- full tree export (octomap's OcTree::write / writeData; DESIGN.md §4b''''''') -----------------------------------
+// Node states here: 0 no known voxel below, 1 leaf, 3 inner; values are float log-odds kept as their bits.
+constexpr int kFullNodeBytes = 5;
+
+// octomap's isNodeCollapsible on values (all 8 children exist, are leaves and compare equal as floats; the collapsed
+// leaf keeps child 0's bits) and updateInnerOccupancy (an inner node holds its largest child, the earliest on ties).
+// Children are added in child order.
+struct FullMerge {
+  int na = 0, nl = 0;
+  bool eq = true;
+  unsigned first = 0, best = 0;
+  __device__ __forceinline__ void add(int s, unsigned v) {
+    if (!s) return;
+    if (na == 0) {
+      first = best = v;
+    } else {
+      eq = eq && __uint_as_float(v) == __uint_as_float(first);
+      if (__uint_as_float(v) > __uint_as_float(best)) best = v;
+    }
+    ++na;
+    nl += s == 1;
+  }
+  __device__ __forceinline__ int state(bool may_prune, unsigned& v) const {
+    if (may_prune && nl == 8 && eq) {
+      v = first;
+      return 1;
+    }
+    v = best;
+    return na ? 3 : 0;
+  }
+};
+
+__device__ __forceinline__ void put_node(unsigned char* p, unsigned v, int mask) {
+  p[0] = (unsigned char)(v & 0xff), p[1] = (unsigned char)((v >> 8) & 0xff), p[2] = (unsigned char)((v >> 16) & 0xff);
+  p[3] = (unsigned char)(v >> 24), p[4] = (unsigned char)mask;
+}
+
+struct FullBrickTree {
+  unsigned v16[512], v15[64], v14[8];
+  unsigned char s16[512], s15[64], s14[8];
+  int n15[64], l15[64], n14[8], l14[8];
+  int st, nodes, leaves;  // the depth-13 node
+  unsigned val;
+};
+
+// One block of 512 threads: thread t reads the voxel of Morton index t, then the brick's levels 15, 14 and 13.
+__device__ void full_brick_tree(const unsigned* __restrict__ known, const float* __restrict__ lo, int b, FullBrickTree& T) {
+  const int t = threadIdx.x;
+  const int v = morton_local(t);
+  T.s16[t] = (unsigned char)((known[(size_t)b * 16 + (v >> 5)] >> (v & 31)) & 1u);
+  T.v16[t] = __float_as_uint(lo[(size_t)b * 512 + v]);
+  __syncthreads();
+  if (t < 64) {
+    FullMerge m;
+    for (int i = 0; i < 8; ++i) m.add(T.s16[8 * t + i], T.v16[8 * t + i]);
+    unsigned val;
+    const int st = m.state(true, val);
+    T.s15[t] = (unsigned char)st, T.v15[t] = val;
+    T.n15[t] = st == 3 ? 1 + m.na : st != 0;
+    T.l15[t] = st == 3 ? m.na : st != 0;
+  }
+  __syncthreads();
+  if (t < 8) {
+    FullMerge m;
+    int n = 0, l = 0;
+    for (int i = 0; i < 8; ++i) m.add(T.s15[8 * t + i], T.v15[8 * t + i]), n += T.n15[8 * t + i], l += T.l15[8 * t + i];
+    unsigned val;
+    const int st = m.state(true, val);
+    T.s14[t] = (unsigned char)st, T.v14[t] = val;
+    T.n14[t] = st == 3 ? 1 + n : st != 0;
+    T.l14[t] = st == 3 ? l : st != 0;
+  }
+  __syncthreads();
+  if (t == 0) {
+    FullMerge m;
+    int n = 0, l = 0;
+    for (int i = 0; i < 8; ++i) m.add(T.s14[i], T.v14[i]), n += T.n14[i], l += T.l14[i];
+    unsigned val;
+    const int st = m.state(true, val);
+    T.st = st, T.val = val;
+    T.nodes = st == 3 ? 1 + n : st != 0;
+    T.leaves = st == 3 ? l : st != 0;
+  }
+  __syncthreads();
+}
+
+// (e') one block per brick record, in pre-order: state, value and subtree totals (nodes, leaves)
+__global__ void __launch_bounds__(512) ful_brick_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
+                                                        Nodes N, unsigned* __restrict__ val) {
+  __shared__ FullBrickTree T;
+  const int r = blockIdx.x;
+  full_brick_tree(known, lo, N.pool[r], T);
+  if (threadIdx.x == 0) {
+    N.st[r] = (unsigned char)T.st;
+    val[r] = T.val;
+    N.nn[r] = (unsigned long long)T.nodes;
+    N.nl[r] = (unsigned long long)T.leaves;
+  }
+}
+
+// (f') levels 12 ... 0 as in (f), merging values; tot: nodes and leaves of the root (0 when no voxel is known)
+__global__ void __launch_bounds__(kTreeThreads) ful_up_kernel(Nodes N, unsigned* __restrict__ val, int n_b, int* levels,
+                                                              unsigned long long* tot) {
+  using Scan = cub::BlockScan<int, kTreeThreads>;
+  __shared__ typename Scan::TempStorage scan;
+  const int t = threadIdx.x;
+  int cb = 0, cn = n_b;  // the level below
+  if (t == 0) levels[2 * kBrickDepth] = 0, levels[2 * kBrickDepth + 1] = n_b;
+  for (int d = kBrickDepth - 1; d >= 0; --d) {
+    const int pb = cb + cn;
+    int pn = 0;
+    for (int c0 = 0; c0 < cn; c0 += kTreeThreads) {
+      const int i = c0 + t;
+      const int head = i < cn && (i == 0 || (N.code[cb + i] >> 3) != (N.code[cb + i - 1] >> 3));
+      int pos, total;
+      Scan(scan).ExclusiveSum(head, pos, total);
+      if (head) {
+        N.code[pb + pn + pos] = N.code[cb + i] >> 3;
+        N.first[pb + pn + pos] = cb + i;
+      }
+      pn += total;
+      __syncthreads();
+    }
+    for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
+      const int f = N.first[p], e = p + 1 < pb + pn ? N.first[p + 1] : pb;
+      FullMerge m;
+      unsigned long long n = 0, l = 0;
+      for (int c = f; c < e; ++c) m.add(N.st[c], val[c]), n += N.nn[c], l += N.nl[c];
+      unsigned v;
+      const int s = m.state(d > 0, v);  // the root is never pruned
+      N.st[p] = (unsigned char)s;
+      val[p] = v;
+      N.end[p] = e;
+      N.nn[p] = s == 3 ? n + 1 : (unsigned long long)(s != 0);
+      N.nl[p] = s == 3 ? l : (unsigned long long)(s != 0);
+    }
+    __syncthreads();
+    if (t == 0) levels[2 * d] = pb, levels[2 * d + 1] = pn;
+    cb = pb, cn = pn;
+  }
+  if (t == 0) tot[0] = N.nn[cb], tot[1] = N.nl[cb];
+}
+
+// (g') levels 0 ... 12: each inner node writes its 5 bytes and its leaf children's, and gives every child its offset (its
+// own + 5 + 5 x the earlier siblings' nodes); inner bricks write themselves in (h')
+__global__ void __launch_bounds__(kTreeThreads) ful_down_kernel(Nodes N, const unsigned* __restrict__ val,
+                                                                const int* __restrict__ levels,
+                                                                unsigned char* __restrict__ payload) {
+  const int t = threadIdx.x;
+  if (t == 0) N.off[levels[0]] = 0;
+  __syncthreads();
+  for (int d = 0; d < kBrickDepth; ++d) {
+    const int pb = levels[2 * d], pn = levels[2 * d + 1];
+    for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
+      if (N.st[p] != 3) continue;  // only an inner node's children are in the tree
+      const int f = N.first[p], e = N.end[p];
+      int mask = 0;
+      for (int c = f; c < e; ++c) mask |= (N.st[c] != 0) << (int)(N.code[c] & 7);
+      unsigned long long o = N.off[p];
+      put_node(payload + o, val[p], mask);
+      o += kFullNodeBytes;
+      for (int c = f; c < e; ++c) {
+        N.off[c] = o;
+        if (N.st[c] == 1) put_node(payload + o, val[c], 0);
+        o += kFullNodeBytes * N.nn[c];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// (h') one block per inner brick record: its nodes below depth 13 placed in parallel.  Thread t owns, in pre-order, the
+// depth-14 node starting at Morton index t (t % 64 == 0), the depth-15 one (t % 8 == 0) and voxel t, each when it is in
+// the tree; a block scan over the owned counts gives each its place.
+__global__ void __launch_bounds__(512) ful_emit_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
+                                                       Nodes N, unsigned char* __restrict__ payload) {
+  using Scan = cub::BlockScan<int, 512>;
+  __shared__ FullBrickTree T;
+  __shared__ typename Scan::TempStorage scan;
+  const int r = blockIdx.x;
+  if (N.st[r] != 3) return;  // a leaf brick is written by its parent in (g')
+  full_brick_tree(known, lo, N.pool[r], T);
+  const int t = threadIdx.x;
+  unsigned char* base = payload + N.off[r];
+  if (t == 0) {
+    int m = 0;
+    for (int i = 0; i < 8; ++i) m |= (T.s14[i] != 0) << i;
+    put_node(base, T.val, m);
+  }
+  const int i14 = t >> 6, i15 = t >> 3;
+  const bool a = (t & 63) == 0 && T.s14[i14] != 0;
+  const bool b = (t & 7) == 0 && T.s14[i14] == 3 && T.s15[i15] != 0;
+  const bool c = T.s14[i14] == 3 && T.s15[i15] == 3 && T.s16[t] != 0;
+  int idx;
+  Scan(scan).ExclusiveSum((int)a + (int)b + (int)c, idx);
+  unsigned char* p = base + (size_t)kFullNodeBytes * (1 + idx);
+  if (a) {
+    int m = 0;
+    if (T.s14[i14] == 3)
+      for (int i = 0; i < 8; ++i) m |= (T.s15[8 * i14 + i] != 0) << i;
+    put_node(p, T.v14[i14], m);
+    p += kFullNodeBytes;
+  }
+  if (b) {
+    int m = 0;
+    if (T.s15[i15] == 3)
+      for (int i = 0; i < 8; ++i) m |= (T.s16[8 * i15 + i] != 0) << i;
+    put_node(p, T.v15[i15], m);
+    p += kFullNodeBytes;
+  }
+  if (c) put_node(p, T.v16[t], 0);
+}
+
 // ---- .bt read (octomap's readBinary; DESIGN.md §4b'''''') ------------------------------------------------
 // Pair i of the payload is the i-th inner node in pre-order.  With c_i its inner children, the excess E_0 = 1,
 // E_{i+1} = E_i + c_i - 1 counts the inner nodes found but not yet read; the tree ends at the first i >= 1 with E_i = 0.
@@ -1115,6 +1338,190 @@ __global__ void rd_leaf_kernel(Dev D, Params P, const unsigned char* __restrict_
         atomicOr(&D.known[b * 16 + (row >> 5)], bitsw);
       }
   }
+}
+
+// ---- full tree read (octomap's AbstractOcTree::read / readData; DESIGN.md §4b''''''') -----------------------------
+// Node i of the payload is 5 bytes: its float value, then the mask of its existing children.  Every node is in the
+// stream, so with c_i = popcount(mask_i) the excess E_0 = 1, E_{i+1} = E_i + c_i - 1 counts the nodes found but not yet
+// read, and the tree ends at the first i >= 1 with E_i = 0.
+constexpr int kMaxFullExcess = 8 + 7 * 15;  // the largest excess of a tree whose nodes lie at depth <= 16
+constexpr int kBadValue = 2;
+
+__device__ __forceinline__ int full_mask(const unsigned char* pay, int i) { return pay[(size_t)kFullNodeBytes * i + 4]; }
+__device__ __forceinline__ unsigned full_value(const unsigned char* pay, int i) {
+  const unsigned char* p = pay + (size_t)kFullNodeBytes * i;
+  return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
+}
+
+// (s1) in[0] = 1 and in[i + 1] = c_i - 1: an inclusive sum gives E_0 ... E_n
+__global__ void fr_excess_kernel(const unsigned char* __restrict__ pay, int n, int* __restrict__ in) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) in[0] = 1;
+  if (i < n) in[i + 1] = __popc(full_mask(pay, i)) - 1;
+}
+
+// (s3) per node j >= 1 of the tree: its parent, the last i < j with E_i <= E_j, and its slot, the (E_p + c_p - 1 - E_j)-th
+// set bit of p's mask.  An excess above kMaxFullExcess proves a node below depth 16.
+__global__ void fr_parent_kernel(const unsigned char* __restrict__ pay, const int* __restrict__ ex,
+                                 const int* __restrict__ bmin, int n, int* __restrict__ par, unsigned char* __restrict__ slot,
+                                 ReadCounters* cnt) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n || j >= cnt->end) return;
+  const int e = ex[j];
+  if (e > kMaxFullExcess) {
+    atomicOr(&cnt->bad, kBadDepth);
+    return;
+  }
+  if (j == 0) {
+    par[0] = -1, slot[0] = 0;
+    return;
+  }
+  const int b0 = j / kReadThreads * kReadThreads;
+  int p = j - 1;
+  while (p >= b0 && ex[p] > e) --p;
+  if (p < b0) {  // E_0 = 1 <= e: some earlier block holds the parent
+    int b = j / kReadThreads - 1;
+    while (bmin[b] > e) --b;
+    p = b * kReadThreads + kReadThreads - 1;
+    while (ex[p] > e) --p;
+  }
+  const int m = full_mask(pay, p);
+  int rank = ex[p] + __popc(m) - 1 - e, s = 0;
+  for (; s < 8; ++s)
+    if (((m >> s) & 1) && rank-- == 0) break;
+  par[j] = p;
+  slot[j] = (unsigned char)s;
+}
+
+// (s4) per node j of the tree: depth and first key from at most 16 parents (more, or children at depth 16: too deep), its
+// depth-13 ancestor, and the counts: nodes with children, leaves by state, known voxels 8^(16-d) and bricks 8^(13-d) per
+// leaf at depth d (d <= 13), one brick for a node with children at depth 13.  A leaf's value must be finite.
+__global__ void __launch_bounds__(kReadThreads) fr_node_kernel(const unsigned char* __restrict__ pay,
+                                                              const int* __restrict__ par,
+                                                              const unsigned char* __restrict__ slot, int n, float l_occ,
+                                                              unsigned char* __restrict__ depth,
+                                                              unsigned long long* __restrict__ key, int* __restrict__ anc,
+                                                              long long* __restrict__ nb, ReadCounters* cnt) {
+  using Reduce = cub::BlockReduce<unsigned long long, kReadThreads>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long v[4] = {0, 0, 0, 0};  // nodes with children, free leaves, occupied leaves, known voxels
+  long long bricks = 0;
+  if (j < n && j < cnt->end && !cnt->bad) {
+    int d = 0, x = j, a1 = j, a2 = j, a3 = j;
+    unsigned long long slots = 0;
+    while (x != 0 && d < 16) {
+      if (d == 1) a1 = x;
+      if (d == 2) a2 = x;
+      if (d == 3) a3 = x;
+      slots |= (unsigned long long)slot[x] << (3 * d);
+      ++d;
+      x = par[x];
+    }
+    const int m = full_mask(pay, j);
+    const float val = __uint_as_float(full_value(pay, j));
+    if (x != 0 || (d == 16 && m)) {
+      atomicOr(&cnt->bad, kBadDepth);
+    } else if (!m && !isfinite(val)) {
+      atomicOr(&cnt->bad, kBadValue);
+    } else {
+      unsigned kx = 0, ky = 0, kz = 0;
+      for (int i = 0; i < d; ++i) {
+        const unsigned s = (unsigned)(slots >> (3 * i)) & 7u, b = (unsigned)(16 - d + i);
+        kx |= (s & 1u) << b, ky |= ((s >> 1) & 1u) << b, kz |= ((s >> 2) & 1u) << b;
+      }
+      depth[j] = (unsigned char)d;
+      key[j] = pack((int)kx, (int)ky, (int)kz);
+      anc[j] = d == kBrickDepth ? j : d == kBrickDepth + 1 ? a1 : d == kBrickDepth + 2 ? a2 : d == kBrickDepth + 3 ? a3 : -1;
+      if (m) {
+        v[0] = 1;
+        if (d == kBrickDepth) bricks = 1;
+      } else {
+        ++v[val >= l_occ ? 2 : 1];
+        v[3] = 1ull << (3 * (16 - d));
+        if (d <= kBrickDepth) bricks = 1LL << (3 * (kBrickDepth - d));
+      }
+    }
+  }
+  if (j <= n) nb[j] = bricks;
+  for (int k = 0; k < 4; ++k) {
+    const unsigned long long t = Reduce(tmp).Sum(v[k]);
+    if (threadIdx.x == 0 && t) atomicAdd(k == 0 ? &cnt->inner : k == 1 ? &cnt->free_leaves : k == 2 ? &cnt->occ_leaves
+                                                                                                     : &cnt->known, t);
+    __syncthreads();
+  }
+}
+
+// The node whose bricks hold brick b: the last j < end with boff[j] <= b (a node without bricks has the next one's boff).
+__device__ __forceinline__ int brick_owner(const long long* __restrict__ boff, int end, long long b) {
+  int lo = 0, hi = end - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (boff[mid] <= b) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// (s5) per new brick, in pre-order: its key and state (1: under a leaf at depth <= 13, in Morton order; 3: below a node
+// with children at depth 13)
+__global__ void fr_brick_kernel(const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
+                                const unsigned long long* __restrict__ key, const long long* __restrict__ boff, int end,
+                                int n_b, unsigned long long* __restrict__ bkey, unsigned char* __restrict__ bst) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= n_b) return;
+  const int j = brick_owner(boff, end, b);
+  const unsigned long long k0 = key[j], r = (unsigned long long)(b - boff[j]);
+  const bool mixed = depth[j] == kBrickDepth && full_mask(pay, j) != 0;
+  const int k[3] = {(int)(k0 & 0xffff) + (mixed ? 0 : squeeze3(r) << 3),
+                    (int)((k0 >> 16) & 0xffff) + (mixed ? 0 : squeeze3(r >> 1) << 3),
+                    (int)((k0 >> 32) & 0xffff) + (mixed ? 0 : squeeze3(r >> 2) << 3)};
+  bkey[b] = brick_key(k);
+  bst[b] = (unsigned char)(mixed ? 3 : 1);
+}
+
+// (s6) one block of 512 threads per new brick: a uniform brick holds its leaf's value and is all known, a mixed one starts
+// empty; marks and touched flags clear
+__global__ void __launch_bounds__(512) fr_fill_kernel(Dev D, const unsigned char* __restrict__ pay,
+                                                      const long long* __restrict__ boff, int end,
+                                                      const unsigned long long* __restrict__ bkey,
+                                                      const unsigned char* __restrict__ bst) {
+  __shared__ float v;
+  const int b = blockIdx.x, t = threadIdx.x, st = bst[b];
+  if (t == 0) v = st == 1 ? __uint_as_float(full_value(pay, brick_owner(boff, end, b))) : 0.0f;
+  __syncthreads();
+  D.lo[(size_t)b * 512 + t] = v;
+  if (t < 16) {
+    D.known[(size_t)b * 16 + t] = st == 3 ? 0u : ~0u;
+    D.mfree[(size_t)b * 16 + t] = 0u;
+    D.mocc[(size_t)b * 16 + t] = 0u;
+  }
+  if (t == 0) D.touched[b] = 0u, D.bkey[b] = bkey[b];
+}
+
+// (s7) per leaf at depth 14 ... 16: its 64, 8 or 1 voxels with its own value, in its depth-13 ancestor's brick
+__global__ void fr_leaf_kernel(Dev D, const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
+                               const unsigned long long* __restrict__ key, const int* __restrict__ anc,
+                               const long long* __restrict__ boff, int end) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= end) return;
+  const int d = depth[j];
+  if (d <= kBrickDepth || full_mask(pay, j)) return;
+  const size_t b = (size_t)boff[anc[j]];
+  const float v = __uint_as_float(full_value(pay, j));
+  const unsigned long long k0 = key[j];
+  const int side = 1 << (16 - d);
+  const int x0 = (int)(k0 & 7), y0 = (int)((k0 >> 16) & 7), z0 = (int)((k0 >> 32) & 7);
+  for (int z = z0; z < z0 + side; ++z)
+    for (int y = y0; y < y0 + side; ++y) {
+      unsigned bitsw = 0;
+      const int row = (y << 3) | (z << 6);  // side <= 4 voxels of one row share a known word
+      for (int x = x0; x < x0 + side; ++x) {
+        D.lo[b * 512 + row + x] = v;
+        bitsw |= 1u << ((row + x) & 31);
+      }
+      atomicOr(&D.known[b * 16 + (row >> 5)], bitsw);
+    }
 }
 
 int code(cudaError_t e) {
@@ -1510,6 +1917,53 @@ int download_octree(const Octree& t, unsigned char* payload, float* centres4, un
   return LS_OK;
 }
 
+namespace {
+
+// The tail of a read whose stream is valid and numbers n_b new bricks: `keys` writes their keys and states to rd_bkey /
+// rd_bst, the pool grows and the new hash is built beside the old one, so the map is unchanged if any of that fails; only
+// then does `fill` write the new bricks (n_b > 0), and the map takes the new hash, n_b bricks and `known` voxels.
+int replace_map(Map& m, int n_b, long long known, const std::function<int()>& keys, const std::function<int(const Dev&)>& fill,
+                const char** why, cudaStream_t st, uint64_t* launches) {
+  const char* nomem = "the map cannot grow";
+  int rc;
+  if (n_b > 0) {
+    cudaError_t e = m.rd_bkey.capacity() >= (size_t)n_b ? cudaSuccess : m.rd_bkey.reserve(n_b, n_b + n_b / 8);
+    if (e == cudaSuccess && m.rd_bst.capacity() < (size_t)n_b) e = m.rd_bst.reserve(n_b, n_b + n_b / 8);
+    if (e != cudaSuccess) {
+      m.rd_bkey.reset(), m.rd_bst.reset();
+      return *why = nomem, code(e);
+    }
+    if ((rc = keys())) return rc;
+  }
+  if (n_b > m.pool_cap()) {
+    long long cap = m.pool_cap() > 0 ? m.pool_cap() : 1;
+    while (cap < n_b) cap *= 2;
+    if ((rc = grow_pool(m, (int)cap, st))) return *why = nomem, rc;
+  }
+  int tab = 1024;
+  while (tab < 2 * n_b) tab *= 2;
+  ls::Buffer<unsigned long long> tkeys;
+  ls::Buffer<int> tvals;
+  if ((rc = build_table(m, m.rd_bkey.get(), n_b, tab, tkeys, tvals, st, launches))) return *why = nomem, rc;
+  // Only now is the map written.
+  if (n_b > 0 && (rc = fill(dev_of(m)))) return rc;
+  if (m.pool_n > n_b) {  // bricks past the new pool start empty, as a grown pool's do
+    const size_t a = (size_t)n_b, k = (size_t)(m.pool_n - n_b);
+    OCC_TRY(cudaMemsetAsync(m.lo.get() + a * 512, 0, k * 512 * sizeof(float), st));
+    OCC_TRY(cudaMemsetAsync(m.known.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.mfree.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.mocc.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.touched.get() + a, 0, k * sizeof(unsigned), st));
+  }
+  OCC_TRY(cudaStreamSynchronize(st));
+  m.tab_keys = std::move(tkeys), m.tab_vals = std::move(tvals);
+  m.pool_n = n_b;
+  m.n_known = known;
+  return LS_OK;
+}
+
+}  // namespace
+
 int read_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes, ReadCounters* out,
                 const char** why, cudaStream_t st, uint64_t* launches) {
   std::memset(out, 0, sizeof(ReadCounters));
@@ -1559,51 +2013,130 @@ int read_octree(Map& m, const Params& P, const unsigned char* payload, long long
     end = c.end;
     n_b = (int)c.bricks;
   }
-  // The file is valid: grow, then build the new hash beside the old one; the map is still unchanged if either fails.
-  const char* nomem = "the map cannot grow";
-  if (n_b > 0) {
-    cudaError_t e = m.rd_bkey.capacity() >= (size_t)n_b ? cudaSuccess : m.rd_bkey.reserve(n_b, n_b + n_b / 8);
-    if (e == cudaSuccess && m.rd_bst.capacity() < (size_t)n_b) e = m.rd_bst.reserve(n_b, n_b + n_b / 8);
-    if (e != cudaSuccess) {
-      m.rd_bkey.reset(), m.rd_bst.reset();
-      return *why = nomem, code(e);
-    }
-    rd_brick_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_boff.get(), end,
-                                                       n_b, m.rd_bkey.get(), m.rd_bst.get());
-    OCC_LAUNCHED();
+  return replace_map(
+      m, n_b, (long long)out->known,
+      [&]() -> int {
+        rd_brick_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_boff.get(),
+                                                           end, n_b, m.rd_bkey.get(), m.rd_bst.get());
+        OCC_LAUNCHED();
+        return LS_OK;
+      },
+      [&](const Dev& D) -> int {
+        rd_fill_kernel<<<n_b, 512, 0, st>>>(D, P, m.rd_bkey.get(), m.rd_bst.get());
+        OCC_LAUNCHED();
+        rd_leaf_kernel<<<(end + 255) / 256, 256, 0, st>>>(D, P, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(),
+                                                          m.rd_anc.get(), m.rd_boff.get(), end);
+        OCC_LAUNCHED();
+        return LS_OK;
+      },
+      why, st, launches);
+}
+
+int build_full_octree(const Map& m, Octree& t, cudaStream_t st, uint64_t* launches) {
+  t.nodes = t.bytes = t.leaves = 0;
+  const int n_b = m.pool_n;
+  if (n_b == 0) return LS_OK;
+  int rc;
+  if ((rc = reserve_tree(t, n_b, st))) return rc;
+  if (t.val.capacity() < t.code.capacity()) {
+    OCC_TRY(cudaStreamSynchronize(st));
+    t.val.reset();
+    OCC_TRY(t.val.reserve(t.code.capacity(), t.code.capacity()));
   }
-  if (n_b > m.pool_cap()) {
-    long long cap = m.pool_cap() > 0 ? m.pool_cap() : 1;
-    while (cap < n_b) cap *= 2;
-    if ((rc = grow_pool(m, (int)cap, st))) return *why = nomem, rc;
-  }
-  int tab = 1024;
-  while (tab < 2 * n_b) tab *= 2;
-  ls::Buffer<unsigned long long> keys;
-  ls::Buffer<int> vals;
-  if ((rc = build_table(m, m.rd_bkey.get(), n_b, tab, keys, vals, st, launches))) return *why = nomem, rc;
-  // Only now is the map written.
-  const Dev D = dev_of(m);
-  if (n_b > 0) {
-    rd_fill_kernel<<<n_b, 512, 0, st>>>(D, P, m.rd_bkey.get(), m.rd_bst.get());
-    OCC_LAUNCHED();
-    rd_leaf_kernel<<<(end + 255) / 256, 256, 0, st>>>(D, P, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(),
-                                                      m.rd_boff.get(), end);
-    OCC_LAUNCHED();
-  }
-  if (m.pool_n > n_b) {  // bricks past the new pool start empty, as a grown pool's do
-    const size_t a = (size_t)n_b, k = (size_t)(m.pool_n - n_b);
-    OCC_TRY(cudaMemsetAsync(m.lo.get() + a * 512, 0, k * 512 * sizeof(float), st));
-    OCC_TRY(cudaMemsetAsync(m.known.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mfree.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mocc.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.touched.get() + a, 0, k * sizeof(unsigned), st));
-  }
+  const Nodes N = nodes_of(t);
+  oct_code_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.bkey.get(), n_b, t.sort_k.get(), t.sort_v.get());
+  OCC_LAUNCHED();
+  size_t bytes = t.cub_bytes;
+  OCC_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp.get(), bytes, t.sort_k.get(), t.code.get(), t.sort_v.get(), t.pool.get(), n_b,
+                                          0, 3 * kBrickDepth, st));
+  ++*launches;
+  ful_brick_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, t.val.get());
+  OCC_LAUNCHED();
+  ful_up_kernel<<<1, kTreeThreads, 0, st>>>(N, t.val.get(), n_b, t.levels.get(), t.tot_dev.get());
+  OCC_LAUNCHED();
+  OCC_TRY(cudaMemcpyAsync(t.tot_host.get(), t.tot_dev.get(), 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   OCC_TRY(cudaStreamSynchronize(st));
-  m.tab_keys = std::move(keys), m.tab_vals = std::move(vals);
-  m.pool_n = n_b;
-  m.n_known = (long long)out->known;
+  const long long nodes = (long long)t.tot_host.get()[0], leaves = (long long)t.tot_host.get()[1];
+  if (nodes == 0) return LS_OK;
+  const long long pay = kFullNodeBytes * nodes;
+  if ((rc = reserve_tree_outputs(t, pay, 0, st))) return rc;
+  ful_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.val.get(), t.levels.get(), t.payload.get());
+  OCC_LAUNCHED();
+  ful_emit_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, t.payload.get());
+  OCC_LAUNCHED();
+  OCC_TRY(cudaStreamSynchronize(st));
+  t.nodes = nodes, t.bytes = pay, t.leaves = leaves;
   return LS_OK;
+}
+
+int read_full_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes,
+                     ReadCounters* out, const char** why, cudaStream_t st, uint64_t* launches) {
+  std::memset(out, 0, sizeof(ReadCounters));
+  *why = "";
+  int rc, n_b = 0, end = 0;
+  // A valid tree has `nodes` nodes, so later bytes cannot belong to it.
+  const long long count = std::min(bytes / kFullNodeBytes, nodes);
+  if (nodes > 0 && count == 0) return *why = "the payload is truncated", LS_ERR_ARG;
+  if (count > kMaxReadPairs) return *why = "more than 2^30 nodes", LS_ERR_NOMEM;
+  if (count > 0) {
+    const int n = (int)count;
+    if ((rc = reserve_read(m, n, kFullNodeBytes * (size_t)n, st))) return *why = "out of device memory for the parse", rc;
+    ReadCounters* cnt = m.rd_cnt_dev.get();
+    ReadCounters init{};
+    init.end = INT_MAX;
+    *m.rd_cnt_host.get() = init;
+    OCC_TRY(cudaMemcpyAsync(cnt, m.rd_cnt_host.get(), sizeof(ReadCounters), cudaMemcpyHostToDevice, st));
+    OCC_TRY(cudaMemcpyAsync(m.rd_pay.get(), payload, kFullNodeBytes * (size_t)n, cudaMemcpyHostToDevice, st));
+    const int blocks = (n + kReadThreads) / kReadThreads;  // n + 1 items
+    fr_excess_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), n, m.rd_tmp.get());
+    OCC_LAUNCHED();
+    size_t tb = m.rd_cub_bytes;
+    OCC_TRY(cub::DeviceScan::InclusiveSum(m.rd_cub.get(), tb, m.rd_tmp.get(), m.rd_ex.get(), n + 1, st));
+    ++*launches;
+    rd_end_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_ex.get(), n, m.rd_bmin.get(), cnt);
+    OCC_LAUNCHED();
+    fr_parent_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_ex.get(), m.rd_bmin.get(), n, m.rd_par.get(),
+                                                      m.rd_slot.get(), cnt);
+    OCC_LAUNCHED();
+    fr_node_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_par.get(), m.rd_slot.get(), n, P.l_occ,
+                                                    m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(), m.rd_nb.get(), cnt);
+    OCC_LAUNCHED();
+    tb = m.rd_cub_bytes;
+    OCC_TRY(cub::DeviceScan::ExclusiveSum(m.rd_cub.get(), tb, m.rd_nb.get(), m.rd_boff.get(), n + 1, st));
+    ++*launches;
+    OCC_TRY(cudaMemcpyAsync(&cnt->bricks, m.rd_boff.get() + n, sizeof(long long), cudaMemcpyDeviceToDevice, st));
+    OCC_TRY(cudaMemcpyAsync(m.rd_cnt_host.get(), cnt, sizeof(ReadCounters), cudaMemcpyDeviceToHost, st));
+    OCC_TRY(cudaStreamSynchronize(st));
+    const ReadCounters c = *m.rd_cnt_host.get();
+    if (c.end == INT_MAX)
+      return *why = count < nodes ? "the payload is truncated" : "the header's size does not count the payload's nodes",
+             LS_ERR_ARG;
+    if (c.bad & kBadDepth) return *why = "a node at depth 16 with children", LS_ERR_ARG;
+    if (c.bad & kBadValue) return *why = "a leaf value that is NaN or infinite", LS_ERR_ARG;
+    if ((long long)c.end != nodes) return *why = "the header's size does not count the payload's nodes", LS_ERR_ARG;
+    if (c.bricks > kMaxReadBricks) return *why = "the file covers more bricks than the map can index", LS_ERR_NOMEM;
+    *out = c;
+    out->nodes = (unsigned long long)c.end;
+    end = c.end;
+    n_b = (int)c.bricks;
+  }
+  return replace_map(
+      m, n_b, (long long)out->known,
+      [&]() -> int {
+        fr_brick_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_boff.get(),
+                                                           end, n_b, m.rd_bkey.get(), m.rd_bst.get());
+        OCC_LAUNCHED();
+        return LS_OK;
+      },
+      [&](const Dev& D) -> int {
+        fr_fill_kernel<<<n_b, 512, 0, st>>>(D, m.rd_pay.get(), m.rd_boff.get(), end, m.rd_bkey.get(), m.rd_bst.get());
+        OCC_LAUNCHED();
+        fr_leaf_kernel<<<(end + 255) / 256, 256, 0, st>>>(D, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(),
+                                                          m.rd_boff.get(), end);
+        OCC_LAUNCHED();
+        return LS_OK;
+      },
+      why, st, launches);
 }
 
 namespace {

@@ -83,7 +83,8 @@ struct Octree {
   ls::Buffer<int> pool;    // bricks: pool index (its capacity is the group's, in bricks)
   ls::Buffer<unsigned long long> code;  // Morton code of the node at its depth
   ls::Buffer<int> first, end;           // upper nodes: their children's records [first, end)
-  ls::Buffer<unsigned char> st;         // 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner
+  ls::Buffer<unsigned char> st;         // 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner (full tree: 1 leaf)
+  ls::Buffer<unsigned> val;             // full tree only: each node's float log-odds bits
   ls::Buffer<unsigned long long> n_nodes, n_bytes, n_leaves;  // subtree totals
   ls::Buffer<unsigned long long> off, loff;  // payload byte and occupied-leaf offsets in pre-order
   ls::Buffer<unsigned long long> sort_k;
@@ -95,7 +96,7 @@ struct Octree {
   ls::Buffer<unsigned char> payload;
   ls::Buffer<float4> centres;  // with depths
   ls::Buffer<unsigned char> depths;
-  long long nodes = 0, bytes = 0, leaves = 0;  // of the last build
+  long long nodes = 0, bytes = 0, leaves = 0;  // of the last build (full tree: every leaf)
 };
 
 // All return LS_OK, LS_ERR_NOMEM or LS_ERR_CUDA (include/ls_b200.h) and count their launches in *launches.
@@ -115,6 +116,10 @@ size_t device_bytes(const Map& m);
 int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches);
 // Copies the last build's payload (t.bytes) and, each when not NULL, its t.leaves centres {x, y, z, 1} and depths.
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st);
+// Builds octomap's full tree of the map (OcTree::write's payload, DESIGN.md §4b') into t: every node's float log-odds
+// and child mask, 5 bytes per node in pre-order, pruned by value.  t.nodes / bytes / leaves hold the counts; the payload
+// stays on the device (download_octree copies it).  Reads the map only.  Synchronous.
+int build_full_octree(const Map& m, Octree& t, cudaStream_t st, uint64_t* launches);
 
 // octomap's readBinary of a .bt payload (`bytes` bytes after "data\n", `nodes` the header's size) into the map, replacing
 // it (DESIGN.md §4b'''''').  P: the map's parameters at the file's resolution.  Synchronous.  Validates the
@@ -123,6 +128,13 @@ int download_octree(const Octree& t, unsigned char* payload, float* centres4, un
 // why).  *out: the counts.
 int read_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes, ReadCounters* out,
                 const char** why, cudaStream_t st, uint64_t* launches);
+
+// octomap's readData of a full-tree payload (`bytes` bytes after "data\n", `nodes` the header's size) into the map,
+// replacing it: every leaf's voxels take its value verbatim.  P: the map's parameters at the file's resolution (P.l_occ
+// classifies the leaves in *out).  Validation and errors as read_octree, and a leaf value that is not finite is LS_ERR_ARG;
+// the map is unchanged after any error.  out->inner: the nodes with children.
+int read_full_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes,
+                     ReadCounters* out, const char** why, cudaStream_t st, uint64_t* launches);
 
 // Queries (oracle/QUERIES.md), reading the map only.  Synchronous; host inputs and outputs, *visited the voxel states the
 // kernels read.  n <= 0 launches nothing.

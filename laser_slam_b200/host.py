@@ -287,6 +287,11 @@ class OccupancyMap:
             L.lsh_occupancy_occupied_cloud.argtypes = [vp, vp, ci]
             L.lsh_occupancy_write_binary.argtypes = [vp, ctypes.c_char_p]
             L.lsh_occupancy_read_binary.argtypes = [vp, ctypes.c_char_p]
+            L.lsh_occupancy_write_full.argtypes = [vp, ctypes.c_char_p]
+            L.lsh_occupancy_read_full.argtypes = [vp, ctypes.c_char_p]
+            L.lsh_occupancy_write_full_data.argtypes = [vp, vp, i64, ctypes.POINTER(i64)]
+            L.lsh_occupancy_write_full_data.restype = i64
+            L.lsh_occupancy_read_full_data.argtypes = [vp, vp, i64, i64, ctypes.c_double]
             L.lsh_occupancy_occupied_leaf_cloud.argtypes = [vp, vp, ci]
             L.lsh_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp]
             L.lsh_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, ci, vp, vp]
@@ -332,6 +337,36 @@ class OccupancyMap:
     def read_binary(self, path):
         """readBinary: the .bt file replaces the map.  False, with the map unchanged, when the file is refused."""
         rc = lib().lsh_occupancy_read_binary(self._h, os.fsencode(path))
+        if rc == -1:  # LS_ERR_ARG
+            return False
+        self._check(rc)
+        return True
+
+    def write_full(self, path):
+        """write: the map as an octomap .ot file (every node's log-odds)."""
+        self._check(lib().lsh_occupancy_write_full(self._h, os.fsencode(path)))
+
+    def read_full(self, path):
+        """read: the .ot file replaces the map.  False, with the map unchanged, when the file is refused."""
+        rc = lib().lsh_occupancy_read_full(self._h, os.fsencode(path))
+        if rc == -1:  # LS_ERR_ARG
+            return False
+        self._check(rc)
+        return True
+
+    def write_data(self):
+        """writeData: (nodes, payload bytes) of the full tree."""
+        nodes = ctypes.c_int64(0)
+        n = self._check(lib().lsh_occupancy_write_full_data(self._h, None, 0, ctypes.byref(nodes)))
+        out = np.zeros(max(n, 1), np.uint8)
+        self._check(lib().lsh_occupancy_write_full_data(self._h, out.ctypes.data, n, ctypes.byref(nodes)))
+        return nodes.value, out[:n].tobytes()
+
+    def read_data(self, payload, nodes, resolution):
+        """readData: a full-tree payload replaces the map.  False, with the map unchanged, when it is refused."""
+        buf = np.frombuffer(bytes(payload), np.uint8)
+        rc = lib().lsh_occupancy_read_full_data(self._h, buf.ctypes.data if len(buf) else None, len(buf), int(nodes),
+                                                float(resolution))
         if rc == -1:  # LS_ERR_ARG
             return False
         self._check(rc)

@@ -473,6 +473,53 @@ int lsh_occupancy_read_binary(void* ov, const char* path) {
   }
 }
 
+// write (.ot); 0 on success, LS_ERR_ARG when the file cannot be written
+int lsh_occupancy_write_full(void* ov, const char* path) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    return h->map->write(path) ? 0 : LS_ERR_ARG;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// read (.ot); 0 on success, LS_ERR_ARG when it returns false
+int lsh_occupancy_read_full(void* ov, const char* path) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    return h->map->read(path) ? 0 : LS_ERR_ARG;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// writeData: the payload's size (0: empty map; nothing copied when it exceeds cap) and node count; LS_ERR_STATE on error
+int64_t lsh_occupancy_write_full_data(void* ov, uint8_t* out, int64_t cap, int64_t* nodes) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<uint8_t> payload;
+    h->map->writeData(&payload, nodes);
+    if ((int64_t)payload.size() <= cap && !payload.empty()) std::memcpy(out, payload.data(), payload.size());
+    return (int64_t)payload.size();
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// readData; 0 on success, LS_ERR_ARG when it returns false
+int lsh_occupancy_read_full_data(void* ov, const uint8_t* payload, int64_t bytes, int64_t nodes, double resolution) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    return h->map->readData(std::vector<uint8_t>(payload, payload + bytes), nodes, resolution) ? 0 : LS_ERR_ARG;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
 // getCellProbabilityPoint per point (single queries): status and probability; 0 or LS_ERR_STATE
 int lsh_occupancy_cell_status(void* ov, const double* pts3, int n, int8_t* status, double* probability) {
   OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);

@@ -108,6 +108,46 @@ bool OccupancyMap::readBinary(const std::string& filename) {
   return true;
 }
 
+bool OccupancyMap::write(const std::string& filename) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  const int rc = ls_occupancy_write_octomap_full(map_, filename.c_str(), NULL);
+  if (rc == LS_ERR_ARG) return false;
+  throwOnError(ctx_, rc, "ls_occupancy_write_octomap_full");
+  return true;
+}
+
+bool OccupancyMap::read(const std::string& filename) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_octomap_read_stats stats;
+  const int rc = ls_occupancy_read_octomap_full(map_, filename.c_str(), &stats);
+  if (rc == LS_ERR_ARG || rc == LS_ERR_NOMEM) return false;
+  throwOnError(ctx_, rc, "ls_occupancy_read_octomap_full");
+  params_.resolution = stats.resolution;
+  return true;
+}
+
+void OccupancyMap::writeData(std::vector<uint8_t>* payload, int64_t* nodes) {
+  if (payload == NULL || nodes == NULL) throw std::invalid_argument("null output");
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_full_octree_stats st;
+  throwOnError(ctx_, ls_occupancy_build_full_octree(map_, &st), "ls_occupancy_build_full_octree");
+  payload->resize((size_t)st.payload_bytes);
+  throwOnError(ctx_, ls_occupancy_download_full_octree(map_, payload->data(), st.payload_bytes),
+               "ls_occupancy_download_full_octree");
+  *nodes = st.nodes;
+}
+
+bool OccupancyMap::readData(const std::vector<uint8_t>& payload, int64_t nodes, double resolution) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_octomap_read_stats stats;
+  const int rc = ls_occupancy_read_full_octree(map_, payload.empty() ? NULL : payload.data(), (int64_t)payload.size(), nodes,
+                                               resolution, &stats);
+  if (rc == LS_ERR_ARG || rc == LS_ERR_NOMEM) return false;
+  throwOnError(ctx_, rc, "ls_occupancy_read_full_octree");
+  params_.resolution = stats.resolution;
+  return true;
+}
+
 void OccupancyMap::getOccupiedLeafCloud(DataPoints* cloud) {
   if (cloud == NULL) throw std::invalid_argument("null output");
   std::lock_guard<std::mutex> lock(mutex_);
