@@ -98,6 +98,25 @@ class OccupancyMap {
                 std::vector<int>* results, std::vector<kindr::minimal::Position>* ends, bool ignore_unknown = false,
                 double max_range = -1.0) const;
 
+  // ---- edits: volumetric_mapping's WorldBase map calls on the device map (ls_occupancy_set_boxes / _clear / _box_voxels /
+  // _bounds; rules in DESIGN.md §4b'''''''').  Errors throw, as every call here.
+  // setFree / setOccupied: every voxel the box's loop reaches becomes known with clamping_thres_min / _max.
+  void setFree(const kindr::minimal::Position& position, const kindr::minimal::Position& bounding_box_size);
+  void setOccupied(const kindr::minimal::Position& position, const kindr::minimal::Position& bounding_box_size);
+  // (new) Both in one call, in order: the last box covering a voxel decides it.  stats may be NULL.
+  void setBoxes(const std::vector<kindr::minimal::Position>& positions,
+                const std::vector<kindr::minimal::Position>& bounding_box_sizes, const std::vector<bool>& occupied,
+                ls_occupancy_edit_stats* stats = NULL);
+  // resetMap: no known voxel; the parameters and the device memory stay.
+  void resetMap();
+  // The occupied voxels the box's loop reaches, in loop order, as their centres ({x, y, z, 1}).
+  void getOccupiedPointcloudInBoundingBox(const kindr::minimal::Position& center,
+                                          const kindr::minimal::Position& bounding_box_size, DataPoints* output_cloud) const;
+  // getMetricMin / getMetricMax over the known voxels (zeros when none), their difference and midpoint.
+  void getMapBounds(kindr::minimal::Position* min_bound, kindr::minimal::Position* max_bound) const;
+  kindr::minimal::Position getMapSize() const;
+  kindr::minimal::Position getMapCenter() const;
+
  private:
   CellStatus cellStatus(const kindr::minimal::Position& point, float* log_odds) const;
   void download(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds, std::vector<float>* centres4) const;

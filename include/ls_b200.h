@@ -521,6 +521,41 @@ int ls_occupancy_line_status(ls_occupancy* om, const double* starts3, const doub
 int ls_occupancy_cast_rays(ls_occupancy* om, const float* origins3, const float* directions3, int n, int ignore_unknown,
                            double max_range, int8_t* result, float* ends3, ls_occupancy_query_stats* stats);
 
+/* Edits of the map: volumetric_mapping's setFree / setOccupied (OctomapWorld::setLogOddsBoundingBox, the set-box-occupancy
+ * service), resetMap, getOccupiedPointcloudInBoundingBox and the extent getMapBounds reads (DESIGN.md §4b'''''''').  Rules:
+ *   box loop    per axis in double: c = res * floor(p / res) + res / 2 (a division), then x = (c - s/2) + 0.001; x <=
+ *               (c + s/2) - 0.001; x += res, y inside x and z innermost; each point is cast to float and keyed as above
+ *               (floor(c * (1/resolution)) + 32768); a point with an invalid key is skipped.  A size of 0 covers nothing
+ *   set         every voxel a loop point keys becomes known with L_min (setFree) or L_max (setOccupied); later inserts update
+ *               it as usual.  Boxes apply in call order: the last box covering a voxel decides its value
+ *   reset       no known voxel, no brick; resolution, parameters and device memory stay (device_bytes is unchanged).  An
+ *               insert afterwards equals the same insert into a new map
+ *   box voxels  per loop point (in loop order, repeats kept) whose voxel is occupied (LS_OCC_OCCUPIED) or known
+ *               (LS_OCC_KNOWN): its packed key, log-odds and voxel centre {x, y, z, 1}
+ *   bounds      per axis over the known keys: min = (double)centre(kmin) - res/2, max = ((double)centre(kmax) - res/2) + res,
+ *               centre(k) the float voxel centre; all zeros for a map without known voxels
+ * Calls run on the map's stream, are synchronous and are legal between ls_icp_register_submap_batch_begin and _end.  A
+ * successful set or reset invalidates both cached tree builds.  Errors: LS_ERR_ARG for n < 0, a NULL array, a centre or
+ * size that is not finite, a negative size, a box axis of more than 2^17 loop points (or a box of more than 2^31 - 1 for
+ * box voxels); LS_ERR_NOMEM, before anything is allocated, when the bricks a set covers and those in use exceed 2^29, or
+ * when the map cannot grow.  Every box is checked before any work, so one bad box refuses the whole call; after any error
+ * the known voxels, their values and both cached builds are unchanged. */
+typedef struct ls_occupancy_edit_stats {
+  int64_t voxels_set;   /* loop points with a valid key, summed over the boxes (repeats counted) */
+  int64_t new_known;    /* voxels that became known */
+  int64_t known_voxels, bricks, device_bytes; /* of the map after the call */
+  float device_ms;      /* the call on the map's stream */
+} ls_occupancy_edit_stats;
+/* n boxes: centres3 / sizes3 double triples; occupied[i] 0 = setFree, otherwise setOccupied.  stats may be NULL. */
+int ls_occupancy_set_boxes(ls_occupancy* om, const double* centres3, const double* sizes3, const int8_t* occupied, int n,
+                           ls_occupancy_edit_stats* stats);
+int ls_occupancy_clear(ls_occupancy* om);
+/* which: LS_OCC_KNOWN / LS_OCC_OCCUPIED; outputs may be NULL; *n always set; LS_ERR_ARG without a copy when *n > cap, so
+ * cap = 0 asks for the count. */
+int ls_occupancy_box_voxels(ls_occupancy* om, const double center3[3], const double size3[3], int which, uint64_t* keys,
+                            float* log_odds, float* centres4, int64_t cap, int64_t* n);
+int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]);
+
 /* ---- per-scan input filters (reference laser_slam/src/laser_track.cpp:24-30 loads them from
  * LaserTrackParams::icp_input_filters_file, :81 and :146 apply them to every scan before it is stored) ----------------
  * A chain is an array of ls_point_filter records applied in order; each filter sees the cloud the previous one produced,

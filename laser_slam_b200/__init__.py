@@ -116,6 +116,13 @@ class OctomapReadStats(ctypes.Structure):
                 ("resolution", ctypes.c_double), ("device_ms", ctypes.c_float)]
 
 
+class OccupancyEditStats(ctypes.Structure):
+    """ls_occupancy_edit_stats: loop points set, voxels newly known, and the map's known voxels, bricks and device bytes
+    after the call."""
+    _fields_ = [("voxels_set", ctypes.c_int64), ("new_known", ctypes.c_int64), ("known_voxels", ctypes.c_int64),
+                ("bricks", ctypes.c_int64), ("device_bytes", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
 class OccupancyQueryStats(ctypes.Structure):
     _fields_ = [("keys_visited", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
@@ -241,6 +248,10 @@ def lib():
         L.ls_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp, QS]
         L.ls_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, vp, vp, QS]
         L.ls_occupancy_cast_rays.argtypes = [vp, vp, vp, ci, ci, ctypes.c_double, vp, vp, QS]
+        L.ls_occupancy_set_boxes.argtypes = [vp, vp, vp, vp, ci, ctypes.POINTER(OccupancyEditStats)]
+        L.ls_occupancy_clear.argtypes = [vp]
+        L.ls_occupancy_box_voxels.argtypes = [vp, vp, vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
+        L.ls_occupancy_bounds.argtypes = [vp, vp, vp]
         _lib = L
     return _lib
 
@@ -1016,6 +1027,60 @@ class OccupancyMap:
                                                      float(max_range), r.ctypes.data, ends.ctypes.data,
                                                      ctypes.byref(self.last_query)))
         return r[:n].copy(), ends[:n].copy()
+
+    # ---- edits (ls_occupancy_set_boxes / _clear / _box_voxels / _bounds)
+    def set_boxes(self, centres, sizes, occupied):
+        """volumetric_mapping's setFree / setOccupied of n boxes in order ((n,3) centres and sizes, taken as float64; occupied
+        (n,) truthy for setOccupied): every voxel a box's loop reaches becomes known with clamp_min or clamp_max, the last
+        box deciding.  Returns OccupancyEditStats; on an error no voxel changes."""
+        c = np.ascontiguousarray(np.asarray(centres, np.float64).reshape(-1, 3))
+        s = np.ascontiguousarray(np.asarray(sizes, np.float64).reshape(-1, 3))
+        o = np.ascontiguousarray(np.asarray(occupied).reshape(-1).astype(bool).astype(np.int8))
+        if not len(c) == len(s) == len(o):
+            raise ValueError(f"{len(c)} centres, {len(s)} sizes and {len(o)} occupied flags")
+        st = OccupancyEditStats()
+        self.ctx._check(lib().ls_occupancy_set_boxes(self._h, c.ctypes.data, s.ctypes.data, o.ctypes.data, len(c),
+                                                     ctypes.byref(st)))
+        return st
+
+    def set_free(self, centres, sizes):
+        """setFree of each box ((n,3) or (3,) centres and sizes)."""
+        c = np.asarray(centres, np.float64).reshape(-1, 3)
+        return self.set_boxes(c, sizes, np.zeros(len(c), bool))
+
+    def set_occupied(self, centres, sizes):
+        """setOccupied of each box ((n,3) or (3,) centres and sizes)."""
+        c = np.asarray(centres, np.float64).reshape(-1, 3)
+        return self.set_boxes(c, sizes, np.ones(len(c), bool))
+
+    def clear(self):
+        """resetMap: no known voxel and no brick; the parameters and the device memory stay."""
+        self.ctx._check(lib().ls_occupancy_clear(self._h))
+
+    def box_voxels(self, center, size, which=OCC_OCCUPIED):
+        """getOccupiedPointcloudInBoundingBox (which=OCC_OCCUPIED) or every known voxel (OCC_KNOWN) the box's loop reaches,
+        in loop order with repeats: (keys uint64, log-odds float32, voxel centres (n,4) float32)."""
+        c = np.ascontiguousarray(np.asarray(center, np.float64).reshape(3))
+        s = np.ascontiguousarray(np.asarray(size, np.float64).reshape(3))
+        n = ctypes.c_int64(0)
+        rc = lib().ls_occupancy_box_voxels(self._h, c.ctypes.data, s.ctypes.data, int(which), None, None, None, 0,
+                                           ctypes.byref(n))
+        if rc != LS_ERR_ARG or n.value == 0:
+            self.ctx._check(rc)
+        m = n.value
+        keys = np.empty(max(m, 1), np.uint64)
+        lo = np.empty(max(m, 1), np.float32)
+        cen = np.empty((max(m, 1), 4), np.float32)
+        if m > 0:
+            self.ctx._check(lib().ls_occupancy_box_voxels(self._h, c.ctypes.data, s.ctypes.data, int(which), keys.ctypes.data,
+                                                          lo.ctypes.data, cen.ctypes.data, m, ctypes.byref(n)))
+        return keys[:m].copy(), lo[:m].copy(), cen[:m].copy()
+
+    def bounds(self):
+        """getMetricMin / getMetricMax over the known voxels: (min (3,) float64, max (3,) float64), zeros when empty."""
+        lo, hi = np.zeros(3, np.float64), np.zeros(3, np.float64)
+        self.ctx._check(lib().ls_occupancy_bounds(self._h, lo.ctypes.data, hi.ctypes.data))
+        return lo, hi
 
 
 Octree = collections.namedtuple("Octree", "nodes payload centres depths device_ms")

@@ -2241,3 +2241,100 @@ int ls_occupancy_cast_rays(ls_occupancy* om, const float* origins3, const float*
 }
 
 }  // extern "C"
+
+namespace {
+// A box centre and size: finite, the size >= 0.  NULL when valid, else why not.
+const char* bad_box(const double* c3, const double* s3) {
+  for (int a = 0; a < 3; ++a) {
+    if (!std::isfinite(c3[a])) return "a box centre is not finite";
+    if (!std::isfinite(s3[a]) || s3[a] < 0.0) return "a box size is not finite and >= 0";
+  }
+  return nullptr;
+}
+}  // namespace
+
+extern "C" {
+
+int ls_occupancy_set_boxes(ls_occupancy* om, const double* centres3, const double* sizes3, const int8_t* occupied, int n,
+                           ls_occupancy_edit_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (n < 0 || (n > 0 && (!centres3 || !sizes3 || !occupied))) return fail(ctx, LS_ERR_ARG, "bad argument");
+  for (int i = 0; i < n; ++i) {
+    const char* why = bad_box(centres3 + 3 * (size_t)i, sizes3 + 3 * (size_t)i);
+    if (why) return fail(ctx, LS_ERR_ARG, "box %d: %s", i, why);
+  }
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  long long set = 0, added = 0;
+  const char* why = "";
+  const int rc = lso::set_boxes(om->map, om->prm, centres3, sizes3, occupied, n, &set, &added, &why, om->stream,
+                                &ctx->launches);
+  if (rc) return fail(ctx, rc, "set boxes refused, the map's voxels are unchanged: %s", why);
+  if (set > 0) om->tree_current = om->full_current = false;
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    stats->voxels_set = set;
+    stats->new_known = added;
+    stats->known_voxels = om->map.n_known;
+    stats->bricks = om->map.pool_n;
+    stats->device_bytes = (int64_t)lso::device_bytes(om->map);
+    stats->device_ms = ms;
+  }
+  return LS_OK;
+}
+
+int ls_occupancy_clear(ls_occupancy* om) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  CU(cudaSetDevice(ctx->device));
+  const int rc = lso::clear(om->map, om->stream);
+  om->tree_current = om->full_current = false;
+  if (rc) return fail(ctx, rc, "occupancy map reset failed");
+  return LS_OK;
+}
+
+int ls_occupancy_box_voxels(ls_occupancy* om, const double center3[3], const double size3[3], int which, uint64_t* keys,
+                            float* log_odds, float* centres4, int64_t cap, int64_t* n) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!n) return fail(ctx, LS_ERR_ARG, "bad argument");
+  *n = 0;
+  if (!center3 || !size3 || cap < 0 || (which != LS_OCC_KNOWN && which != LS_OCC_OCCUPIED))
+    return fail(ctx, LS_ERR_ARG, "bad argument");
+  const char* why = bad_box(center3, size3);
+  if (why) return fail(ctx, LS_ERR_ARG, "%s", why);
+  CU(cudaSetDevice(ctx->device));
+  long long m = 0;
+  const int rc = lso::box_voxels(om->map, om->prm, center3, size3, which, keys, log_odds, centres4, cap, &m, om->stream,
+                                 &ctx->launches);
+  *n = m;
+  if (rc == LS_ERR_ARG && m > cap) return fail(ctx, rc, "buffers of %lld voxels for %lld", (long long)cap, m);
+  if (rc == LS_ERR_ARG) return fail(ctx, rc, "the box has more than 2^17 loop points on an axis or 2^31 - 1 in all");
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "box voxels: out of device memory" : "box voxels failed");
+  return LS_OK;
+}
+
+int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!min3 || !max3) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  int kmin[3], kmax[3];
+  bool empty = true;
+  const int rc = lso::key_bounds(om->map, kmin, kmax, &empty, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "bounds: out of device memory" : "bounds failed");
+  const double res = om->prm.res;
+  for (int a = 0; a < 3; ++a) {
+    // octomap's calcMinMax over depth-16 leaves: the lower corner, and the lower corner plus the voxel size
+    const auto centre = [res](int k) { return (double)(float)(((double)(k - 32768) + 0.5) * res); };
+    min3[a] = empty ? 0.0 : centre(kmin[a]) - res / 2.0;
+    max3[a] = empty ? 0.0 : (centre(kmax[a]) - res / 2.0) + res;
+  }
+  return LS_OK;
+}
+
+}  // extern "C"

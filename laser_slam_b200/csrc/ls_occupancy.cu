@@ -69,6 +69,8 @@ constexpr unsigned long long kEmpty = ~0ull;
 constexpr int kPending = -1, kFull = -2;
 constexpr int kMaxProbe = 64;
 constexpr int kKeyMax = 32768;
+constexpr long long kMaxEditAxis = 1LL << 17;    // loop points per box axis (the key space has 2^16 per axis)
+constexpr long long kMaxEditBricks = 1LL << 29;  // bricks of an edit plus those in use (the read's bound)
 constexpr int kOverflowTable = 1, kOverflowPool = 2;
 
 struct Xform16 {
@@ -1524,6 +1526,124 @@ __global__ void fr_leaf_kernel(Dev D, const unsigned char* __restrict__ pay, con
     }
 }
 
+// ---- edits (volumetric_mapping's setLogOddsBoundingBox, resetMap, getOccupiedPointcloudInBoundingBox and the map's
+// extent; DESIGN.md §4b'''''''') -----------------------------------------------------------------------------------------
+// A set box as the kernels see it: per axis, the bricks its loop reaches, axes[off[a] .. off[a] + n[a]) (brick index << 8 |
+// the 8-bit mask of the brick's keys the loop reaches), and its first (box, brick) item over the whole call.
+struct EditBox {
+  int off[3], n[3];
+  long long item0;
+};
+
+// Brick key of item j of box B (bricks x outer, z inner) and the masks of its keys in the box.
+__device__ __forceinline__ unsigned long long edit_brick(const EditBox& B, const unsigned* __restrict__ axes, long long j,
+                                                         unsigned m[3]) {
+  const long long nyz = (long long)B.n[1] * B.n[2];
+  const unsigned ax = axes[B.off[0] + (int)(j / nyz)], ay = axes[B.off[1] + (int)((j / B.n[2]) % B.n[1])],
+                 az = axes[B.off[2] + (int)(j % B.n[2])];
+  m[0] = ax & 0xffu, m[1] = ay & 0xffu, m[2] = az & 0xffu;
+  return (unsigned long long)(ax >> 8) | ((unsigned long long)(ay >> 8) << 13) | ((unsigned long long)(az >> 8) << 26);
+}
+
+// One thread per (box, brick) item of the call.  kClaim false: the items whose brick the hash lacks, counted into
+// cnt->n_out (a brick missing from several boxes counts once per box).  kClaim true: every item's brick placed with
+// brick_of, after the pool and the hash have grown for the count.
+template <bool kClaim>
+__global__ void ed_bricks_kernel(const EditBox* __restrict__ boxes, int nb, const unsigned* __restrict__ axes, long long items,
+                                 Dev D, Counters* cnt) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  bool miss = false;
+  if (i < items) {
+    int lo = 0, hi = nb - 1;  // the last box whose first item is <= i (boxes without items share the next one's)
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (boxes[mid].item0 <= i) lo = mid;
+      else hi = mid - 1;
+    }
+    unsigned m[3];
+    const unsigned long long bk = edit_brick(boxes[lo], axes, i - boxes[lo].item0, m);
+    if (kClaim) brick_of(D, cnt, bk);
+    else miss = find_brick(D, bk) < 0;
+  }
+  if (!kClaim) {
+    const unsigned bal = __ballot_sync(0xffffffffu, miss);
+    if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&cnt->n_out, (unsigned long long)__popc(bal));
+  }
+}
+
+// One box: one block of 512 threads per brick item, one thread per voxel.  A voxel is in the box iff its key is in the
+// box's key list on every axis; it takes `value` and becomes known.  Newly known voxels: one popcount per warp.
+__global__ void __launch_bounds__(512) ed_write_kernel(EditBox B, const unsigned* __restrict__ axes, float value, Dev D,
+                                                       Counters* cnt) {
+  __shared__ int sb;
+  unsigned m[3];
+  const unsigned long long bk = edit_brick(B, axes, blockIdx.x, m);
+  const int t = threadIdx.x, lane = t & 31;
+  if (t == 0) sb = find_brick(D, bk);
+  __syncthreads();
+  const int b = sb;
+  if (b < 0) return;
+  const bool in = ((m[0] >> (t & 7)) & (m[1] >> ((t >> 3) & 7)) & (m[2] >> (t >> 6)) & 1u) != 0u;
+  if (in) D.lo[(size_t)b * 512 + t] = value;
+  const unsigned bits = __ballot_sync(0xffffffffu, in);
+  if (lane == 0 && bits) {
+    unsigned* w = D.known + (size_t)b * 16 + (t >> 5);
+    const unsigned old = *w;
+    *w = old | bits;
+    const unsigned nk = __popc(bits & ~old);
+    if (nk) atomicAdd(&cnt->new_known, (unsigned long long)nk);
+  }
+}
+
+// The crop: one thread per loop point (x outer, z inner) over the valid keys of each axis (keys: x's, then y's, then
+// z's); flag 1 when its voxel is in `which`.
+__global__ void ed_flag_kernel(const int* __restrict__ keys, int nx, int ny, int nz, long long n, Dev D, Params P, int which,
+                               int* __restrict__ flag) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int k[3] = {keys[(int)(i / ((long long)ny * nz))], keys[nx + (int)((i / nz) % ny)], keys[nx + ny + (int)(i % nz)]};
+  Cursor cur;
+  const int s = state_of(D, P, cur, k, nullptr);
+  flag[i] = s == LS_CELL_OCCUPIED || (which == LS_OCC_KNOWN && s == LS_CELL_FREE);
+}
+
+// The flagged points in loop order at their inclusive-scan positions: packed key, log-odds bits and voxel centre.
+__global__ void ed_scatter_kernel(const int* __restrict__ keys, int nx, int ny, int nz, long long n, Dev D, double res,
+                                  const int* __restrict__ flag, const int* __restrict__ pos, unsigned long long* __restrict__ ok,
+                                  unsigned* __restrict__ ov, float4* __restrict__ oc) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !flag[i]) return;
+  const int k[3] = {keys[(int)(i / ((long long)ny * nz))], keys[nx + (int)((i / nz) % ny)], keys[nx + ny + (int)(i % nz)]};
+  const int b = find_brick(D, brick_key(k));
+  const int local = (k[0] & 7) | ((k[1] & 7) << 3) | ((k[2] & 7) << 6);
+  const int p = pos[i] - 1;
+  ok[p] = pack(k[0], k[1], k[2]);
+  ov[p] = __float_as_uint(D.lo[(size_t)b * 512 + local]);
+  oc[p] = make_float4(centre_of(k[0], res), centre_of(k[1], res), centre_of(k[2], res), 1.0f);
+}
+
+// The extent: one block per brick in use; the smallest and largest known key per axis, one atomicMin / atomicMax per axis
+// and block into mm (min x, y, z, then max x, y, z).
+__global__ void __launch_bounds__(512) ed_bounds_kernel(Dev D, int* mm) {
+  using Reduce = cub::BlockReduce<int, 512>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const int b = blockIdx.x, t = threadIdx.x;
+  const bool kn = (D.known[(size_t)b * 16 + (t >> 5)] >> (t & 31)) & 1u;
+  const unsigned long long bk = D.bkey[b];
+  const int k[3] = {(int)(bk & 0x1fff) * 8 + (t & 7), (int)((bk >> 13) & 0x1fff) * 8 + ((t >> 3) & 7),
+                    (int)((bk >> 26) & 0x1fff) * 8 + (t >> 6)};
+  for (int a = 0; a < 3; ++a) {
+    const int lo = Reduce(tmp).Reduce(kn ? k[a] : INT_MAX, cub::Min());
+    __syncthreads();
+    const int hi = Reduce(tmp).Reduce(kn ? k[a] : -1, cub::Max());
+    __syncthreads();
+    if (t == 0 && hi >= 0) {
+      atomicMin(&mm[a], lo);
+      atomicMax(&mm[3 + a], hi);
+    }
+  }
+}
+
 int code(cudaError_t e) {
   if (e == cudaSuccess) return LS_OK;
   cudaGetLastError();
@@ -2286,6 +2406,209 @@ int query_rays(Map& m, const Params& P, const float* origins3, const float* dire
   OCC_TRY(cudaMemcpyAsync(result, q + o_r, (size_t)n, cudaMemcpyDeviceToHost, st));
   if (ends3) OCC_TRY(cudaMemcpyAsync(ends3, q + o_e, vec_bytes, cudaMemcpyDeviceToHost, st));
   return finish_query(m, st, visited);
+}
+
+// ---- edits -------------------------------------------------------------------------------------------------------------
+namespace {
+
+// One axis of setLogOddsBoundingBox's loop around p of size s: the keys of its points whose key is valid, in loop order
+// (ascending, repeats kept).  False when the axis has more than kMaxEditAxis points.
+bool edit_axis(double p, double s, const Params& P, std::vector<int>* keys) {
+  keys->clear();
+  const double c = P.res * std::floor(p / P.res) + P.res / 2.0;
+  const double lo = (c - s / 2) + 0.001, hi = (c + s / 2) - 0.001;
+  if (!((hi - lo) / P.res <= (double)kMaxEditAxis)) return false;  // bounds the loop below; a NaN is refused too
+  long long points = 0;
+  for (double x = lo; x <= hi; x += P.res) {
+    if (++points > kMaxEditAxis) return false;
+    const double f = std::floor((double)(float)x * P.inv);
+    if (f >= -(double)kKeyMax && f < (double)kKeyMax) keys->push_back((int)f + kKeyMax);
+  }
+  return true;
+}
+
+// The bricks of one axis's keys appended to out: brick index << 8 | the mask of its keys (keys ascending, so each brick
+// is one run).  Returns their number.
+int axis_bricks(const std::vector<int>& keys, std::vector<unsigned>* out) {
+  const size_t first = out->size();
+  for (const int k : keys) {
+    const unsigned b = (unsigned)(k >> 3) << 8, bit = 1u << (k & 7);
+    if (out->size() > first && (out->back() & ~0xffu) == b) out->back() |= bit;
+    else out->push_back(b | bit);
+  }
+  return (int)(out->size() - first);
+}
+
+}  // namespace
+
+int set_boxes(Map& m, const Params& P, const double* centres3, const double* sizes3, const int8_t* occupied, int n,
+              long long* voxels_set, long long* new_known, const char** why, cudaStream_t st, uint64_t* launches) {
+  *voxels_set = *new_known = 0;
+  *why = "";
+  // Every box's loop first, on the host: nothing is allocated or written before the whole call is known to be valid.
+  std::vector<EditBox> boxes((size_t)n);
+  std::vector<unsigned> axes;
+  std::vector<int> keys;
+  long long items = 0, set = 0;
+  for (int i = 0; i < n; ++i) {
+    EditBox& B = boxes[(size_t)i];
+    long long pts = 1, bricks = 1;
+    for (int a = 0; a < 3; ++a) {
+      if (!edit_axis(centres3[3 * (size_t)i + a], sizes3[3 * (size_t)i + a], P, &keys))
+        return *why = "a box axis has more than 2^17 loop points", LS_ERR_ARG;
+      B.off[a] = (int)axes.size();
+      B.n[a] = axis_bricks(keys, &axes);
+      pts *= (long long)keys.size();
+      bricks *= B.n[a];
+    }
+    B.item0 = items;
+    items += bricks;
+    set += pts;
+    if (items + m.pool_n > kMaxEditBricks) return *why = "the boxes cover more than 2^29 bricks", LS_ERR_NOMEM;
+  }
+  *voxels_set = set;
+  if (items == 0) return LS_OK;
+  size_t off = 0;
+  const size_t o_box = take(off, boxes.size() * sizeof(EditBox)), o_ax = take(off, axes.size() * sizeof(unsigned));
+  int rc;
+  if ((rc = reserve_query(m, off, st))) return *why = "out of device memory for the boxes", rc;
+  char* q = m.qbuf.get();
+  const EditBox* dbox = (const EditBox*)(q + o_box);
+  const unsigned* dax = (const unsigned*)(q + o_ax);
+  OCC_TRY(cudaMemcpyAsync(q + o_box, boxes.data(), boxes.size() * sizeof(EditBox), cudaMemcpyHostToDevice, st));
+  OCC_TRY(cudaMemcpyAsync(q + o_ax, axes.data(), axes.size() * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+  const int blocks = (int)((items + 255) / 256);
+  // Count the missing bricks, grow the pool and the hash for them, then place them (the insert's retry when a probe
+  // sequence overflows).  A failure here (a growth refused after some bricks were placed) leaves the known voxels as they
+  // were: placed bricks hold none, as after a failed insert.  Both tree builds give a brick without a known voxel state 0
+  // and no node, and the queries and the bounds test the known bits, so the cached trees and every answer stay current.
+  if ((rc = upload_counters(m, st))) return rc;
+  ed_bricks_kernel<false><<<blocks, 256, 0, st>>>(dbox, n, dax, items, dev_of(m), m.cnt_dev.get());
+  OCC_LAUNCHED();
+  if ((rc = read_counters(m, st))) return rc;
+  const long long missing = (long long)m.cnt_host.get()->n_out;
+  if (missing > 0) {
+    const long long need = m.pool_n + missing;
+    if (need > m.pool_cap()) {
+      long long cap = m.pool_cap() > 0 ? m.pool_cap() : 1;
+      while (cap < need) cap *= 2;
+      if ((rc = grow_pool(m, (int)cap, st))) return *why = "the map cannot grow", rc;
+    }
+    long long tab = m.tab_cap();
+    while (2 * need > tab) tab *= 2;
+    if (tab > m.tab_cap() && (rc = rebuild_table(m, (int)tab, st, launches))) return *why = "the map cannot grow", rc;
+    for (;;) {
+      if ((rc = upload_counters(m, st))) return rc;
+      ed_bricks_kernel<true><<<blocks, 256, 0, st>>>(dbox, n, dax, items, dev_of(m), m.cnt_dev.get());
+      OCC_LAUNCHED();
+      if ((rc = read_counters(m, st))) return rc;
+      const Counters c = *m.cnt_host.get();
+      m.pool_n = c.pool_n < m.pool_cap() ? c.pool_n : m.pool_cap();
+      if (!c.overflow) break;
+      if ((rc = rebuild_table(m, m.tab_cap() * 2, st, launches))) return *why = "the map cannot grow", rc;
+    }
+  }
+  // Only now is the map written: one launch per box, in call order, so the last box covering a voxel sets it.
+  if ((rc = upload_counters(m, st))) return rc;
+  const Dev D = dev_of(m);
+  for (int i = 0; i < n; ++i) {
+    const EditBox& B = boxes[(size_t)i];
+    const long long nb = (long long)B.n[0] * B.n[1] * B.n[2];
+    if (nb == 0) continue;
+    const float value = occupied[i] ? P.l_max : P.l_min;
+    ed_write_kernel<<<(unsigned)nb, 512, 0, st>>>(B, dax, value, D, m.cnt_dev.get());
+    OCC_LAUNCHED();
+  }
+  if ((rc = read_counters(m, st))) return rc;
+  *new_known = (long long)m.cnt_host.get()->new_known;
+  m.n_known += *new_known;
+  return LS_OK;
+}
+
+int clear(Map& m, cudaStream_t st) {
+  const size_t a = (size_t)m.pool_n;
+  if (a > 0) {  // a claimed pool brick must start zeroed, as a grown pool's do
+    OCC_TRY(cudaMemsetAsync(m.lo.get(), 0, a * 512 * sizeof(float), st));
+    OCC_TRY(cudaMemsetAsync(m.known.get(), 0, a * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.mfree.get(), 0, a * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.mocc.get(), 0, a * 16 * sizeof(unsigned), st));
+    OCC_TRY(cudaMemsetAsync(m.touched.get(), 0, a * sizeof(unsigned), st));
+  }
+  OCC_TRY(cudaMemsetAsync(m.tab_keys.get(), 0xff, (size_t)m.tab_cap() * sizeof(unsigned long long), st));
+  OCC_TRY(cudaMemsetAsync(m.tab_vals.get(), 0xff, (size_t)m.tab_cap() * sizeof(int), st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  m.pool_n = 0;
+  m.n_known = 0;
+  return LS_OK;
+}
+
+int box_voxels(Map& m, const Params& P, const double center3[3], const double size3[3], int which, uint64_t* keys,
+               float* log_odds, float* centres4, long long cap, long long* n, cudaStream_t st, uint64_t* launches) {
+  *n = 0;
+  std::vector<int> axis[3];
+  long long pts = 1;
+  for (int a = 0; a < 3; ++a) {
+    if (!edit_axis(center3[a], size3[a], P, &axis[a])) return LS_ERR_ARG;
+    pts *= (long long)axis[a].size();
+  }
+  if (pts > 0x7fffffffLL) return LS_ERR_ARG;
+  if (pts == 0) return LS_OK;
+  const int nx = (int)axis[0].size(), ny = (int)axis[1].size(), nz = (int)axis[2].size();
+  std::vector<int> flat;
+  for (int a = 0; a < 3; ++a) flat.insert(flat.end(), axis[a].begin(), axis[a].end());
+  size_t scan_bytes = 0;
+  OCC_TRY(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (int*)nullptr, (int*)nullptr, (int)pts, st));
+  size_t off = 0;
+  const size_t o_k = take(off, flat.size() * sizeof(int)), o_f = take(off, (size_t)pts * sizeof(int)),
+               o_p = take(off, (size_t)pts * sizeof(int)), o_t = take(off, scan_bytes);
+  int rc;
+  if ((rc = reserve_query(m, off, st))) return rc;
+  char* q = m.qbuf.get();
+  const int* dk = (const int*)(q + o_k);
+  int* flag = (int*)(q + o_f);
+  int* pos = (int*)(q + o_p);
+  OCC_TRY(cudaMemcpyAsync(q + o_k, flat.data(), flat.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const Dev D = dev_of(m);
+  ed_flag_kernel<<<blocks_of(pts), 256, 0, st>>>(dk, nx, ny, nz, pts, D, P, which, flag);
+  OCC_LAUNCHED();
+  OCC_TRY(cub::DeviceScan::InclusiveSum(q + o_t, scan_bytes, flag, pos, (int)pts, st));
+  ++*launches;
+  int total = 0;
+  OCC_TRY(cudaMemcpyAsync(&total, pos + (pts - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  *n = total;
+  if (total > cap) return LS_ERR_ARG;
+  if (total == 0 || (!keys && !log_odds && !centres4)) return LS_OK;
+  if ((rc = reserve_export(m, total, st))) return rc;
+  ed_scatter_kernel<<<blocks_of(pts), 256, 0, st>>>(dk, nx, ny, nz, pts, D, P.res, flag, pos, m.ex_k[0].get(), m.ex_v[0].get(),
+                                                    m.ex_c.get());
+  OCC_LAUNCHED();
+  if (keys) OCC_TRY(cudaMemcpyAsync(keys, m.ex_k[0].get(), (size_t)total * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, m.ex_v[0].get(), (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (centres4) OCC_TRY(cudaMemcpyAsync(centres4, m.ex_c.get(), (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  return LS_OK;
+}
+
+int key_bounds(Map& m, int kmin[3], int kmax[3], bool* empty, cudaStream_t st, uint64_t* launches) {
+  *empty = true;
+  if (m.n_known == 0 || m.pool_n == 0) return LS_OK;
+  size_t off = 0;
+  const size_t o_mm = take(off, 6 * sizeof(int));
+  int rc;
+  if ((rc = reserve_query(m, off, st))) return rc;
+  int* mm = (int*)(m.qbuf.get() + o_mm);
+  OCC_TRY(cudaMemsetAsync(mm, 0x7f, 3 * sizeof(int), st));      // 0x7f7f7f7f: above any key
+  OCC_TRY(cudaMemsetAsync(mm + 3, 0xff, 3 * sizeof(int), st));  // -1
+  ed_bounds_kernel<<<m.pool_n, 512, 0, st>>>(dev_of(m), mm);
+  OCC_LAUNCHED();
+  int h[6];
+  OCC_TRY(cudaMemcpyAsync(h, mm, sizeof h, cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  if (h[3] < 0) return LS_OK;
+  for (int a = 0; a < 3; ++a) kmin[a] = h[a], kmax[a] = h[3 + a];
+  *empty = false;
+  return LS_OK;
 }
 
 }  // namespace lso

@@ -151,4 +151,22 @@ int query_lines(Map& m, const Params& P, const double* starts3, const double* en
 int query_rays(Map& m, const Params& P, const float* origins3, const float* directions3, int n, int ignore_unknown,
                double max_range, int8_t* result, float* ends3, long long* visited, cudaStream_t st, uint64_t* launches);
 
+// Edits (DESIGN.md §4b'''''''').  Synchronous.  The box loop per axis: c = res * floor(p / res) + res / 2, points from
+// (c - s/2) + 0.001 while <= (c + s/2) - 0.001 in steps of res (double), each cast to float and keyed; invalid keys skipped.
+// setLogOddsBoundingBox of n boxes (double triples; finite, sizes >= 0, checked by the caller) in call order: every voxel a
+// loop point keys becomes known with L_max (occupied[i] != 0) or L_min.  LS_ERR_ARG when an axis has more than 2^17 points,
+// LS_ERR_NOMEM before any allocation when the call's bricks and those in use exceed 2^29, or when the map cannot grow; the
+// known voxels and their values are unchanged after any error (*why says why).  *voxels_set: loop points with a valid key.
+int set_boxes(Map& m, const Params& P, const double* centres3, const double* sizes3, const int8_t* occupied, int n,
+              long long* voxels_set, long long* new_known, const char** why, cudaStream_t st, uint64_t* launches);
+// resetMap: no known voxel and no brick; the capacity stays.
+int clear(Map& m, cudaStream_t st);
+// getOccupiedPointcloudInBoundingBox: per loop point of the box (x outer, z inner) whose voxel is in `which` (LS_OCC_*),
+// its packed key, log-odds and voxel centre {x, y, z, 1}, in loop order.  *n: their number; LS_ERR_ARG without a copy when
+// it exceeds cap, or when an axis has more than 2^17 points or the box more than 2^31 - 1.  Outputs may be NULL.
+int box_voxels(Map& m, const Params& P, const double center3[3], const double size3[3], int which, uint64_t* keys,
+               float* log_odds, float* centres4, long long cap, long long* n, cudaStream_t st, uint64_t* launches);
+// The smallest and largest known key per axis; *empty when no voxel is known.
+int key_bounds(Map& m, int kmin[3], int kmax[3], bool* empty, cudaStream_t st, uint64_t* launches);
+
 }  // namespace lso

@@ -296,6 +296,10 @@ class OccupancyMap:
             L.lsh_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp]
             L.lsh_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, ci, vp, vp]
             L.lsh_occupancy_cast_rays.argtypes = [vp, vp, vp, ci, ci, ctypes.c_double, ci, vp, vp]
+            L.lsh_occupancy_set_boxes.argtypes = [vp, vp, vp, vp, ci, ci, vp]
+            L.lsh_occupancy_reset.argtypes = [vp]
+            L.lsh_occupancy_box_cloud.argtypes = [vp, vp, vp, vp, ci]
+            L.lsh_occupancy_bounds.argtypes = [vp, vp]
             L._occ_bound = True
         prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range], np.float64)
         err = ctypes.create_string_buffer(512)
@@ -414,3 +418,31 @@ class OccupancyMap:
         self._check(lib().lsh_occupancy_cast_rays(self._h, o.ctypes.data, d.ctypes.data, n, int(bool(ignore_unknown)),
                                                   float(max_range), int(bool(single)), r.ctypes.data, ends.ctypes.data))
         return r[:n], ends[:n]
+
+    def set_boxes(self, centres, sizes, occupied, single=False):
+        """setBoxes ((voxels_set, new_known, known voxels)), or with single=True one setFree / setOccupied per box (None)."""
+        c = np.ascontiguousarray(np.asarray(centres, np.float64).reshape(-1, 3))
+        s = np.ascontiguousarray(np.asarray(sizes, np.float64).reshape(-1, 3))
+        o = np.ascontiguousarray(np.asarray(occupied).reshape(-1).astype(bool).astype(np.int8))
+        st = np.zeros(3, np.int64)
+        self._check(lib().lsh_occupancy_set_boxes(self._h, c.ctypes.data, s.ctypes.data, o.ctypes.data, len(c),
+                                                  int(bool(single)), st.ctypes.data))
+        return None if single else tuple(int(x) for x in st)
+
+    def reset_map(self):
+        self._check(lib().lsh_occupancy_reset(self._h))
+
+    def occupied_cloud_in_box(self, center, size):
+        """getOccupiedPointcloudInBoundingBox: (n,4) float32 voxel centres in loop order."""
+        c = np.ascontiguousarray(np.asarray(center, np.float64).reshape(3))
+        s = np.ascontiguousarray(np.asarray(size, np.float64).reshape(3))
+        n = self._check(lib().lsh_occupancy_box_cloud(self._h, c.ctypes.data, s.ctypes.data, None, 0))
+        out = np.zeros((max(n, 1), 4), np.float32)
+        self._check(lib().lsh_occupancy_box_cloud(self._h, c.ctypes.data, s.ctypes.data, out.ctypes.data, n))
+        return out[:n]
+
+    def map_bounds(self):
+        """getMapBounds, getMapSize, getMapCenter: (min, max, size, centre), each (3,) float64."""
+        out = np.zeros(12, np.float64)
+        self._check(lib().lsh_occupancy_bounds(self._h, out.ctypes.data))
+        return out[0:3], out[3:6], out[6:9], out[9:12]

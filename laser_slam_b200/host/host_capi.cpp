@@ -612,4 +612,69 @@ int lsh_occupancy_occupied_leaf_cloud(void* ov, float* out4, int cap) {
     return LS_ERR_STATE;
   }
 }
+
+// Edits.  single = 1: setFree / setOccupied once per box, else one setBoxes call; stats (voxels_set, new_known, known voxels)
+// of the batched call.  0 or LS_ERR_STATE.
+int lsh_occupancy_set_boxes(void* ov, const double* c3, const double* s3, const int8_t* occupied, int n, int single,
+                            int64_t* stats3) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<kindr::minimal::Position> c(n), s(n);
+    std::vector<bool> o(n);
+    for (int i = 0; i < n; ++i)
+      c[i] = {c3[3 * i], c3[3 * i + 1], c3[3 * i + 2]}, s[i] = {s3[3 * i], s3[3 * i + 1], s3[3 * i + 2]}, o[i] = occupied[i] != 0;
+    if (single) {
+      for (int i = 0; i < n; ++i) o[i] ? h->map->setOccupied(c[i], s[i]) : h->map->setFree(c[i], s[i]);
+      return 0;
+    }
+    ls_occupancy_edit_stats st;
+    h->map->setBoxes(c, s, o, &st);
+    stats3[0] = st.voxels_set, stats3[1] = st.new_known, stats3[2] = st.known_voxels;
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+int lsh_occupancy_reset(void* ov) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    h->map->resetMap();
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// getOccupiedPointcloudInBoundingBox; returns its number of points, written when it is <= cap
+int lsh_occupancy_box_cloud(void* ov, const double* c3, const double* s3, float* out4, int cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    DataPoints d;
+    h->map->getOccupiedPointcloudInBoundingBox({c3[0], c3[1], c3[2]}, {s3[0], s3[1], s3[2]}, &d);
+    const int n = (int)d.getNbPoints();
+    if (out4 && n <= cap) std::memcpy(out4, static_cast<const DataPoints&>(d).features.data(), sizeof(float) * 4 * (size_t)n);
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// getMapBounds, getMapSize and getMapCenter: out12 = min, max, size, centre
+int lsh_occupancy_bounds(void* ov, double* out12) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    kindr::minimal::Position lo, hi;
+    h->map->getMapBounds(&lo, &hi);
+    const kindr::minimal::Position size = h->map->getMapSize(), centre = h->map->getMapCenter();
+    for (int a = 0; a < 3; ++a) out12[a] = lo[a], out12[3 + a] = hi[a], out12[6 + a] = size[a], out12[9 + a] = centre[a];
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
 }  // extern "C"

@@ -263,4 +263,70 @@ void OccupancyMap::castRays(const std::vector<kindr::minimal::Position>& origins
   }
 }
 
+// ---- edits ---------------------------------------------------------------------------------------------------------
+void OccupancyMap::setFree(const kindr::minimal::Position& position, const kindr::minimal::Position& bounding_box_size) {
+  setBoxes({position}, {bounding_box_size}, {false});
+}
+
+void OccupancyMap::setOccupied(const kindr::minimal::Position& position, const kindr::minimal::Position& bounding_box_size) {
+  setBoxes({position}, {bounding_box_size}, {true});
+}
+
+void OccupancyMap::setBoxes(const std::vector<kindr::minimal::Position>& positions,
+                            const std::vector<kindr::minimal::Position>& bounding_box_sizes, const std::vector<bool>& occupied,
+                            ls_occupancy_edit_stats* stats) {
+  const size_t n = positions.size();
+  if (bounding_box_sizes.size() != n || occupied.size() != n)
+    throw std::invalid_argument("positions, sizes and occupied flags differ in length");
+  std::vector<double> c(3 * n), s(3 * n);
+  std::vector<int8_t> o(n > 0 ? n : 1);
+  for (size_t i = 0; i < n; ++i) {
+    for (int a = 0; a < 3; ++a) c[3 * i + a] = positions[i][a], s[3 * i + a] = bounding_box_sizes[i][a];
+    o[i] = occupied[i] ? 1 : 0;
+  }
+  std::lock_guard<std::mutex> lock(mutex_);
+  throwOnError(ctx_, ls_occupancy_set_boxes(map_, c.data(), s.data(), o.data(), (int)n, stats), "ls_occupancy_set_boxes");
+}
+
+void OccupancyMap::resetMap() {
+  std::lock_guard<std::mutex> lock(mutex_);
+  throwOnError(ctx_, ls_occupancy_clear(map_), "ls_occupancy_clear");
+}
+
+void OccupancyMap::getOccupiedPointcloudInBoundingBox(const kindr::minimal::Position& center,
+                                                      const kindr::minimal::Position& bounding_box_size,
+                                                      DataPoints* output_cloud) const {
+  if (output_cloud == NULL) throw std::invalid_argument("null output");
+  std::lock_guard<std::mutex> lock(mutex_);
+  int64_t n = 0;
+  int rc = ls_occupancy_box_voxels(map_, center.data(), bounding_box_size.data(), LS_OCC_OCCUPIED, NULL, NULL, NULL, 0, &n);
+  if (!(rc == LS_ERR_ARG && n > 0)) throwOnError(ctx_, rc, "ls_occupancy_box_voxels");
+  std::vector<float> c(4 * (size_t)(n > 0 ? n : 1));
+  if (n > 0)
+    throwOnError(ctx_, ls_occupancy_box_voxels(map_, center.data(), bounding_box_size.data(), LS_OCC_OCCUPIED, NULL, NULL,
+                                               c.data(), n, &n),
+                 "ls_occupancy_box_voxels");
+  *output_cloud = DataPoints::fromArrays(c.data(), NULL, (size_t)n);
+}
+
+void OccupancyMap::getMapBounds(kindr::minimal::Position* min_bound, kindr::minimal::Position* max_bound) const {
+  if (min_bound == NULL || max_bound == NULL) throw std::invalid_argument("null output");
+  std::lock_guard<std::mutex> lock(mutex_);
+  throwOnError(ctx_, ls_occupancy_bounds(map_, min_bound->data(), max_bound->data()), "ls_occupancy_bounds");
+}
+
+kindr::minimal::Position OccupancyMap::getMapSize() const {
+  kindr::minimal::Position lo, hi;
+  getMapBounds(&lo, &hi);
+  return kindr::minimal::Position{hi[0] - lo[0], hi[1] - lo[1], hi[2] - lo[2]};
+}
+
+kindr::minimal::Position OccupancyMap::getMapCenter() const {
+  kindr::minimal::Position lo, hi;
+  getMapBounds(&lo, &hi);
+  kindr::minimal::Position c;
+  for (int a = 0; a < 3; ++a) c[a] = lo[a] + (hi[a] - lo[a]) / 2.0;
+  return c;
+}
+
 }  // namespace laser_slam

@@ -98,6 +98,19 @@ with tempfile.TemporaryDirectory() as tmp:
     wk, wv = rr.expand(ls.read_octomap(bt), *rr.clamps())
     assert np.array_equal(rk, wk) and np.array_equal(rv.view(np.uint32), wv.view(np.uint32)) and len(rk) > 0
     rm.close()
+# edits of that map: a set that grows it from 16 bricks, the crop, the bounds and a reset, against the edit restatement
+import occupancy_edits_ref as er
+e = er.Edits(0.2, *rr.clamps(), oc.logodds(0.7))
+vox = er.as_dict(*oom.download())
+bc, bs = [truth[0][:3, 3], truth[0][:3, 3] + 20.0], [(3.0, 3.0, 1.0), (4.0, 4.0, 4.0)]
+om.set_boxes(bc, bs, [False, True])
+e.set_boxes(vox, bc, bs, [False, True])
+ek, ev, _ = om.download(ls.OCC_KNOWN)
+assert np.array_equal(ek, er.as_arrays(vox)[0]) and np.array_equal(ev.view(np.uint32), er.as_arrays(vox)[1].view(np.uint32))
+assert np.array_equal(om.box_voxels(bc[1], (6.0, 6.0, 6.0))[0], e.crop(vox, bc[1], (6.0, 6.0, 6.0))[0])
+assert all(np.array_equal(a, b) for a, b in zip(om.bounds(), e.bounds(vox)))
+om.clear()
+assert om.size(ls.OCC_KNOWN) == 0
 om.close()
 launches = ctx.launch_count
 # every handle closed, so a leak check sees only what the library failed to free
