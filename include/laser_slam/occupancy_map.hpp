@@ -18,6 +18,8 @@
 
 namespace laser_slam {
 
+class DistanceMap;
+
 // laser_to_octomap's defaults (:18-21) and volumetric_mapping's clamping and threshold.
 struct OccupancyMapParams {
   double resolution = 0.075;
@@ -118,6 +120,8 @@ class OccupancyMap {
   kindr::minimal::Position getMapCenter() const;
 
  private:
+  friend class DistanceMap;  // reads map_ under mutex_ in its update (include/laser_slam/distance_map.hpp)
+
   CellStatus cellStatus(const kindr::minimal::Position& point, float* log_odds) const;
   void download(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds, std::vector<float>* centres4) const;
 

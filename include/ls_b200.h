@@ -556,6 +556,64 @@ int ls_occupancy_box_voxels(ls_occupancy* om, const double center3[3], const dou
                             float* log_odds, float* centres4, int64_t cap, int64_t* n);
 int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]);
 
+/* Euclidean distance map of the occupancy map: octomap's DynamicEDTOctomap(maxdist, octree, bbxMin, bbxMax,
+ * treatUnknownAsOccupied) over the finest cells of a box, recomputed in full on the device at every update and queried in
+ * batches (DESIGN.md §4b''''''''').  Rules:
+ *   box         each corner keyed as the map's points: k = floor((double)c * (1/res)) + 32768 per axis.  The grid covers keys
+ *               kmin ... kmax per axis, both included; cell (x, y, z) is key kmin + (x, y, z); x fastest, then y, then z
+ *   obstacles   a cell inside the box whose voxel is occupied (known, v >= L_occ); with treat_unknown_as_occupied, every
+ *               unknown cell too.  Voxels outside the box do not count
+ *   cap         m = (int)((double)max_dist / res + 1.0), M = m * m; max_dist (getMaxDist) = (float)(m * res)
+ *   field       per cell s = the squared distance in cells to the nearest obstacle (dx^2 + dy^2 + dz^2).  s <= M: s and that
+ *               obstacle; otherwise M and no obstacle (also when the box has none).  An obstacle cell has s = 0 and is its own
+ *   ties        among obstacles at the least s, the smallest packed key (smallest z, then y, then x)
+ *   queries     float triples keyed as the corners.  distance = (float)((double)(float)sqrt((double)s) * res), sqdist = s,
+ *               obstacle = its voxel centre (float)(((double)(k - 32768) + 0.5) * res) per axis, NaN when the cell has none.
+ *               A point whose key is invalid (non-finite included) or outside the box: -1.0f, -1 and NaN
+ *   snapshot    the field is the map as of the last successful update; the box, the resolution, L_occ and M are taken from
+ *               the map then.  Queries and downloads before the first update return LS_ERR_STATE
+ * Unlike DynamicEDT3D, which propagates obstacles through the 26-neighbourhood with a priority queue and updates from
+ * octomap's change detection, the transform is exact and recomputed in full.  The handle has its own stream and buffers and
+ * uses none of the context's workspaces, so every call is legal between ls_icp_register_submap_batch_begin and _end.  Calls
+ * are synchronous and never change the occupancy map.  Errors: LS_ERR_ARG, checked before any work and leaving the previous
+ * field intact, for max_dist not finite or <= 0, m > 46340, a corner that is not finite or has an invalid key, bbx_min >
+ * bbx_max on an axis, more than 2^30 cells, n < 0, a NULL required array, a map on another device or a too-small buffer;
+ * LS_ERR_NOMEM when the field's buffers cannot grow, after which the handle has no field. */
+typedef struct ls_distance_map ls_distance_map;
+typedef struct ls_distance_map_params {
+  float max_dist;                 /* [m], finite and > 0 */
+  float bbx_min[3], bbx_max[3];   /* the box's corners [m] */
+  int treat_unknown_as_occupied;
+} ls_distance_map_params;
+
+typedef struct ls_distance_map_stats {
+  int32_t min_key[3];        /* kmin */
+  int32_t size[3];           /* cells per axis */
+  int64_t cells;
+  int64_t obstacles;         /* obstacle cells in the box */
+  double resolution;         /* the map's at the update */
+  int32_t max_sqdist_cells;  /* M */
+  float max_dist;            /* getMaxDist */
+  int64_t device_bytes;      /* device memory the handle holds */
+  float device_ms;           /* the update on the handle's stream */
+} ls_distance_map_stats;
+
+typedef struct ls_distance_map_query_stats {
+  int64_t outside;  /* points with an invalid key or outside the box */
+  float device_ms;  /* the call on the handle's stream, copies included */
+} ls_distance_map_query_stats;
+
+int ls_distance_map_create(ls_ctx* ctx, const ls_distance_map_params* params, ls_distance_map** out);
+void ls_distance_map_destroy(ls_distance_map* dm);
+/* The field of om's current state.  stats may be NULL. */
+int ls_distance_map_update(ls_distance_map* dm, ls_occupancy* om, ls_distance_map_stats* stats);
+/* points3: n float triples.  distance, sqdist_cells, obstacles3 (n float triples) and stats may be NULL. */
+int ls_distance_map_query(ls_distance_map* dm, const float* points3, int n, float* distance, int32_t* sqdist_cells,
+                          float* obstacles3, ls_distance_map_query_stats* stats);
+/* The whole field in layout order: s per cell and its obstacle's packed key (all ones when none); either output may be NULL.
+ * *n always set to the cells (after an update); LS_ERR_ARG without a copy when cap_cells is below it. */
+int ls_distance_map_download(ls_distance_map* dm, int32_t* sqdist, uint64_t* obstacle_keys, int64_t cap_cells, int64_t* n);
+
 /* ---- per-scan input filters (reference laser_slam/src/laser_track.cpp:24-30 loads them from
  * LaserTrackParams::icp_input_filters_file, :81 and :146 apply them to every scan before it is stored) ----------------
  * A chain is an array of ls_point_filter records applied in order; each filter sees the cloud the previous one produced,

@@ -127,6 +127,23 @@ class OccupancyQueryStats(ctypes.Structure):
     _fields_ = [("keys_visited", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
 
+class DistanceMapParams(ctypes.Structure):
+    _fields_ = [("max_dist", ctypes.c_float), ("bbx_min", ctypes.c_float * 3), ("bbx_max", ctypes.c_float * 3),
+                ("treat_unknown_as_occupied", ctypes.c_int)]
+
+
+class DistanceMapStats(ctypes.Structure):
+    """ls_distance_map_stats: the box (first key and cells per axis), cells, obstacles, the map's resolution, M, getMaxDist,
+    the handle's device bytes and the update's device ms."""
+    _fields_ = [("min_key", ctypes.c_int32 * 3), ("size", ctypes.c_int32 * 3), ("cells", ctypes.c_int64),
+                ("obstacles", ctypes.c_int64), ("resolution", ctypes.c_double), ("max_sqdist_cells", ctypes.c_int32),
+                ("max_dist", ctypes.c_float), ("device_bytes", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
+class DistanceMapQueryStats(ctypes.Structure):
+    _fields_ = [("outside", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
 OCC_KNOWN, OCC_OCCUPIED = 1, 2
 CELL_FREE, CELL_OCCUPIED, CELL_UNKNOWN = 0, 1, 2
 RAY_INVALID, RAY_HIT, RAY_UNKNOWN, RAY_MAX_RANGE, RAY_KEY_BOUND = 0, 1, 2, 3, 4
@@ -252,6 +269,12 @@ def lib():
         L.ls_occupancy_clear.argtypes = [vp]
         L.ls_occupancy_box_voxels.argtypes = [vp, vp, vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
         L.ls_occupancy_bounds.argtypes = [vp, vp, vp]
+        L.ls_distance_map_create.argtypes = [vp, ctypes.POINTER(DistanceMapParams), ctypes.POINTER(vp)]
+        L.ls_distance_map_destroy.argtypes = [vp]
+        L.ls_distance_map_destroy.restype = None
+        L.ls_distance_map_update.argtypes = [vp, vp, ctypes.POINTER(DistanceMapStats)]
+        L.ls_distance_map_query.argtypes = [vp, vp, ci, vp, vp, vp, ctypes.POINTER(DistanceMapQueryStats)]
+        L.ls_distance_map_download.argtypes = [vp, vp, vp, ctypes.c_int64, i64p]
         _lib = L
     return _lib
 
@@ -1081,6 +1104,68 @@ class OccupancyMap:
         lo, hi = np.zeros(3, np.float64), np.zeros(3, np.float64)
         self.ctx._check(lib().ls_occupancy_bounds(self._h, lo.ctypes.data, hi.ctypes.data))
         return lo, hi
+
+
+class DistanceMap:
+    """octomap's DynamicEDTOctomap on the device (ls_distance_map_*): the Euclidean distance of every finest cell of the box
+    bbx_min ... bbx_max (float triples) to its nearest obstacle, an occupied voxel (or, with treat_unknown_as_occupied, an
+    unknown one), capped at max_dist.  update() recomputes it from an OccupancyMap's current state; queries read the last
+    update only."""
+
+    def __init__(self, ctx, max_dist, bbx_min, bbx_max, treat_unknown_as_occupied=False):
+        self.ctx = ctx
+        self.params = DistanceMapParams(float(max_dist), (ctypes.c_float * 3)(*[float(x) for x in bbx_min]),
+                                        (ctypes.c_float * 3)(*[float(x) for x in bbx_max]), int(bool(treat_unknown_as_occupied)))
+        self._h = ctypes.c_void_p()
+        ctx._check(lib().ls_distance_map_create(ctx._h, ctypes.byref(self.params), ctypes.byref(self._h)))
+        self.stats = None
+
+    def close(self):
+        if self._h:
+            lib().ls_distance_map_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def update(self, occupancy_map):
+        """The field of occupancy_map as it is now (ls_distance_map_update).  Returns DistanceMapStats; on an error the
+        previous field stays (LS_ERR_ARG) or the handle has none (LS_ERR_NOMEM)."""
+        st = DistanceMapStats()
+        self.ctx._check(lib().ls_distance_map_update(self._h, occupancy_map._h, ctypes.byref(st)))
+        self.stats = st
+        return st
+
+    def query(self, points):
+        """getDistanceAndClosestObstacle and getSquaredDistanceInCells per point ((n,3), taken as float32): (distance
+        float32 [m], squared distance in cells int32, closest obstacle's voxel centre (n,3) float32).  -1, -1 and NaN
+        outside the box; NaN obstacles where none is within max_dist."""
+        p = np.ascontiguousarray(np.asarray(points, np.float32).reshape(-1, 3))
+        n = len(p)
+        d = np.empty(max(n, 1), np.float32)
+        s = np.empty(max(n, 1), np.int32)
+        o = np.empty((max(n, 1), 3), np.float32)
+        self.last_query = DistanceMapQueryStats()
+        self.ctx._check(lib().ls_distance_map_query(self._h, p.ctypes.data if n else None, n, d.ctypes.data, s.ctypes.data,
+                                                    o.ctypes.data, ctypes.byref(self.last_query)))
+        return d[:n].copy(), s[:n].copy(), o[:n].copy()
+
+    def download(self):
+        """The whole field: (squared distances (sz, sy, sx) int32, closest obstacles' packed keys (sz, sy, sx) uint64, all
+        ones when none)."""
+        n = ctypes.c_int64(0)
+        rc = lib().ls_distance_map_download(self._h, None, None, 0, ctypes.byref(n))
+        if rc != LS_ERR_ARG or n.value == 0:
+            self.ctx._check(rc)
+        m = n.value
+        s = np.empty(max(m, 1), np.int32)
+        k = np.empty(max(m, 1), np.uint64)
+        self.ctx._check(lib().ls_distance_map_download(self._h, s.ctypes.data, k.ctypes.data, m, ctypes.byref(n)))
+        shape = tuple(self.stats.size[::-1]) if self.stats is not None else (m,)
+        return s[:m].reshape(shape), k[:m].reshape(shape)
 
 
 Octree = collections.namedtuple("Octree", "nodes payload centres depths device_ms")

@@ -2338,3 +2338,159 @@ int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]) {
 }
 
 }  // extern "C"
+
+// ---- Euclidean distance map of the occupancy map (DynamicEDTOctomap; kernels in ls_distance.cu) --------------------------
+struct ls_distance_map {
+  ls_ctx* ctx = nullptr;
+  ls_distance_map_params prm{};
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  lso::DistanceField field;
+  bool has_field = false;
+  float max_dist = 0.f;  // getMaxDist of the field
+};
+
+namespace {
+// The map's key of a float coordinate: floor((double)c * inv) + 32768; false when outside [0, 65535] (NaN included).
+bool corner_key(double inv, float c, int* k) {
+  const double s = std::floor((double)c * inv);
+  if (!(s >= -32768.0 && s < 32768.0)) return false;
+  *k = (int)s + 32768;
+  return true;
+}
+
+void distance_stats(const ls_distance_map* dm, float ms, ls_distance_map_stats* stats) {
+  if (!stats) return;
+  const lso::DistanceField& f = dm->field;
+  for (int a = 0; a < 3; ++a) stats->min_key[a] = f.kmin[a], stats->size[a] = f.size[a];
+  stats->cells = f.cells;
+  stats->obstacles = f.obstacles;
+  stats->resolution = f.res;
+  stats->max_sqdist_cells = f.M;
+  stats->max_dist = dm->max_dist;
+  stats->device_bytes = (int64_t)lso::distance_bytes(f);
+  stats->device_ms = ms;
+}
+}  // namespace
+
+extern "C" {
+
+int ls_distance_map_create(ls_ctx* ctx, const ls_distance_map_params* params, ls_distance_map** out) {
+  if (!ctx || !out) return LS_ERR_ARG;
+  *out = nullptr;
+  if (!params) return fail(ctx, LS_ERR_ARG, "bad argument");
+  const ls_distance_map_params& p = *params;
+  if (!std::isfinite(p.max_dist) || !(p.max_dist > 0.f))
+    return fail(ctx, LS_ERR_ARG, "distance map max_dist %g (finite and > 0)", (double)p.max_dist);
+  for (int a = 0; a < 3; ++a) {
+    if (!std::isfinite(p.bbx_min[a]) || !std::isfinite(p.bbx_max[a]))
+      return fail(ctx, LS_ERR_ARG, "distance map box corner not finite on axis %d", a);
+    if (p.bbx_min[a] > p.bbx_max[a])
+      return fail(ctx, LS_ERR_ARG, "distance map box min %g > max %g on axis %d", (double)p.bbx_min[a], (double)p.bbx_max[a], a);
+  }
+  CU(cudaSetDevice(ctx->device));
+  ls_distance_map* dm = new ls_distance_map();
+  dm->ctx = ctx;
+  dm->prm = p;
+  if (cudaStreamCreateWithFlags(&dm->stream, cudaStreamNonBlocking) != cudaSuccess ||
+      cudaEventCreate(&dm->ev0) != cudaSuccess || cudaEventCreate(&dm->ev1) != cudaSuccess) {
+    cudaGetLastError();
+    ls_distance_map_destroy(dm);
+    return fail(ctx, LS_ERR_NOMEM, "distance map creation failed");
+  }
+  *out = dm;
+  return LS_OK;
+}
+
+void ls_distance_map_destroy(ls_distance_map* dm) {
+  if (!dm) return;
+  cudaSetDevice(dm->ctx->device);
+  if (dm->stream) cudaStreamSynchronize(dm->stream);
+  if (dm->ev0) cudaEventDestroy(dm->ev0);
+  if (dm->ev1) cudaEventDestroy(dm->ev1);
+  if (dm->stream) cudaStreamDestroy(dm->stream);
+  delete dm;
+}
+
+int ls_distance_map_update(ls_distance_map* dm, ls_occupancy* om, ls_distance_map_stats* stats) {
+  if (!dm) return LS_ERR_ARG;
+  ls_ctx* ctx = dm->ctx;
+  if (!om) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (om->ctx->device != ctx->device)
+    return fail(ctx, LS_ERR_ARG, "the occupancy map is on device %d, the distance map on device %d", om->ctx->device,
+                ctx->device);
+  const ls_distance_map_params& p = dm->prm;
+  const double res = om->prm.res, inv = om->prm.inv;
+  const double mf = (double)p.max_dist / res + 1.0;
+  if (!(mf < 46341.0)) return fail(ctx, LS_ERR_ARG, "max_dist %g is more than 46340 cells of %g m", (double)p.max_dist, res);
+  const int m = (int)mf;
+  int kmin[3], kmax[3];
+  long long cells = 1;
+  for (int a = 0; a < 3; ++a) {
+    if (!corner_key(inv, p.bbx_min[a], &kmin[a]) || !corner_key(inv, p.bbx_max[a], &kmax[a]))
+      return fail(ctx, LS_ERR_ARG, "a box corner has no valid key on axis %d at resolution %g", a, res);
+    if (kmin[a] > kmax[a]) return fail(ctx, LS_ERR_ARG, "box min key above max key on axis %d", a);
+    cells *= kmax[a] - kmin[a] + 1;
+  }
+  if (cells > (1LL << 30)) return fail(ctx, LS_ERR_ARG, "the box has %lld cells (at most 2^30)", cells);
+  CU(cudaSetDevice(ctx->device));
+  lso::DistanceField& f = dm->field;
+  dm->has_field = false;
+  int rc = lso::distance_reserve(f, cells);
+  if (rc) return fail(ctx, rc, "distance map: out of device memory for %lld cells", cells);
+  for (int a = 0; a < 3; ++a) f.kmin[a] = kmin[a], f.size[a] = kmax[a] - kmin[a] + 1;
+  f.cells = cells;
+  f.res = res, f.inv = inv;
+  f.M = m * m;
+  dm->max_dist = (float)(m * res);
+  CU(cudaEventRecord(dm->ev0, dm->stream));
+  rc = lso::distance_update(f, om->map, om->prm.l_occ, p.treat_unknown_as_occupied != 0, dm->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "distance map update failed");
+  CU(cudaEventRecord(dm->ev1, dm->stream));
+  CU(cudaEventSynchronize(dm->ev1));
+  dm->has_field = true;
+  float ms = 0.f;
+  CU(cudaEventElapsedTime(&ms, dm->ev0, dm->ev1));
+  distance_stats(dm, ms, stats);
+  return LS_OK;
+}
+
+int ls_distance_map_query(ls_distance_map* dm, const float* points3, int n, float* distance, int32_t* sqdist_cells,
+                          float* obstacles3, ls_distance_map_query_stats* stats) {
+  if (!dm) return LS_ERR_ARG;
+  ls_ctx* ctx = dm->ctx;
+  if (n < 0 || (n > 0 && !points3)) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!dm->has_field) return fail(ctx, LS_ERR_STATE, "the distance map has no field: update it first");
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(dm->ev0, dm->stream));
+  long long outside = 0;
+  const int rc = lso::distance_query(dm->field, points3, n, distance, sqdist_cells, obstacles3, &outside, dm->stream,
+                                     &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "distance query: out of device memory" : "distance query failed");
+  CU(cudaEventRecord(dm->ev1, dm->stream));
+  CU(cudaEventSynchronize(dm->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, dm->ev0, dm->ev1));
+    stats->outside = outside;
+    stats->device_ms = ms;
+  }
+  return LS_OK;
+}
+
+int ls_distance_map_download(ls_distance_map* dm, int32_t* sqdist, uint64_t* obstacle_keys, int64_t cap_cells, int64_t* n) {
+  if (!dm) return LS_ERR_ARG;
+  ls_ctx* ctx = dm->ctx;
+  if (!n) return fail(ctx, LS_ERR_ARG, "bad argument");
+  *n = 0;
+  if (!dm->has_field) return fail(ctx, LS_ERR_STATE, "the distance map has no field: update it first");
+  *n = dm->field.cells;
+  if (cap_cells < dm->field.cells)
+    return fail(ctx, LS_ERR_ARG, "buffers of %lld cells for %lld", (long long)cap_cells, dm->field.cells);
+  CU(cudaSetDevice(ctx->device));
+  const int rc = lso::distance_download(dm->field, sqdist, obstacle_keys, dm->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "distance map download failed");
+  return LS_OK;
+}
+
+}  // extern "C"

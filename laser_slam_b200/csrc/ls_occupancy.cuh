@@ -169,4 +169,35 @@ int box_voxels(Map& m, const Params& P, const double center3[3], const double si
 // The smallest and largest known key per axis; *empty when no voxel is known.
 int key_bounds(Map& m, int kmin[3], int kmax[3], bool* empty, cudaStream_t st, uint64_t* launches);
 
+// Euclidean distance map of a box of the map (ls_distance.cu; DESIGN.md §4b''''''''').  The grid covers keys kmin ...
+// kmin + size - 1 per axis, cell (x, y, z) at (z * size[1] + y) * size[0] + x.  The field is val[0] (the squared distance in
+// cells, M where no obstacle is within it) and site[0] (the obstacle's cell index, -1 when none).  The other buffers are
+// scratch: the obstacle grid (one byte per cell), val[1] / site[1] between the passes and the per-column stacks.
+struct DistanceField {
+  ls::Buffer<unsigned char> grid;
+  ls::Buffer<int> val[2], site[2];
+  ls::Buffer<uint2> stack;
+  ls::Buffer<unsigned long long> cnt_dev;
+  ls::PinnedBuffer<unsigned long long> cnt_host;
+  ls::Buffer<char> qbuf;  // query staging, grown by doubling
+  int kmin[3] = {0, 0, 0}, size[3] = {0, 0, 0};
+  long long cells = 0, obstacles = 0;
+  double res = 0.0, inv = 0.0;
+  int M = 0;
+};
+// Every buffer of a field of `cells` cells, all or nothing: after LS_ERR_NOMEM every buffer is empty.
+int distance_reserve(DistanceField& f, long long cells);
+// The field of the map's known voxels inside f's box (kmin, size, cells and M set by the caller, buffers reserved): an
+// obstacle is an occupied voxel (v >= l_occ), and with unknown_occ every unknown cell too.  Reads the map only.  Synchronous;
+// sets f.obstacles.
+int distance_update(DistanceField& f, const Map& m, float l_occ, bool unknown_occ, cudaStream_t st, uint64_t* launches);
+// One thread per point (host float triples): distance [m], squared distance in cells and the obstacle's voxel centre, each
+// output may be NULL; -1 / -1 / NaN for a point whose key is invalid or outside the box (*outside counts them), NaN obstacle
+// centres where the cell has no obstacle.  Synchronous.
+int distance_query(DistanceField& f, const float* pts3, int n, float* dist, int* sq, float* obst3, long long* outside,
+                   cudaStream_t st, uint64_t* launches);
+// The whole field in cell order (each output may be NULL): squared distances, obstacles as packed keys (all ones when none).
+int distance_download(DistanceField& f, int* sq, uint64_t* keys, cudaStream_t st, uint64_t* launches);
+size_t distance_bytes(const DistanceField& f);
+
 }  // namespace lso

@@ -446,3 +446,58 @@ class OccupancyMap:
         out = np.zeros(12, np.float64)
         self._check(lib().lsh_occupancy_bounds(self._h, out.ctypes.data))
         return out[0:3], out[3:6], out[6:9], out[9:12]
+
+
+class DistanceMap:
+    """laser_slam::DistanceMap (include/laser_slam/distance_map.hpp) on an OccupancyMap of this module: DynamicEDTOctomap's
+    calls over the device distance map.  Close it before the occupancy map."""
+
+    def __init__(self, occupancy_map, max_dist, bbx_min, bbx_max, treat_unknown_as_occupied=False):
+        L = lib()
+        if not hasattr(L, "_dist_bound"):
+            vp, ci = ctypes.c_void_p, ctypes.c_int
+            L.lsh_distance_create.restype = vp
+            L.lsh_distance_create.argtypes = [vp, ctypes.c_float, vp, ci, ctypes.c_char_p, ci]
+            L.lsh_distance_destroy.argtypes = [vp]
+            L.lsh_distance_destroy.restype = None
+            L.lsh_distance_last_error.argtypes = [vp]
+            L.lsh_distance_last_error.restype = ctypes.c_char_p
+            L.lsh_distance_update.argtypes = [vp, vp]
+            L.lsh_distance_query.argtypes = [vp, vp, ci, ci, vp, vp, vp]
+            L._dist_bound = True
+        box = np.ascontiguousarray(np.concatenate([np.asarray(bbx_min, np.float64).reshape(3),
+                                                   np.asarray(bbx_max, np.float64).reshape(3)]))
+        err = ctypes.create_string_buffer(512)
+        self._h = L.lsh_distance_create(occupancy_map._h, float(max_dist), box.ctypes.data, int(bool(treat_unknown_as_occupied)),
+                                        err, 512)
+        if not self._h:
+            raise LsError(err.value.decode() or "lsh_distance_create failed")
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().lsh_distance_destroy(self._h)
+            self._h = None
+
+    def _check(self, rc):
+        if rc < 0:
+            raise LsError(lib().lsh_distance_last_error(self._h).decode())
+        return rc
+
+    def update(self):
+        """update; returns (getMaxDist, getSquaredMaxDistCells)."""
+        out = np.zeros(2, np.float64)
+        self._check(lib().lsh_distance_update(self._h, out.ctypes.data))
+        return float(out[0]), int(out[1])
+
+    def query(self, points, single=False):
+        """The batched getDistances, or with single=True getDistance / getDistanceAndClosestObstacle /
+        getSquaredDistanceInCells once per point: (distance float32, squared distance in cells int32, closest (n,3)
+        float64)."""
+        p = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
+        n = len(p)
+        d = np.zeros(max(n, 1), np.float32)
+        s = np.zeros(max(n, 1), np.int32)
+        c = np.zeros((max(n, 1), 3), np.float64)
+        self._check(lib().lsh_distance_query(self._h, p.ctypes.data, n, int(bool(single)), d.ctypes.data, s.ctypes.data,
+                                             c.ctypes.data))
+        return d[:n], s[:n], c[:n]

@@ -8,6 +8,7 @@
 
 #include "laser_slam/incremental_estimator.hpp"
 #include "laser_slam/local_map.hpp"
+#include "laser_slam/distance_map.hpp"
 #include "laser_slam/occupancy_map.hpp"
 #include "laser_slam/velodyne_assembler.hpp"
 
@@ -671,6 +672,72 @@ int lsh_occupancy_bounds(void* ov, double* out12) {
     h->map->getMapBounds(&lo, &hi);
     const kindr::minimal::Position size = h->map->getMapSize(), centre = h->map->getMapCenter();
     for (int a = 0; a < 3; ++a) out12[a] = lo[a], out12[3 + a] = hi[a], out12[6 + a] = size[a], out12[9 + a] = centre[a];
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+// ---- laser_slam::DistanceMap (include/laser_slam/distance_map.hpp) on an OccupancyMap handle, for the tests.  Destroy it
+// before the occupancy map.  box6: bbx_min, bbx_max.
+struct DistanceHandle {
+  std::unique_ptr<DistanceMap> map;
+  std::string err;
+};
+
+void* lsh_distance_create(void* ov, float maxdist, const double* box6, int unknown_occ, char* err, int errlen) {
+  try {
+    DistanceHandle* h = new DistanceHandle();
+    h->map.reset(new DistanceMap(maxdist, *static_cast<OccupancyHandle*>(ov)->map, {box6[0], box6[1], box6[2]},
+                                 {box6[3], box6[4], box6[5]}, unknown_occ != 0));
+    return h;
+  } catch (const std::exception& e) {
+    if (err && errlen > 0) std::strncpy(err, e.what(), (size_t)errlen - 1), err[errlen - 1] = 0;
+    return nullptr;
+  }
+}
+void lsh_distance_destroy(void* dv) { delete static_cast<DistanceHandle*>(dv); }
+const char* lsh_distance_last_error(void* dv) { return static_cast<DistanceHandle*>(dv)->err.c_str(); }
+
+// update; out2: getMaxDist, getSquaredMaxDistCells.  0 or LS_ERR_STATE
+int lsh_distance_update(void* dv, double* out2) {
+  DistanceHandle* h = static_cast<DistanceHandle*>(dv);
+  try {
+    h->map->update();
+    out2[0] = h->map->getMaxDist(), out2[1] = h->map->getSquaredMaxDistCells();
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// single = 1: getDistance, getDistanceAndClosestObstacle and getSquaredDistanceInCells once per point (the two distances
+// must agree); single = 0: the batched getDistances.  closest3 as the C++ layer returns it.  0 or LS_ERR_STATE
+int lsh_distance_query(void* dv, const double* pts3, int n, int single, float* dist, int* sq, double* closest3) {
+  DistanceHandle* h = static_cast<DistanceHandle*>(dv);
+  try {
+    std::vector<kindr::minimal::Position> p(n);
+    for (int i = 0; i < n; ++i) p[i] = {pts3[3 * i], pts3[3 * i + 1], pts3[3 * i + 2]};
+    if (single) {
+      for (int i = 0; i < n; ++i) {
+        kindr::minimal::Position c;
+        h->map->getDistanceAndClosestObstacle(p[i], dist[i], c);
+        const float d = h->map->getDistance(p[i]);
+        if (!(d == dist[i])) throw std::runtime_error("getDistance and getDistanceAndClosestObstacle disagree");
+        sq[i] = h->map->getSquaredDistanceInCells(p[i]);
+        for (int a = 0; a < 3; ++a) closest3[3 * i + a] = c[a];
+      }
+      return 0;
+    }
+    std::vector<float> d;
+    std::vector<int> s;
+    std::vector<kindr::minimal::Position> c;
+    h->map->getDistances(p, &d, &s, &c);
+    for (int i = 0; i < n; ++i) {
+      dist[i] = d[(size_t)i], sq[i] = s[(size_t)i];
+      for (int a = 0; a < 3; ++a) closest3[3 * i + a] = c[(size_t)i][a];
+    }
     return 0;
   } catch (const std::exception& e) {
     h->err = e.what();

@@ -109,6 +109,17 @@ ek, ev, _ = om.download(ls.OCC_KNOWN)
 assert np.array_equal(ek, er.as_arrays(vox)[0]) and np.array_equal(ev.view(np.uint32), er.as_arrays(vox)[1].view(np.uint32))
 assert np.array_equal(om.box_voxels(bc[1], (6.0, 6.0, 6.0))[0], e.crop(vox, bc[1], (6.0, 6.0, 6.0))[0])
 assert all(np.array_equal(a, b) for a, b in zip(om.bounds(), e.bounds(vox)))
+# the distance map of that map in both modes (ls_distance.cu): one update, the field and one query against the reference
+import distance_map_ref as dmr
+dk, dv, _ = om.download(ls.OCC_KNOWN)
+dlo, dhi = truth[0][:3, 3] - 3.0, truth[0][:3, 3] + 3.0
+dq = truth[0][:3, 3] + rng.uniform(-4.0, 4.0, (256, 3))
+for unknown in (False, True):
+    dm = ls.DistanceMap(ctx, 1.0, dlo, dhi, unknown)
+    dm.update(om)
+    df = dmr.Field(dk, dv, 0.2, oc.logodds(0.7), 1.0, dlo, dhi, unknown)
+    assert np.array_equal(dm.download()[0], df.s) and np.array_equal(dm.query(dq)[1], df.query(dq)[1])
+    dm.close()
 om.clear()
 assert om.size(ls.OCC_KNOWN) == 0
 om.close()
