@@ -119,16 +119,36 @@ class OccupancyMap {
   kindr::minimal::Position getMapSize() const;
   kindr::minimal::Position getMapCenter() const;
 
+  // ---- change detection: octomap's calls and volumetric_mapping's getChangedPoints on the device map
+  // (ls_occupancy_track_changes / _changes; rules in DESIGN.md §4b'''''''''').  A change is a voxel whose state (free,
+  // occupied, unknown) differs from its state at the last enable or reset.
+  // true takes the map as it is now as the baseline (again when enabled); false turns tracking off.
+  void enableChangeDetection(bool enable);
+  bool isChangeDetectionEnabled() const;
+  // The map as it is now becomes the baseline; nothing while tracking is off.
+  void resetChangeDetection();
+  // 0 while tracking is off.
+  size_t numChangesDetected() const;
+  // (new) The changed voxels by ascending key: packed keys, LS_CELL_* now and at the baseline; empty while tracking is off.
+  void getChangedKeys(std::vector<uint64_t>* keys, std::vector<int8_t>* status, std::vector<int8_t>* previous) const;
+  // The changed voxels' centres and whether each is occupied now, by ascending key, then resetChangeDetection; empty
+  // while tracking is off.
+  void getChangedPoints(std::vector<kindr::minimal::Position>* changed_points, std::vector<bool>* changed_states);
+
  private:
   friend class DistanceMap;  // reads map_ under mutex_ in its update (include/laser_slam/distance_map.hpp)
 
   CellStatus cellStatus(const kindr::minimal::Position& point, float* log_odds) const;
   void download(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds, std::vector<float>* centres4) const;
+  // Under mutex_: the changes (each output may be NULL), then a reset when `reset`.  Returns their number.
+  size_t changes(std::vector<uint64_t>* keys, std::vector<int8_t>* status, std::vector<int8_t>* previous,
+                 std::vector<float>* centres4, bool reset) const;
 
   OccupancyMapParams params_;
   IncrementalEstimator& estimator_;
   ls_ctx* ctx_ = nullptr;
   ls_occupancy* map_ = nullptr;
+  bool change_detection_ = false;
   mutable std::mutex mutex_;
 };
 

@@ -556,6 +556,39 @@ int ls_occupancy_box_voxels(ls_occupancy* om, const double center3[3], const dou
                             float* log_odds, float* centres4, int64_t cap, int64_t* n);
 int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]);
 
+/* Change detection: octomap's enableChangeDetection / changedKeysBegin / numChangesDetected / resetChangeDetection, as
+ * volumetric_mapping's getChangedPoints reads them, kept as a diff against a baseline (DESIGN.md §4b'''''''''').  Rules:
+ *   state     per voxel: LS_CELL_UNKNOWN, LS_CELL_FREE (known, v < L_occ) or LS_CELL_OCCUPIED (known, v >= L_occ)
+ *   baseline  the state of every voxel known when tracking was enabled or last reset, stored by brick key (not by pool
+ *             index), with the map's resolution then
+ *   changed   a voxel whose state now differs from its state at the baseline: one known now and unknown then (octomap's
+ *             `true`), one whose occupied state differs (an odd number of flips; an even number leaves nothing), and one
+ *             known then and unknown now (only ls_occupancy_clear or a .bt / .ot read does that).  A log-odds change that
+ *             keeps the state is not a change.  The result does not depend on the order of the updates since the baseline,
+ *             so inserts, edits and reads run exactly as without tracking
+ *   outputs   per changed voxel, by ascending packed key: the key, the state now (status) and then (previous), LS_CELL_*,
+ *             and the voxel centre {x, y, z, 1}: (float)(((double)(k - 32768) + 0.5) * res) per axis, res the map's
+ *             resolution for a voxel known now and the baseline's for one unknown now
+ *   reset     reset != 0 makes the map as it is now the new baseline after a successful copy (getChangedPoints followed by
+ *             resetChangeDetection); a refused call does not reset
+ * ls_occupancy_track_changes(om, 1) takes a fresh baseline (again when tracking is on); (om, 0) turns tracking off and
+ * frees the baseline.  Calls run on the map's stream, are synchronous, never change the map and are legal between
+ * ls_icp_register_submap_batch_begin and _end.  Errors: LS_ERR_STATE from ls_occupancy_changes while tracking is off;
+ * LS_ERR_ARG, without a copy and without a reset, for a NULL n, cap < 0 or more changes than cap (so cap = 0 asks for the
+ * count); LS_ERR_NOMEM when the baseline or the scratch cannot grow.  After any error the baseline, the tracking state and
+ * the map are as they were. */
+typedef struct ls_occupancy_change_stats {
+  int64_t bricks_compared; /* the map's bricks plus the baseline's, each read once per pass */
+  int64_t changed;         /* voxels changed (= *n) */
+  int64_t baseline_bricks; /* bricks of the baseline after the call */
+  int64_t device_bytes;    /* device memory change detection holds: baselines and scratch */
+  float device_ms;         /* the call on the map's stream, the reset's capture included */
+} ls_occupancy_change_stats;
+int ls_occupancy_track_changes(ls_occupancy* om, int enable);
+/* keys, status, previous, centres4 and stats may be NULL; *n always set. */
+int ls_occupancy_changes(ls_occupancy* om, uint64_t* keys, int8_t* status, int8_t* previous, float* centres4, int64_t cap,
+                         int64_t* n, int reset, ls_occupancy_change_stats* stats);
+
 /* Euclidean distance map of the occupancy map: octomap's DynamicEDTOctomap(maxdist, octree, bbxMin, bbxMax,
  * treatUnknownAsOccupied) over the finest cells of a box, recomputed in full on the device at every update and queried in
  * batches (DESIGN.md §4b''''''''').  Rules:

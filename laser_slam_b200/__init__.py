@@ -123,6 +123,13 @@ class OccupancyEditStats(ctypes.Structure):
                 ("bricks", ctypes.c_int64), ("device_bytes", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
 
+class OccupancyChangeStats(ctypes.Structure):
+    """ls_occupancy_change_stats: bricks compared (the map's plus the baseline's), voxels changed, the baseline's bricks
+    after the call, device bytes change detection holds and the call's device ms."""
+    _fields_ = [("bricks_compared", ctypes.c_int64), ("changed", ctypes.c_int64), ("baseline_bricks", ctypes.c_int64),
+                ("device_bytes", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
 class OccupancyQueryStats(ctypes.Structure):
     _fields_ = [("keys_visited", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
@@ -269,6 +276,9 @@ def lib():
         L.ls_occupancy_clear.argtypes = [vp]
         L.ls_occupancy_box_voxels.argtypes = [vp, vp, vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
         L.ls_occupancy_bounds.argtypes = [vp, vp, vp]
+        L.ls_occupancy_track_changes.argtypes = [vp, ci]
+        L.ls_occupancy_changes.argtypes = [vp, vp, vp, vp, vp, ctypes.c_int64, i64p, ci,
+                                           ctypes.POINTER(OccupancyChangeStats)]
         L.ls_distance_map_create.argtypes = [vp, ctypes.POINTER(DistanceMapParams), ctypes.POINTER(vp)]
         L.ls_distance_map_destroy.argtypes = [vp]
         L.ls_distance_map_destroy.restype = None
@@ -1104,6 +1114,33 @@ class OccupancyMap:
         lo, hi = np.zeros(3, np.float64), np.zeros(3, np.float64)
         self.ctx._check(lib().ls_occupancy_bounds(self._h, lo.ctypes.data, hi.ctypes.data))
         return lo, hi
+
+    # ---- change detection (ls_occupancy_track_changes / _changes); self.last_changes holds the last call's stats
+    def track_changes(self, enable=True):
+        """enableChangeDetection: True takes the map as it is now as the baseline (again when tracking is on); False turns
+        tracking off and frees the baseline."""
+        self.ctx._check(lib().ls_occupancy_track_changes(self._h, int(bool(enable))))
+
+    def changes(self, reset=False):
+        """The voxels whose state (CELL_*) differs from the baseline's, by ascending packed key: (keys uint64, status int8
+        now, previous int8 at the baseline, centres (n,4) float32).  reset=True then makes the map the new baseline
+        (getChangedPoints followed by resetChangeDetection)."""
+        n = ctypes.c_int64(0)
+        self.last_changes = OccupancyChangeStats()
+        rc = lib().ls_occupancy_changes(self._h, None, None, None, None, 0, ctypes.byref(n), int(bool(reset)),
+                                        ctypes.byref(self.last_changes))
+        if rc != LS_ERR_ARG or n.value == 0:
+            self.ctx._check(rc)
+        m = n.value
+        keys = np.empty(max(m, 1), np.uint64)
+        st = np.empty(max(m, 1), np.int8)
+        prev = np.empty(max(m, 1), np.int8)
+        cen = np.empty((max(m, 1), 4), np.float32)
+        if m > 0:
+            self.ctx._check(lib().ls_occupancy_changes(self._h, keys.ctypes.data, st.ctypes.data, prev.ctypes.data,
+                                                       cen.ctypes.data, m, ctypes.byref(n), int(bool(reset)),
+                                                       ctypes.byref(self.last_changes)))
+        return keys[:m].copy(), st[:m].copy(), prev[:m].copy(), cen[:m].copy()
 
 
 class DistanceMap:

@@ -1739,6 +1739,8 @@ struct ls_occupancy {
   lso::Octree full;           // the full tree (.ot), cached apart from the .bt build
   bool full_current = false;
   float full_ms = 0.f;
+  lso::Changes changes;  // change detection's baseline and scratch (ls_changes.cu)
+  bool tracking = false;
 };
 
 namespace {
@@ -2333,6 +2335,57 @@ int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]) {
     const auto centre = [res](int k) { return (double)(float)(((double)(k - 32768) + 0.5) * res); };
     min3[a] = empty ? 0.0 : centre(kmin[a]) - res / 2.0;
     max3[a] = empty ? 0.0 : (centre(kmax[a]) - res / 2.0) + res;
+  }
+  return LS_OK;
+}
+
+int ls_occupancy_track_changes(ls_occupancy* om, int enable) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  CU(cudaSetDevice(ctx->device));
+  if (!enable) {
+    CU(cudaStreamSynchronize(om->stream));
+    lso::release_changes(om->changes);
+    om->tracking = false;
+    return LS_OK;
+  }
+  const int rc = lso::capture_baseline(om->changes, om->map, om->prm, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "change detection: out of device memory for the baseline" :
+                                                    "change detection: baseline capture failed");
+  om->tracking = true;
+  return LS_OK;
+}
+
+int ls_occupancy_changes(ls_occupancy* om, uint64_t* keys, int8_t* status, int8_t* previous, float* centres4, int64_t cap,
+                         int64_t* n, int reset, ls_occupancy_change_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!n) return fail(ctx, LS_ERR_ARG, "bad argument");
+  *n = 0;
+  if (cap < 0) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!om->tracking) return fail(ctx, LS_ERR_STATE, "change detection is off: enable it with ls_occupancy_track_changes");
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  const long long compared = (long long)om->map.pool_n + om->changes.base.n;
+  long long m = 0;
+  int rc = lso::diff_changes(om->changes, om->map, om->prm, keys, status, previous, centres4, cap, &m, om->stream,
+                             &ctx->launches);
+  *n = m;
+  if (rc == LS_ERR_ARG) return fail(ctx, rc, "buffers of %lld changes for %lld", (long long)cap, m);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "changes: out of device memory" : "changes failed");
+  if (reset && (rc = lso::capture_baseline(om->changes, om->map, om->prm, om->stream, &ctx->launches)))
+    return fail(ctx, rc, rc == LS_ERR_NOMEM ? "changes copied, the reset is refused: out of device memory for the baseline"
+                                            : "changes copied, the reset failed");
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    stats->bricks_compared = compared;
+    stats->changed = m;
+    stats->baseline_bricks = om->changes.base.n;
+    stats->device_bytes = (int64_t)lso::changes_bytes(om->changes);
+    stats->device_ms = ms;
   }
   return LS_OK;
 }

@@ -67,7 +67,6 @@ namespace {
 
 constexpr unsigned long long kEmpty = ~0ull;
 constexpr int kPending = -1, kFull = -2;
-constexpr int kMaxProbe = 64;
 constexpr int kKeyMax = 32768;
 constexpr long long kMaxEditAxis = 1LL << 17;    // loop points per box axis (the key space has 2^16 per axis)
 constexpr long long kMaxEditBricks = 1LL << 29;  // bricks of an edit plus those in use (the read's bound)
@@ -101,15 +100,6 @@ struct Dev {
 Dev dev_of(const Map& m) {
   return Dev{m.tab_keys.get(), m.tab_vals.get(), (unsigned)m.tab_cap() - 1u, m.pool_cap(), m.lo.get(), m.known.get(),
              m.mfree.get(), m.mocc.get(), m.bkey.get(), m.touched.get(), m.tlist.get()};
-}
-
-__device__ __forceinline__ unsigned hash64(unsigned long long k) {
-  k ^= k >> 33;
-  k *= 0xff51afd7ed558ccdull;
-  k ^= k >> 33;
-  k *= 0xc4ceb9fe1a85ec53ull;
-  k ^= k >> 33;
-  return (unsigned)k;
 }
 
 // floor(c * (1/res)) + 32768, valid iff in [0, 65535]
@@ -420,19 +410,8 @@ __global__ void occ_centres_kernel(const unsigned long long* __restrict__ keys, 
 // They read tab_keys / tab_vals, the known bits and the log-odds only; no insert runs during a query.
 constexpr unsigned kNanBits = 0x7fc00000u;  // the NaN of an unknown cell's log-odds and an invalid ray's end
 
-// Pool index of brick bk, or -1 when the hash does not hold it.  Read-only: no CAS, no allocation, no wait on a pending
-// slot.  A slot whose value is negative (left by an insert whose pool filled) is absent.
 __device__ __forceinline__ int find_brick(const Dev& D, unsigned long long bk) {
-  unsigned h = hash64(bk) & D.tab_mask;
-  for (int p = 0; p < kMaxProbe; ++p, h = (h + 1u) & D.tab_mask) {
-    const unsigned long long k = D.tab_keys[h];
-    if (k == bk) {
-      const int v = D.tab_vals[h];
-      return v >= 0 ? v : -1;
-    }
-    if (k == kEmpty) return -1;
-  }
-  return -1;
+  return lookup_brick(D.tab_keys, D.tab_vals, D.tab_mask, bk);
 }
 
 // State of voxel k (LS_CELL_*), the brick of the last lookup cached in cur.  The known bit decides "unknown", not the

@@ -76,6 +76,59 @@ struct Map {
   int pool_cap() const { return (int)tlist.capacity(); }
 };
 
+// The brick hash: a brick key's home slot (before the mask) and the probe bound of its linear probing.  The insert places
+// keys with it (ls_occupancy.cu); the queries and change detection (ls_changes.cu) look them up.
+constexpr int kMaxProbe = 64;
+__device__ __forceinline__ unsigned hash64(unsigned long long k) {
+  k ^= k >> 33;
+  k *= 0xff51afd7ed558ccdull;
+  k ^= k >> 33;
+  k *= 0xc4ceb9fe1a85ec53ull;
+  k ^= k >> 33;
+  return (unsigned)k;
+}
+
+// Pool index of brick bk, or -1 when the hash does not hold it.  Read-only: no CAS, no allocation, no wait on a pending
+// slot.  A slot whose value is negative (left by an insert whose pool filled) is absent.
+__device__ __forceinline__ int lookup_brick(const unsigned long long* tab_keys, const int* tab_vals, unsigned mask,
+                                            unsigned long long bk) {
+  unsigned h = hash64(bk) & mask;
+  for (int p = 0; p < kMaxProbe; ++p, h = (h + 1u) & mask) {
+    const unsigned long long k = tab_keys[h];
+    if (k == bk) {
+      const int v = tab_vals[h];
+      return v >= 0 ? v : -1;
+    }
+    if (k == ~0ull) return -1;
+  }
+  return -1;
+}
+
+// Change detection (ls_changes.cu; DESIGN.md §4b'''''''''').  A baseline holds, per brick with a known voxel when it was
+// taken, its brick key (ascending) and 32 words: 16 of known bits, then 16 of occupied bits (known and v >= L_occ); res is
+// the map's resolution then.  Keys, not pool indices, so growth, rehashing, clear and reads cannot corrupt it.
+struct Baseline {
+  ls::Buffer<unsigned long long> keys;
+  ls::Buffer<unsigned> bits;
+  long long n = 0;
+  double res = 0.0;
+};
+struct Changes {
+  Baseline base, next;  // next: a capture in progress, swapped with base when it completes
+  // capture records before the sort (key, order, bits); the diff's voxels (packed key, states) before and after the sort,
+  // their status / previous bytes and centres
+  ls::Buffer<unsigned long long> rec_key;
+  ls::Buffer<int> rec_idx[2];
+  ls::Buffer<unsigned> rec_bits;
+  ls::Buffer<unsigned long long> out_key[2];
+  ls::Buffer<unsigned> out_val[2];
+  ls::Buffer<signed char> out_st;
+  ls::Buffer<float4> out_c;
+  ls::Buffer<unsigned char> cub_tmp;
+  ls::Buffer<unsigned long long> cnt_dev;
+  ls::PinnedBuffer<unsigned long long> cnt_host;
+};
+
 // The map as octomap's pruned tree: depth 16 over the map's keys, each brick a depth-13 node.  Node records hold the
 // bricks by Morton code, then each upper level (12 ... 0) in turn; all scratch is O(bricks) plus the outputs.
 struct Octree {
@@ -199,5 +252,16 @@ int distance_query(DistanceField& f, const float* pts3, int n, float* dist, int*
 // The whole field in cell order (each output may be NULL): squared distances, obstacles as packed keys (all ones when none).
 int distance_download(DistanceField& f, int* sq, uint64_t* keys, cudaStream_t st, uint64_t* launches);
 size_t distance_bytes(const DistanceField& f);
+
+// Change detection (ls_changes.cu).  Both read the map only and are synchronous.
+// The map's state now (P.res, P.l_occ) becomes c.base.  On an error c.base is as it was.
+int capture_baseline(Changes& c, const Map& m, const Params& P, cudaStream_t st, uint64_t* launches);
+// The voxels whose state (LS_CELL_*) differs from c.base's, by ascending packed key: keys, states now and then, centres
+// {x, y, z, 1} (at P.res when known now, at c.base.res otherwise), each output may be NULL.  *n: their number;
+// LS_ERR_ARG without a copy when it exceeds cap.
+int diff_changes(Changes& c, const Map& m, const Params& P, uint64_t* keys, int8_t* status, int8_t* previous, float* centres4,
+                 long long cap, long long* n, cudaStream_t st, uint64_t* launches);
+void release_changes(Changes& c);
+size_t changes_bytes(const Changes& c);
 
 }  // namespace lso

@@ -300,6 +300,11 @@ class OccupancyMap:
             L.lsh_occupancy_reset.argtypes = [vp]
             L.lsh_occupancy_box_cloud.argtypes = [vp, vp, vp, vp, ci]
             L.lsh_occupancy_bounds.argtypes = [vp, vp]
+            L.lsh_occupancy_track_changes.argtypes = [vp, ci]
+            L.lsh_occupancy_changed_keys.argtypes = [vp, vp, vp, vp, i64]
+            L.lsh_occupancy_changed_keys.restype = i64
+            L.lsh_occupancy_changed_points.argtypes = [vp, vp, vp, i64]
+            L.lsh_occupancy_changed_points.restype = i64
             L._occ_bound = True
         prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range], np.float64)
         err = ctypes.create_string_buffer(512)
@@ -446,6 +451,35 @@ class OccupancyMap:
         out = np.zeros(12, np.float64)
         self._check(lib().lsh_occupancy_bounds(self._h, out.ctypes.data))
         return out[0:3], out[3:6], out[6:9], out[9:12]
+
+    def enable_change_detection(self, enable=True):
+        """enableChangeDetection; returns isChangeDetectionEnabled."""
+        return bool(self._check(lib().lsh_occupancy_track_changes(self._h, int(bool(enable)))))
+
+    def reset_change_detection(self):
+        """resetChangeDetection; returns isChangeDetectionEnabled."""
+        return bool(self._check(lib().lsh_occupancy_track_changes(self._h, -1)))
+
+    def num_changes(self):
+        """numChangesDetected."""
+        return self._check(lib().lsh_occupancy_changed_keys(self._h, None, None, None, 0))
+
+    def changed_keys(self):
+        """getChangedKeys: (keys uint64, status int8, previous int8) by ascending key."""
+        n = self.num_changes()
+        k = np.zeros(max(n, 1), np.uint64)
+        s = np.zeros(max(n, 1), np.int8)
+        p = np.zeros(max(n, 1), np.int8)
+        self._check(lib().lsh_occupancy_changed_keys(self._h, k.ctypes.data, s.ctypes.data, p.ctypes.data, n))
+        return k[:n], s[:n], p[:n]
+
+    def changed_points(self, cap):
+        """getChangedPoints (then a reset): (centres (n,3) float64, occupied (n,) bool), at most cap of them."""
+        pts = np.zeros((max(cap, 1), 3), np.float64)
+        occ = np.zeros(max(cap, 1), np.uint8)
+        n = self._check(lib().lsh_occupancy_changed_points(self._h, pts.ctypes.data, occ.ctypes.data, int(cap)))
+        m = min(n, cap)
+        return pts[:m], occ[:m].astype(bool)
 
 
 class DistanceMap:

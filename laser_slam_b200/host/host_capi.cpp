@@ -678,6 +678,57 @@ int lsh_occupancy_bounds(void* ov, double* out12) {
     return LS_ERR_STATE;
   }
 }
+// Change detection.  enableChangeDetection (enable >= 0) or resetChangeDetection (enable < 0); returns
+// isChangeDetectionEnabled, or LS_ERR_STATE.
+int lsh_occupancy_track_changes(void* ov, int enable) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    if (enable < 0) h->map->resetChangeDetection();
+    else h->map->enableChangeDetection(enable != 0);
+    return h->map->isChangeDetectionEnabled() ? 1 : 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// numChangesDetected, then (when keys is not NULL and it is <= cap) getChangedKeys; returns the count or LS_ERR_STATE
+int64_t lsh_occupancy_changed_keys(void* ov, uint64_t* keys, int8_t* status, int8_t* previous, int64_t cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    const int64_t n = (int64_t)h->map->numChangesDetected();
+    if (!keys || n > cap) return n;
+    std::vector<uint64_t> k;
+    std::vector<int8_t> s, p;
+    h->map->getChangedKeys(&k, &s, &p);
+    if ((int64_t)k.size() != n) throw std::runtime_error("numChangesDetected and getChangedKeys disagree");
+    for (int64_t i = 0; i < n; ++i) keys[i] = k[(size_t)i], status[i] = s[(size_t)i], previous[i] = p[(size_t)i];
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// getChangedPoints (which resets); returns its number of points, the first min(n, cap) written: centres and occupied
+int64_t lsh_occupancy_changed_points(void* ov, double* pts3, uint8_t* occupied, int64_t cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<kindr::minimal::Position> p;
+    std::vector<bool> s;
+    h->map->getChangedPoints(&p, &s);
+    const int64_t n = (int64_t)p.size();
+    for (int64_t i = 0; i < n && i < cap; ++i) {
+      for (int a = 0; a < 3; ++a) pts3[3 * i + a] = p[(size_t)i][a];
+      occupied[i] = s[(size_t)i] ? 1 : 0;
+    }
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
 // ---- laser_slam::DistanceMap (include/laser_slam/distance_map.hpp) on an OccupancyMap handle, for the tests.  Destroy it
 // before the occupancy map.  box6: bbx_min, bbx_max.
 struct DistanceHandle {

@@ -329,4 +329,71 @@ kindr::minimal::Position OccupancyMap::getMapCenter() const {
   return c;
 }
 
+// ---- change detection ----------------------------------------------------------------------------------------------
+void OccupancyMap::enableChangeDetection(bool enable) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  throwOnError(ctx_, ls_occupancy_track_changes(map_, enable ? 1 : 0), "ls_occupancy_track_changes");
+  change_detection_ = enable;
+}
+
+bool OccupancyMap::isChangeDetectionEnabled() const {
+  std::lock_guard<std::mutex> lock(mutex_);
+  return change_detection_;
+}
+
+void OccupancyMap::resetChangeDetection() {
+  std::lock_guard<std::mutex> lock(mutex_);
+  if (change_detection_) throwOnError(ctx_, ls_occupancy_track_changes(map_, 1), "ls_occupancy_track_changes");
+}
+
+size_t OccupancyMap::changes(std::vector<uint64_t>* keys, std::vector<int8_t>* status, std::vector<int8_t>* previous,
+                             std::vector<float>* centres4, bool reset) const {
+  std::lock_guard<std::mutex> lock(mutex_);
+  if (!change_detection_) {
+    if (keys) keys->clear();
+    if (status) status->clear();
+    if (previous) previous->clear();
+    if (centres4) centres4->clear();
+    return 0;
+  }
+  // the count (with cap 0 a reset happens only when nothing changed), then the copy and the reset
+  int64_t n = 0;
+  const int rc = ls_occupancy_changes(map_, NULL, NULL, NULL, NULL, 0, &n, reset ? 1 : 0, NULL);
+  if (!(rc == LS_ERR_ARG && n > 0)) throwOnError(ctx_, rc, "ls_occupancy_changes");
+  if (n == 0 || !(keys || status || previous || centres4)) return (size_t)n;
+  const size_t m = (size_t)n;
+  if (keys) keys->resize(m);
+  if (status) status->resize(m);
+  if (previous) previous->resize(m);
+  if (centres4) centres4->resize(4 * m);
+  throwOnError(ctx_,
+               ls_occupancy_changes(map_, keys ? keys->data() : NULL, status ? status->data() : NULL,
+                                    previous ? previous->data() : NULL, centres4 ? centres4->data() : NULL, n, &n,
+                                    reset ? 1 : 0, NULL),
+               "ls_occupancy_changes");
+  return m;
+}
+
+size_t OccupancyMap::numChangesDetected() const { return changes(NULL, NULL, NULL, NULL, false); }
+
+void OccupancyMap::getChangedKeys(std::vector<uint64_t>* keys, std::vector<int8_t>* status,
+                                  std::vector<int8_t>* previous) const {
+  if (keys == NULL || status == NULL || previous == NULL) throw std::invalid_argument("null output");
+  changes(keys, status, previous, NULL, false);
+}
+
+void OccupancyMap::getChangedPoints(std::vector<kindr::minimal::Position>* changed_points,
+                                    std::vector<bool>* changed_states) {
+  if (changed_points == NULL || changed_states == NULL) throw std::invalid_argument("null output");
+  std::vector<int8_t> status;
+  std::vector<float> c;
+  const size_t n = changes(NULL, &status, NULL, &c, true);
+  changed_points->resize(n);
+  changed_states->resize(n);
+  for (size_t i = 0; i < n; ++i) {
+    (*changed_points)[i] = kindr::minimal::Position{c[4 * i], c[4 * i + 1], c[4 * i + 2]};
+    (*changed_states)[i] = status[i] == LS_CELL_OCCUPIED;
+  }
+}
+
 }  // namespace laser_slam

@@ -120,6 +120,14 @@ for unknown in (False, True):
     df = dmr.Field(dk, dv, 0.2, oc.logodds(0.7), 1.0, dlo, dhi, unknown)
     assert np.array_equal(dm.download()[0], df.s) and np.array_equal(dm.query(dq)[1], df.query(dq)[1])
     dm.close()
+# change detection of that map (ls_changes.cu): one capture, an edit, one diff with a reset, against two downloads
+import occupancy_changes_ref as ocr
+om.track_changes()
+ck0 = om.download(ls.OCC_KNOWN)[:2]
+om.set_boxes([bc[0]], [(2.0, 2.0, 2.0)], [True])
+cg = om.changes(reset=True)
+cw = ocr.diff_arrays(*ck0, *om.download(ls.OCC_KNOWN)[:2], oc.logodds(0.7))
+assert len(cg[0]) > 0 and all(np.array_equal(x, y) for x, y in zip(cg[:3], cw))
 om.clear()
 assert om.size(ls.OCC_KNOWN) == 0
 om.close()
