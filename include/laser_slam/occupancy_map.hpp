@@ -30,6 +30,9 @@ struct OccupancyMapParams {
   double occupancy_thres = 0.7;
   double sensor_max_range = 20.0;  // < 0: unlimited
   int initial_capacity_bricks = 0;  // 8x8x8-voxel bricks to start with; <= 0: the library's default
+  // volumetric_mapping's: robot collision checks count unknown space as a collision (recalled, unverified).  The status
+  // calls report unknown either way.
+  bool treat_unknown_as_occupied = true;
 };
 
 class OccupancyMap {
@@ -100,6 +103,26 @@ class OccupancyMap {
                 std::vector<int>* results, std::vector<kindr::minimal::Position>* ends, bool ignore_unknown = false,
                 double max_range = -1.0) const;
 
+  // ---- box status and robot collision: volumetric_mapping's getCellStatusBoundingBox and robot calls on the device map
+  // (ls_occupancy_box_status / _check_paths; rules in DESIGN.md §4b''''''''''').  The robot is an axis-aligned box of
+  // getRobotSize() (zero until set) at each position; a pose collides when its box is occupied, or, with
+  // treat_unknown_as_occupied, when it is not free.
+  CellStatus getCellStatusBoundingBox(const kindr::minimal::Position& point,
+                                      const kindr::minimal::Position& bounding_box_size) const;
+  // (new) One status per box.
+  void getCellStatusBoundingBox(const std::vector<kindr::minimal::Position>& points,
+                                const std::vector<kindr::minimal::Position>& bounding_box_sizes,
+                                std::vector<CellStatus>* statuses) const;
+  void setRobotSize(const kindr::minimal::Position& robot_size);
+  kindr::minimal::Position getRobotSize() const;
+  bool checkCollisionWithRobot(const kindr::minimal::Position& robot_position) const;
+  // True when a pose collides; *collision_index (may be NULL) the first one.
+  bool checkPathForCollisionsWithRobot(const std::vector<kindr::minimal::Position>& robot_positions,
+                                       size_t* collision_index) const;
+  // (new) Per path the first colliding pose's index, -1 when none (an empty path included).
+  void checkPathsForCollisionsWithRobot(const std::vector<std::vector<kindr::minimal::Position> >& paths,
+                                        std::vector<int64_t>* first_collisions) const;
+
   // ---- edits: volumetric_mapping's WorldBase map calls on the device map (ls_occupancy_set_boxes / _clear / _box_voxels /
   // _bounds; rules in DESIGN.md §4b'''''''').  Errors throw, as every call here.
   // setFree / setOccupied: every voxel the box's loop reaches becomes known with clamping_thres_min / _max.
@@ -149,6 +172,7 @@ class OccupancyMap {
   ls_ctx* ctx_ = nullptr;
   ls_occupancy* map_ = nullptr;
   bool change_detection_ = false;
+  kindr::minimal::Position robot_size_{0.0, 0.0, 0.0};
   mutable std::mutex mutex_;
 };
 

@@ -521,6 +521,36 @@ int ls_occupancy_line_status(ls_occupancy* om, const double* starts3, const doub
 int ls_occupancy_cast_rays(ls_occupancy* om, const float* origins3, const float* directions3, int n, int ignore_unknown,
                            double max_range, int8_t* result, float* ends3, ls_occupancy_query_stats* stats);
 
+/* Box status and robot collision: volumetric_mapping's getCellStatusBoundingBox, checkCollisionWithRobot and
+ * checkPathForCollisionsWithRobot, batched (DESIGN.md §4b''''''''''').  Per box (centre p, size s, double triples):
+ *   1  the centre's state by the cell rule above (double key); when it is not free, that is the box's status
+ *   2  the float centre (float)p with an invalid key: unknown
+ *   3  corners bmin = (float)(p - s/2), bmax = (float)(p + s/2) per axis
+ *   4  occupied pass, only when both corners have valid keys: every known voxel with keys between key(bmin) and key(bmax)
+ *      on all axes whose cube c +- res/2 (c = ((double)(k - 32768) + 0.5) * res) is not wholly outside [bmin, bmax] on an
+ *      axis; an occupied one makes the box occupied
+ *   5  unknown pass: per axis x = bmin; x <= bmax; x += res in double (y inside x, z innermost), each point cast to float
+ *      and keyed; an invalid key or a voxel that is not known makes the box unknown
+ *   6  otherwise free.  Occupied beats unknown beats free, so the order of the work does not matter
+ * A pose collides when its box (the robot's size at the position) is occupied, or with unknown_as_occupied when it is not
+ * free.  Path p is positions3[offsets[p] ... offsets[p + 1]); its result is the first colliding pose's index within the
+ * path, or -1 (an empty path included).  checkCollisionWithRobot is a path of one pose.
+ * Calls read the map only, on the map's stream, are synchronous and are legal between ls_icp_register_submap_batch_begin
+ * and _end; n = 0 (n_paths = 0) is LS_OK without a launch.  keys_visited counts the centres and the voxel states the
+ * passes read (it depends on the scheduling).  Errors, before any result: LS_ERR_ARG for n < 0, a NULL required array, a
+ * size that is negative or not finite (the robot size even when every path is empty), more than 2^17 loop points on an
+ * axis of a box whose centre has a valid key, boxes that span more than 2^36 (box, brick) items in all (per box with a
+ * valid centre, the product over the axes of the 8-voxel bricks its passes touch, whatever the map holds), path offsets
+ * that are not non-decreasing from 0, or more than 2^31 - 1 poses; LS_ERR_NOMEM when the staging cannot grow.  A centre that is NaN or infinite is not refused: it is unknown by step 1. */
+/* getCellStatusBoundingBox per box: centres3 / sizes3 n double triples; status LS_CELL_*.  stats may be NULL. */
+int ls_occupancy_box_status(ls_occupancy* om, const double* centres3, const double* sizes3, int n, int8_t* status,
+                            ls_occupancy_query_stats* stats);
+/* checkPathForCollisionsWithRobot per path: path p is positions3[offsets[p] .. offsets[p+1]); first_collision[p] the
+ * first colliding pose's index within its path, -1 when none.  stats may be NULL. */
+int ls_occupancy_check_paths(ls_occupancy* om, const double* positions3, const int64_t* offsets, int n_paths,
+                             const double robot_size3[3], int unknown_as_occupied, int64_t* first_collision,
+                             ls_occupancy_query_stats* stats);
+
 /* Edits of the map: volumetric_mapping's setFree / setOccupied (OctomapWorld::setLogOddsBoundingBox, the set-box-occupancy
  * service), resetMap, getOccupiedPointcloudInBoundingBox and the extent getMapBounds reads (DESIGN.md §4b'''''''').  Rules:
  *   box loop    per axis in double: c = res * floor(p / res) + res / 2 (a division), then x = (c - s/2) + 0.001; x <=

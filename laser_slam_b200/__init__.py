@@ -272,6 +272,8 @@ def lib():
         L.ls_occupancy_cell_status.argtypes = [vp, vp, ci, vp, vp, QS]
         L.ls_occupancy_line_status.argtypes = [vp, vp, vp, ci, vp, ci, vp, vp, QS]
         L.ls_occupancy_cast_rays.argtypes = [vp, vp, vp, ci, ci, ctypes.c_double, vp, vp, QS]
+        L.ls_occupancy_box_status.argtypes = [vp, vp, vp, ci, vp, QS]
+        L.ls_occupancy_check_paths.argtypes = [vp, vp, vp, ci, vp, ci, vp, QS]
         L.ls_occupancy_set_boxes.argtypes = [vp, vp, vp, vp, ci, ctypes.POINTER(OccupancyEditStats)]
         L.ls_occupancy_clear.argtypes = [vp]
         L.ls_occupancy_box_voxels.argtypes = [vp, vp, vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
@@ -1060,6 +1062,40 @@ class OccupancyMap:
                                                      float(max_range), r.ctypes.data, ends.ctypes.data,
                                                      ctypes.byref(self.last_query)))
         return r[:n].copy(), ends[:n].copy()
+
+    # ---- box status and robot collision (ls_occupancy_box_status / _check_paths); self.last_query holds the stats
+    def box_status(self, centres, sizes):
+        """getCellStatusBoundingBox per box ((n,3) centres and sizes, or (3,) sizes for every box; taken as float64):
+        status int8 CELL_* (DESIGN.md §4b''''''''''')."""
+        c = np.ascontiguousarray(np.asarray(centres, np.float64).reshape(-1, 3))
+        s = np.asarray(sizes, np.float64)
+        s = np.ascontiguousarray(np.broadcast_to(s.reshape(-1, 3) if s.size != 3 else s.reshape(1, 3), c.shape))
+        if len(s) != len(c):
+            raise ValueError(f"{len(c)} centres for {len(s)} sizes")
+        n = len(c)
+        st = np.empty(max(n, 1), np.int8)
+        self.last_query = OccupancyQueryStats()
+        self.ctx._check(lib().ls_occupancy_box_status(self._h, c.ctypes.data, s.ctypes.data, n, st.ctypes.data,
+                                                      ctypes.byref(self.last_query)))
+        return st[:n].copy()
+
+    def check_paths(self, positions, offsets, robot_size, unknown_as_occupied=True):
+        """checkPathForCollisionsWithRobot per path: path p is positions[offsets[p]:offsets[p + 1]] ((m,3), taken as
+        float64; offsets (n_paths + 1,) non-decreasing from 0), the robot a box of robot_size (3,) at each pose.  Returns
+        int64 per path: the first colliding pose's index within the path, -1 when none.  A pose collides when its box is
+        occupied, or, with unknown_as_occupied, when it is not free."""
+        p = np.ascontiguousarray(np.asarray(positions, np.float64).reshape(-1, 3))
+        o = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1))
+        r = np.ascontiguousarray(np.asarray(robot_size, np.float64).reshape(3))
+        n = max(len(o) - 1, 0)
+        if n > 0 and o[-1] != len(p):
+            raise ValueError(f"offsets end at {o[-1]} for {len(p)} positions")
+        first = np.empty(max(n, 1), np.int64)
+        self.last_query = OccupancyQueryStats()
+        self.ctx._check(lib().ls_occupancy_check_paths(self._h, p.ctypes.data if len(p) else None, o.ctypes.data, n,
+                                                       r.ctypes.data, int(bool(unknown_as_occupied)), first.ctypes.data,
+                                                       ctypes.byref(self.last_query)))
+        return first[:n].copy()
 
     # ---- edits (ls_occupancy_set_boxes / _clear / _box_voxels / _bounds)
     def set_boxes(self, centres, sizes, occupied):

@@ -2242,6 +2242,51 @@ int ls_occupancy_cast_rays(ls_occupancy* om, const float* origins3, const float*
   return query_done(om, visited, stats);
 }
 
+int ls_occupancy_box_status(ls_occupancy* om, const double* centres3, const double* sizes3, int n, int8_t* status,
+                            ls_occupancy_query_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (n < 0 || (n > 0 && (!centres3 || !sizes3 || !status))) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (n == 0) return query_none(stats), LS_OK;
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  long long visited = 0;
+  const int rc = lso::box_status(om->map, om->prm, centres3, sizes3, n, status, &visited, om->stream, &ctx->launches);
+  if (rc == LS_ERR_ARG)
+    return fail(ctx, rc, "box status refused: a size is negative or not finite, a box axis has more than 2^17 loop points, "
+                         "or the boxes span more than 2^36 (box, brick) items");
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "box status: out of device memory" : "box status failed");
+  return query_done(om, visited, stats);
+}
+
+int ls_occupancy_check_paths(ls_occupancy* om, const double* positions3, const int64_t* offsets, int n_paths,
+                             const double robot_size3[3], int unknown_as_occupied, int64_t* first_collision,
+                             ls_occupancy_query_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (n_paths < 0 || (n_paths > 0 && (!offsets || !robot_size3 || !first_collision)))
+    return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (n_paths == 0) return query_none(stats), LS_OK;
+  for (int a = 0; a < 3; ++a)  // checked here too, so a call whose paths are all empty refuses a bad size as well
+    if (!std::isfinite(robot_size3[a]) || robot_size3[a] < 0.0)
+      return fail(ctx, LS_ERR_ARG, "robot size %g on axis %d (finite and >= 0)", robot_size3[a], a);
+  if (offsets[0] != 0) return fail(ctx, LS_ERR_ARG, "path offsets start at %lld, not 0", (long long)offsets[0]);
+  for (int p = 0; p < n_paths; ++p)
+    if (offsets[p + 1] < offsets[p]) return fail(ctx, LS_ERR_ARG, "path offsets decrease at path %d", p);
+  if (offsets[n_paths] > 0x7fffffffLL) return fail(ctx, LS_ERR_ARG, "%lld poses (at most 2^31 - 1)", (long long)offsets[n_paths]);
+  if (offsets[n_paths] > 0 && !positions3) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  long long visited = 0;
+  const int rc = lso::check_paths(om->map, om->prm, positions3, offsets, n_paths, robot_size3, unknown_as_occupied,
+                                  first_collision, &visited, om->stream, &ctx->launches);
+  if (rc == LS_ERR_ARG)
+    return fail(ctx, rc, "path check refused: the robot box has more than 2^17 loop points on an axis, or the poses span "
+                         "more than 2^36 (box, brick) items");
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "path check: out of device memory" : "path check failed");
+  return query_done(om, visited, stats);
+}
+
 }  // extern "C"
 
 namespace {

@@ -264,4 +264,18 @@ int diff_changes(Changes& c, const Map& m, const Params& P, uint64_t* keys, int8
 void release_changes(Changes& c);
 size_t changes_bytes(const Changes& c);
 
+// Box status and robot collision (ls_collision.cu; DESIGN.md §4b''''''''''').  Both read the map only, stage in m.qbuf
+// and are synchronous; *visited: the voxel states read.  LS_ERR_ARG, before any result, for a size that is negative or
+// not finite, an axis of more than 2^17 loop points in a box whose centre has a valid key, or boxes spanning more than
+// 2^36 (box, brick) items in all.
+// getCellStatusBoundingBox per box (double triples): LS_CELL_*.  n <= 0 launches nothing.
+int box_status(Map& m, const Params& P, const double* centres3, const double* sizes3, int n, int8_t* status,
+               long long* visited, cudaStream_t st, uint64_t* launches);
+// checkPathForCollisionsWithRobot per path: the robot box robot3 at positions3[offsets[p] ... offsets[p + 1]) (offsets
+// checked by the caller: non-decreasing from 0, at most 2^31 - 1 poses); first[p] the first colliding pose's index
+// within its path, -1 when none.  A pose collides when its status is occupied, or not free with unknown_occ.
+int check_paths(Map& m, const Params& P, const double* positions3, const int64_t* offsets, int n_paths,
+                const double robot3[3], int unknown_occ, int64_t* first, long long* visited, cudaStream_t st,
+                uint64_t* launches);
+
 }  // namespace lso

@@ -271,7 +271,7 @@ class OccupancyMap:
     every track's scans.  Keyword arguments are laser_slam_b200.OccupancyParams' fields.  Close it before the estimator."""
 
     def __init__(self, estimator, resolution=0.075, prob_hit=0.9, prob_miss=0.4, clamp_min=0.12, clamp_max=0.97,
-                 occupancy_threshold=0.7, max_range=20.0, initial_capacity=0):
+                 occupancy_threshold=0.7, max_range=20.0, initial_capacity=0, treat_unknown_as_occupied=True):
         L = lib()
         if not hasattr(L, "_occ_bound"):
             vp, ci, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
@@ -305,8 +305,11 @@ class OccupancyMap:
             L.lsh_occupancy_changed_keys.restype = i64
             L.lsh_occupancy_changed_points.argtypes = [vp, vp, vp, i64]
             L.lsh_occupancy_changed_points.restype = i64
+            L.lsh_occupancy_box_status.argtypes = [vp, vp, vp, ci, ci, vp]
+            L.lsh_occupancy_check_paths.argtypes = [vp, vp, vp, ci, vp, ci, vp]
             L._occ_bound = True
-        prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range], np.float64)
+        prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range,
+                        float(bool(treat_unknown_as_occupied))], np.float64)
         err = ctypes.create_string_buffer(512)
         self._h = L.lsh_occupancy_create(estimator._h, prm.ctypes.data, int(initial_capacity), err, 512)
         if not self._h:
@@ -480,6 +483,28 @@ class OccupancyMap:
         n = self._check(lib().lsh_occupancy_changed_points(self._h, pts.ctypes.data, occ.ctypes.data, int(cap)))
         m = min(n, cap)
         return pts[:m], occ[:m].astype(bool)
+
+    def box_status(self, centres, sizes, single=False):
+        """The batched getCellStatusBoundingBox overload, or with single=True one call per box: int8 CELL_* per box."""
+        c = np.ascontiguousarray(np.asarray(centres, np.float64).reshape(-1, 3))
+        s = np.ascontiguousarray(np.asarray(sizes, np.float64).reshape(-1, 3))
+        st = np.zeros(max(len(c), 1), np.int8)
+        self._check(lib().lsh_occupancy_box_status(self._h, c.ctypes.data, s.ctypes.data, len(c), int(bool(single)),
+                                                   st.ctypes.data))
+        return st[:len(c)]
+
+    def check_paths(self, positions, offsets, robot_size, single=False):
+        """setRobotSize(robot_size), then checkPathsForCollisionsWithRobot, or with single=True one
+        checkPathForCollisionsWithRobot per path: int64 per path, the first colliding pose's index or -1.  The collision
+        mode is the map's treat_unknown_as_occupied."""
+        p = np.ascontiguousarray(np.asarray(positions, np.float64).reshape(-1, 3))
+        o = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1))
+        r = np.ascontiguousarray(np.asarray(robot_size, np.float64).reshape(3))
+        n = max(len(o) - 1, 0)
+        first = np.zeros(max(n, 1), np.int64)
+        self._check(lib().lsh_occupancy_check_paths(self._h, p.ctypes.data, o.ctypes.data, n, r.ctypes.data,
+                                                    int(bool(single)), first.ctypes.data))
+        return first[:n]
 
 
 class DistanceMap:

@@ -379,7 +379,8 @@ int lsh_assembler_add_packet(void* av, const float* pts4, int n, const float* T_
 }
 
 // ---- laser_slam::OccupancyMap (include/laser_slam/occupancy_map.hpp) on an estimator, for the tests.  Destroy it before
-// the estimator.  prm: resolution, hit, miss, clamp min, clamp max, occupancy threshold, max range.
+// the estimator.  prm: resolution, hit, miss, clamp min, clamp max, occupancy threshold, max range, treat unknown as
+// occupied (0 or 1).
 struct OccupancyHandle {
   std::unique_ptr<OccupancyMap> map;
   std::string err;
@@ -396,6 +397,7 @@ void* lsh_occupancy_create(void* hv, const double* prm, int initial_capacity_bri
     p.occupancy_thres = prm[5];
     p.sensor_max_range = prm[6];
     p.initial_capacity_bricks = initial_capacity_bricks;
+    p.treat_unknown_as_occupied = prm[7] != 0.0;
     OccupancyHandle* h = new OccupancyHandle();
     h->map.reset(new OccupancyMap(p, *static_cast<Handle*>(hv)->est));
     return h;
@@ -723,6 +725,60 @@ int64_t lsh_occupancy_changed_points(void* ov, double* pts3, uint8_t* occupied, 
       occupied[i] = s[(size_t)i] ? 1 : 0;
     }
     return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// Box status.  single = 1: getCellStatusBoundingBox once per box, else the batched overload.  0 or LS_ERR_STATE
+int lsh_occupancy_box_status(void* ov, const double* c3, const double* s3, int n, int single, int8_t* status) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<kindr::minimal::Position> c(n), s(n);
+    for (int i = 0; i < n; ++i) c[i] = {c3[3 * i], c3[3 * i + 1], c3[3 * i + 2]}, s[i] = {s3[3 * i], s3[3 * i + 1], s3[3 * i + 2]};
+    if (single) {
+      for (int i = 0; i < n; ++i) status[i] = (int8_t)h->map->getCellStatusBoundingBox(c[i], s[i]);
+      return 0;
+    }
+    std::vector<OccupancyMap::CellStatus> st;
+    h->map->getCellStatusBoundingBox(c, s, &st);
+    for (int i = 0; i < n; ++i) status[i] = (int8_t)st[(size_t)i];
+    return 0;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// Robot collision after setRobotSize(robot3) (getRobotSize must return it).  single = 1: checkPathForCollisionsWithRobot
+// per path (first[p] its collision_index, -1 when false; a path of one pose also through checkCollisionWithRobot, which
+// must agree); single = 0: checkPathsForCollisionsWithRobot.  0 or LS_ERR_STATE
+int lsh_occupancy_check_paths(void* ov, const double* p3, const int64_t* offsets, int n_paths, const double* robot3,
+                              int single, int64_t* first) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    const kindr::minimal::Position r{robot3[0], robot3[1], robot3[2]};
+    h->map->setRobotSize(r);
+    const kindr::minimal::Position got = h->map->getRobotSize();
+    if (!(got[0] == r[0] && got[1] == r[1] && got[2] == r[2])) throw std::runtime_error("getRobotSize differs");
+    std::vector<std::vector<kindr::minimal::Position> > paths((size_t)n_paths);
+    for (int p = 0; p < n_paths; ++p)
+      for (int64_t i = offsets[p]; i < offsets[p + 1]; ++i) paths[(size_t)p].push_back({p3[3 * i], p3[3 * i + 1], p3[3 * i + 2]});
+    if (single) {
+      for (int p = 0; p < n_paths; ++p) {
+        size_t idx = 0;
+        const bool hit = h->map->checkPathForCollisionsWithRobot(paths[(size_t)p], &idx);
+        first[p] = hit ? (int64_t)idx : -1;
+        if (paths[(size_t)p].size() == 1 && h->map->checkCollisionWithRobot(paths[(size_t)p][0]) != hit)
+          throw std::runtime_error("checkCollisionWithRobot and checkPathForCollisionsWithRobot disagree");
+      }
+      return 0;
+    }
+    std::vector<int64_t> f;
+    h->map->checkPathsForCollisionsWithRobot(paths, &f);
+    for (int p = 0; p < n_paths; ++p) first[p] = f[(size_t)p];
+    return 0;
   } catch (const std::exception& e) {
     h->err = e.what();
     return LS_ERR_STATE;

@@ -263,6 +263,75 @@ void OccupancyMap::castRays(const std::vector<kindr::minimal::Position>& origins
   }
 }
 
+// ---- box status and robot collision --------------------------------------------------------------------------------
+OccupancyMap::CellStatus OccupancyMap::getCellStatusBoundingBox(const kindr::minimal::Position& point,
+                                                                const kindr::minimal::Position& bounding_box_size) const {
+  std::vector<CellStatus> st;
+  getCellStatusBoundingBox(std::vector<kindr::minimal::Position>{point}, std::vector<kindr::minimal::Position>{bounding_box_size},
+                           &st);
+  return st[0];
+}
+
+void OccupancyMap::getCellStatusBoundingBox(const std::vector<kindr::minimal::Position>& points,
+                                            const std::vector<kindr::minimal::Position>& bounding_box_sizes,
+                                            std::vector<CellStatus>* statuses) const {
+  if (statuses == NULL) throw std::invalid_argument("null output");
+  if (points.size() != bounding_box_sizes.size()) throw std::invalid_argument("points and sizes differ in length");
+  const size_t n = points.size();
+  std::vector<double> c(3 * n), s(3 * n);
+  for (size_t i = 0; i < n; ++i)
+    for (int a = 0; a < 3; ++a) c[3 * i + a] = points[i][a], s[3 * i + a] = bounding_box_sizes[i][a];
+  std::vector<int8_t> st(n > 0 ? n : 1);
+  {
+    std::lock_guard<std::mutex> lock(mutex_);
+    throwOnError(ctx_, ls_occupancy_box_status(map_, c.data(), s.data(), (int)n, st.data(), NULL), "ls_occupancy_box_status");
+  }
+  statuses->resize(n);
+  for (size_t i = 0; i < n; ++i) (*statuses)[i] = static_cast<CellStatus>(st[i]);
+}
+
+void OccupancyMap::setRobotSize(const kindr::minimal::Position& robot_size) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  robot_size_ = robot_size;
+}
+
+kindr::minimal::Position OccupancyMap::getRobotSize() const {
+  std::lock_guard<std::mutex> lock(mutex_);
+  return robot_size_;
+}
+
+bool OccupancyMap::checkCollisionWithRobot(const kindr::minimal::Position& robot_position) const {
+  return checkPathForCollisionsWithRobot(std::vector<kindr::minimal::Position>{robot_position}, NULL);
+}
+
+bool OccupancyMap::checkPathForCollisionsWithRobot(const std::vector<kindr::minimal::Position>& robot_positions,
+                                                   size_t* collision_index) const {
+  std::vector<int64_t> first;
+  checkPathsForCollisionsWithRobot(std::vector<std::vector<kindr::minimal::Position> >{robot_positions}, &first);
+  if (first[0] < 0) return false;
+  if (collision_index) *collision_index = (size_t)first[0];
+  return true;
+}
+
+void OccupancyMap::checkPathsForCollisionsWithRobot(const std::vector<std::vector<kindr::minimal::Position> >& paths,
+                                                    std::vector<int64_t>* first_collisions) const {
+  if (first_collisions == NULL) throw std::invalid_argument("null output");
+  std::vector<int64_t> offsets(1, 0);
+  std::vector<double> pos;
+  for (const auto& path : paths) {
+    for (const auto& p : path)
+      for (int a = 0; a < 3; ++a) pos.push_back(p[a]);
+    offsets.push_back(offsets.back() + (int64_t)path.size());
+  }
+  first_collisions->assign(paths.size(), -1);
+  std::lock_guard<std::mutex> lock(mutex_);
+  throwOnError(ctx_,
+               ls_occupancy_check_paths(map_, pos.empty() ? NULL : pos.data(), offsets.data(), (int)paths.size(),
+                                        robot_size_.data(), params_.treat_unknown_as_occupied ? 1 : 0,
+                                        first_collisions->empty() ? NULL : first_collisions->data(), NULL),
+               "ls_occupancy_check_paths");
+}
+
 // ---- edits ---------------------------------------------------------------------------------------------------------
 void OccupancyMap::setFree(const kindr::minimal::Position& position, const kindr::minimal::Position& bounding_box_size) {
   setBoxes({position}, {bounding_box_size}, {false});

@@ -128,6 +128,18 @@ om.set_boxes([bc[0]], [(2.0, 2.0, 2.0)], [True])
 cg = om.changes(reset=True)
 cw = ocr.diff_arrays(*ck0, *om.download(ls.OCC_KNOWN)[:2], oc.logodds(0.7))
 assert len(cg[0]) > 0 and all(np.array_equal(x, y) for x, y in zip(cg[:3], cw))
+# box status and robot collision of that map (ls_collision.cu): one box call and one path call, each in both modes,
+# against the restatement
+import occupancy_collision_ref as ocl
+xk, xv, _ = om.download(ls.OCC_KNOWN)
+xvox = ocl.as_dict(xk, xv)
+xc = truth[0][:3, 3] + rng.uniform(-4.0, 4.0, (64, 3))
+for xs in ((1.0, 1.0, 0.5), (0.0, 0.6, 0.3)):
+    assert om.box_status(xc, xs).tolist() == [ocl.box_status(xvox, c, xs, 0.2, oc.logodds(0.7)) for c in xc]
+xo = np.array([0, 10, 10, 40, 64], np.int64)
+for unknown in (True, False):
+    xw = ocl.check_paths(xvox, xc, xo, (1.0, 1.0, 0.5), 0.2, oc.logodds(0.7), unknown)
+    assert np.array_equal(om.check_paths(xc, xo, (1.0, 1.0, 0.5), unknown), xw)
 om.clear()
 assert om.size(ls.OCC_KNOWN) == 0
 om.close()
