@@ -1733,49 +1733,50 @@ struct ls_occupancy {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   lso::Map map;
-  lso::Octree tree;
-  bool tree_current = false;  // the last octree build reflects every insert
-  float tree_ms = 0.f;
-  lso::Octree full;           // the full tree (.ot), cached apart from the .bt build
-  bool full_current = false;
-  float full_ms = 0.f;
+  // The last build of each tree format (indexed by lso::TreeFormat), cached apart; current while it reflects every change
+  // to the map.
+  struct Tree {
+    lso::Octree tree;
+    bool current = false;
+    float ms = 0.f;
+  } trees[2];
   lso::Changes changes;  // change detection's baseline and scratch (ls_changes.cu)
   bool tracking = false;
 };
 
 namespace {
-int build_tree(ls_occupancy* om) {
-  ls_ctx* ctx = om->ctx;
-  om->tree_current = false;
-  CU(cudaEventRecord(om->ev0, om->stream));
-  const int rc = lso::build_octree(om->map, om->prm, om->tree, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "octree export: out of device memory" : "octree export failed");
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
-  CU(cudaEventElapsedTime(&om->tree_ms, om->ev0, om->ev1));
-  om->tree_current = true;
-  return LS_OK;
+using lso::TreeFormat;
+
+ls_occupancy::Tree& tree_of(ls_occupancy* om, TreeFormat f) { return om->trees[(int)f]; }
+
+void trees_stale(ls_occupancy* om) {
+  for (ls_occupancy::Tree& t : om->trees) t.current = false;
 }
 
-int build_full(ls_occupancy* om) {
+// The error texts' name of a format: "octree" or "full octree".
+const char* tree_name(TreeFormat f) { return f == TreeFormat::Full ? "full octree" : "octree"; }
+
+int build_tree(ls_occupancy* om, TreeFormat f) {
   ls_ctx* ctx = om->ctx;
-  om->full_current = false;
+  ls_occupancy::Tree& t = tree_of(om, f);
+  t.current = false;
   CU(cudaEventRecord(om->ev0, om->stream));
-  const int rc = lso::build_full_octree(om->map, om->full, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "full octree export: out of device memory" : "full octree export failed");
+  const int rc = lso::build_tree(om->map, om->prm, f, t.tree, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "%s export: out of device memory" : "%s export failed", tree_name(f));
   CU(cudaEventRecord(om->ev1, om->stream));
   CU(cudaEventSynchronize(om->ev1));
-  CU(cudaEventElapsedTime(&om->full_ms, om->ev0, om->ev1));
-  om->full_current = true;
+  CU(cudaEventElapsedTime(&t.ms, om->ev0, om->ev1));
+  t.current = true;
   return LS_OK;
 }
 
 void full_stats(const ls_occupancy* om, ls_full_octree_stats* stats) {
   if (!stats) return;
-  stats->nodes = om->full.nodes;
-  stats->leaves = om->full.leaves;
-  stats->payload_bytes = om->full.bytes;
-  stats->device_ms = om->full_ms;
+  const ls_occupancy::Tree& t = om->trees[(int)TreeFormat::Full];
+  stats->nodes = t.tree.nodes;
+  stats->leaves = t.tree.leaves;
+  stats->payload_bytes = t.tree.bytes;
+  stats->device_ms = t.ms;
 }
 
 // The file at `path`, whole.  NULL on success, else why not.
@@ -1792,10 +1793,11 @@ const char* read_file(const char* path, std::vector<uint8_t>* data) {
 
 void octree_stats(const ls_occupancy* om, ls_octree_stats* stats) {
   if (!stats) return;
-  stats->nodes = om->tree.nodes;
-  stats->payload_bytes = om->tree.bytes;
-  stats->occupied_leaves = om->tree.leaves;
-  stats->device_ms = om->tree_ms;
+  const ls_occupancy::Tree& t = om->trees[(int)TreeFormat::Binary];
+  stats->nodes = t.tree.nodes;
+  stats->payload_bytes = t.tree.bytes;
+  stats->occupied_leaves = t.tree.leaves;
+  stats->device_ms = t.ms;
 }
 
 // A .bt header (with `full`, a .ot header) as laser_slam_b200.read_octomap (read_octomap_full) parses it: the first line
@@ -1844,6 +1846,98 @@ const char* parse_bt_header(const std::vector<uint8_t>& d, size_t* off, long lon
   if (n < 0) return "negative size";
   *off = pos, *nodes = n, *res = r;
   return nullptr;
+}
+int download_tree(ls_occupancy* om, TreeFormat f, uint8_t* payload, int64_t payload_cap, float* centres4, uint8_t* depths,
+                  int64_t leaf_cap) {
+  ls_ctx* ctx = om->ctx;
+  if (!tree_of(om, f).current)
+    return fail(ctx, LS_ERR_STATE, f == TreeFormat::Full ? "no current full octree: build it after the last insert or read"
+                                                         : "no current octree: build it after the last insert");
+  const lso::Octree& t = tree_of(om, f).tree;
+  if ((t.bytes > 0 && !payload) || payload_cap < t.bytes)
+    return fail(ctx, LS_ERR_ARG, "a payload buffer of %lld bytes for %lld", (long long)payload_cap, t.bytes);
+  if ((centres4 || depths) && leaf_cap < t.leaves)
+    return fail(ctx, LS_ERR_ARG, "leaf buffers of %lld for %lld occupied leaves", (long long)leaf_cap, t.leaves);
+  CU(cudaSetDevice(ctx->device));
+  const int rc = lso::download_octree(t, payload, centres4, depths, om->stream);
+  if (rc) return fail(ctx, rc, "%s download failed", tree_name(f));
+  return LS_OK;
+}
+
+// octomap's writeBinaryConst (.bt) or AbstractOcTree::write (.ot): the header, then the payload of the current build
+int write_tree(ls_occupancy* om, TreeFormat f, const char* path) {
+  ls_ctx* ctx = om->ctx;
+  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
+  CU(cudaSetDevice(ctx->device));
+  ls_occupancy::Tree& t = tree_of(om, f);
+  int rc;
+  if (!t.current && (rc = build_tree(om, f))) return rc;
+  std::vector<uint8_t> payload((size_t)t.tree.bytes);
+  if ((rc = lso::download_octree(t.tree, payload.data(), nullptr, nullptr, om->stream)))
+    return fail(ctx, rc, "%s download failed", tree_name(f));
+  // the resolution as a default std::ostream prints a double (%g)
+  char head[256];
+  const int n = std::snprintf(head, sizeof head,
+                              "%s\n# (feel free to add / change comments, but leave the first line as it is!)\n#\nid OcTree\n"
+                              "size %lld\nres %g\ndata\n",
+                              f == TreeFormat::Full ? "# Octomap OcTree file" : "# Octomap OcTree binary file", t.tree.nodes,
+                              om->prm.res);
+  FILE* file = std::fopen(path, "wb");
+  if (!file) return fail(ctx, LS_ERR_ARG, "cannot open %s for writing", path);
+  bool ok = std::fwrite(head, 1, (size_t)n, file) == (size_t)n;
+  if (ok && !payload.empty()) ok = std::fwrite(payload.data(), 1, payload.size(), file) == payload.size();
+  ok = std::fclose(file) == 0 && ok;
+  if (!ok) return fail(ctx, LS_ERR_ARG, "writing %s failed", path);
+  return LS_OK;
+}
+
+int read_tree(ls_occupancy* om, TreeFormat f, const uint8_t* payload, int64_t payload_bytes, int64_t nodes, double resolution,
+              ls_octomap_read_stats* stats) {
+  ls_ctx* ctx = om->ctx;
+  if (nodes < 0 || payload_bytes < 0 || (payload_bytes > 0 && !payload)) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!(resolution > 0.0) || !std::isfinite(resolution))
+    return fail(ctx, LS_ERR_ARG, "octomap resolution %g (finite and > 0)", resolution);
+  CU(cudaSetDevice(ctx->device));
+  CU(cudaEventRecord(om->ev0, om->stream));
+  lso::Params P = om->prm;
+  P.res = resolution;
+  P.inv = 1.0 / resolution;
+  lso::ReadCounters c;
+  const char* why = "";
+  const int rc = lso::read_tree(om->map, P, f, payload, payload_bytes, nodes, &c, &why, om->stream, &ctx->launches);
+  if (rc)
+    return fail(ctx, rc, "octomap %sread refused, the map is unchanged: %s", f == TreeFormat::Full ? "full tree " : "", why);
+  om->prm = P;
+  trees_stale(om);
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    stats->nodes = (int64_t)c.nodes;
+    stats->inner_nodes = (int64_t)c.inner;
+    stats->free_leaves = (int64_t)c.free_leaves;
+    stats->occupied_leaves = (int64_t)c.occ_leaves;
+    stats->known_voxels = om->map.n_known;
+    stats->bricks = om->map.pool_n;
+    stats->resolution = P.res;
+    stats->device_ms = ms;
+  }
+  return LS_OK;
+}
+
+int read_tree_file(ls_occupancy* om, TreeFormat f, const char* path, ls_octomap_read_stats* stats) {
+  ls_ctx* ctx = om->ctx;
+  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
+  std::vector<uint8_t> data;
+  const char* why = read_file(path, &data);
+  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
+  size_t off = 0;
+  long long nodes = 0;
+  double res = 0.0;
+  why = parse_bt_header(data, &off, &nodes, &res, f == TreeFormat::Full);
+  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
+  return read_tree(om, f, data.data() + off, (int64_t)(data.size() - off), nodes, res, stats);
 }
 }  // namespace
 
@@ -1915,8 +2009,7 @@ int ls_occupancy_insert_scan(ls_occupancy* om, const ls_map* ring, uint64_t scan
   if (!s) return fail(ctx, LS_ERR_STATE, "scan %llu is not resident (evicted or never pushed)", (unsigned long long)scan_id);
   if (wait_slot(s, om->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
   CU(cudaEventRecord(om->ev0, om->stream));
-  om->tree_current = false;
-  om->full_current = false;
+  trees_stale(om);
   lso::Counters c;
   const int rc = lso::insert(om->map, om->prm, s->pts.get(), s->n, T_w_scan, is_identity16(T_w_scan), om->stream, &c,
                              &ctx->launches);
@@ -1970,203 +2063,65 @@ int ls_occupancy_build_octree(ls_occupancy* om, ls_octree_stats* stats) {
   if (!om) return LS_ERR_ARG;
   ls_ctx* ctx = om->ctx;
   CU(cudaSetDevice(ctx->device));
-  const int rc = build_tree(om);
-  if (rc) return rc;
-  octree_stats(om, stats);
-  return LS_OK;
+  const int rc = build_tree(om, TreeFormat::Binary);
+  if (!rc) octree_stats(om, stats);
+  return rc;
 }
 
 int ls_occupancy_download_octree(ls_occupancy* om, uint8_t* payload, int64_t payload_cap, float* centres4, uint8_t* depths,
                                  int64_t leaf_cap) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (!om->tree_current) return fail(ctx, LS_ERR_STATE, "no current octree: build it after the last insert");
-  const lso::Octree& t = om->tree;
-  if ((t.bytes > 0 && !payload) || payload_cap < t.bytes)
-    return fail(ctx, LS_ERR_ARG, "a payload buffer of %lld bytes for %lld", (long long)payload_cap, t.bytes);
-  if ((centres4 || depths) && leaf_cap < t.leaves)
-    return fail(ctx, LS_ERR_ARG, "leaf buffers of %lld for %lld occupied leaves", (long long)leaf_cap, t.leaves);
-  CU(cudaSetDevice(ctx->device));
-  const int rc = lso::download_octree(t, payload, centres4, depths, om->stream);
-  if (rc) return fail(ctx, rc, "octree download failed");
-  return LS_OK;
+  return download_tree(om, TreeFormat::Binary, payload, payload_cap, centres4, depths, leaf_cap);
 }
 
 int ls_occupancy_write_octomap(ls_occupancy* om, const char* path, ls_octree_stats* stats) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
-  CU(cudaSetDevice(ctx->device));
-  int rc;
-  if (!om->tree_current && (rc = build_tree(om))) return rc;
-  std::vector<uint8_t> payload((size_t)om->tree.bytes);
-  if ((rc = lso::download_octree(om->tree, payload.data(), nullptr, nullptr, om->stream)))
-    return fail(ctx, rc, "octree download failed");
-  // octomap's writeBinaryConst: the resolution as a default std::ostream prints a double (%g)
-  char head[256];
-  const int n = std::snprintf(head, sizeof head,
-                              "# Octomap OcTree binary file\n# (feel free to add / change comments, but leave the first line "
-                              "as it is!)\n#\nid OcTree\nsize %lld\nres %g\ndata\n",
-                              om->tree.nodes, om->prm.res);
-  FILE* f = std::fopen(path, "wb");
-  if (!f) return fail(ctx, LS_ERR_ARG, "cannot open %s for writing", path);
-  bool ok = std::fwrite(head, 1, (size_t)n, f) == (size_t)n;
-  if (ok && !payload.empty()) ok = std::fwrite(payload.data(), 1, payload.size(), f) == payload.size();
-  ok = std::fclose(f) == 0 && ok;
-  if (!ok) return fail(ctx, LS_ERR_ARG, "writing %s failed", path);
-  octree_stats(om, stats);
-  return LS_OK;
+  const int rc = write_tree(om, TreeFormat::Binary, path);
+  if (!rc) octree_stats(om, stats);
+  return rc;
 }
 
 int ls_occupancy_read_octree(ls_occupancy* om, const uint8_t* payload, int64_t payload_bytes, int64_t nodes,
                              double resolution, ls_octomap_read_stats* stats) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (nodes < 0 || payload_bytes < 0 || (payload_bytes > 0 && !payload)) return fail(ctx, LS_ERR_ARG, "bad argument");
-  if (!(resolution > 0.0) || !std::isfinite(resolution))
-    return fail(ctx, LS_ERR_ARG, "octomap resolution %g (finite and > 0)", resolution);
-  CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
-  lso::Params P = om->prm;
-  P.res = resolution;
-  P.inv = 1.0 / resolution;
-  lso::ReadCounters c;
-  const char* why = "";
-  const int rc = lso::read_octree(om->map, P, payload, payload_bytes, nodes, &c, &why, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, "octomap read refused, the map is unchanged: %s", why);
-  om->prm = P;
-  om->tree_current = false;
-  om->full_current = false;
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
-  if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
-    stats->nodes = (int64_t)c.nodes;
-    stats->inner_nodes = (int64_t)c.inner;
-    stats->free_leaves = (int64_t)c.free_leaves;
-    stats->occupied_leaves = (int64_t)c.occ_leaves;
-    stats->known_voxels = om->map.n_known;
-    stats->bricks = om->map.pool_n;
-    stats->resolution = P.res;
-    stats->device_ms = ms;
-  }
-  return LS_OK;
+  return read_tree(om, TreeFormat::Binary, payload, payload_bytes, nodes, resolution, stats);
 }
 
 int ls_occupancy_read_octomap(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
-  std::vector<uint8_t> data;
-  const char* why = read_file(path, &data);
-  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
-  size_t off = 0;
-  long long nodes = 0;
-  double res = 0.0;
-  why = parse_bt_header(data, &off, &nodes, &res);
-  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
-  return ls_occupancy_read_octree(om, data.data() + off, (int64_t)(data.size() - off), nodes, res, stats);
+  return read_tree_file(om, TreeFormat::Binary, path, stats);
 }
 
 int ls_occupancy_build_full_octree(ls_occupancy* om, ls_full_octree_stats* stats) {
   if (!om) return LS_ERR_ARG;
   ls_ctx* ctx = om->ctx;
   CU(cudaSetDevice(ctx->device));
-  const int rc = build_full(om);
-  if (rc) return rc;
-  full_stats(om, stats);
-  return LS_OK;
+  const int rc = build_tree(om, TreeFormat::Full);
+  if (!rc) full_stats(om, stats);
+  return rc;
 }
 
 int ls_occupancy_download_full_octree(ls_occupancy* om, uint8_t* payload, int64_t payload_cap) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (!om->full_current) return fail(ctx, LS_ERR_STATE, "no current full octree: build it after the last insert or read");
-  const lso::Octree& t = om->full;
-  if ((t.bytes > 0 && !payload) || payload_cap < t.bytes)
-    return fail(ctx, LS_ERR_ARG, "a payload buffer of %lld bytes for %lld", (long long)payload_cap, t.bytes);
-  CU(cudaSetDevice(ctx->device));
-  const int rc = lso::download_octree(t, payload, nullptr, nullptr, om->stream);
-  if (rc) return fail(ctx, rc, "full octree download failed");
-  return LS_OK;
+  return download_tree(om, TreeFormat::Full, payload, payload_cap, nullptr, nullptr, 0);
 }
 
 int ls_occupancy_write_octomap_full(ls_occupancy* om, const char* path, ls_full_octree_stats* stats) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
-  CU(cudaSetDevice(ctx->device));
-  int rc;
-  if (!om->full_current && (rc = build_full(om))) return rc;
-  std::vector<uint8_t> payload((size_t)om->full.bytes);
-  if ((rc = lso::download_octree(om->full, payload.data(), nullptr, nullptr, om->stream)))
-    return fail(ctx, rc, "full octree download failed");
-  // octomap's AbstractOcTree::write: the resolution as a default std::ostream prints a double (%g)
-  char head[256];
-  const int n = std::snprintf(head, sizeof head,
-                              "# Octomap OcTree file\n# (feel free to add / change comments, but leave the first line as it "
-                              "is!)\n#\nid OcTree\nsize %lld\nres %g\ndata\n",
-                              om->full.nodes, om->prm.res);
-  FILE* f = std::fopen(path, "wb");
-  if (!f) return fail(ctx, LS_ERR_ARG, "cannot open %s for writing", path);
-  bool ok = std::fwrite(head, 1, (size_t)n, f) == (size_t)n;
-  if (ok && !payload.empty()) ok = std::fwrite(payload.data(), 1, payload.size(), f) == payload.size();
-  ok = std::fclose(f) == 0 && ok;
-  if (!ok) return fail(ctx, LS_ERR_ARG, "writing %s failed", path);
-  full_stats(om, stats);
-  return LS_OK;
+  const int rc = write_tree(om, TreeFormat::Full, path);
+  if (!rc) full_stats(om, stats);
+  return rc;
 }
 
 int ls_occupancy_read_full_octree(ls_occupancy* om, const uint8_t* payload, int64_t payload_bytes, int64_t nodes,
                                   double resolution, ls_octomap_read_stats* stats) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (nodes < 0 || payload_bytes < 0 || (payload_bytes > 0 && !payload)) return fail(ctx, LS_ERR_ARG, "bad argument");
-  if (!(resolution > 0.0) || !std::isfinite(resolution))
-    return fail(ctx, LS_ERR_ARG, "octomap resolution %g (finite and > 0)", resolution);
-  CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
-  lso::Params P = om->prm;
-  P.res = resolution;
-  P.inv = 1.0 / resolution;
-  lso::ReadCounters c;
-  const char* why = "";
-  const int rc = lso::read_full_octree(om->map, P, payload, payload_bytes, nodes, &c, &why, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, "octomap full tree read refused, the map is unchanged: %s", why);
-  om->prm = P;
-  om->tree_current = false;
-  om->full_current = false;
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
-  if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
-    stats->nodes = (int64_t)c.nodes;
-    stats->inner_nodes = (int64_t)c.inner;
-    stats->free_leaves = (int64_t)c.free_leaves;
-    stats->occupied_leaves = (int64_t)c.occ_leaves;
-    stats->known_voxels = om->map.n_known;
-    stats->bricks = om->map.pool_n;
-    stats->resolution = P.res;
-    stats->device_ms = ms;
-  }
-  return LS_OK;
+  return read_tree(om, TreeFormat::Full, payload, payload_bytes, nodes, resolution, stats);
 }
 
 int ls_occupancy_read_octomap_full(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats) {
   if (!om) return LS_ERR_ARG;
-  ls_ctx* ctx = om->ctx;
-  if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
-  std::vector<uint8_t> data;
-  const char* why = read_file(path, &data);
-  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
-  size_t off = 0;
-  long long nodes = 0;
-  double res = 0.0;
-  why = parse_bt_header(data, &off, &nodes, &res, true);
-  if (why) return fail(ctx, LS_ERR_ARG, "%s: %s", path, why);
-  return ls_occupancy_read_full_octree(om, data.data() + off, (int64_t)(data.size() - off), nodes, res, stats);
+  return read_tree_file(om, TreeFormat::Full, path, stats);
 }
 
 }  // extern "C"
@@ -2318,7 +2273,7 @@ int ls_occupancy_set_boxes(ls_occupancy* om, const double* centres3, const doubl
   const int rc = lso::set_boxes(om->map, om->prm, centres3, sizes3, occupied, n, &set, &added, &why, om->stream,
                                 &ctx->launches);
   if (rc) return fail(ctx, rc, "set boxes refused, the map's voxels are unchanged: %s", why);
-  if (set > 0) om->tree_current = om->full_current = false;
+  if (set > 0) trees_stale(om);
   CU(cudaEventRecord(om->ev1, om->stream));
   CU(cudaEventSynchronize(om->ev1));
   if (stats) {
@@ -2339,7 +2294,7 @@ int ls_occupancy_clear(ls_occupancy* om) {
   ls_ctx* ctx = om->ctx;
   CU(cudaSetDevice(ctx->device));
   const int rc = lso::clear(om->map, om->stream);
-  om->tree_current = om->full_current = false;
+  trees_stale(om);
   if (rc) return fail(ctx, rc, "occupancy map reset failed");
   return LS_OK;
 }

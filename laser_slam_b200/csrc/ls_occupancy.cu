@@ -11,41 +11,38 @@
 // Log-odds change only in (c).  When the pool or the hash overflows in (b) the host clears every mark, grows what filled
 // and runs (b) again, so a failed insert leaves the known voxels and their values as they were.
 //
-// Octree export (octomap's writeBinary after toMaxLikelihood and prune; rules in oracle/OCTREE.md), reading the map only:
+// Octree export and read, one pipeline each over a format trait (BinaryTree: octomap's writeBinary / readBinary after
+// toMaxLikelihood and prune, the .bt payload, rules in oracle/OCTREE.md; FullTree: OcTree::write / readData, the .ot
+// payload with every node's float value, DESIGN.md §4b''''''').  Each kernel below is a template over the format, which
+// supplies the node record, the merge of 8 children and its subtree totals, a brick's levels, and which nodes the stream
+// holds.
+// Export, reading the map only:
 //   (d) oct_code_kernel      Morton code of each brick key; a CUB radix sort puts the bricks in pre-order at depth 13
-//   (e) oct_brick_kernel     one block per brick: max-likelihood states of its 512 voxels, levels 15, 14 and 13 pruned in
-//                            shared memory, the brick's state and subtree totals (nodes, payload bytes, occupied leaves)
+//   (e) oct_brick_kernel     one block per brick: its 512 voxels merged in shared memory through levels 15, 14 and 13
+//                            (the format's levels), the brick's state, value and subtree totals
 //   (f) oct_up_kernel        one block: levels 12 ... 0, each level's sorted list segmented by code >> 3 with a block scan,
-//                            collapse or inner per parent (the root never collapses), subtree totals summed
-//   the three totals of the root come back once and size the outputs
-//   (g) oct_down_kernel      one block: levels 0 ... 12, each inner node's two bytes, its children's offsets (its own + 2 +
-//                            the earlier siblings' totals) and the centres of occupied leaves above the bricks
-//   (h) oct_emit_kernel      one block per inner brick: (e)'s tree again, its pre-order bytes and occupied leaves written at
-//                            the offsets (g) gave it, so no per-brick staging is kept
+//                            the format's merge per parent (the root never collapses), subtree totals summed
+//   the root's totals come back once and size the outputs
+//   (g) oct_down_kernel      one block: levels 0 ... 12, each inner node's record and its children's offsets (its own +
+//                            its record + the earlier siblings' totals); .bt writes occupied leaves' centres, .ot leaf nodes
+//   (h) oct_emit_kernel      one block per inner brick: (e)'s levels again, its nodes below depth 13 written at the offset
+//                            (g) gave it, so no per-brick staging is kept; one specialisation per format
 // A brick without a known voxel (an insert that failed after placing it leaves one) has state 0 and adds nothing.
 //
-// .bt read (octomap's readBinary; DESIGN.md §4b''''''), replacing the map.  The payload is uploaded once and
-// parsed without a walk, one thread per pair (= inner node):
-//   (r1) rd_excess_kernel + a CUB scan   the excess E_i of each pair: inner nodes found but not yet read
+// Read (DESIGN.md §4b''''''), replacing the map.  The payload is uploaded once and parsed without a walk, one thread per
+// stream record (.bt: inner nodes only; .ot: every node):
+//   (r1) rd_excess_kernel + a CUB scan   the excess E_i of each record: stream nodes found but not yet read
 //   (r2) rd_end_kernel                   the tree's end (the first E_i = 0) and each block's least excess
-//   (r3) rd_parent_kernel                each inner node's parent (the last earlier pair with E <= its own) and slot
-//   (r4) rd_node_kernel                  depth and first key (at most 15 parents up), the depth-13 ancestor, and the
-//                                        counts: nodes, leaves, known voxels and bricks; a CUB scan gives each inner node
-//                                        its first brick, so the bricks are numbered in pre-order with no deduplication
+//   (r3) rd_parent_kernel                each node's parent (the last earlier record with E <= its own) and slot
+//   (r4) rd_node_kernel                  depth and first key (at most 15 / 16 parents up), the depth-13 ancestor, the
+//                                        format's checks and counts: nodes, leaves, known voxels and bricks; a CUB scan
+//                                        gives each node its first brick, so the bricks are numbered in pre-order with
+//                                        no deduplication
 //   one readback validates the stream, checks the size line and the brick bound, and sizes the pool
-//   (r5) rd_brick_kernel                 each new brick's key and state (uniform free / occupied, or mixed)
-//   the hash is built from those keys beside the old one, so a failure up to here leaves the map as it was
+//   (r5) rd_brick_kernel                 each new brick's key and state (uniform, or mixed)
+//   the hash is built from those keys beside the old one (replace_map), so a failure up to here leaves the map as it was
 //   (r6) rd_fill_kernel                  one block per brick: uniform bricks written whole, mixed ones cleared
 //   (r7) rd_leaf_kernel                  the voxels of each leaf at depth 14 ... 16, each written once
-//
-// Full tree export (octomap's OcTree::write, the .ot payload; DESIGN.md §4b'), reading the map only: (d) and its
-// sort, then (e') ful_brick_kernel, (f') ful_up_kernel, (g') ful_down_kernel and (h') ful_emit_kernel as (e) ... (h) with
-// every node's float value in place of its state (value-equality pruning, inner nodes holding their largest child) and
-// 5 payload bytes per node; (h') places a brick's up to 585 nodes in parallel with a block scan.
-// Full tree read (octomap's readData; DESIGN.md §4b'), replacing the map: (s1) fr_excess_kernel over every node
-// (c_i = the popcount of its child mask), (r2), (s3) fr_parent_kernel, (s4) fr_node_kernel (depth up to 16, the leaf
-// checks and counts), one readback, then the tail the .bt read shares (replace_map) with (s5) fr_brick_kernel, (s6)
-// fr_fill_kernel and (s7) fr_leaf_kernel writing each leaf's own value.
 #include <algorithm>
 #include <cfloat>
 #include <climits>
@@ -631,11 +628,11 @@ __global__ void occ_ray_kernel(const float* __restrict__ o3, const float* __rest
   add_visited(cnt, visited);
 }
 
-// ---- octree export ---------------------------------------------------------------------------------------------------
+// ---- octree export and read ------------------------------------------------------------------------------------------
 constexpr int kTreeThreads = 1024;  // (f) and (g)
 constexpr int kBrickDepth = 13;
 
-// Node states: 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner -- also the bit pair of the payload.
+// .bt node states: 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner -- also the bit pair of the payload.
 // octomap's isNodeCollapsible after toMaxLikelihood: all 8 children exist, are leaves and have one state.
 __device__ __forceinline__ int parent_state(int n_free, int n_occ, int n_any, bool may_prune) {
   if (may_prune && n_free == 8) return 1;
@@ -682,70 +679,409 @@ __device__ __forceinline__ void put_leaf(float4* cen, unsigned char* dep, unsign
   dep[i] = (unsigned char)depth;
 }
 
-struct BrickTree {
-  unsigned char s16[512], s15[64], s14[8];
-  int n15[64], l15[64], n14[8], l14[8], b14[8];
-  int st, nodes, bytes, leaves;  // the depth-13 node
-};
-
-// One block of 512 threads: thread t reads the voxel of Morton index t, then the brick's levels 15, 14 and 13.
-__device__ void brick_tree(const unsigned* __restrict__ known, const float* __restrict__ lo, int b, float l_occ, BrickTree& T) {
-  const int t = threadIdx.x;
-  const int v = morton_local(t);
-  int s = 0;
-  if ((known[(size_t)b * 16 + (v >> 5)] >> (v & 31)) & 1u) s = lo[(size_t)b * 512 + v] >= l_occ ? 2 : 1;
-  T.s16[t] = (unsigned char)s;
-  __syncthreads();
-  if (t < 64) {
-    int nf = 0, no = 0, na = 0;
-    for (int i = 0; i < 8; ++i) {
-      const int c = T.s16[8 * t + i];
-      nf += c == 1, no += c == 2, na += c != 0;
-    }
-    const int st = parent_state(nf, no, na, true);
-    T.s15[t] = (unsigned char)st;
-    T.n15[t] = st == 3 ? 1 + na : st != 0;
-    T.l15[t] = st == 3 ? no : st == 2;
-  }
-  __syncthreads();
-  if (t < 8) {
-    int nf = 0, no = 0, na = 0, n = 0, l = 0, by = 0;
-    for (int i = 0; i < 8; ++i) {
-      const int c = T.s15[8 * t + i];
-      nf += c == 1, no += c == 2, na += c != 0;
-      n += T.n15[8 * t + i], l += T.l15[8 * t + i], by += c == 3 ? 2 : 0;
-    }
-    const int st = parent_state(nf, no, na, true);
-    T.s14[t] = (unsigned char)st;
-    T.n14[t] = st == 3 ? 1 + n : st != 0;
-    T.l14[t] = st == 3 ? l : st == 2;
-    T.b14[t] = st == 3 ? 2 + by : 0;
-  }
-  __syncthreads();
-  if (t == 0) {
-    int nf = 0, no = 0, na = 0, n = 0, l = 0, by = 0;
-    for (int i = 0; i < 8; ++i) {
-      const int c = T.s14[i];
-      nf += c == 1, no += c == 2, na += c != 0;
-      n += T.n14[i], l += T.l14[i], by += T.b14[i];
-    }
-    const int st = parent_state(nf, no, na, true);
-    T.st = st;
-    T.nodes = st == 3 ? 1 + n : st != 0;
-    T.leaves = st == 3 ? l : st == 2;
-    T.bytes = st == 3 ? 2 + by : 0;
-  }
-  __syncthreads();
-}
-
-// Node records (Octree): bricks first, then each upper level.
+// Node records (Octree): bricks first, then each upper level.  tot: the subtree totals the format keeps, in its order.
 struct Nodes {
   unsigned long long* code;
   int *pool, *first, *end;
   unsigned char* st;
-  unsigned long long *nn, *nb, *nl, *off, *loff;
+  unsigned* val;  // FullTree only
+  unsigned long long *tot[3], *off, *loff;
 };
 
+// ---- the two payloads ------------------------------------------------------------------------------------------------
+// The export and the read below are written once over a format: BinaryTree (octomap's writeBinary / readBinary, the .bt
+// payload; DESIGN.md §4b'''' and §4b'''''') or FullTree (OcTree::write / readData, the .ot payload; §4b''''''').  A
+// format holds only what differs: the node record, the merge of 8 children and its totals, which nodes the stream holds
+// and what a leaf writes into the map.
+constexpr int kReadThreads = 256;
+constexpr long long kMaxReadBricks = 1LL << 29;  // a hash of at most 2^30 slots at load <= 1/2
+constexpr long long kMaxReadPairs = 1LL << 30;
+constexpr int kBadDepth = 1, kBadValue = 2;
+
+// The node whose bricks hold brick b: the last j < end with boff[j] <= b (a node without bricks has the next one's boff).
+__device__ __forceinline__ int brick_owner(const long long* __restrict__ boff, int end, long long b) {
+  int lo = 0, hi = end - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (boff[mid] <= b) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// The voxels [x0, x0 + side) x [y0, ...) x [z0, ...) of pool brick b hold v and become known.
+__device__ __forceinline__ void fill_cube(const Dev& D, size_t b, int x0, int y0, int z0, int side, float v) {
+  for (int z = z0; z < z0 + side; ++z)
+    for (int y = y0; y < y0 + side; ++y) {
+      unsigned bitsw = 0;
+      const int row = (y << 3) | (z << 6);  // side <= 4 voxels of one row share a known word
+      for (int x = x0; x < x0 + side; ++x) {
+        D.lo[b * 512 + row + x] = v;
+        bitsw |= 1u << ((row + x) & 31);
+      }
+      atomicOr(&D.known[b * 16 + (row >> 5)], bitsw);
+    }
+}
+
+// .bt: node states as parent_state's.  Only inner nodes are in the stream, 2 bytes each (the bit pairs of their 8 children).  Totals: nodes, occupied leaves,
+// payload bytes.
+struct BinaryTree {
+  static constexpr int kNodeBytes = 2, kTotals = 3;
+  static constexpr bool kValued = false;
+  static constexpr int kMaxDepth = 15;             // of a stream node
+  static constexpr int kMaxExcess = 8 + 7 * 14;    // the largest excess of a tree whose inner nodes lie at depth <= 15
+  static constexpr const char* kTooMany = "more than 2^30 inner nodes";
+  static constexpr bool kCentres = true;  // (g) and (h) write the occupied leaves' centres and depths
+  static long long payload_bytes(const unsigned long long* tot) { return (long long)tot[2]; }
+
+  struct Merge {
+    int nf = 0, no = 0, na = 0;
+    __device__ __forceinline__ void add(int s, unsigned) { nf += s == 1, no += s == 2, na += s != 0; }
+    __device__ __forceinline__ int state(bool may_prune, unsigned& v) const {
+      v = 0;
+      return parent_state(nf, no, na, may_prune);
+    }
+  };
+  // (e) a brick's levels 16 ... 13 in shared memory, one block of 512 threads: thread t reads the voxel of Morton index t,
+  // then levels 15, 14 and 13 merge their 8 children each
+  struct Levels {
+    unsigned char s16[512], s15[64], s14[8];
+    int n15[64], l15[64], n14[8], l14[8], b14[8];
+    int st, nodes, bytes, leaves;  // the depth-13 node
+  };
+  __device__ static void levels(const unsigned* __restrict__ known, const float* __restrict__ lo, int b, float l_occ,
+                                Levels& T) {
+    const int t = threadIdx.x;
+    const int v = morton_local(t);
+    int s = 0;
+    if ((known[(size_t)b * 16 + (v >> 5)] >> (v & 31)) & 1u) s = lo[(size_t)b * 512 + v] >= l_occ ? 2 : 1;
+    T.s16[t] = (unsigned char)s;
+    __syncthreads();
+    if (t < 64) {
+      int nf = 0, no = 0, na = 0;
+      for (int i = 0; i < 8; ++i) {
+        const int c = T.s16[8 * t + i];
+        nf += c == 1, no += c == 2, na += c != 0;
+      }
+      const int st = parent_state(nf, no, na, true);
+      T.s15[t] = (unsigned char)st;
+      T.n15[t] = st == 3 ? 1 + na : st != 0;
+      T.l15[t] = st == 3 ? no : st == 2;
+    }
+    __syncthreads();
+    if (t < 8) {
+      int nf = 0, no = 0, na = 0, n = 0, l = 0, by = 0;
+      for (int i = 0; i < 8; ++i) {
+        const int c = T.s15[8 * t + i];
+        nf += c == 1, no += c == 2, na += c != 0;
+        n += T.n15[8 * t + i], l += T.l15[8 * t + i], by += c == 3 ? 2 : 0;
+      }
+      const int st = parent_state(nf, no, na, true);
+      T.s14[t] = (unsigned char)st;
+      T.n14[t] = st == 3 ? 1 + n : st != 0;
+      T.l14[t] = st == 3 ? l : st == 2;
+      T.b14[t] = st == 3 ? 2 + by : 0;
+    }
+    __syncthreads();
+    if (t == 0) {
+      int nf = 0, no = 0, na = 0, n = 0, l = 0, by = 0;
+      for (int i = 0; i < 8; ++i) {
+        const int c = T.s14[i];
+        nf += c == 1, no += c == 2, na += c != 0;
+        n += T.n14[i], l += T.l14[i], by += T.b14[i];
+      }
+      const int st = parent_state(nf, no, na, true);
+      T.st = st;
+      T.nodes = st == 3 ? 1 + n : st != 0;
+      T.leaves = st == 3 ? l : st == 2;
+      T.bytes = st == 3 ? 2 + by : 0;
+    }
+    __syncthreads();
+  }
+  __device__ __forceinline__ static void record(const Levels& T, const Nodes& N, int r) {
+    N.st[r] = (unsigned char)T.st;
+    N.tot[0][r] = (unsigned long long)T.nodes;
+    N.tot[1][r] = (unsigned long long)T.leaves;
+    N.tot[2][r] = (unsigned long long)T.bytes;
+  }
+  // c: the children's totals summed, then the node's
+  template <class T>
+  __device__ __forceinline__ static void totals(int s, T* c) {
+    c[0] = s == 3 ? c[0] + 1 : (T)(s != 0);
+    c[1] = s == 3 ? c[1] : (T)(s == 2);
+    c[2] = s == 3 ? c[2] + 2 : (T)0;
+  }
+  __device__ __forceinline__ static int child_bits(int s, int slot) { return s << (2 * slot); }
+  __device__ __forceinline__ static void put_inner(unsigned char* p, const Nodes&, int, int mask) {
+    p[0] = (unsigned char)(mask & 0xff), p[1] = (unsigned char)(mask >> 8);
+  }
+  // (g) child c of an inner node at depth d - 1 takes its offsets; an occupied leaf writes its centre
+  __device__ __forceinline__ static void place(const Nodes& N, int c, int d, unsigned long long& o, unsigned long long& l,
+                                               double res, unsigned char*, float4* cen, unsigned char* dep) {
+    N.off[c] = o, N.loff[c] = l;
+    if (N.st[c] == 2) {
+      const unsigned long long k = N.code[c];
+      const int sh = 16 - d;
+      put_leaf(cen, dep, l, squeeze3(k) << sh, squeeze3(k >> 1) << sh, squeeze3(k >> 2) << sh, d, res);
+    }
+    o += N.tot[2][c], l += N.tot[1][c];
+  }
+
+  __device__ __forceinline__ static int pair(const unsigned char* pay, int i) {
+    return (int)pay[2 * (size_t)i] | ((int)pay[2 * (size_t)i + 1] << 8);
+  }
+  // the children of stream item i that are stream items too: its inner children
+  __device__ __forceinline__ static int streamed(const unsigned char* pay, int i) {
+    const int m = pair(pay, i);
+    int c = 0;
+    for (int s = 0; s < 8; ++s) c |= (((m >> (2 * s)) & 3) == 3) << s;
+    return c;
+  }
+  __device__ __forceinline__ static unsigned long long* node_count(ReadCounters* cnt) { return &cnt->nodes; }
+  // (r4) inner node j at depth d: its children's counts (nodes, free and occupied leaves, known voxels 8^(16-d) per leaf at
+  // depth d) and bricks: 8^(13-d) per leaf at depth d <= 13, one for the node itself at depth 13
+  __device__ __forceinline__ static int count(const unsigned char* pay, int j, int d, float, unsigned long long v[4],
+                                              long long& bricks) {
+    const int m = pair(pay, j);
+    for (int s = 0; s < 8; ++s) {
+      const int b = (m >> (2 * s)) & 3;
+      if (!b) continue;
+      ++v[0];
+      if (b == 3) continue;
+      ++v[b];
+      v[3] += 1ull << (3 * (15 - d));
+      if (d + 1 <= kBrickDepth) bricks += 1LL << (3 * (kBrickDepth - 1 - d));
+    }
+    if (d == kBrickDepth) bricks += 1;
+    return 0;
+  }
+  // (r5) brick r of inner node j (depth d, first key k0): under a leaf child (its state; a leaf's bricks in Morton order),
+  // or, at depth 13, the node's own brick (3: mixed)
+  __device__ __forceinline__ static int brick(const unsigned char* pay, int j, int d, unsigned long long k0, long long r,
+                                              int k[3]) {
+    k[0] = (int)(k0 & 0xffff), k[1] = (int)((k0 >> 16) & 0xffff), k[2] = (int)((k0 >> 32) & 0xffff);
+    if (d == kBrickDepth) return 3;
+    const int m = pair(pay, j), sh = 15 - d;
+    for (int s = 0; s < 8; ++s) {
+      const int bits = (m >> (2 * s)) & 3;
+      if (bits == 0 || bits == 3) continue;
+      const long long c = 1LL << (3 * (kBrickDepth - 1 - d));
+      if (r >= c) {
+        r -= c;
+        continue;
+      }
+      k[0] += ((s & 1) << sh) + (squeeze3((unsigned long long)r) << 3);
+      k[1] += (((s >> 1) & 1) << sh) + (squeeze3((unsigned long long)r >> 1) << 3);
+      k[2] += (((s >> 2) & 1) << sh) + (squeeze3((unsigned long long)r >> 2) << 3);
+      return bits;
+    }
+    return 3;
+  }
+  // (r6) a uniform brick holds L_min or L_max
+  __device__ __forceinline__ static float uniform(const Params& P, const unsigned char*, const long long*, int, int, int st) {
+    return st == 1 ? P.l_min : st == 2 ? P.l_max : 0.0f;
+  }
+  // (r7) inner nodes at depth 13 ... 15 write the 64, 8 or 1 voxels of each of their leaves
+  __device__ __forceinline__ static bool writes_leaves(const unsigned char*, int, int d) { return d >= kBrickDepth; }
+  template <class Cube>
+  __device__ __forceinline__ static void leaves(const Params& P, const unsigned char* pay, int j, int d,
+                                                unsigned long long k0, Cube&& cube) {
+    const int m = pair(pay, j), sh = 15 - d;
+    for (int s = 0; s < 8; ++s) {
+      const int bits = (m >> (2 * s)) & 3;
+      if (bits == 0 || bits == 3) continue;
+      cube(((int)(k0 & 7)) | ((s & 1) << sh), ((int)((k0 >> 16) & 7)) | (((s >> 1) & 1) << sh),
+           ((int)((k0 >> 32) & 7)) | (((s >> 2) & 1) << sh), 1 << sh, bits == 1 ? P.l_min : P.l_max);
+    }
+  }
+
+  static int check(const ReadCounters& c, long long, long long nodes, const char** why) {
+    if (c.end == INT_MAX) return *why = "the payload is truncated", LS_ERR_ARG;
+    if (c.bad) return *why = "an inner node at depth 16", LS_ERR_ARG;
+    if ((long long)c.nodes + 1 != nodes) return *why = "the header's size does not count the payload's nodes", LS_ERR_ARG;
+    return LS_OK;
+  }
+  static void counts(ReadCounters* out) {  // the root counts as a node; every stream item is inner
+    out->nodes += 1;
+    out->inner = (unsigned long long)out->end;
+  }
+};
+
+// .ot: node states 0 no known voxel below, 1 leaf, 3 inner; values are float log-odds kept as their bits.  Every node is
+// in the stream, 5 bytes each: its value, then the mask of its existing children.  Totals: nodes, leaves.
+struct FullTree {
+  static constexpr int kNodeBytes = 5, kTotals = 2;
+  static constexpr bool kValued = true;
+  static constexpr int kMaxDepth = 16;
+  static constexpr int kMaxExcess = 8 + 7 * 15;  // the largest excess of a tree whose nodes lie at depth <= 16
+  static constexpr const char* kTooMany = "more than 2^30 nodes";
+  static constexpr bool kCentres = false;
+  static long long payload_bytes(const unsigned long long* tot) { return kNodeBytes * (long long)tot[0]; }
+
+  // octomap's isNodeCollapsible on values (all 8 children exist, are leaves and compare equal as floats; the collapsed
+  // leaf keeps child 0's bits) and updateInnerOccupancy (an inner node holds its largest child, the earliest on ties).
+  // Children are added in child order.
+  struct Merge {
+    int na = 0, nl = 0;
+    bool eq = true;
+    unsigned first = 0, best = 0;
+    __device__ __forceinline__ void add(int s, unsigned v) {
+      if (!s) return;
+      if (na == 0) {
+        first = best = v;
+      } else {
+        eq = eq && __uint_as_float(v) == __uint_as_float(first);
+        if (__uint_as_float(v) > __uint_as_float(best)) best = v;
+      }
+      ++na;
+      nl += s == 1;
+    }
+    __device__ __forceinline__ int state(bool may_prune, unsigned& v) const {
+      if (may_prune && nl == 8 && eq) {
+        v = first;
+        return 1;
+      }
+      v = best;
+      return na ? 3 : 0;
+    }
+  };
+  // (e) as BinaryTree's, merging values
+  struct Levels {
+    unsigned v16[512], v15[64], v14[8];
+    unsigned char s16[512], s15[64], s14[8];
+    int n15[64], l15[64], n14[8], l14[8];
+    int st, nodes, leaves;  // the depth-13 node
+    unsigned val;
+  };
+  __device__ static void levels(const unsigned* __restrict__ known, const float* __restrict__ lo, int b, float, Levels& T) {
+    const int t = threadIdx.x;
+    const int v = morton_local(t);
+    T.s16[t] = (unsigned char)((known[(size_t)b * 16 + (v >> 5)] >> (v & 31)) & 1u);
+    T.v16[t] = __float_as_uint(lo[(size_t)b * 512 + v]);
+    __syncthreads();
+    if (t < 64) {
+      Merge m;
+      for (int i = 0; i < 8; ++i) m.add(T.s16[8 * t + i], T.v16[8 * t + i]);
+      unsigned val;
+      const int st = m.state(true, val);
+      T.s15[t] = (unsigned char)st, T.v15[t] = val;
+      T.n15[t] = st == 3 ? 1 + m.na : st != 0;
+      T.l15[t] = st == 3 ? m.na : st != 0;
+    }
+    __syncthreads();
+    if (t < 8) {
+      Merge m;
+      int n = 0, l = 0;
+      for (int i = 0; i < 8; ++i) m.add(T.s15[8 * t + i], T.v15[8 * t + i]), n += T.n15[8 * t + i], l += T.l15[8 * t + i];
+      unsigned val;
+      const int st = m.state(true, val);
+      T.s14[t] = (unsigned char)st, T.v14[t] = val;
+      T.n14[t] = st == 3 ? 1 + n : st != 0;
+      T.l14[t] = st == 3 ? l : st != 0;
+    }
+    __syncthreads();
+    if (t == 0) {
+      Merge m;
+      int n = 0, l = 0;
+      for (int i = 0; i < 8; ++i) m.add(T.s14[i], T.v14[i]), n += T.n14[i], l += T.l14[i];
+      unsigned val;
+      const int st = m.state(true, val);
+      T.st = st, T.val = val;
+      T.nodes = st == 3 ? 1 + n : st != 0;
+      T.leaves = st == 3 ? l : st != 0;
+    }
+    __syncthreads();
+  }
+  __device__ __forceinline__ static void record(const Levels& T, const Nodes& N, int r) {
+    N.st[r] = (unsigned char)T.st;
+    N.val[r] = T.val;
+    N.tot[0][r] = (unsigned long long)T.nodes;
+    N.tot[1][r] = (unsigned long long)T.leaves;
+  }
+  template <class T>
+  __device__ __forceinline__ static void totals(int s, T* c) {
+    c[0] = s == 3 ? c[0] + 1 : (T)(s != 0);
+    c[1] = s == 3 ? c[1] : (T)(s != 0);
+  }
+  __device__ __forceinline__ static void put_node(unsigned char* p, unsigned v, int mask) {
+    p[0] = (unsigned char)(v & 0xff), p[1] = (unsigned char)((v >> 8) & 0xff), p[2] = (unsigned char)((v >> 16) & 0xff);
+    p[3] = (unsigned char)(v >> 24), p[4] = (unsigned char)mask;
+  }
+  __device__ __forceinline__ static int child_bits(int s, int slot) { return (s != 0) << slot; }
+  __device__ __forceinline__ static void put_inner(unsigned char* p, const Nodes& N, int i, int mask) {
+    put_node(p, N.val[i], mask);
+  }
+  // (g) child c takes its offset; a leaf writes its node (an inner brick writes itself in (h))
+  __device__ __forceinline__ static void place(const Nodes& N, int c, int, unsigned long long& o, unsigned long long&,
+                                               double, unsigned char* payload, float4*, unsigned char*) {
+    N.off[c] = o;
+    if (N.st[c] == 1) put_node(payload + o, N.val[c], 0);
+    o += kNodeBytes * N.tot[0][c];
+  }
+
+  __device__ __forceinline__ static int mask(const unsigned char* pay, int i) { return pay[(size_t)kNodeBytes * i + 4]; }
+  __device__ __forceinline__ static unsigned value(const unsigned char* pay, int i) {
+    const unsigned char* p = pay + (size_t)kNodeBytes * i;
+    return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
+  }
+  __device__ __forceinline__ static int streamed(const unsigned char* pay, int i) { return mask(pay, i); }
+  __device__ __forceinline__ static unsigned long long* node_count(ReadCounters* cnt) { return &cnt->inner; }
+  // (r4) node j at depth d: a node with children (one brick of its own at depth 13), or a leaf by state with 8^(16-d)
+  // known voxels and 8^(13-d) bricks (d <= 13).  Children at depth 16 and leaf values that are not finite are refused.
+  __device__ __forceinline__ static int count(const unsigned char* pay, int j, int d, float l_occ, unsigned long long v[4],
+                                              long long& bricks) {
+    const int m = mask(pay, j);
+    const float val = __uint_as_float(value(pay, j));
+    if (d == 16 && m) return kBadDepth;
+    if (!m && !isfinite(val)) return kBadValue;
+    if (m) {
+      v[0] = 1;
+      if (d == kBrickDepth) bricks = 1;
+    } else {
+      ++v[val >= l_occ ? 2 : 1];
+      v[3] = 1ull << (3 * (16 - d));
+      if (d <= kBrickDepth) bricks = 1LL << (3 * (kBrickDepth - d));
+    }
+    return 0;
+  }
+  // (r5) brick r of node j: a leaf's bricks in Morton order (1), or, at depth 13, the node's own brick (3: mixed)
+  __device__ __forceinline__ static int brick(const unsigned char* pay, int j, int d, unsigned long long k0, long long r,
+                                              int k[3]) {
+    const bool mixed = d == kBrickDepth && mask(pay, j) != 0;
+    const unsigned long long u = (unsigned long long)r;
+    k[0] = (int)(k0 & 0xffff) + (mixed ? 0 : squeeze3(u) << 3);
+    k[1] = (int)((k0 >> 16) & 0xffff) + (mixed ? 0 : squeeze3(u >> 1) << 3);
+    k[2] = (int)((k0 >> 32) & 0xffff) + (mixed ? 0 : squeeze3(u >> 2) << 3);
+    return mixed ? 3 : 1;
+  }
+  // (r6) a uniform brick holds its leaf's value
+  __device__ __forceinline__ static float uniform(const Params&, const unsigned char* pay, const long long* boff, int end,
+                                                  int b, int st) {
+    return st == 1 ? __uint_as_float(value(pay, brick_owner(boff, end, b))) : 0.0f;
+  }
+  // (r7) leaves at depth 14 ... 16 write their 64, 8 or 1 voxels
+  __device__ __forceinline__ static bool writes_leaves(const unsigned char* pay, int j, int d) {
+    return d > kBrickDepth && !mask(pay, j);
+  }
+  template <class Cube>
+  __device__ __forceinline__ static void leaves(const Params&, const unsigned char* pay, int j, int d, unsigned long long k0,
+                                                Cube&& cube) {
+    cube((int)(k0 & 7), (int)((k0 >> 16) & 7), (int)((k0 >> 32) & 7), 1 << (16 - d), __uint_as_float(value(pay, j)));
+  }
+
+  static int check(const ReadCounters& c, long long count, long long nodes, const char** why) {
+    if (c.end == INT_MAX)
+      return *why = count < nodes ? "the payload is truncated" : "the header's size does not count the payload's nodes",
+             LS_ERR_ARG;
+    if (c.bad & kBadDepth) return *why = "a node at depth 16 with children", LS_ERR_ARG;
+    if (c.bad & kBadValue) return *why = "a leaf value that is NaN or infinite", LS_ERR_ARG;
+    if ((long long)c.end != nodes) return *why = "the header's size does not count the payload's nodes", LS_ERR_ARG;
+    return LS_OK;
+  }
+  static void counts(ReadCounters* out) { out->nodes = (unsigned long long)out->end; }
+};
+
+// ---- export: (d) ... (h) ---------------------------------------------------------------------------------------------
 // (d)
 __global__ void oct_code_kernel(const unsigned long long* __restrict__ bkey, int n, unsigned long long* __restrict__ code,
                                 int* __restrict__ idx) {
@@ -757,22 +1093,19 @@ __global__ void oct_code_kernel(const unsigned long long* __restrict__ bkey, int
   idx[i] = i;
 }
 
-// (e) one block per brick record, in pre-order
+// (e) one block per brick record, in pre-order: state, value and subtree totals
+template <class F>
 __global__ void __launch_bounds__(512) oct_brick_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
                                                         Nodes N, float l_occ) {
-  __shared__ BrickTree T;
+  __shared__ typename F::Levels T;
   const int r = blockIdx.x;
-  brick_tree(known, lo, N.pool[r], l_occ, T);
-  if (threadIdx.x == 0) {
-    N.st[r] = (unsigned char)T.st;
-    N.nn[r] = (unsigned long long)T.nodes;
-    N.nb[r] = (unsigned long long)T.bytes;
-    N.nl[r] = (unsigned long long)T.leaves;
-  }
+  F::levels(known, lo, N.pool[r], l_occ, T);
+  if (threadIdx.x == 0) F::record(T, N, r);
 }
 
 // (f) levels 12 ... 0 appended after the n_b brick records; levels[2d], levels[2d + 1]: first record and count at depth d.
-// tot: nodes, payload bytes and occupied leaves of the root (all 0 when no voxel is known).
+// tot: the root's totals (all 0 when no voxel is known).
+template <class F>
 __global__ void __launch_bounds__(kTreeThreads) oct_up_kernel(Nodes N, int n_b, int* levels, unsigned long long* tot) {
   using Scan = cub::BlockScan<int, kTreeThreads>;
   __shared__ typename Scan::TempStorage scan;
@@ -796,28 +1129,31 @@ __global__ void __launch_bounds__(kTreeThreads) oct_up_kernel(Nodes N, int n_b, 
     }
     for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
       const int f = N.first[p], e = p + 1 < pb + pn ? N.first[p + 1] : pb;
-      int nf = 0, no = 0, na = 0;
-      unsigned long long n = 0, by = 0, l = 0;
+      typename F::Merge m;
+      unsigned long long sum[F::kTotals] = {};
       for (int c = f; c < e; ++c) {
-        const int s = N.st[c];
-        nf += s == 1, no += s == 2, na += s != 0;
-        n += N.nn[c], by += N.nb[c], l += N.nl[c];
+        m.add(N.st[c], F::kValued ? N.val[c] : 0u);
+        for (int k = 0; k < F::kTotals; ++k) sum[k] += N.tot[k][c];
       }
-      const int s = parent_state(nf, no, na, d > 0);  // octomap's prune() stops at depth 1: the root stays inner
+      unsigned v;
+      const int s = m.state(d > 0, v);  // octomap's prune() stops at depth 1: the root stays inner
       N.st[p] = (unsigned char)s;
+      if (F::kValued) N.val[p] = v;
       N.end[p] = e;
-      N.nn[p] = s == 3 ? n + 1 : (unsigned long long)(s != 0);
-      N.nb[p] = s == 3 ? by + 2 : 0ull;
-      N.nl[p] = s == 3 ? l : (unsigned long long)(s == 2);
+      F::totals(s, sum);
+      for (int k = 0; k < F::kTotals; ++k) N.tot[k][p] = sum[k];
     }
     __syncthreads();
     if (t == 0) levels[2 * d] = pb, levels[2 * d + 1] = pn;
     cb = pb, cn = pn;
   }
-  if (t == 0) tot[0] = N.nn[cb], tot[1] = N.nb[cb], tot[2] = N.nl[cb];
+  if (t == 0)
+    for (int k = 0; k < F::kTotals; ++k) tot[k] = N.tot[k][cb];
 }
 
-// (g)
+// (g) levels 0 ... 12: each inner node writes its record and gives every child its offsets (its own + its record + the
+// earlier siblings' totals)
+template <class F>
 __global__ void __launch_bounds__(kTreeThreads) oct_down_kernel(Nodes N, const int* __restrict__ levels, double res,
                                                                 unsigned char* __restrict__ payload, float4* __restrict__ cen,
                                                                 unsigned char* __restrict__ dep) {
@@ -830,37 +1166,36 @@ __global__ void __launch_bounds__(kTreeThreads) oct_down_kernel(Nodes N, const i
       if (N.st[p] != 3) continue;  // only an inner node's children are in the tree
       const int f = N.first[p], e = N.end[p];
       int mask = 0;
-      for (int c = f; c < e; ++c) mask |= (int)N.st[c] << (2 * (int)(N.code[c] & 7));
+      for (int c = f; c < e; ++c) mask |= F::child_bits(N.st[c], (int)(N.code[c] & 7));
       unsigned long long o = N.off[p], l = N.loff[p];
-      payload[o] = (unsigned char)(mask & 0xff);
-      payload[o + 1] = (unsigned char)(mask >> 8);
-      o += 2;
-      for (int c = f; c < e; ++c) {
-        N.off[c] = o, N.loff[c] = l;
-        if (N.st[c] == 2) {
-          const unsigned long long k = N.code[c];
-          const int sh = 16 - (d + 1);
-          put_leaf(cen, dep, l, squeeze3(k) << sh, squeeze3(k >> 1) << sh, squeeze3(k >> 2) << sh, d + 1, res);
-        }
-        o += N.nb[c], l += N.nl[c];
-      }
+      F::put_inner(payload + o, N, p, mask);
+      o += F::kNodeBytes;
+      for (int c = f; c < e; ++c) F::place(N, c, d + 1, o, l, res, payload, cen, dep);
     }
     __syncthreads();
   }
 }
 
-// (h) one block per brick record; the inner ones write their bytes and occupied leaves
-__global__ void __launch_bounds__(512) oct_emit_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
-                                                       const unsigned long long* __restrict__ bkey, Nodes N, float l_occ,
-                                                       double res, unsigned char* __restrict__ payload,
-                                                       float4* __restrict__ cen, unsigned char* __restrict__ dep) {
+// (h) one block per brick record; the inner ones write their nodes below depth 13 at the offset (g) gave them
+template <class F>
+__global__ void oct_emit_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
+                                const unsigned long long* __restrict__ bkey, Nodes N, float l_occ, double res,
+                                unsigned char* __restrict__ payload, float4* __restrict__ cen, unsigned char* __restrict__ dep);
+
+// .bt: the brick's pre-order bytes, and its occupied leaves
+template <>
+__global__ void __launch_bounds__(512) oct_emit_kernel<BinaryTree>(const unsigned* __restrict__ known,
+                                                                   const float* __restrict__ lo,
+                                                                   const unsigned long long* __restrict__ bkey, Nodes N,
+                                                                   float l_occ, double res, unsigned char* __restrict__ payload,
+                                                                   float4* __restrict__ cen, unsigned char* __restrict__ dep) {
   using Scan = cub::BlockScan<int, 512>;
-  __shared__ BrickTree T;
+  __shared__ BinaryTree::Levels T;
   __shared__ typename Scan::TempStorage scan;
   const int r = blockIdx.x;
   if (N.st[r] != 3) return;  // a leaf brick is written by its parent in (g)
   const int b = N.pool[r];
-  brick_tree(known, lo, b, l_occ, T);
+  BinaryTree::levels(known, lo, b, l_occ, T);
   const int t = threadIdx.x;
   if (t == 0) {  // pre-order: the brick, then each inner depth-14 node followed by its inner depth-15 nodes
     unsigned char* p = payload + N.off[r];
@@ -893,194 +1228,26 @@ __global__ void __launch_bounds__(512) oct_emit_kernel(const unsigned* __restric
   }
 }
 
-// ---- full tree export (octomap's OcTree::write / writeData; DESIGN.md §4b''''''') -----------------------------------
-// Node states here: 0 no known voxel below, 1 leaf, 3 inner; values are float log-odds kept as their bits.
-constexpr int kFullNodeBytes = 5;
-
-// octomap's isNodeCollapsible on values (all 8 children exist, are leaves and compare equal as floats; the collapsed
-// leaf keeps child 0's bits) and updateInnerOccupancy (an inner node holds its largest child, the earliest on ties).
-// Children are added in child order.
-struct FullMerge {
-  int na = 0, nl = 0;
-  bool eq = true;
-  unsigned first = 0, best = 0;
-  __device__ __forceinline__ void add(int s, unsigned v) {
-    if (!s) return;
-    if (na == 0) {
-      first = best = v;
-    } else {
-      eq = eq && __uint_as_float(v) == __uint_as_float(first);
-      if (__uint_as_float(v) > __uint_as_float(best)) best = v;
-    }
-    ++na;
-    nl += s == 1;
-  }
-  __device__ __forceinline__ int state(bool may_prune, unsigned& v) const {
-    if (may_prune && nl == 8 && eq) {
-      v = first;
-      return 1;
-    }
-    v = best;
-    return na ? 3 : 0;
-  }
-};
-
-__device__ __forceinline__ void put_node(unsigned char* p, unsigned v, int mask) {
-  p[0] = (unsigned char)(v & 0xff), p[1] = (unsigned char)((v >> 8) & 0xff), p[2] = (unsigned char)((v >> 16) & 0xff);
-  p[3] = (unsigned char)(v >> 24), p[4] = (unsigned char)mask;
-}
-
-struct FullBrickTree {
-  unsigned v16[512], v15[64], v14[8];
-  unsigned char s16[512], s15[64], s14[8];
-  int n15[64], l15[64], n14[8], l14[8];
-  int st, nodes, leaves;  // the depth-13 node
-  unsigned val;
-};
-
-// One block of 512 threads: thread t reads the voxel of Morton index t, then the brick's levels 15, 14 and 13.
-__device__ void full_brick_tree(const unsigned* __restrict__ known, const float* __restrict__ lo, int b, FullBrickTree& T) {
-  const int t = threadIdx.x;
-  const int v = morton_local(t);
-  T.s16[t] = (unsigned char)((known[(size_t)b * 16 + (v >> 5)] >> (v & 31)) & 1u);
-  T.v16[t] = __float_as_uint(lo[(size_t)b * 512 + v]);
-  __syncthreads();
-  if (t < 64) {
-    FullMerge m;
-    for (int i = 0; i < 8; ++i) m.add(T.s16[8 * t + i], T.v16[8 * t + i]);
-    unsigned val;
-    const int st = m.state(true, val);
-    T.s15[t] = (unsigned char)st, T.v15[t] = val;
-    T.n15[t] = st == 3 ? 1 + m.na : st != 0;
-    T.l15[t] = st == 3 ? m.na : st != 0;
-  }
-  __syncthreads();
-  if (t < 8) {
-    FullMerge m;
-    int n = 0, l = 0;
-    for (int i = 0; i < 8; ++i) m.add(T.s15[8 * t + i], T.v15[8 * t + i]), n += T.n15[8 * t + i], l += T.l15[8 * t + i];
-    unsigned val;
-    const int st = m.state(true, val);
-    T.s14[t] = (unsigned char)st, T.v14[t] = val;
-    T.n14[t] = st == 3 ? 1 + n : st != 0;
-    T.l14[t] = st == 3 ? l : st != 0;
-  }
-  __syncthreads();
-  if (t == 0) {
-    FullMerge m;
-    int n = 0, l = 0;
-    for (int i = 0; i < 8; ++i) m.add(T.s14[i], T.v14[i]), n += T.n14[i], l += T.l14[i];
-    unsigned val;
-    const int st = m.state(true, val);
-    T.st = st, T.val = val;
-    T.nodes = st == 3 ? 1 + n : st != 0;
-    T.leaves = st == 3 ? l : st != 0;
-  }
-  __syncthreads();
-}
-
-// (e') one block per brick record, in pre-order: state, value and subtree totals (nodes, leaves)
-__global__ void __launch_bounds__(512) ful_brick_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
-                                                        Nodes N, unsigned* __restrict__ val) {
-  __shared__ FullBrickTree T;
-  const int r = blockIdx.x;
-  full_brick_tree(known, lo, N.pool[r], T);
-  if (threadIdx.x == 0) {
-    N.st[r] = (unsigned char)T.st;
-    val[r] = T.val;
-    N.nn[r] = (unsigned long long)T.nodes;
-    N.nl[r] = (unsigned long long)T.leaves;
-  }
-}
-
-// (f') levels 12 ... 0 as in (f), merging values; tot: nodes and leaves of the root (0 when no voxel is known)
-__global__ void __launch_bounds__(kTreeThreads) ful_up_kernel(Nodes N, unsigned* __restrict__ val, int n_b, int* levels,
-                                                              unsigned long long* tot) {
-  using Scan = cub::BlockScan<int, kTreeThreads>;
-  __shared__ typename Scan::TempStorage scan;
-  const int t = threadIdx.x;
-  int cb = 0, cn = n_b;  // the level below
-  if (t == 0) levels[2 * kBrickDepth] = 0, levels[2 * kBrickDepth + 1] = n_b;
-  for (int d = kBrickDepth - 1; d >= 0; --d) {
-    const int pb = cb + cn;
-    int pn = 0;
-    for (int c0 = 0; c0 < cn; c0 += kTreeThreads) {
-      const int i = c0 + t;
-      const int head = i < cn && (i == 0 || (N.code[cb + i] >> 3) != (N.code[cb + i - 1] >> 3));
-      int pos, total;
-      Scan(scan).ExclusiveSum(head, pos, total);
-      if (head) {
-        N.code[pb + pn + pos] = N.code[cb + i] >> 3;
-        N.first[pb + pn + pos] = cb + i;
-      }
-      pn += total;
-      __syncthreads();
-    }
-    for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
-      const int f = N.first[p], e = p + 1 < pb + pn ? N.first[p + 1] : pb;
-      FullMerge m;
-      unsigned long long n = 0, l = 0;
-      for (int c = f; c < e; ++c) m.add(N.st[c], val[c]), n += N.nn[c], l += N.nl[c];
-      unsigned v;
-      const int s = m.state(d > 0, v);  // the root is never pruned
-      N.st[p] = (unsigned char)s;
-      val[p] = v;
-      N.end[p] = e;
-      N.nn[p] = s == 3 ? n + 1 : (unsigned long long)(s != 0);
-      N.nl[p] = s == 3 ? l : (unsigned long long)(s != 0);
-    }
-    __syncthreads();
-    if (t == 0) levels[2 * d] = pb, levels[2 * d + 1] = pn;
-    cb = pb, cn = pn;
-  }
-  if (t == 0) tot[0] = N.nn[cb], tot[1] = N.nl[cb];
-}
-
-// (g') levels 0 ... 12: each inner node writes its 5 bytes and its leaf children's, and gives every child its offset (its
-// own + 5 + 5 x the earlier siblings' nodes); inner bricks write themselves in (h')
-__global__ void __launch_bounds__(kTreeThreads) ful_down_kernel(Nodes N, const unsigned* __restrict__ val,
-                                                                const int* __restrict__ levels,
-                                                                unsigned char* __restrict__ payload) {
-  const int t = threadIdx.x;
-  if (t == 0) N.off[levels[0]] = 0;
-  __syncthreads();
-  for (int d = 0; d < kBrickDepth; ++d) {
-    const int pb = levels[2 * d], pn = levels[2 * d + 1];
-    for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
-      if (N.st[p] != 3) continue;  // only an inner node's children are in the tree
-      const int f = N.first[p], e = N.end[p];
-      int mask = 0;
-      for (int c = f; c < e; ++c) mask |= (N.st[c] != 0) << (int)(N.code[c] & 7);
-      unsigned long long o = N.off[p];
-      put_node(payload + o, val[p], mask);
-      o += kFullNodeBytes;
-      for (int c = f; c < e; ++c) {
-        N.off[c] = o;
-        if (N.st[c] == 1) put_node(payload + o, val[c], 0);
-        o += kFullNodeBytes * N.nn[c];
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// (h') one block per inner brick record: its nodes below depth 13 placed in parallel.  Thread t owns, in pre-order, the
-// depth-14 node starting at Morton index t (t % 64 == 0), the depth-15 one (t % 8 == 0) and voxel t, each when it is in
-// the tree; a block scan over the owned counts gives each its place.
-__global__ void __launch_bounds__(512) ful_emit_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
-                                                       Nodes N, unsigned char* __restrict__ payload) {
+// .ot: the brick's up to 585 nodes placed in parallel.  Thread t owns, in pre-order, the depth-14 node starting at Morton
+// index t (t % 64 == 0), the depth-15 one (t % 8 == 0) and voxel t, each when it is in the tree; a block scan over the
+// owned counts gives each its place.
+template <>
+__global__ void __launch_bounds__(512) oct_emit_kernel<FullTree>(const unsigned* __restrict__ known, const float* __restrict__ lo,
+                                                                 const unsigned long long* __restrict__, Nodes N, float l_occ,
+                                                                 double, unsigned char* __restrict__ payload,
+                                                                 float4* __restrict__, unsigned char* __restrict__) {
   using Scan = cub::BlockScan<int, 512>;
-  __shared__ FullBrickTree T;
+  __shared__ FullTree::Levels T;
   __shared__ typename Scan::TempStorage scan;
   const int r = blockIdx.x;
-  if (N.st[r] != 3) return;  // a leaf brick is written by its parent in (g')
-  full_brick_tree(known, lo, N.pool[r], T);
+  if (N.st[r] != 3) return;  // a leaf brick is written by its parent in (g)
+  FullTree::levels(known, lo, N.pool[r], l_occ, T);
   const int t = threadIdx.x;
   unsigned char* base = payload + N.off[r];
   if (t == 0) {
     int m = 0;
     for (int i = 0; i < 8; ++i) m |= (T.s14[i] != 0) << i;
-    put_node(base, T.val, m);
+    FullTree::put_node(base, T.val, m);
   }
   const int i14 = t >> 6, i15 = t >> 3;
   const bool a = (t & 63) == 0 && T.s14[i14] != 0;
@@ -1088,54 +1255,40 @@ __global__ void __launch_bounds__(512) ful_emit_kernel(const unsigned* __restric
   const bool c = T.s14[i14] == 3 && T.s15[i15] == 3 && T.s16[t] != 0;
   int idx;
   Scan(scan).ExclusiveSum((int)a + (int)b + (int)c, idx);
-  unsigned char* p = base + (size_t)kFullNodeBytes * (1 + idx);
+  unsigned char* p = base + (size_t)FullTree::kNodeBytes * (1 + idx);
   if (a) {
     int m = 0;
     if (T.s14[i14] == 3)
       for (int i = 0; i < 8; ++i) m |= (T.s15[8 * i14 + i] != 0) << i;
-    put_node(p, T.v14[i14], m);
-    p += kFullNodeBytes;
+    FullTree::put_node(p, T.v14[i14], m);
+    p += FullTree::kNodeBytes;
   }
   if (b) {
     int m = 0;
     if (T.s15[i15] == 3)
       for (int i = 0; i < 8; ++i) m |= (T.s16[8 * i15 + i] != 0) << i;
-    put_node(p, T.v15[i15], m);
-    p += kFullNodeBytes;
+    FullTree::put_node(p, T.v15[i15], m);
+    p += FullTree::kNodeBytes;
   }
-  if (c) put_node(p, T.v16[t], 0);
+  if (c) FullTree::put_node(p, T.v16[t], 0);
 }
 
-// ---- .bt read (octomap's readBinary; DESIGN.md §4b'''''') ------------------------------------------------
-// Pair i of the payload is the i-th inner node in pre-order.  With c_i its inner children, the excess E_0 = 1,
-// E_{i+1} = E_i + c_i - 1 counts the inner nodes found but not yet read; the tree ends at the first i >= 1 with E_i = 0.
-constexpr int kReadThreads = 256;
-constexpr int kMaxInnerExcess = 8 + 7 * 14;      // the largest excess of a tree whose inner nodes lie at depth <= 15
-constexpr long long kMaxReadBricks = 1LL << 29;  // a hash of at most 2^30 slots at load <= 1/2
-constexpr long long kMaxReadPairs = 1LL << 30;
-constexpr int kBadDepth = 1;
-
+// ---- read: (r1) ... (r7) ---------------------------------------------------------------------------------------------
+// Item i of the stream is the i-th node of it in pre-order.  With c_i its children in the stream, the excess E_0 = 1,
+// E_{i+1} = E_i + c_i - 1 counts the stream nodes found but not yet read; the tree ends at the first i >= 1 with E_i = 0.
 struct MinOp {
   __device__ __forceinline__ int operator()(int a, int b) const { return a < b ? a : b; }
 };
 
-__device__ __forceinline__ int pair_mask(const unsigned char* pay, int i) {
-  return (int)pay[2 * (size_t)i] | ((int)pay[2 * (size_t)i + 1] << 8);
-}
-__device__ __forceinline__ int inner_children(int mask) {
-  int c = 0;
-  for (int s = 0; s < 8; ++s) c += ((mask >> (2 * s)) & 3) == 3;
-  return c;
-}
-
 // (r1) in[0] = 1 and in[i + 1] = c_i - 1: an inclusive sum gives E_0 ... E_n
+template <class F>
 __global__ void rd_excess_kernel(const unsigned char* __restrict__ pay, int n, int* __restrict__ in) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) in[0] = 1;
-  if (i < n) in[i + 1] = inner_children(pair_mask(pay, i)) - 1;
+  if (i < n) in[i + 1] = __popc(F::streamed(pay, i)) - 1;
 }
 
-// (r2) the tree's end and, per block of kReadThreads pairs, the least excess (r3) skips blocks by
+// (r2) the tree's end and, per block of kReadThreads items, the least excess (r3) skips blocks by
 __global__ void __launch_bounds__(kReadThreads) rd_end_kernel(const int* __restrict__ ex, int n, int* __restrict__ bmin,
                                                              ReadCounters* cnt) {
   using Reduce = cub::BlockReduce<int, kReadThreads>;
@@ -1147,15 +1300,16 @@ __global__ void __launch_bounds__(kReadThreads) rd_end_kernel(const int* __restr
   if (threadIdx.x == 0) bmin[blockIdx.x] = m;
 }
 
-// (r3) per inner node j >= 1 of the tree: its parent, the last i < j with E_i <= E_j, and its slot, the child index of the
-// (E_p + c_p - 1 - E_j)-th inner child of p.  An excess above kMaxInnerExcess proves an inner node at depth 16.
+// (r3) per stream node j >= 1: its parent, the last i < j with E_i <= E_j, and its slot, the (E_p + c_p - 1 - E_j)-th
+// stream child of p.  An excess above the format's bound proves a stream node too deep.
+template <class F>
 __global__ void rd_parent_kernel(const unsigned char* __restrict__ pay, const int* __restrict__ ex,
                                  const int* __restrict__ bmin, int n, int* __restrict__ par, unsigned char* __restrict__ slot,
                                  ReadCounters* cnt) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n || j >= cnt->end) return;
   const int e = ex[j];
-  if (e > kMaxInnerExcess) {
+  if (e > F::kMaxExcess) {
     atomicOr(&cnt->bad, kBadDepth);
     return;
   }
@@ -1172,201 +1326,7 @@ __global__ void rd_parent_kernel(const unsigned char* __restrict__ pay, const in
     p = b * kReadThreads + kReadThreads - 1;
     while (ex[p] > e) --p;
   }
-  const int m = pair_mask(pay, p);
-  int rank = ex[p] + inner_children(m) - 1 - e, s = 0;
-  for (; s < 8; ++s)
-    if (((m >> (2 * s)) & 3) == 3 && rank-- == 0) break;
-  par[j] = p;
-  slot[j] = (unsigned char)s;
-}
-
-// (r4) per inner node j of the tree: depth and first key from at most 15 parents (more: an inner node at depth 16), its
-// depth-13 ancestor, and its children's counts: nodes, leaves, known voxels 8^(16-d) and bricks 8^(13-d) per leaf at depth
-// d (d <= 13), one brick for the node itself at depth 13.  nb[j] = its bricks (0 past the tree, nb[n] = 0).
-__global__ void __launch_bounds__(kReadThreads) rd_node_kernel(const unsigned char* __restrict__ pay,
-                                                              const int* __restrict__ par,
-                                                              const unsigned char* __restrict__ slot, int n,
-                                                              unsigned char* __restrict__ depth,
-                                                              unsigned long long* __restrict__ key, int* __restrict__ anc,
-                                                              long long* __restrict__ nb, ReadCounters* cnt) {
-  using Reduce = cub::BlockReduce<unsigned long long, kReadThreads>;
-  __shared__ typename Reduce::TempStorage tmp;
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  unsigned long long v[4] = {0, 0, 0, 0};  // child nodes, free leaves, occupied leaves, known voxels
-  long long bricks = 0;
-  if (j < n && j < cnt->end && !cnt->bad) {
-    // step i visits the ancestor at depth d - i: its slot is key bit 16 - d + i; the depth-13 one is among steps 0 ... 2
-    int d = 0, x = j, a1 = j, a2 = j;
-    unsigned long long slots = 0;
-    while (x != 0 && d < 15) {
-      if (d == 1) a1 = x;
-      if (d == 2) a2 = x;
-      slots |= (unsigned long long)slot[x] << (3 * d);
-      ++d;
-      x = par[x];
-    }
-    if (x != 0) {
-      atomicOr(&cnt->bad, kBadDepth);
-    } else {
-      unsigned kx = 0, ky = 0, kz = 0;
-      for (int i = 0; i < d; ++i) {
-        const unsigned s = (unsigned)(slots >> (3 * i)) & 7u, b = (unsigned)(16 - d + i);
-        kx |= (s & 1u) << b, ky |= ((s >> 1) & 1u) << b, kz |= ((s >> 2) & 1u) << b;
-      }
-      depth[j] = (unsigned char)d;
-      key[j] = pack((int)kx, (int)ky, (int)kz);
-      anc[j] = d == kBrickDepth ? j : d == kBrickDepth + 1 ? a1 : d == kBrickDepth + 2 ? a2 : -1;
-      const int m = pair_mask(pay, j);
-      for (int s = 0; s < 8; ++s) {
-        const int b = (m >> (2 * s)) & 3;
-        if (!b) continue;
-        ++v[0];
-        if (b == 3) continue;
-        ++v[b];
-        v[3] += 1ull << (3 * (15 - d));
-        if (d + 1 <= kBrickDepth) bricks += 1LL << (3 * (kBrickDepth - 1 - d));
-      }
-      if (d == kBrickDepth) bricks += 1;
-    }
-  }
-  if (j <= n) nb[j] = bricks;
-  for (int k = 0; k < 4; ++k) {
-    const unsigned long long t = Reduce(tmp).Sum(v[k]);
-    if (threadIdx.x == 0 && t) atomicAdd(k == 0 ? &cnt->nodes : k == 1 ? &cnt->free_leaves : k == 2 ? &cnt->occ_leaves
-                                                                                                     : &cnt->known, t);
-    __syncthreads();
-  }
-}
-
-// (r5) per new brick, in pre-order: its key and state (1 free, 2 occupied: under a leaf at depth <= 13; 3: below an inner
-// node at depth 13).  Its inner node is the last j with boff[j] <= b; a leaf's bricks are in Morton order.
-__global__ void rd_brick_kernel(const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
-                                const unsigned long long* __restrict__ key, const long long* __restrict__ boff, int end,
-                                int n_b, unsigned long long* __restrict__ bkey, unsigned char* __restrict__ bst) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= n_b) return;
-  int lo = 0, hi = end - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (boff[mid] <= b) lo = mid;
-    else hi = mid - 1;
-  }
-  const int j = lo, d = depth[j];
-  const unsigned long long k0 = key[j];
-  int kx = (int)(k0 & 0xffff), ky = (int)((k0 >> 16) & 0xffff), kz = (int)((k0 >> 32) & 0xffff), st = 3;
-  if (d != kBrickDepth) {
-    const int m = pair_mask(pay, j), sh = 15 - d;
-    long long r = b - boff[j];
-    for (int s = 0; s < 8; ++s) {
-      const int bits = (m >> (2 * s)) & 3;
-      if (bits == 0 || bits == 3) continue;
-      const long long c = 1LL << (3 * (kBrickDepth - 1 - d));
-      if (r >= c) {
-        r -= c;
-        continue;
-      }
-      st = bits;
-      kx += ((s & 1) << sh) + (squeeze3((unsigned long long)r) << 3);
-      ky += (((s >> 1) & 1) << sh) + (squeeze3((unsigned long long)r >> 1) << 3);
-      kz += (((s >> 2) & 1) << sh) + (squeeze3((unsigned long long)r >> 2) << 3);
-      break;
-    }
-  }
-  const int k[3] = {kx, ky, kz};
-  bkey[b] = brick_key(k);
-  bst[b] = (unsigned char)st;
-}
-
-// (r6) one block of 512 threads per new brick: a uniform brick holds L_min or L_max and is all known, a mixed one starts
-// empty; marks and touched flags clear
-__global__ void __launch_bounds__(512) rd_fill_kernel(Dev D, Params P, const unsigned long long* __restrict__ bkey,
-                                                      const unsigned char* __restrict__ bst) {
-  const int b = blockIdx.x, t = threadIdx.x, st = bst[b];
-  D.lo[(size_t)b * 512 + t] = st == 1 ? P.l_min : st == 2 ? P.l_max : 0.0f;
-  if (t < 16) {
-    D.known[(size_t)b * 16 + t] = st == 3 ? 0u : ~0u;
-    D.mfree[(size_t)b * 16 + t] = 0u;
-    D.mocc[(size_t)b * 16 + t] = 0u;
-  }
-  if (t == 0) D.touched[b] = 0u, D.bkey[b] = bkey[b];
-}
-
-// (r7) per inner node at depth 13 ... 15: the 64, 8 or 1 voxels of each of its leaves, in its depth-13 ancestor's brick
-__global__ void rd_leaf_kernel(Dev D, Params P, const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
-                               const unsigned long long* __restrict__ key, const int* __restrict__ anc,
-                               const long long* __restrict__ boff, int end) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= end) return;
-  const int d = depth[j];
-  if (d < kBrickDepth) return;
-  const size_t b = (size_t)boff[anc[j]];
-  const unsigned long long k0 = key[j];
-  const int m = pair_mask(pay, j), sh = 15 - d, side = 1 << sh;
-  for (int s = 0; s < 8; ++s) {
-    const int bits = (m >> (2 * s)) & 3;
-    if (bits == 0 || bits == 3) continue;
-    const float v = bits == 1 ? P.l_min : P.l_max;
-    const int x0 = ((int)(k0 & 7)) | ((s & 1) << sh), y0 = ((int)((k0 >> 16) & 7)) | (((s >> 1) & 1) << sh),
-              z0 = ((int)((k0 >> 32) & 7)) | (((s >> 2) & 1) << sh);
-    for (int z = z0; z < z0 + side; ++z)
-      for (int y = y0; y < y0 + side; ++y) {
-        unsigned bitsw = 0;
-        const int row = (y << 3) | (z << 6);  // side <= 4 voxels of one row share a known word
-        for (int x = x0; x < x0 + side; ++x) {
-          D.lo[b * 512 + row + x] = v;
-          bitsw |= 1u << ((row + x) & 31);
-        }
-        atomicOr(&D.known[b * 16 + (row >> 5)], bitsw);
-      }
-  }
-}
-
-// ---- full tree read (octomap's AbstractOcTree::read / readData; DESIGN.md §4b''''''') -----------------------------
-// Node i of the payload is 5 bytes: its float value, then the mask of its existing children.  Every node is in the
-// stream, so with c_i = popcount(mask_i) the excess E_0 = 1, E_{i+1} = E_i + c_i - 1 counts the nodes found but not yet
-// read, and the tree ends at the first i >= 1 with E_i = 0.
-constexpr int kMaxFullExcess = 8 + 7 * 15;  // the largest excess of a tree whose nodes lie at depth <= 16
-constexpr int kBadValue = 2;
-
-__device__ __forceinline__ int full_mask(const unsigned char* pay, int i) { return pay[(size_t)kFullNodeBytes * i + 4]; }
-__device__ __forceinline__ unsigned full_value(const unsigned char* pay, int i) {
-  const unsigned char* p = pay + (size_t)kFullNodeBytes * i;
-  return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
-}
-
-// (s1) in[0] = 1 and in[i + 1] = c_i - 1: an inclusive sum gives E_0 ... E_n
-__global__ void fr_excess_kernel(const unsigned char* __restrict__ pay, int n, int* __restrict__ in) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i == 0) in[0] = 1;
-  if (i < n) in[i + 1] = __popc(full_mask(pay, i)) - 1;
-}
-
-// (s3) per node j >= 1 of the tree: its parent, the last i < j with E_i <= E_j, and its slot, the (E_p + c_p - 1 - E_j)-th
-// set bit of p's mask.  An excess above kMaxFullExcess proves a node below depth 16.
-__global__ void fr_parent_kernel(const unsigned char* __restrict__ pay, const int* __restrict__ ex,
-                                 const int* __restrict__ bmin, int n, int* __restrict__ par, unsigned char* __restrict__ slot,
-                                 ReadCounters* cnt) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n || j >= cnt->end) return;
-  const int e = ex[j];
-  if (e > kMaxFullExcess) {
-    atomicOr(&cnt->bad, kBadDepth);
-    return;
-  }
-  if (j == 0) {
-    par[0] = -1, slot[0] = 0;
-    return;
-  }
-  const int b0 = j / kReadThreads * kReadThreads;
-  int p = j - 1;
-  while (p >= b0 && ex[p] > e) --p;
-  if (p < b0) {  // E_0 = 1 <= e: some earlier block holds the parent
-    int b = j / kReadThreads - 1;
-    while (bmin[b] > e) --b;
-    p = b * kReadThreads + kReadThreads - 1;
-    while (ex[p] > e) --p;
-  }
-  const int m = full_mask(pay, p);
+  const int m = F::streamed(pay, p);
   int rank = ex[p] + __popc(m) - 1 - e, s = 0;
   for (; s < 8; ++s)
     if (((m >> s) & 1) && rank-- == 0) break;
@@ -1374,10 +1334,10 @@ __global__ void fr_parent_kernel(const unsigned char* __restrict__ pay, const in
   slot[j] = (unsigned char)s;
 }
 
-// (s4) per node j of the tree: depth and first key from at most 16 parents (more, or children at depth 16: too deep), its
-// depth-13 ancestor, and the counts: nodes with children, leaves by state, known voxels 8^(16-d) and bricks 8^(13-d) per
-// leaf at depth d (d <= 13), one brick for a node with children at depth 13.  A leaf's value must be finite.
-__global__ void __launch_bounds__(kReadThreads) fr_node_kernel(const unsigned char* __restrict__ pay,
+// (r4) per stream node j: depth and first key from at most F::kMaxDepth parents (more: too deep), its depth-13 ancestor,
+// and the format's counts.  nb[j] = its bricks (0 past the tree, nb[n] = 0).
+template <class F>
+__global__ void __launch_bounds__(kReadThreads) rd_node_kernel(const unsigned char* __restrict__ pay,
                                                               const int* __restrict__ par,
                                                               const unsigned char* __restrict__ slot, int n, float l_occ,
                                                               unsigned char* __restrict__ depth,
@@ -1386,12 +1346,13 @@ __global__ void __launch_bounds__(kReadThreads) fr_node_kernel(const unsigned ch
   using Reduce = cub::BlockReduce<unsigned long long, kReadThreads>;
   __shared__ typename Reduce::TempStorage tmp;
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  unsigned long long v[4] = {0, 0, 0, 0};  // nodes with children, free leaves, occupied leaves, known voxels
+  unsigned long long v[4] = {0, 0, 0, 0};  // F::node_count, free leaves, occupied leaves, known voxels
   long long bricks = 0;
   if (j < n && j < cnt->end && !cnt->bad) {
+    // step i visits the ancestor at depth d - i: its slot is key bit 16 - d + i; the depth-13 one is among steps 0 ... 3
     int d = 0, x = j, a1 = j, a2 = j, a3 = j;
     unsigned long long slots = 0;
-    while (x != 0 && d < 16) {
+    while (x != 0 && d < F::kMaxDepth) {
       if (d == 1) a1 = x;
       if (d == 2) a2 = x;
       if (d == 3) a3 = x;
@@ -1399,12 +1360,9 @@ __global__ void __launch_bounds__(kReadThreads) fr_node_kernel(const unsigned ch
       ++d;
       x = par[x];
     }
-    const int m = full_mask(pay, j);
-    const float val = __uint_as_float(full_value(pay, j));
-    if (x != 0 || (d == 16 && m)) {
-      atomicOr(&cnt->bad, kBadDepth);
-    } else if (!m && !isfinite(val)) {
-      atomicOr(&cnt->bad, kBadValue);
+    const int bad = x != 0 ? kBadDepth : F::count(pay, j, d, l_occ, v, bricks);
+    if (bad) {
+      atomicOr(&cnt->bad, bad);
     } else {
       unsigned kx = 0, ky = 0, kz = 0;
       for (int i = 0; i < d; ++i) {
@@ -1414,62 +1372,42 @@ __global__ void __launch_bounds__(kReadThreads) fr_node_kernel(const unsigned ch
       depth[j] = (unsigned char)d;
       key[j] = pack((int)kx, (int)ky, (int)kz);
       anc[j] = d == kBrickDepth ? j : d == kBrickDepth + 1 ? a1 : d == kBrickDepth + 2 ? a2 : d == kBrickDepth + 3 ? a3 : -1;
-      if (m) {
-        v[0] = 1;
-        if (d == kBrickDepth) bricks = 1;
-      } else {
-        ++v[val >= l_occ ? 2 : 1];
-        v[3] = 1ull << (3 * (16 - d));
-        if (d <= kBrickDepth) bricks = 1LL << (3 * (kBrickDepth - d));
-      }
     }
   }
   if (j <= n) nb[j] = bricks;
   for (int k = 0; k < 4; ++k) {
     const unsigned long long t = Reduce(tmp).Sum(v[k]);
-    if (threadIdx.x == 0 && t) atomicAdd(k == 0 ? &cnt->inner : k == 1 ? &cnt->free_leaves : k == 2 ? &cnt->occ_leaves
-                                                                                                     : &cnt->known, t);
+    if (threadIdx.x == 0 && t) atomicAdd(k == 0 ? F::node_count(cnt) : k == 1 ? &cnt->free_leaves : k == 2 ? &cnt->occ_leaves
+                                                                                                       : &cnt->known, t);
     __syncthreads();
   }
 }
 
-// The node whose bricks hold brick b: the last j < end with boff[j] <= b (a node without bricks has the next one's boff).
-__device__ __forceinline__ int brick_owner(const long long* __restrict__ boff, int end, long long b) {
-  int lo = 0, hi = end - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (boff[mid] <= b) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
-}
-
-// (s5) per new brick, in pre-order: its key and state (1: under a leaf at depth <= 13, in Morton order; 3: below a node
-// with children at depth 13)
-__global__ void fr_brick_kernel(const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
+// (r5) per new brick, in pre-order: its key and state (1 free, 2 occupied: uniform; 3: below a node with children at depth
+// 13), from the stream node whose bricks hold it
+template <class F>
+__global__ void rd_brick_kernel(const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
                                 const unsigned long long* __restrict__ key, const long long* __restrict__ boff, int end,
                                 int n_b, unsigned long long* __restrict__ bkey, unsigned char* __restrict__ bst) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= n_b) return;
   const int j = brick_owner(boff, end, b);
-  const unsigned long long k0 = key[j], r = (unsigned long long)(b - boff[j]);
-  const bool mixed = depth[j] == kBrickDepth && full_mask(pay, j) != 0;
-  const int k[3] = {(int)(k0 & 0xffff) + (mixed ? 0 : squeeze3(r) << 3),
-                    (int)((k0 >> 16) & 0xffff) + (mixed ? 0 : squeeze3(r >> 1) << 3),
-                    (int)((k0 >> 32) & 0xffff) + (mixed ? 0 : squeeze3(r >> 2) << 3)};
+  int k[3];
+  const int st = F::brick(pay, j, depth[j], key[j], b - boff[j], k);
   bkey[b] = brick_key(k);
-  bst[b] = (unsigned char)(mixed ? 3 : 1);
+  bst[b] = (unsigned char)st;
 }
 
-// (s6) one block of 512 threads per new brick: a uniform brick holds its leaf's value and is all known, a mixed one starts
-// empty; marks and touched flags clear
-__global__ void __launch_bounds__(512) fr_fill_kernel(Dev D, const unsigned char* __restrict__ pay,
+// (r6) one block of 512 threads per new brick: a uniform brick holds the format's value and is all known, a mixed one
+// starts empty; marks and touched flags clear
+template <class F>
+__global__ void __launch_bounds__(512) rd_fill_kernel(Dev D, Params P, const unsigned char* __restrict__ pay,
                                                       const long long* __restrict__ boff, int end,
                                                       const unsigned long long* __restrict__ bkey,
                                                       const unsigned char* __restrict__ bst) {
   __shared__ float v;
   const int b = blockIdx.x, t = threadIdx.x, st = bst[b];
-  if (t == 0) v = st == 1 ? __uint_as_float(full_value(pay, brick_owner(boff, end, b))) : 0.0f;
+  if (t == 0) v = F::uniform(P, pay, boff, end, b, st);
   __syncthreads();
   D.lo[(size_t)b * 512 + t] = v;
   if (t < 16) {
@@ -1480,29 +1418,17 @@ __global__ void __launch_bounds__(512) fr_fill_kernel(Dev D, const unsigned char
   if (t == 0) D.touched[b] = 0u, D.bkey[b] = bkey[b];
 }
 
-// (s7) per leaf at depth 14 ... 16: its 64, 8 or 1 voxels with its own value, in its depth-13 ancestor's brick
-__global__ void fr_leaf_kernel(Dev D, const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
+// (r7) per stream node: the voxels of the leaves below depth 13 it writes, each in its depth-13 ancestor's brick
+template <class F>
+__global__ void rd_leaf_kernel(Dev D, Params P, const unsigned char* __restrict__ pay, const unsigned char* __restrict__ depth,
                                const unsigned long long* __restrict__ key, const int* __restrict__ anc,
                                const long long* __restrict__ boff, int end) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= end) return;
   const int d = depth[j];
-  if (d <= kBrickDepth || full_mask(pay, j)) return;
+  if (!F::writes_leaves(pay, j, d)) return;
   const size_t b = (size_t)boff[anc[j]];
-  const float v = __uint_as_float(full_value(pay, j));
-  const unsigned long long k0 = key[j];
-  const int side = 1 << (16 - d);
-  const int x0 = (int)(k0 & 7), y0 = (int)((k0 >> 16) & 7), z0 = (int)((k0 >> 32) & 7);
-  for (int z = z0; z < z0 + side; ++z)
-    for (int y = y0; y < y0 + side; ++y) {
-      unsigned bitsw = 0;
-      const int row = (y << 3) | (z << 6);  // side <= 4 voxels of one row share a known word
-      for (int x = x0; x < x0 + side; ++x) {
-        D.lo[b * 512 + row + x] = v;
-        bitsw |= 1u << ((row + x) & 31);
-      }
-      atomicOr(&D.known[b * 16 + (row >> 5)], bitsw);
-    }
+  F::leaves(P, pay, j, d, key[j], [&](int x0, int y0, int z0, int side, float v) { fill_cube(D, b, x0, y0, z0, side, v); });
 }
 
 // ---- edits (volumetric_mapping's setLogOddsBoundingBox, resetMap, getOccupiedPointcloudInBoundingBox and the map's
@@ -1723,7 +1649,7 @@ int rebuild_table(Map& m, int cap, cudaStream_t st, uint64_t* launches) {
   return LS_OK;
 }
 
-// The read's per-pair scratch for n pairs of `bytes` payload bytes, grown all or nothing.
+// The read's per-record scratch for n stream records of `bytes` payload bytes, grown all or nothing.
 int reserve_read(Map& m, int n, size_t bytes, cudaStream_t st) {
   OCC_TRY(m.rd_cnt_dev.reserve(1, 1));
   OCC_TRY(m.rd_cnt_host.reserve(1, 1));
@@ -1809,8 +1735,8 @@ int select(Map& m, const Params& P, int which, unsigned long long* keys, unsigne
 }
 
 Nodes nodes_of(const Octree& t) {
-  return Nodes{t.code.get(), t.pool.get(), t.first.get(), t.end.get(), t.st.get(),
-               t.n_nodes.get(), t.n_bytes.get(), t.n_leaves.get(), t.off.get(), t.loff.get()};
+  return Nodes{t.code.get(), t.pool.get(), t.first.get(), t.end.get(), t.st.get(), t.val.get(),
+               {t.n_nodes.get(), t.n_leaves.get(), t.n_bytes.get()}, t.off.get(), t.loff.get()};
 }
 
 // Records for n_b bricks and every upper node they can have: at most min(n_b, 8^d) at depth d.
@@ -1974,39 +1900,6 @@ int download(Map& m, const Params& P, int which, long long n, uint64_t* keys, fl
   return LS_OK;
 }
 
-int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches) {
-  t.nodes = t.bytes = t.leaves = 0;
-  const int n_b = m.pool_n;
-  if (n_b == 0) return LS_OK;
-  int rc;
-  if ((rc = reserve_tree(t, n_b, st))) return rc;
-  const Nodes N = nodes_of(t);
-  oct_code_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.bkey.get(), n_b, t.sort_k.get(), t.sort_v.get());
-  OCC_LAUNCHED();
-  size_t bytes = t.cub_bytes;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp.get(), bytes, t.sort_k.get(), t.code.get(), t.sort_v.get(), t.pool.get(), n_b,
-                                          0, 3 * kBrickDepth, st));
-  ++*launches;
-  oct_brick_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, P.l_occ);
-  OCC_LAUNCHED();
-  oct_up_kernel<<<1, kTreeThreads, 0, st>>>(N, n_b, t.levels.get(), t.tot_dev.get());
-  OCC_LAUNCHED();
-  OCC_TRY(cudaMemcpyAsync(t.tot_host.get(), t.tot_dev.get(), 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  OCC_TRY(cudaStreamSynchronize(st));
-  const unsigned long long* tot = t.tot_host.get();
-  const long long nodes = (long long)tot[0], pay = (long long)tot[1], leaves = (long long)tot[2];
-  if (nodes == 0) return LS_OK;
-  if ((rc = reserve_tree_outputs(t, pay, leaves, st))) return rc;
-  oct_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), P.res, t.payload.get(), t.centres.get(), t.depths.get());
-  OCC_LAUNCHED();
-  oct_emit_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, P.res, t.payload.get(),
-                                       t.centres.get(), t.depths.get());
-  OCC_LAUNCHED();
-  OCC_TRY(cudaStreamSynchronize(st));
-  t.nodes = nodes, t.bytes = pay, t.leaves = leaves;
-  return LS_OK;
-}
-
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st) {
   if (t.bytes > 0 && payload) OCC_TRY(cudaMemcpyAsync(payload, t.payload.get(), (size_t)t.bytes, cudaMemcpyDeviceToHost, st));
   if (t.leaves > 0 && centres4)
@@ -2061,83 +1954,14 @@ int replace_map(Map& m, int n_b, long long known, const std::function<int()>& ke
   return LS_OK;
 }
 
-}  // namespace
-
-int read_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes, ReadCounters* out,
-                const char** why, cudaStream_t st, uint64_t* launches) {
-  std::memset(out, 0, sizeof(ReadCounters));
-  *why = "";
-  int rc, n_b = 0, end = 0;
-  // A valid tree has at most `nodes` inner nodes, so later pairs cannot belong to it.
-  const long long pairs = nodes > 0 ? std::min(bytes / 2, nodes) : 0;
-  if (nodes > 0 && pairs == 0) return *why = "the payload is truncated", LS_ERR_ARG;
-  if (pairs > kMaxReadPairs) return *why = "more than 2^30 inner nodes", LS_ERR_NOMEM;
-  if (pairs > 0) {
-    const int n = (int)pairs;
-    if ((rc = reserve_read(m, n, 2 * (size_t)n, st))) return *why = "out of device memory for the parse", rc;
-    ReadCounters* cnt = m.rd_cnt_dev.get();
-    ReadCounters init{};
-    init.end = INT_MAX;
-    *m.rd_cnt_host.get() = init;
-    OCC_TRY(cudaMemcpyAsync(cnt, m.rd_cnt_host.get(), sizeof(ReadCounters), cudaMemcpyHostToDevice, st));
-    OCC_TRY(cudaMemcpyAsync(m.rd_pay.get(), payload, 2 * (size_t)n, cudaMemcpyHostToDevice, st));
-    const int blocks = (n + kReadThreads) / kReadThreads;  // n + 1 items
-    rd_excess_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), n, m.rd_tmp.get());
-    OCC_LAUNCHED();
-    size_t tb = m.rd_cub_bytes;
-    OCC_TRY(cub::DeviceScan::InclusiveSum(m.rd_cub.get(), tb, m.rd_tmp.get(), m.rd_ex.get(), n + 1, st));
-    ++*launches;
-    rd_end_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_ex.get(), n, m.rd_bmin.get(), cnt);
-    OCC_LAUNCHED();
-    rd_parent_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_ex.get(), m.rd_bmin.get(), n, m.rd_par.get(),
-                                                      m.rd_slot.get(), cnt);
-    OCC_LAUNCHED();
-    rd_node_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_par.get(), m.rd_slot.get(), n, m.rd_depth.get(),
-                                                    m.rd_key.get(), m.rd_anc.get(), m.rd_nb.get(), cnt);
-    OCC_LAUNCHED();
-    tb = m.rd_cub_bytes;
-    OCC_TRY(cub::DeviceScan::ExclusiveSum(m.rd_cub.get(), tb, m.rd_nb.get(), m.rd_boff.get(), n + 1, st));
-    ++*launches;
-    OCC_TRY(cudaMemcpyAsync(&cnt->bricks, m.rd_boff.get() + n, sizeof(long long), cudaMemcpyDeviceToDevice, st));
-    OCC_TRY(cudaMemcpyAsync(m.rd_cnt_host.get(), cnt, sizeof(ReadCounters), cudaMemcpyDeviceToHost, st));
-    OCC_TRY(cudaStreamSynchronize(st));
-    const ReadCounters c = *m.rd_cnt_host.get();
-    if (c.end == INT_MAX) return *why = "the payload is truncated", LS_ERR_ARG;
-    if (c.bad) return *why = "an inner node at depth 16", LS_ERR_ARG;
-    if ((long long)c.nodes + 1 != nodes) return *why = "the header's size does not count the payload's nodes", LS_ERR_ARG;
-    if (c.bricks > kMaxReadBricks) return *why = "the file covers more bricks than the map can index", LS_ERR_NOMEM;
-    *out = c;
-    out->nodes = c.nodes + 1;
-    out->inner = (unsigned long long)c.end;
-    end = c.end;
-    n_b = (int)c.bricks;
-  }
-  return replace_map(
-      m, n_b, (long long)out->known,
-      [&]() -> int {
-        rd_brick_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_boff.get(),
-                                                           end, n_b, m.rd_bkey.get(), m.rd_bst.get());
-        OCC_LAUNCHED();
-        return LS_OK;
-      },
-      [&](const Dev& D) -> int {
-        rd_fill_kernel<<<n_b, 512, 0, st>>>(D, P, m.rd_bkey.get(), m.rd_bst.get());
-        OCC_LAUNCHED();
-        rd_leaf_kernel<<<(end + 255) / 256, 256, 0, st>>>(D, P, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(),
-                                                          m.rd_anc.get(), m.rd_boff.get(), end);
-        OCC_LAUNCHED();
-        return LS_OK;
-      },
-      why, st, launches);
-}
-
-int build_full_octree(const Map& m, Octree& t, cudaStream_t st, uint64_t* launches) {
+template <class F>
+int build_tree_as(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches) {
   t.nodes = t.bytes = t.leaves = 0;
   const int n_b = m.pool_n;
   if (n_b == 0) return LS_OK;
   int rc;
   if ((rc = reserve_tree(t, n_b, st))) return rc;
-  if (t.val.capacity() < t.code.capacity()) {
+  if (F::kValued && t.val.capacity() < t.code.capacity()) {
     OCC_TRY(cudaStreamSynchronize(st));
     t.val.reset();
     OCC_TRY(t.val.reserve(t.code.capacity(), t.code.capacity()));
@@ -2149,56 +1973,60 @@ int build_full_octree(const Map& m, Octree& t, cudaStream_t st, uint64_t* launch
   OCC_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp.get(), bytes, t.sort_k.get(), t.code.get(), t.sort_v.get(), t.pool.get(), n_b,
                                           0, 3 * kBrickDepth, st));
   ++*launches;
-  ful_brick_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, t.val.get());
+  oct_brick_kernel<F><<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, P.l_occ);
   OCC_LAUNCHED();
-  ful_up_kernel<<<1, kTreeThreads, 0, st>>>(N, t.val.get(), n_b, t.levels.get(), t.tot_dev.get());
+  oct_up_kernel<F><<<1, kTreeThreads, 0, st>>>(N, n_b, t.levels.get(), t.tot_dev.get());
   OCC_LAUNCHED();
-  OCC_TRY(cudaMemcpyAsync(t.tot_host.get(), t.tot_dev.get(), 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  OCC_TRY(cudaMemcpyAsync(t.tot_host.get(), t.tot_dev.get(), F::kTotals * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                          st));
   OCC_TRY(cudaStreamSynchronize(st));
-  const long long nodes = (long long)t.tot_host.get()[0], leaves = (long long)t.tot_host.get()[1];
+  const unsigned long long* tot = t.tot_host.get();
+  const long long nodes = (long long)tot[0], leaves = (long long)tot[1], pay = F::payload_bytes(tot);
   if (nodes == 0) return LS_OK;
-  const long long pay = kFullNodeBytes * nodes;
-  if ((rc = reserve_tree_outputs(t, pay, 0, st))) return rc;
-  ful_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.val.get(), t.levels.get(), t.payload.get());
+  if ((rc = reserve_tree_outputs(t, pay, F::kCentres ? leaves : 0, st))) return rc;
+  oct_down_kernel<F><<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), P.res, t.payload.get(), t.centres.get(), t.depths.get());
   OCC_LAUNCHED();
-  ful_emit_kernel<<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, t.payload.get());
+  oct_emit_kernel<F><<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, P.res, t.payload.get(),
+                                          t.centres.get(), t.depths.get());
   OCC_LAUNCHED();
   OCC_TRY(cudaStreamSynchronize(st));
   t.nodes = nodes, t.bytes = pay, t.leaves = leaves;
   return LS_OK;
 }
 
-int read_full_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes,
-                     ReadCounters* out, const char** why, cudaStream_t st, uint64_t* launches) {
+template <class F>
+int read_tree_as(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes, ReadCounters* out,
+                 const char** why, cudaStream_t st, uint64_t* launches) {
   std::memset(out, 0, sizeof(ReadCounters));
   *why = "";
   int rc, n_b = 0, end = 0;
-  // A valid tree has `nodes` nodes, so later bytes cannot belong to it.
-  const long long count = std::min(bytes / kFullNodeBytes, nodes);
+  // A valid tree has at most `nodes` stream nodes, so later records cannot belong to it.
+  const long long count = nodes > 0 ? std::min(bytes / F::kNodeBytes, nodes) : 0;
   if (nodes > 0 && count == 0) return *why = "the payload is truncated", LS_ERR_ARG;
-  if (count > kMaxReadPairs) return *why = "more than 2^30 nodes", LS_ERR_NOMEM;
+  if (count > kMaxReadPairs) return *why = F::kTooMany, LS_ERR_NOMEM;
   if (count > 0) {
     const int n = (int)count;
-    if ((rc = reserve_read(m, n, kFullNodeBytes * (size_t)n, st))) return *why = "out of device memory for the parse", rc;
+    const size_t pay = (size_t)F::kNodeBytes * n;
+    if ((rc = reserve_read(m, n, pay, st))) return *why = "out of device memory for the parse", rc;
     ReadCounters* cnt = m.rd_cnt_dev.get();
     ReadCounters init{};
     init.end = INT_MAX;
     *m.rd_cnt_host.get() = init;
     OCC_TRY(cudaMemcpyAsync(cnt, m.rd_cnt_host.get(), sizeof(ReadCounters), cudaMemcpyHostToDevice, st));
-    OCC_TRY(cudaMemcpyAsync(m.rd_pay.get(), payload, kFullNodeBytes * (size_t)n, cudaMemcpyHostToDevice, st));
+    OCC_TRY(cudaMemcpyAsync(m.rd_pay.get(), payload, pay, cudaMemcpyHostToDevice, st));
     const int blocks = (n + kReadThreads) / kReadThreads;  // n + 1 items
-    fr_excess_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), n, m.rd_tmp.get());
+    rd_excess_kernel<F><<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), n, m.rd_tmp.get());
     OCC_LAUNCHED();
     size_t tb = m.rd_cub_bytes;
     OCC_TRY(cub::DeviceScan::InclusiveSum(m.rd_cub.get(), tb, m.rd_tmp.get(), m.rd_ex.get(), n + 1, st));
     ++*launches;
     rd_end_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_ex.get(), n, m.rd_bmin.get(), cnt);
     OCC_LAUNCHED();
-    fr_parent_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_ex.get(), m.rd_bmin.get(), n, m.rd_par.get(),
-                                                      m.rd_slot.get(), cnt);
+    rd_parent_kernel<F><<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_ex.get(), m.rd_bmin.get(), n, m.rd_par.get(),
+                                                         m.rd_slot.get(), cnt);
     OCC_LAUNCHED();
-    fr_node_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_par.get(), m.rd_slot.get(), n, P.l_occ,
-                                                    m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(), m.rd_nb.get(), cnt);
+    rd_node_kernel<F><<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_par.get(), m.rd_slot.get(), n, P.l_occ,
+                                                       m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(), m.rd_nb.get(), cnt);
     OCC_LAUNCHED();
     tb = m.rd_cub_bytes;
     OCC_TRY(cub::DeviceScan::ExclusiveSum(m.rd_cub.get(), tb, m.rd_nb.get(), m.rd_boff.get(), n + 1, st));
@@ -2207,35 +2035,42 @@ int read_full_octree(Map& m, const Params& P, const unsigned char* payload, long
     OCC_TRY(cudaMemcpyAsync(m.rd_cnt_host.get(), cnt, sizeof(ReadCounters), cudaMemcpyDeviceToHost, st));
     OCC_TRY(cudaStreamSynchronize(st));
     const ReadCounters c = *m.rd_cnt_host.get();
-    if (c.end == INT_MAX)
-      return *why = count < nodes ? "the payload is truncated" : "the header's size does not count the payload's nodes",
-             LS_ERR_ARG;
-    if (c.bad & kBadDepth) return *why = "a node at depth 16 with children", LS_ERR_ARG;
-    if (c.bad & kBadValue) return *why = "a leaf value that is NaN or infinite", LS_ERR_ARG;
-    if ((long long)c.end != nodes) return *why = "the header's size does not count the payload's nodes", LS_ERR_ARG;
+    if ((rc = F::check(c, count, nodes, why))) return rc;
     if (c.bricks > kMaxReadBricks) return *why = "the file covers more bricks than the map can index", LS_ERR_NOMEM;
     *out = c;
-    out->nodes = (unsigned long long)c.end;
+    F::counts(out);
     end = c.end;
     n_b = (int)c.bricks;
   }
   return replace_map(
       m, n_b, (long long)out->known,
       [&]() -> int {
-        fr_brick_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_boff.get(),
-                                                           end, n_b, m.rd_bkey.get(), m.rd_bst.get());
+        rd_brick_kernel<F><<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(),
+                                                              m.rd_boff.get(), end, n_b, m.rd_bkey.get(), m.rd_bst.get());
         OCC_LAUNCHED();
         return LS_OK;
       },
       [&](const Dev& D) -> int {
-        fr_fill_kernel<<<n_b, 512, 0, st>>>(D, m.rd_pay.get(), m.rd_boff.get(), end, m.rd_bkey.get(), m.rd_bst.get());
+        rd_fill_kernel<F><<<n_b, 512, 0, st>>>(D, P, m.rd_pay.get(), m.rd_boff.get(), end, m.rd_bkey.get(), m.rd_bst.get());
         OCC_LAUNCHED();
-        fr_leaf_kernel<<<(end + 255) / 256, 256, 0, st>>>(D, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(),
-                                                          m.rd_boff.get(), end);
+        rd_leaf_kernel<F><<<(end + 255) / 256, 256, 0, st>>>(D, P, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(),
+                                                             m.rd_anc.get(), m.rd_boff.get(), end);
         OCC_LAUNCHED();
         return LS_OK;
       },
       why, st, launches);
+}
+
+}  // namespace
+
+int build_tree(const Map& m, const Params& P, TreeFormat f, Octree& t, cudaStream_t st, uint64_t* launches) {
+  return f == TreeFormat::Full ? build_tree_as<FullTree>(m, P, t, st, launches) : build_tree_as<BinaryTree>(m, P, t, st, launches);
+}
+
+int read_tree(Map& m, const Params& P, TreeFormat f, const unsigned char* payload, long long bytes, long long nodes,
+              ReadCounters* out, const char** why, cudaStream_t st, uint64_t* launches) {
+  return f == TreeFormat::Full ? read_tree_as<FullTree>(m, P, payload, bytes, nodes, out, why, st, launches)
+                               : read_tree_as<BinaryTree>(m, P, payload, bytes, nodes, out, why, st, launches);
 }
 
 namespace {

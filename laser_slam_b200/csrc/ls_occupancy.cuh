@@ -22,7 +22,7 @@ struct Counters {
   int pool_n, n_touched, overflow, rays_cast, rays_skipped, pad[3];
 };
 
-// Device counters of one .bt read, copied back once after the parse: the node counts, the pair after the tree (INT_MAX
+// Device counters of one tree read, copied back once after the parse: the node counts, the record after the tree (INT_MAX
 // while none is found), the known voxels and bricks the file covers, and why it is malformed (0 when it is not).
 struct ReadCounters {
   unsigned long long nodes, inner, free_leaves, occ_leaves, known;
@@ -56,7 +56,7 @@ struct Map {
   size_t cub_bytes = 0;
   // query staging (inputs and outputs of one call), grown by doubling
   ls::Buffer<char> qbuf;
-  // .bt read scratch: per payload pair (the excess, parent, depth, first key, bricks) and per new brick (key, state)
+  // tree read scratch: per stream record (the excess, parent, depth, first key, bricks) and per new brick (key, state)
   ls::Buffer<unsigned char> rd_pay;
   ls::Buffer<int> rd_ex, rd_tmp, rd_par, rd_anc, rd_bmin;
   ls::Buffer<unsigned char> rd_slot, rd_depth;
@@ -138,7 +138,7 @@ struct Octree {
   ls::Buffer<int> first, end;           // upper nodes: their children's records [first, end)
   ls::Buffer<unsigned char> st;         // 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner (full tree: 1 leaf)
   ls::Buffer<unsigned> val;             // full tree only: each node's float log-odds bits
-  ls::Buffer<unsigned long long> n_nodes, n_bytes, n_leaves;  // subtree totals
+  ls::Buffer<unsigned long long> n_nodes, n_bytes, n_leaves;  // subtree totals: nodes, payload bytes (.bt only), leaves
   ls::Buffer<unsigned long long> off, loff;  // payload byte and occupied-leaf offsets in pre-order
   ls::Buffer<unsigned long long> sort_k;
   ls::Buffer<int> sort_v;
@@ -164,30 +164,25 @@ int count(Map& m, const Params& P, int which, long long* n, cudaStream_t st, uin
 int download(Map& m, const Params& P, int which, long long n, uint64_t* keys, float* log_odds, float* centres4, cudaStream_t st,
              uint64_t* launches);
 size_t device_bytes(const Map& m);
-// Builds the pruned tree of the map's max-likelihood states (oracle/OCTREE.md) into t: payload and occupied leaves stay
-// on the device, t.nodes / bytes / leaves hold the counts.  Reads the map only.  Synchronous.
-int build_octree(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches);
+// octomap's two tree payloads: the pruned max-likelihood tree of writeBinary (.bt, oracle/OCTREE.md) and the
+// full-probability tree of OcTree::write (.ot, DESIGN.md §4b''''''': every node's float log-odds and child mask, 5 bytes
+// per node in pre-order, pruned by value).
+enum class TreeFormat { Binary, Full };
+// Builds the map's tree in format f into t: the payload (and, for .bt, the occupied leaves' centres and depths) stays on
+// the device, t.nodes / bytes / leaves hold the counts (leaves: occupied ones for .bt, every leaf for .ot).  Reads the map
+// only.  Synchronous.
+int build_tree(const Map& m, const Params& P, TreeFormat f, Octree& t, cudaStream_t st, uint64_t* launches);
 // Copies the last build's payload (t.bytes) and, each when not NULL, its t.leaves centres {x, y, z, 1} and depths.
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st);
-// Builds octomap's full tree of the map (OcTree::write's payload, DESIGN.md §4b') into t: every node's float log-odds
-// and child mask, 5 bytes per node in pre-order, pruned by value.  t.nodes / bytes / leaves hold the counts; the payload
-// stays on the device (download_octree copies it).  Reads the map only.  Synchronous.
-int build_full_octree(const Map& m, Octree& t, cudaStream_t st, uint64_t* launches);
 
-// octomap's readBinary of a .bt payload (`bytes` bytes after "data\n", `nodes` the header's size) into the map, replacing
-// it (DESIGN.md §4b'''''').  P: the map's parameters at the file's resolution.  Synchronous.  Validates the
-// whole stream and the brick count before it grows or writes anything: LS_ERR_ARG for a malformed payload, LS_ERR_NOMEM
-// for more bricks than the map can index or a failed growth, and the map is unchanged after any error (*why then says
-// why).  *out: the counts.
-int read_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes, ReadCounters* out,
-                const char** why, cudaStream_t st, uint64_t* launches);
-
-// octomap's readData of a full-tree payload (`bytes` bytes after "data\n", `nodes` the header's size) into the map,
-// replacing it: every leaf's voxels take its value verbatim.  P: the map's parameters at the file's resolution (P.l_occ
-// classifies the leaves in *out).  Validation and errors as read_octree, and a leaf value that is not finite is LS_ERR_ARG;
-// the map is unchanged after any error.  out->inner: the nodes with children.
-int read_full_octree(Map& m, const Params& P, const unsigned char* payload, long long bytes, long long nodes,
-                     ReadCounters* out, const char** why, cudaStream_t st, uint64_t* launches);
+// octomap's readBinary (.bt) or readData (.ot) of a payload (`bytes` bytes after "data\n", `nodes` the header's size) into
+// the map, replacing it (DESIGN.md §4b'''''' and §4b''''''').  P: the map's parameters at the file's resolution (P.l_occ
+// classifies a .ot's leaves in *out; a .ot leaf's voxels take its value verbatim).  Synchronous.  Validates the whole
+// stream and the brick count before it grows or writes anything: LS_ERR_ARG for a malformed payload (for .ot, a leaf
+// value that is not finite too), LS_ERR_NOMEM for more bricks than the map can index or a failed growth, and the map is
+// unchanged after any error (*why then says why).  *out: the counts; out->inner: the nodes with children.
+int read_tree(Map& m, const Params& P, TreeFormat f, const unsigned char* payload, long long bytes, long long nodes,
+              ReadCounters* out, const char** why, cudaStream_t st, uint64_t* launches);
 
 // Queries (oracle/QUERIES.md), reading the map only.  Synchronous; host inputs and outputs, *visited the voxel states the
 // kernels read.  n <= 0 launches nothing.

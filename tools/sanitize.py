@@ -85,7 +85,7 @@ for got, want in ((om.cell_status(qs), qo.cell_status(qs)), (om.line_status(qs, 
                   (om.cast_rays(qorg, qd, False, 10.0), qo.cast_rays(qorg, qd, False, 10.0)),
                   (om.cast_rays(qorg, qd, True, 10.0), qo.cast_rays(qorg, qd, True, 10.0))):
     assert np.array_equal(got[0], want[0]) and np.array_equal(np.asarray(got[1]).view(np.uint8), np.asarray(want[1]).view(np.uint8))
-# that map's .bt file read back into a map of 16 bricks (parse, growth, expansion) against the reference expansion
+# that map's .bt and .ot files read back into maps of 16 bricks (parse, growth, expansion) against the reference expansions
 import tempfile
 sys.path.insert(1, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import octomap_read_ref as rr
@@ -96,6 +96,19 @@ with tempfile.TemporaryDirectory() as tmp:
     rm.read_octomap(bt)
     rk, rv, _ = rm.download(ls.OCC_KNOWN)
     wk, wv = rr.expand(ls.read_octomap(bt), *rr.clamps())
+    assert np.array_equal(rk, wk) and np.array_equal(rv.view(np.uint32), wv.view(np.uint32)) and len(rk) > 0
+    rm.close()
+    # the same map as a full tree: the .ot payload against the full-tree reference, and its file read back
+    import octomap_full_ref as fr
+    ft, oft = om.full_octree(), fr.of_map(oom)
+    assert ft.nodes == oft.nodes > 0 and ft.payload == oft.payload
+    oft.close()
+    ot = os.path.join(tmp, "map.ot")
+    om.save_octomap_full(ot)
+    rm = ls.OccupancyMap(ctx, resolution=0.05, max_range=10.0, initial_capacity=16)
+    rm.read_octomap_full(ot)
+    rk, rv, _ = rm.download(ls.OCC_KNOWN)
+    wk, wv = fr.expand(ls.read_octomap_full(ot))
     assert np.array_equal(rk, wk) and np.array_equal(rv.view(np.uint32), wv.view(np.uint32)) and len(rk) > 0
     rm.close()
 # edits of that map: a set that grows it from 16 bricks, the crop, the bounds and a reset, against the edit restatement
