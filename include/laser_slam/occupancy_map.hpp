@@ -7,9 +7,11 @@
 #ifndef LASER_SLAM_OCCUPANCY_MAP_HPP_
 #define LASER_SLAM_OCCUPANCY_MAP_HPP_
 
+#include <array>
 #include <cstdint>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "laser_slam/common.hpp"
@@ -142,6 +144,31 @@ class OccupancyMap {
   kindr::minimal::Position getMapSize() const;
   kindr::minimal::Position getMapCenter() const;
 
+  // ---- leaf boxes and marker cubes: volumetric_mapping's getAllFreeBoxes / getAllOccupiedBoxes and generateMarkerArray on
+  // the device map (ls_occupancy_build_leaves / _download_leaves / _marker_cubes; rules in DESIGN.md §4b'''''''''''').  A box
+  // is a leaf of the value-pruned tree (octomap's tree in memory, not the .bt file's), as (centre, edge), in octomap's leaf
+  // order.
+  typedef std::vector<std::pair<kindr::minimal::Position, double> > BoxVector;
+  void getAllFreeBoxes(BoxVector* free_boxes) const;
+  void getAllOccupiedBoxes(BoxVector* occupied_boxes) const;
+  // (new) Only the leaves whose key cube meets the box [region_min, region_max] (metres, each corner keyed and clamped to
+  // the key range); a region that is not finite or is inverted throws.
+  void getAllFreeBoxes(const kindr::minimal::Position& region_min, const kindr::minimal::Position& region_max,
+                       BoxVector* free_boxes) const;
+  void getAllOccupiedBoxes(const kindr::minimal::Position& region_min, const kindr::minimal::Position& region_max,
+                           BoxVector* occupied_boxes) const;
+  // One of generateMarkerArray's cube lists: the cube edge of its depth, the cubes' centres and, for occupied cubes, one
+  // colour {r, g, b, a} per cube (free lists carry none: the marker's own colour is set by the caller).
+  struct CubeList {
+    double size;
+    std::vector<kindr::minimal::Position> points;
+    std::vector<std::array<float, 4> > colors;
+  };
+  // One list per depth 0..16 for the occupied leaves, coloured by height (octomap_server's heightMapColor over min_z ...
+  // max_z, times color_factor), and for the free ones.  min_z < max_z, all finite, or it throws.
+  void generateMarkerArray(double min_z, double max_z, double color_factor, std::vector<CubeList>* occupied_nodes,
+                           std::vector<CubeList>* free_nodes) const;
+
   // ---- change detection: octomap's calls and volumetric_mapping's getChangedPoints on the device map
   // (ls_occupancy_track_changes / _changes; rules in DESIGN.md §4b'''''''''').  A change is a voxel whose state (free,
   // occupied, unknown) differs from its state at the last enable or reset.
@@ -162,6 +189,9 @@ class OccupancyMap {
   friend class DistanceMap;  // reads map_ under mutex_ in its update (include/laser_slam/distance_map.hpp)
 
   CellStatus cellStatus(const kindr::minimal::Position& point, float* log_odds) const;
+  // Under mutex_: the leaves of LS_LEAVES_FREE or LS_LEAVES_OCCUPIED, of the region when region_min is not NULL.
+  void boxes(int which, const kindr::minimal::Position* region_min, const kindr::minimal::Position* region_max,
+             BoxVector* out) const;
   void download(int which, std::vector<uint64_t>* keys, std::vector<float>* log_odds, std::vector<float>* centres4) const;
   // Under mutex_: the changes (each output may be NULL), then a reset when `reset`.  Returns their number.
   size_t changes(std::vector<uint64_t>* keys, std::vector<int8_t>* status, std::vector<int8_t>* previous,

@@ -472,6 +472,49 @@ int ls_occupancy_read_full_octree(ls_occupancy* om, const uint8_t* payload, int6
  * above. */
 int ls_occupancy_read_octomap_full(ls_occupancy* om, const char* path, ls_octomap_read_stats* stats);
 
+/* The map's leaves as boxes: volumetric_mapping's getAllFreeBoxes / getAllOccupiedBoxes and generateMarkerArray's cube lists
+ * (DESIGN.md §4b'''''''''''').  Rules:
+ *   tree        the leaves of the value-pruned tree the .ot build writes (octomap's tree in memory), not the .bt file's
+ *               max-likelihood tree, so occupied leaves can be finer than ls_occupancy_download_octree's; for a map read
+ *               from a .bt file the two coincide
+ *   state       LS_CELL_OCCUPIED iff the leaf's log-odds >= L_occ, else LS_CELL_FREE
+ *   order       octomap's leaf iterator: pre-order, children 0..7
+ *   box         depth d (1..16), centre keyToCoord(key, d) per axis as the .bt leaves above (float), edge res * 2^(16-d)
+ *   region      region_min3 / region_max3 in metres, keyed as the map's points in double (floor(c * (1/res)) + 32768) and
+ *               clamped to [0, 65535]: a leaf is listed iff its key cube [k0, k0 + 2^(16-d)) meets [key(min), key(max)] on
+ *               every axis.  Both NULL: every leaf
+ *   cubes       the listed leaves ordered by state (occupied first), then depth 0..16, then the leaf order.  An occupied
+ *               cube's colour is octomap_server's heightMapColor(h), h = (1 - min(max((z - min_z) / (max_z - min_z), 0), 1))
+ *               * color_factor, z the float centre's z widened to double, all in double and cast to float once, alpha 1
+ * ls_occupancy_build_leaves lists the leaves (building the .ot tree first unless its cached build is current; neither
+ * cached build is invalidated, and their outputs do not change).  Only the counts come back; the list stays on the device
+ * until an insert, edit, read or reset of the map invalidates it, and a download then returns LS_ERR_STATE.  Calls run on
+ * the map's stream, are synchronous, never change the map and are legal between ls_icp_register_submap_batch_begin and
+ * _end.  Errors: LS_ERR_ARG for a region that is not finite, inverted (min > max on an axis) or given by one pointer only,
+ * bad `which`, NULL n, cap < 0, a NULL output with cap > 0, more leaves than cap (*n then holds their number, nothing is
+ * copied), or colour arguments that are not finite, have min_z >= max_z or a difference that overflows; LS_ERR_NOMEM when the list cannot grow.  A
+ * refused call leaves the map, both cached builds and the last list as they were. */
+#define LS_LEAVES_FREE 1
+#define LS_LEAVES_OCCUPIED 2
+#define LS_LEAVES_ALL 3
+typedef struct ls_leaf_stats {
+  int64_t free_leaves, occupied_leaves;           /* listed leaves */
+  int64_t free_by_depth[17], occupied_by_depth[17]; /* listed leaves per depth 0..16 */
+  float device_ms;                                /* the call on the map's stream, a .ot build it needed included */
+} ls_leaf_stats;
+/* stats may be NULL. */
+int ls_occupancy_build_leaves(ls_occupancy* om, const double* region_min3, const double* region_max3, ls_leaf_stats* stats);
+/* which: LS_LEAVES_*; per listed leaf of that state, in leaf order: centre {x, y, z, 1}, depth and state LS_CELL_*.  *n always
+ * set, so cap = 0 asks for the count. */
+int ls_occupancy_download_leaves(ls_occupancy* om, int which, float* centres4, uint8_t* depths, int8_t* states, int64_t cap,
+                                 int64_t* n);
+/* The cube lists of the last list: centres4 holds *n cubes {x, y, z, 1} in the cube order, the occupied cubes of depth d at
+ * [occupied_offsets[d], occupied_offsets[d + 1]) and the free ones at [free_offsets[d], free_offsets[d + 1]) (so
+ * occupied_offsets[17] = free_offsets[0]); colors4 {r, g, b, a} per occupied cube.  Offsets and *n always set; cap: cubes
+ * centres4 can hold. */
+int ls_occupancy_marker_cubes(ls_occupancy* om, double min_z, double max_z, double color_factor, float* centres4,
+                              float* colors4, int64_t occupied_offsets[18], int64_t free_offsets[18], int64_t cap, int64_t* n);
+
 /* Queries of the map: volumetric_mapping's WorldBase (getCellStatusPoint, getLineStatus, getVisibility,
  * getLineStatusBoundingBox) and octomap's castRay, batched, one device thread per query.  The rules (oracle/QUERIES.md):
  *   cell        the key of the double point (octomap's search(x, y, z): floor(c * (1/resolution)) + 32768, no float cast);

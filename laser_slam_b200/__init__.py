@@ -130,6 +130,13 @@ class OccupancyChangeStats(ctypes.Structure):
                 ("device_bytes", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
 
+class LeafStats(ctypes.Structure):
+    """ls_leaf_stats: the listed leaves per state, and per state and depth 0..16, and the call's device ms."""
+    _fields_ = [("free_leaves", ctypes.c_int64), ("occupied_leaves", ctypes.c_int64),
+                ("free_by_depth", ctypes.c_int64 * 17), ("occupied_by_depth", ctypes.c_int64 * 17),
+                ("device_ms", ctypes.c_float)]
+
+
 class OccupancyQueryStats(ctypes.Structure):
     _fields_ = [("keys_visited", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
@@ -152,6 +159,7 @@ class DistanceMapQueryStats(ctypes.Structure):
 
 
 OCC_KNOWN, OCC_OCCUPIED = 1, 2
+LEAVES_FREE, LEAVES_OCCUPIED, LEAVES_ALL = 1, 2, 3
 CELL_FREE, CELL_OCCUPIED, CELL_UNKNOWN = 0, 1, 2
 RAY_INVALID, RAY_HIT, RAY_UNKNOWN, RAY_MAX_RANGE, RAY_KEY_BOUND = 0, 1, 2, 3, 4
 LS_ERR_NOMEM, LS_ERR_STATE = -3, -4
@@ -281,6 +289,10 @@ def lib():
         L.ls_occupancy_track_changes.argtypes = [vp, ci]
         L.ls_occupancy_changes.argtypes = [vp, vp, vp, vp, vp, ctypes.c_int64, i64p, ci,
                                            ctypes.POINTER(OccupancyChangeStats)]
+        L.ls_occupancy_build_leaves.argtypes = [vp, vp, vp, ctypes.POINTER(LeafStats)]
+        L.ls_occupancy_download_leaves.argtypes = [vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
+        L.ls_occupancy_marker_cubes.argtypes = [vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp, vp, vp,
+                                                ctypes.c_int64, i64p]
         L.ls_distance_map_create.argtypes = [vp, ctypes.POINTER(DistanceMapParams), ctypes.POINTER(vp)]
         L.ls_distance_map_destroy.argtypes = [vp]
         L.ls_distance_map_destroy.restype = None
@@ -1178,6 +1190,70 @@ class OccupancyMap:
                                                        ctypes.byref(self.last_changes)))
         return keys[:m].copy(), st[:m].copy(), prev[:m].copy(), cen[:m].copy()
 
+    # ---- leaf boxes and marker cubes (ls_occupancy_build_leaves / _download_leaves / _marker_cubes)
+    def build_leaves(self, region=None):
+        """Lists the leaves of the value-pruned tree whose key cube meets region = (min (3,), max (3,)) in metres, or every
+        leaf (DESIGN.md §4b'''''''''''').  Returns LeafStats; the list stays on the device for download_leaves and
+        marker_cubes until the map changes."""
+        st = LeafStats()
+        if region is None:
+            self.ctx._check(lib().ls_occupancy_build_leaves(self._h, None, None, ctypes.byref(st)))
+        else:
+            lo = np.ascontiguousarray(np.asarray(region[0], np.float64).reshape(3))
+            hi = np.ascontiguousarray(np.asarray(region[1], np.float64).reshape(3))
+            self.ctx._check(lib().ls_occupancy_build_leaves(self._h, lo.ctypes.data, hi.ctypes.data, ctypes.byref(st)))
+        return st
+
+    def download_leaves(self, which=LEAVES_ALL):
+        """The last list's leaves of `which` (LEAVES_*) in octomap's leaf order: (centres (n,4) float32, depths uint8,
+        states int8 CELL_*)."""
+        n = ctypes.c_int64(0)
+        rc = lib().ls_occupancy_download_leaves(self._h, int(which), None, None, None, 0, ctypes.byref(n))
+        if rc != LS_ERR_ARG or n.value == 0:
+            self.ctx._check(rc)
+        m = n.value
+        cen = np.empty((max(m, 1), 4), np.float32)
+        dep = np.empty(max(m, 1), np.uint8)
+        st = np.empty(max(m, 1), np.int8)
+        if m > 0:
+            self.ctx._check(lib().ls_occupancy_download_leaves(self._h, int(which), cen.ctypes.data, dep.ctypes.data,
+                                                               st.ctypes.data, m, ctypes.byref(n)))
+        return cen[:m].copy(), dep[:m].copy(), st[:m].copy()
+
+    def leaf_boxes(self, which=LEAVES_ALL, region=None):
+        """getAllFreeBoxes (which=LEAVES_FREE) / getAllOccupiedBoxes (LEAVES_OCCUPIED), or both in one list, optionally
+        limited to a region (min (3,), max (3,)): LeafBoxes(centres (n,3) float32, edges float64 = res * 2^(16 - depth),
+        depths uint8, states int8 CELL_*), in octomap's leaf order.  self.last_leaves holds the build's LeafStats."""
+        self.last_leaves = self.build_leaves(region)
+        cen, dep, st = self.download_leaves(which)
+        edges = self.params.resolution * np.exp2(16 - dep.astype(np.float64))
+        return LeafBoxes(cen[:, :3].copy(), edges, dep, st)
+
+    def marker_cubes(self, min_z, max_z, color_factor=0.8, region=None):
+        """generateMarkerArray's cube lists: MarkerCubes(occupied, free), each a list of 17 CubeList(size, points (k,3)
+        float32, colors (k,4) float32) for depths 0..16; occupied cubes are coloured by height (heightMapColor), free ones
+        carry no colours (an empty (0,4) array).  self.last_leaves holds the build's LeafStats."""
+        self.last_leaves = self.build_leaves(region)
+        occ_off, free_off = np.zeros(18, np.int64), np.zeros(18, np.int64)
+        n = ctypes.c_int64(0)
+        rc = lib().ls_occupancy_marker_cubes(self._h, float(min_z), float(max_z), float(color_factor), None, None,
+                                             occ_off.ctypes.data, free_off.ctypes.data, 0, ctypes.byref(n))
+        if rc != LS_ERR_ARG or n.value == 0:
+            self.ctx._check(rc)
+        m = n.value
+        cen = np.empty((max(m, 1), 4), np.float32)
+        rgba = np.empty((max(m, 1), 4), np.float32)
+        if m > 0:
+            self.ctx._check(lib().ls_occupancy_marker_cubes(self._h, float(min_z), float(max_z), float(color_factor),
+                                                            cen.ctypes.data, rgba.ctypes.data, occ_off.ctypes.data,
+                                                            free_off.ctypes.data, m, ctypes.byref(n)))
+        res = self.params.resolution
+        occ = [CubeList(res * 2.0 ** (16 - d), cen[occ_off[d]:occ_off[d + 1], :3].copy(),
+                        rgba[occ_off[d]:occ_off[d + 1]].copy()) for d in range(17)]
+        free = [CubeList(res * 2.0 ** (16 - d), cen[free_off[d]:free_off[d + 1], :3].copy(), np.zeros((0, 4), np.float32))
+                for d in range(17)]
+        return MarkerCubes(occ, free)
+
 
 class DistanceMap:
     """octomap's DynamicEDTOctomap on the device (ls_distance_map_*): the Euclidean distance of every finest cell of the box
@@ -1243,6 +1319,9 @@ class DistanceMap:
 
 Octree = collections.namedtuple("Octree", "nodes payload centres depths device_ms")
 FullOctree = collections.namedtuple("FullOctree", "nodes payload device_ms")
+LeafBoxes = collections.namedtuple("LeafBoxes", "centres edges depths states")
+CubeList = collections.namedtuple("CubeList", "size points colors")
+MarkerCubes = collections.namedtuple("MarkerCubes", "occupied free")
 
 _BT_FIRST_LINE = b"# Octomap OcTree binary file"
 _OT_FIRST_LINE = b"# Octomap OcTree file"

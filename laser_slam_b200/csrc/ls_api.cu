@@ -1742,6 +1742,8 @@ struct ls_occupancy {
   } trees[2];
   lso::Changes changes;  // change detection's baseline and scratch (ls_changes.cu)
   bool tracking = false;
+  lso::Leaves leaves;  // the last leaf list (ls_occupancy_build_leaves), current while it reflects every change to the map
+  bool leaves_current = false;
 };
 
 namespace {
@@ -1749,8 +1751,10 @@ using lso::TreeFormat;
 
 ls_occupancy::Tree& tree_of(ls_occupancy* om, TreeFormat f) { return om->trees[(int)f]; }
 
+// A change to the map invalidates both cached builds and the leaf list.
 void trees_stale(ls_occupancy* om) {
   for (ls_occupancy::Tree& t : om->trees) t.current = false;
+  om->leaves_current = false;
 }
 
 // The error texts' name of a format: "octree" or "full octree".
@@ -2336,6 +2340,108 @@ int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]) {
     min3[a] = empty ? 0.0 : centre(kmin[a]) - res / 2.0;
     max3[a] = empty ? 0.0 : (centre(kmax[a]) - res / 2.0) + res;
   }
+  return LS_OK;
+}
+
+}  // extern "C"
+
+namespace {
+// The key of a region corner in double, clamped to the key range: floor(c * (1/res)) + 32768 in [0, 65535].
+int clamped_key(double inv, double c) {
+  const double s = std::floor(c * inv) + 32768.0;
+  return s < 0.0 ? 0 : s > 65535.0 ? 65535 : (int)s;
+}
+}  // namespace
+
+extern "C" {
+
+int ls_occupancy_build_leaves(ls_occupancy* om, const double* region_min3, const double* region_max3, ls_leaf_stats* stats) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!region_min3 != !region_max3) return fail(ctx, LS_ERR_ARG, "a region needs both corners");
+  int kmin[3] = {0, 0, 0}, kmax[3] = {65535, 65535, 65535};
+  if (region_min3) {
+    for (int a = 0; a < 3; ++a) {
+      if (!std::isfinite(region_min3[a]) || !std::isfinite(region_max3[a]))
+        return fail(ctx, LS_ERR_ARG, "region axis %d is not finite", a);
+      if (region_min3[a] > region_max3[a]) return fail(ctx, LS_ERR_ARG, "region axis %d is inverted (min > max)", a);
+      kmin[a] = clamped_key(om->prm.inv, region_min3[a]);
+      kmax[a] = clamped_key(om->prm.inv, region_max3[a]);
+    }
+  }
+  CU(cudaSetDevice(ctx->device));
+  om->leaves_current = false;
+  ls_occupancy::Tree& t = tree_of(om, TreeFormat::Full);
+  const bool build = !t.current;
+  int rc;
+  if (build && (rc = build_tree(om, TreeFormat::Full))) return rc;
+  CU(cudaEventRecord(om->ev0, om->stream));
+  rc = lso::build_leaves(om->map, om->prm, t.tree, kmin, kmax, om->leaves, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "leaf list: out of device memory" : "leaf list failed");
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  om->leaves_current = true;
+  if (stats) {
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+    const lso::Leaves& L = om->leaves;
+    stats->free_leaves = L.n - L.n_occupied;
+    stats->occupied_leaves = L.n_occupied;
+    for (int d = 0; d < 17; ++d) stats->free_by_depth[d] = L.free[d], stats->occupied_by_depth[d] = L.occupied[d];
+    stats->device_ms = ms + (build ? t.ms : 0.f);
+  }
+  return LS_OK;
+}
+
+int ls_occupancy_download_leaves(ls_occupancy* om, int which, float* centres4, uint8_t* depths, int8_t* states, int64_t cap,
+                                 int64_t* n) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!n) return fail(ctx, LS_ERR_ARG, "bad argument");
+  *n = 0;
+  if (cap < 0 || (which != LS_LEAVES_FREE && which != LS_LEAVES_OCCUPIED && which != LS_LEAVES_ALL) ||
+      (cap > 0 && (!centres4 || !depths || !states)))
+    return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!om->leaves_current) return fail(ctx, LS_ERR_STATE, "no current leaf list: build it after the last change to the map");
+  const lso::Leaves& L = om->leaves;
+  const long long m = which == LS_LEAVES_ALL ? L.n : which == LS_LEAVES_OCCUPIED ? L.n_occupied : L.n - L.n_occupied;
+  *n = m;
+  if (m > cap) return fail(ctx, LS_ERR_ARG, "buffers of %lld leaves for %lld", (long long)cap, m);
+  if (m == 0) return LS_OK;
+  CU(cudaSetDevice(ctx->device));
+  std::vector<uint8_t> tags((size_t)m);
+  const int rc = lso::download_leaves(om->leaves, which, centres4, tags.data(), om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "leaf download failed");
+  for (long long i = 0; i < m; ++i) {
+    depths[i] = tags[i] & 31;
+    states[i] = tags[i] & 32 ? LS_CELL_FREE : LS_CELL_OCCUPIED;
+  }
+  return LS_OK;
+}
+
+int ls_occupancy_marker_cubes(ls_occupancy* om, double min_z, double max_z, double color_factor, float* centres4,
+                              float* colors4, int64_t occupied_offsets[18], int64_t free_offsets[18], int64_t cap, int64_t* n) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!n) return fail(ctx, LS_ERR_ARG, "bad argument");
+  *n = 0;
+  if (cap < 0 || !occupied_offsets || !free_offsets || (cap > 0 && (!centres4 || !colors4)))
+    return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (!std::isfinite(min_z) || !std::isfinite(max_z) || !std::isfinite(color_factor) || !(min_z < max_z) ||
+      !std::isfinite(max_z - min_z))
+    return fail(ctx, LS_ERR_ARG, "colour arguments min_z %g, max_z %g, color_factor %g (finite, min_z < max_z)", min_z, max_z,
+                color_factor);
+  if (!om->leaves_current) return fail(ctx, LS_ERR_STATE, "no current leaf list: build it after the last change to the map");
+  const lso::Leaves& L = om->leaves;
+  occupied_offsets[0] = 0;
+  for (int d = 0; d < 17; ++d) occupied_offsets[d + 1] = occupied_offsets[d] + L.occupied[d];
+  free_offsets[0] = occupied_offsets[17];
+  for (int d = 0; d < 17; ++d) free_offsets[d + 1] = free_offsets[d] + L.free[d];
+  *n = free_offsets[17];
+  if (*n > cap) return fail(ctx, LS_ERR_ARG, "buffers of %lld cubes for %lld", (long long)cap, (long long)*n);
+  CU(cudaSetDevice(ctx->device));
+  const int rc = lso::marker_cubes(om->leaves, min_z, max_z, color_factor, centres4, colors4, om->stream, &ctx->launches);
+  if (rc) return fail(ctx, rc, "marker cubes failed");
   return LS_OK;
 }
 

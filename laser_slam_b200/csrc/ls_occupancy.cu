@@ -28,6 +28,11 @@
 //   (h) oct_emit_kernel      one block per inner brick: (e)'s levels again, its nodes below depth 13 written at the offset
 //                            (g) gave it, so no per-brick staging is kept; one specialisation per format
 // A brick without a known voxel (an insert that failed after placing it leaves one) has state 0 and adds nothing.
+// Leaf lists (DESIGN.md §4b''''''''''''), over the records of a current .ot build, reading them and the map only:
+//   (l1) lv_down_kernel      one block: levels 0 ... 12 as (g), each node's leaf offset; leaves above the bricks written
+//   (l2) lv_emit_kernel      one block per inner brick: (e)'s levels again, its leaves placed by a block scan
+//   (l3) lv_compact_kernel   after a CUB scan of the region flags: the kept leaves in order, counts per (state, depth)
+//   (l4) lv_gather_kernel    after a CUB radix sort by state (or state and depth): centres, tags and height colours
 //
 // Read (DESIGN.md §4b''''''), replacing the map.  The payload is uploaded once and parsed without a walk, one thread per
 // stream record (.bt: inner nodes only; .ot: every node):
@@ -1273,6 +1278,146 @@ __global__ void __launch_bounds__(512) oct_emit_kernel<FullTree>(const unsigned*
   if (c) FullTree::put_node(p, T.v16[t], 0);
 }
 
+// ---- leaf lists: (l1) ... (l4), over the records of a .ot build ---------------------------------------------------------
+// A leaf's tag: its depth, plus kFreeTag when its value is below L_occ.  A radix sort over bit 5 splits the list by state,
+// over bits 0 ... 5 by (state, depth), occupied first; both sorts are stable, so each part keeps the leaf iterator's order.
+constexpr int kFreeTag = 32, kLeafBuckets = 34;  // bucket: depth, or 17 + depth for a free leaf
+
+// The key range of a listing per axis: a leaf is kept iff its key cube [k0, k0 + side) meets [lo, hi] on every axis.
+struct KeyRange {
+  int lo[3], hi[3];
+};
+
+__device__ __forceinline__ void put_tree_leaf(int kx, int ky, int kz, int depth, unsigned v, float l_occ, double res,
+                                              const KeyRange& R, unsigned long long i, float4* __restrict__ cen,
+                                              unsigned char* __restrict__ tag, int* __restrict__ keep) {
+  const int s = 16 - depth, side = 1 << s;
+  cen[i] = make_float4(leaf_coord(kx, s, res), leaf_coord(ky, s, res), leaf_coord(kz, s, res), 1.0f);
+  tag[i] = (unsigned char)(depth | (__uint_as_float(v) >= l_occ ? 0 : kFreeTag));
+  keep[i] = kx <= R.hi[0] && kx + side - 1 >= R.lo[0] && ky <= R.hi[1] && ky + side - 1 >= R.lo[1] && kz <= R.hi[2] &&
+            kz + side - 1 >= R.lo[2];
+}
+
+// (l1) levels 0 ... 12 as (g): each inner node gives its children their leaf offsets (its own + the earlier siblings'
+// leaves); a leaf child, bricks at depth 13 included, writes itself
+__global__ void __launch_bounds__(kTreeThreads) lv_down_kernel(Nodes N, const int* __restrict__ levels, float l_occ, double res,
+                                                               KeyRange R, float4* __restrict__ cen,
+                                                               unsigned char* __restrict__ tag, int* __restrict__ keep) {
+  const int t = threadIdx.x;
+  if (t == 0) N.loff[levels[0]] = 0;
+  __syncthreads();
+  for (int d = 0; d < kBrickDepth; ++d) {
+    const int pb = levels[2 * d], pn = levels[2 * d + 1];
+    for (int p = pb + t; p < pb + pn; p += kTreeThreads) {
+      if (N.st[p] != 3) continue;
+      unsigned long long l = N.loff[p];
+      for (int c = N.first[p]; c < N.end[p]; ++c) {
+        N.loff[c] = l;
+        if (N.st[c] == 1) {
+          const unsigned long long k = N.code[c];
+          const int sh = 15 - d;
+          put_tree_leaf(squeeze3(k) << sh, squeeze3(k >> 1) << sh, squeeze3(k >> 2) << sh, d + 1, N.val[c], l_occ, res, R, l,
+                        cen, tag, keep);
+        }
+        l += N.tot[1][c];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// (l2) one block per inner brick: (e)'s levels again; thread t owns the leaf whose first voxel has Morton index t, if
+// any (a depth-14 leaf at t % 64 == 0, a depth-15 one at t % 8 == 0 or voxel t), and a block scan places it
+__global__ void __launch_bounds__(512) lv_emit_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
+                                                      const unsigned long long* __restrict__ bkey, Nodes N, float l_occ,
+                                                      double res, KeyRange R, float4* __restrict__ cen,
+                                                      unsigned char* __restrict__ tag, int* __restrict__ keep) {
+  using Scan = cub::BlockScan<int, 512>;
+  __shared__ FullTree::Levels T;
+  __shared__ typename Scan::TempStorage scan;
+  const int r = blockIdx.x;
+  if (N.st[r] != 3) return;  // a leaf brick is written in (l1)
+  const int b = N.pool[r];
+  FullTree::levels(known, lo, b, l_occ, T);
+  const int t = threadIdx.x, i14 = t >> 6, i15 = t >> 3;
+  int depth = 0;
+  unsigned v = 0;
+  if (T.s14[i14] != 3) {
+    if ((t & 63) == 0 && T.s14[i14] == 1) depth = 14, v = T.v14[i14];
+  } else if (T.s15[i15] != 3) {
+    if ((t & 7) == 0 && T.s15[i15] == 1) depth = 15, v = T.v15[i15];
+  } else if (T.s16[t]) {
+    depth = 16, v = T.v16[t];
+  }
+  int idx;
+  Scan(scan).ExclusiveSum(depth != 0 ? 1 : 0, idx);
+  if (depth) {
+    const unsigned long long bk = bkey[b];
+    const int u = morton_local(t);
+    put_tree_leaf((int)(bk & 0x1fff) * 8 + (u & 7), (int)((bk >> 13) & 0x1fff) * 8 + ((u >> 3) & 7),
+                  (int)((bk >> 26) & 0x1fff) * 8 + (u >> 6), depth, v, l_occ, res, R, N.loff[r] + (unsigned long long)idx,
+                  cen, tag, keep);
+  }
+}
+
+// (l3) after an exclusive scan of keep into pos: the kept leaves in order, their positions and the count per bucket
+__global__ void __launch_bounds__(256) lv_compact_kernel(const float4* __restrict__ raw_c, const unsigned char* __restrict__ raw_tag,
+                                                         const int* __restrict__ keep, const int* __restrict__ pos, int n,
+                                                         float4* __restrict__ cen, unsigned char* __restrict__ tag,
+                                                         int* __restrict__ idx, unsigned long long* __restrict__ count) {
+  __shared__ unsigned hist[kLeafBuckets];
+  if (threadIdx.x < kLeafBuckets) hist[threadIdx.x] = 0;
+  __syncthreads();
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (!keep[i]) continue;
+    const int j = pos[i], g = raw_tag[i];
+    cen[j] = raw_c[i], tag[j] = (unsigned char)g, idx[j] = j;
+    atomicAdd(&hist[(g & kFreeTag ? 17 : 0) + (g & 31)], 1u);
+  }
+  __syncthreads();
+  if (threadIdx.x < kLeafBuckets && hist[threadIdx.x]) atomicAdd(&count[threadIdx.x], (unsigned long long)hist[threadIdx.x]);
+}
+
+// octomap_server's heightMapColor(h), in double and cast to float once: s = v = 1, so m = 0 and n = 1 - f
+__device__ __forceinline__ float4 height_colour(double h) {
+  h -= floor(h);
+  h *= 6.0;
+  const int i = (int)floor(h);
+  double f = h - (double)i;
+  if (!(i & 1)) f = 1.0 - f;
+  const double n = 1.0 - f;
+  double r = 1.0, g = 0.5, b = 0.5;
+  switch (i) {
+    case 6:
+    case 0: r = 1.0, g = n, b = 0.0; break;
+    case 1: r = n, g = 1.0, b = 0.0; break;
+    case 2: r = 0.0, g = 1.0, b = n; break;
+    case 3: r = 0.0, g = n, b = 1.0; break;
+    case 4: r = n, g = 0.0, b = 1.0; break;
+    case 5: r = 1.0, g = 0.0, b = n; break;
+  }
+  return make_float4((float)r, (float)g, (float)b, 1.0f);
+}
+
+// (l4) entries [first, first + n) of the sorted order gathered: centres and tags; the first n_col of them also take
+// generateMarkerArray's height colour h = (1 - min(max((z - min_z) / (max_z - min_z), 0), 1)) * color_factor
+__global__ void lv_gather_kernel(const float4* __restrict__ cen, const unsigned char* __restrict__ tag,
+                                 const int* __restrict__ order, long long first, long long n, long long n_col, double min_z,
+                                 double max_z, double color_factor, float4* __restrict__ out_c,
+                                 unsigned char* __restrict__ out_tag, float4* __restrict__ rgba) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int j = order[first + i];
+    const float4 c = cen[j];
+    out_c[i] = c, out_tag[i] = tag[j];
+    if (i < n_col) {
+      double x = ((double)c.z - min_z) / (max_z - min_z);
+      x = x < 0.0 ? 0.0 : x;  // std::max(x, 0.0)
+      x = 1.0 < x ? 1.0 : x;  // std::min(x, 1.0)
+      rgba[i] = height_colour((1.0 - x) * color_factor);
+    }
+  }
+}
+
 // ---- read: (r1) ... (r7) ---------------------------------------------------------------------------------------------
 // Item i of the stream is the i-th node of it in pre-order.  With c_i its children in the stream, the excess E_0 = 1,
 // E_{i+1} = E_i + c_i - 1 counts the stream nodes found but not yet read; the tree ends at the first i >= 1 with E_i = 0.
@@ -1957,6 +2102,7 @@ int replace_map(Map& m, int n_b, long long known, const std::function<int()>& ke
 template <class F>
 int build_tree_as(const Map& m, const Params& P, Octree& t, cudaStream_t st, uint64_t* launches) {
   t.nodes = t.bytes = t.leaves = 0;
+  t.bricks = 0;
   const int n_b = m.pool_n;
   if (n_b == 0) return LS_OK;
   int rc;
@@ -1991,6 +2137,7 @@ int build_tree_as(const Map& m, const Params& P, Octree& t, cudaStream_t st, uin
   OCC_LAUNCHED();
   OCC_TRY(cudaStreamSynchronize(st));
   t.nodes = nodes, t.bytes = pay, t.leaves = leaves;
+  t.bricks = n_b;
   return LS_OK;
 }
 
@@ -2071,6 +2218,120 @@ int read_tree(Map& m, const Params& P, TreeFormat f, const unsigned char* payloa
               ReadCounters* out, const char** why, cudaStream_t st, uint64_t* launches) {
   return f == TreeFormat::Full ? read_tree_as<FullTree>(m, P, payload, bytes, nodes, out, why, st, launches)
                                : read_tree_as<BinaryTree>(m, P, payload, bytes, nodes, out, why, st, launches);
+}
+
+// ---- leaf lists ----------------------------------------------------------------------------------------------------------
+namespace {
+
+// Every buffer of a list of n leaves, all or nothing.
+int reserve_leaves(Leaves& L, long long n, cudaStream_t st) {
+  OCC_TRY(L.cnt_dev.reserve(kLeafBuckets, kLeafBuckets));
+  OCC_TRY(L.cnt_host.reserve(kLeafBuckets, kLeafBuckets));
+  if ((size_t)n <= L.raw_c.capacity()) return LS_OK;
+  if (n > (1LL << 30)) return LS_ERR_NOMEM;  // CUB's item counts are int
+  OCC_TRY(cudaStreamSynchronize(st));
+  const size_t c = (size_t)(n + n / 8);
+  size_t scan = 0, sort = 0;
+  cudaError_t e;
+  if ((e = L.raw_c.reserve(c, c)) || (e = L.cen.reserve(c, c)) || (e = L.rgba.reserve(c, c)) || (e = L.raw_tag.reserve(c, c)) ||
+      (e = L.tag.reserve(c, c)) || (e = L.stag.reserve(c, c)) || (e = L.keep.reserve(c, c)) || (e = L.pos.reserve(c, c)) ||
+      (e = L.idx.reserve(c, c)) || (e = L.sorted.reserve(c, c)) ||
+      (e = cub::DeviceScan::ExclusiveSum(nullptr, scan, L.keep.get(), L.pos.get(), (int)c, st)) ||
+      (e = cub::DeviceRadixSort::SortPairs(nullptr, sort, L.tag.get(), L.stag.get(), L.idx.get(), L.sorted.get(), (int)c, 0, 6,
+                                           st)) ||
+      (e = L.cub_tmp.reserve(std::max(scan, sort), std::max(scan, sort)))) {
+    L.raw_c.reset(), L.cen.reset(), L.rgba.reset(), L.raw_tag.reset(), L.tag.reset(), L.stag.reset(), L.keep.reset();
+    L.pos.reset(), L.idx.reset(), L.sorted.reset(), L.cub_tmp.reset();
+    L.cub_bytes = 0;
+    return code(e);
+  }
+  L.cub_bytes = std::max(scan, sort);
+  return LS_OK;
+}
+
+int grid_of(long long n) { return (int)std::min<long long>((n + 255) / 256, 4096); }
+
+// The list's positions stably sorted by tag bits [begin, 6) into L.sorted (tags into L.stag).
+int sort_leaves(Leaves& L, int begin, cudaStream_t st, uint64_t* launches) {
+  size_t bytes = L.cub_bytes;
+  OCC_TRY(cub::DeviceRadixSort::SortPairs(L.cub_tmp.get(), bytes, L.tag.get(), L.stag.get(), L.idx.get(), L.sorted.get(),
+                                          (int)L.n, begin, 6, st));
+  ++*launches;
+  return LS_OK;
+}
+
+// Entries [first, first + n) of L.sorted gathered into raw_c / raw_tag (the first n_col with colours), then copied out.
+int gather_leaves(Leaves& L, long long first, long long n, long long n_col, double min_z, double max_z, double color_factor,
+                  float* centres4, unsigned char* tags, float* rgba4, cudaStream_t st, uint64_t* launches) {
+  if (n > 0) {
+    lv_gather_kernel<<<grid_of(n), 256, 0, st>>>(L.cen.get(), L.tag.get(), L.sorted.get(), first, n, n_col, min_z, max_z,
+                                                 color_factor, L.raw_c.get(), L.raw_tag.get(), L.rgba.get());
+    OCC_LAUNCHED();
+    if (centres4) OCC_TRY(cudaMemcpyAsync(centres4, L.raw_c.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    if (tags) OCC_TRY(cudaMemcpyAsync(tags, L.raw_tag.get(), (size_t)n, cudaMemcpyDeviceToHost, st));
+    if (rgba4 && n_col > 0)
+      OCC_TRY(cudaMemcpyAsync(rgba4, L.rgba.get(), (size_t)n_col * sizeof(float4), cudaMemcpyDeviceToHost, st));
+  }
+  OCC_TRY(cudaStreamSynchronize(st));
+  return LS_OK;
+}
+
+}  // namespace
+
+int build_leaves(const Map& m, const Params& P, Octree& t, const int kmin[3], const int kmax[3], Leaves& L, cudaStream_t st,
+                 uint64_t* launches) {
+  L.n = L.n_occupied = 0;
+  std::fill(L.occupied, L.occupied + 17, 0LL), std::fill(L.free, L.free + 17, 0LL);
+  const long long nl = t.leaves;
+  if (nl == 0) return LS_OK;
+  int rc;
+  if ((rc = reserve_leaves(L, nl, st))) return rc;
+  const KeyRange R{{kmin[0], kmin[1], kmin[2]}, {kmax[0], kmax[1], kmax[2]}};
+  const Nodes N = nodes_of(t);
+  lv_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), P.l_occ, P.res, R, L.raw_c.get(), L.raw_tag.get(),
+                                             L.keep.get());
+  OCC_LAUNCHED();
+  lv_emit_kernel<<<t.bricks, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, P.res, R, L.raw_c.get(),
+                                           L.raw_tag.get(), L.keep.get());
+  OCC_LAUNCHED();
+  size_t bytes = L.cub_bytes;
+  OCC_TRY(cub::DeviceScan::ExclusiveSum(L.cub_tmp.get(), bytes, L.keep.get(), L.pos.get(), (int)nl, st));
+  ++*launches;
+  OCC_TRY(cudaMemsetAsync(L.cnt_dev.get(), 0, kLeafBuckets * sizeof(unsigned long long), st));
+  lv_compact_kernel<<<grid_of(nl), 256, 0, st>>>(L.raw_c.get(), L.raw_tag.get(), L.keep.get(), L.pos.get(), (int)nl,
+                                                 L.cen.get(), L.tag.get(), L.idx.get(), L.cnt_dev.get());
+  OCC_LAUNCHED();
+  OCC_TRY(cudaMemcpyAsync(L.cnt_host.get(), L.cnt_dev.get(), kLeafBuckets * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                          st));
+  OCC_TRY(cudaStreamSynchronize(st));
+  for (int d = 0; d < 17; ++d) {
+    L.occupied[d] = (long long)L.cnt_host.get()[d], L.free[d] = (long long)L.cnt_host.get()[17 + d];
+    L.n_occupied += L.occupied[d], L.n += L.occupied[d] + L.free[d];
+  }
+  return LS_OK;
+}
+
+int download_leaves(Leaves& L, int which, float* centres4, unsigned char* tags, cudaStream_t st, uint64_t* launches) {
+  if (L.n == 0) return LS_OK;
+  if (which == 3) {
+    if (centres4) OCC_TRY(cudaMemcpyAsync(centres4, L.cen.get(), (size_t)L.n * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    if (tags) OCC_TRY(cudaMemcpyAsync(tags, L.tag.get(), (size_t)L.n, cudaMemcpyDeviceToHost, st));
+    OCC_TRY(cudaStreamSynchronize(st));
+    return LS_OK;
+  }
+  int rc;
+  if ((rc = sort_leaves(L, 5, st, launches))) return rc;
+  const long long n_occ = L.n_occupied;
+  return which == 2 ? gather_leaves(L, 0, n_occ, 0, 0.0, 1.0, 0.0, centres4, tags, nullptr, st, launches)
+                    : gather_leaves(L, n_occ, L.n - n_occ, 0, 0.0, 1.0, 0.0, centres4, tags, nullptr, st, launches);
+}
+
+int marker_cubes(Leaves& L, double min_z, double max_z, double color_factor, float* centres4, float* rgba4, cudaStream_t st,
+                 uint64_t* launches) {
+  if (L.n == 0) return LS_OK;
+  int rc;
+  if ((rc = sort_leaves(L, 0, st, launches))) return rc;
+  return gather_leaves(L, 0, L.n, L.n_occupied, min_z, max_z, color_factor, centres4, nullptr, rgba4, st, launches);
 }
 
 namespace {

@@ -150,6 +150,9 @@ struct Octree {
   ls::Buffer<float4> centres;  // with depths
   ls::Buffer<unsigned char> depths;
   long long nodes = 0, bytes = 0, leaves = 0;  // of the last build (full tree: every leaf)
+  // The last build's brick records (the map's pool_n then).  A failed edit can place empty bricks without invalidating a
+  // build, so a pass over the build's records takes their number from here, not from the map.
+  int bricks = 0;
 };
 
 // All return LS_OK, LS_ERR_NOMEM or LS_ERR_CUDA (include/ls_b200.h) and count their launches in *launches.
@@ -174,6 +177,33 @@ enum class TreeFormat { Binary, Full };
 int build_tree(const Map& m, const Params& P, TreeFormat f, Octree& t, cudaStream_t st, uint64_t* launches);
 // Copies the last build's payload (t.bytes) and, each when not NULL, its t.leaves centres {x, y, z, 1} and depths.
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st);
+
+// The leaves of the value-pruned tree as boxes (DESIGN.md §4b''''''''''''): getAllFreeBoxes / getAllOccupiedBoxes and
+// generateMarkerArray's cube lists.  raw_*: every leaf of the tree in pre-order, then the gather target of a download;
+// cen / tag: the listed leaves in pre-order, a tag being the depth plus 32 for a free leaf; idx / sorted: their
+// positions, and those positions and tags after a stable sort by state (or state and depth).
+struct Leaves {
+  ls::Buffer<float4> raw_c, cen, rgba;
+  ls::Buffer<unsigned char> raw_tag, tag, stag;
+  ls::Buffer<int> keep, pos, idx, sorted;
+  ls::Buffer<unsigned char> cub_tmp;
+  size_t cub_bytes = 0;
+  ls::Buffer<unsigned long long> cnt_dev;
+  ls::PinnedBuffer<unsigned long long> cnt_host;
+  long long n = 0, n_occupied = 0;              // listed leaves, of them occupied
+  long long occupied[17] = {}, free[17] = {};  // listed leaves per depth
+};
+// Lists the leaves of t, which must be the current .ot build of m (TreeFormat::Full), whose key cube meets kmin ... kmax
+// on every axis: L.n and the counts per state and depth are set.  Reads the map and t only; synchronous.
+int build_leaves(const Map& m, const Params& P, Octree& t, const int kmin[3], const int kmax[3], Leaves& L, cudaStream_t st,
+                 uint64_t* launches);
+// Of the last list: which = 1 the free leaves, 2 the occupied ones, 3 all, each part in pre-order.  Writes their centres
+// {x, y, z, 1} and tags (n of them, as counted).
+int download_leaves(Leaves& L, int which, float* centres4, unsigned char* tags, cudaStream_t st, uint64_t* launches);
+// The last list ordered by (occupied first, depth, pre-order): centres {x, y, z, 1} and, for the occupied leaves, the
+// height colour {r, g, b, 1} (min_z < max_z, finite: checked by the caller).
+int marker_cubes(Leaves& L, double min_z, double max_z, double color_factor, float* centres4, float* rgba4, cudaStream_t st,
+                 uint64_t* launches);
 
 // octomap's readBinary (.bt) or readData (.ot) of a payload (`bytes` bytes after "data\n", `nodes` the header's size) into
 // the map, replacing it (DESIGN.md §4b'''''' and §4b''''''').  P: the map's parameters at the file's resolution (P.l_occ

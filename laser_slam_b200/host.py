@@ -307,6 +307,11 @@ class OccupancyMap:
             L.lsh_occupancy_changed_points.restype = i64
             L.lsh_occupancy_box_status.argtypes = [vp, vp, vp, ci, ci, vp]
             L.lsh_occupancy_check_paths.argtypes = [vp, vp, vp, ci, vp, ci, vp]
+            L.lsh_occupancy_boxes.argtypes = [vp, ci, vp, vp, vp, vp, i64]
+            L.lsh_occupancy_boxes.restype = i64
+            L.lsh_occupancy_marker_array.argtypes = [vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp, vp, vp,
+                                                     i64]
+            L.lsh_occupancy_marker_array.restype = i64
             L._occ_bound = True
         prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range,
                         float(bool(treat_unknown_as_occupied))], np.float64)
@@ -483,6 +488,35 @@ class OccupancyMap:
         n = self._check(lib().lsh_occupancy_changed_points(self._h, pts.ctypes.data, occ.ctypes.data, int(cap)))
         m = min(n, cap)
         return pts[:m], occ[:m].astype(bool)
+
+    def boxes(self, occupied, region=None):
+        """getAllOccupiedBoxes (occupied) or getAllFreeBoxes, with region = (min (3,), max (3,)) the region overload:
+        (centres (n,3) float64, edges (n,) float64) in octomap's leaf order."""
+        lo = hi = None
+        if region is not None:
+            lo = np.ascontiguousarray(np.asarray(region[0], np.float64).reshape(3))
+            hi = np.ascontiguousarray(np.asarray(region[1], np.float64).reshape(3))
+        args = (int(bool(occupied)), None if lo is None else lo.ctypes.data, None if hi is None else hi.ctypes.data)
+        n = self._check(lib().lsh_occupancy_boxes(self._h, *args, None, None, 0))
+        c = np.zeros((max(n, 1), 3), np.float64)
+        e = np.zeros(max(n, 1), np.float64)
+        m = self._check(lib().lsh_occupancy_boxes(self._h, *args, c.ctypes.data, e.ctypes.data, n))
+        return c[:m], e[:m]
+
+    def marker_array(self, min_z, max_z, color_factor=0.8):
+        """generateMarkerArray: (occupied, free), each 17 (size, centres (k,3) float64, colours (k,4) float32) for depths
+        0..16; free lists have no colours."""
+        sizes, counts = np.zeros(34, np.float64), np.zeros(34, np.int64)
+        n = self._check(lib().lsh_occupancy_marker_array(self._h, float(min_z), float(max_z), float(color_factor), None, None,
+                                                         sizes.ctypes.data, counts.ctypes.data, 0))
+        c = np.zeros((max(n, 1), 3), np.float64)
+        rgba = np.zeros((max(n, 1), 4), np.float32)
+        self._check(lib().lsh_occupancy_marker_array(self._h, float(min_z), float(max_z), float(color_factor), c.ctypes.data,
+                                                     rgba.ctypes.data, sizes.ctypes.data, counts.ctypes.data, n))
+        off = np.concatenate([[0], np.cumsum(counts)])
+        lists = [(sizes[k], c[off[k]:off[k + 1]], rgba[off[k]:off[k + 1]] if k < 17 else np.zeros((0, 4), np.float32))
+                 for k in range(34)]
+        return lists[:17], lists[17:]
 
     def box_status(self, centres, sizes, single=False):
         """The batched getCellStatusBoundingBox overload, or with single=True one call per box: int8 CELL_* per box."""

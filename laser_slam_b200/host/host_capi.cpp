@@ -731,6 +731,60 @@ int64_t lsh_occupancy_changed_points(void* ov, double* pts3, uint8_t* occupied, 
   }
 }
 
+// getAllFreeBoxes (occupied = 0) or getAllOccupiedBoxes, of the region when min3 is not NULL; returns the number of boxes,
+// the first min(n, cap) written: centres and edges.  LS_ERR_STATE on an error
+int64_t lsh_occupancy_boxes(void* ov, int occupied, const double* min3, const double* max3, double* centres3, double* edges,
+                            int64_t cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    if (!min3 != !max3) throw std::invalid_argument("a region needs both corners");
+    OccupancyMap::BoxVector b;
+    if (min3) {
+      const kindr::minimal::Position lo{min3[0], min3[1], min3[2]}, hi{max3[0], max3[1], max3[2]};
+      occupied ? h->map->getAllOccupiedBoxes(lo, hi, &b) : h->map->getAllFreeBoxes(lo, hi, &b);
+    } else {
+      occupied ? h->map->getAllOccupiedBoxes(&b) : h->map->getAllFreeBoxes(&b);
+    }
+    const int64_t n = (int64_t)b.size();
+    for (int64_t i = 0; i < n && i < cap; ++i) {
+      for (int a = 0; a < 3; ++a) centres3[3 * i + a] = b[(size_t)i].first[a];
+      edges[i] = b[(size_t)i].second;
+    }
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// generateMarkerArray; returns the number of cubes, the first min(n, cap) written in list order (occupied depths 0..16,
+// then free depths 0..16): centres, colours (occupied cubes only, rgba4 holds cap of them), and per list its size and
+// length (sizes34, counts34).  LS_ERR_STATE on an error
+int64_t lsh_occupancy_marker_array(void* ov, double min_z, double max_z, double color_factor, double* centres3, float* rgba4,
+                                   double* sizes34, int64_t* counts34, int64_t cap) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    std::vector<OccupancyMap::CubeList> lists[2];
+    h->map->generateMarkerArray(min_z, max_z, color_factor, &lists[0], &lists[1]);
+    int64_t n = 0, k = 0;
+    for (int part = 0; part < 2; ++part)
+      for (size_t d = 0; d < lists[part].size(); ++d, ++k) {
+        const OccupancyMap::CubeList& l = lists[part][d];
+        sizes34[k] = l.size, counts34[k] = (int64_t)l.points.size();
+        for (size_t i = 0; i < l.points.size(); ++i, ++n) {
+          if (n >= cap) continue;
+          for (int a = 0; a < 3; ++a) centres3[3 * n + a] = l.points[i][a];
+          if (part == 0)
+            for (int a = 0; a < 4; ++a) rgba4[4 * n + a] = l.colors[i][(size_t)a];
+        }
+      }
+    return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
 // Box status.  single = 1: getCellStatusBoundingBox once per box, else the batched overload.  0 or LS_ERR_STATE
 int lsh_occupancy_box_status(void* ov, const double* c3, const double* s3, int n, int single, int8_t* status) {
   OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);

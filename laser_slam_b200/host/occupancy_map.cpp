@@ -165,6 +165,72 @@ void OccupancyMap::getVoxels(int which, std::vector<uint64_t>* keys, std::vector
   download(which, keys, log_odds, NULL);
 }
 
+// ---- leaf boxes and marker cubes ------------------------------------------------------------------------------------
+void OccupancyMap::boxes(int which, const kindr::minimal::Position* region_min, const kindr::minimal::Position* region_max,
+                         BoxVector* out) const {
+  if (out == NULL) throw std::invalid_argument("null output");
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_leaf_stats st;
+  throwOnError(ctx_, ls_occupancy_build_leaves(map_, region_min ? region_min->data() : NULL,
+                                               region_max ? region_max->data() : NULL, &st),
+               "ls_occupancy_build_leaves");
+  const int64_t n = which == LS_LEAVES_FREE ? st.free_leaves : st.occupied_leaves;
+  const size_t m = (size_t)(n > 0 ? n : 1);
+  std::vector<float> c(4 * m);
+  std::vector<uint8_t> depth(m);
+  std::vector<int8_t> state(m);
+  int64_t got = 0;
+  throwOnError(ctx_, ls_occupancy_download_leaves(map_, which, c.data(), depth.data(), state.data(), n, &got),
+               "ls_occupancy_download_leaves");
+  out->clear();
+  out->reserve((size_t)got);
+  for (int64_t i = 0; i < got; ++i)
+    out->emplace_back(kindr::minimal::Position{c[4 * i], c[4 * i + 1], c[4 * i + 2]},
+                      params_.resolution * std::ldexp(1.0, 16 - depth[(size_t)i]));
+}
+
+void OccupancyMap::getAllFreeBoxes(BoxVector* free_boxes) const { boxes(LS_LEAVES_FREE, NULL, NULL, free_boxes); }
+
+void OccupancyMap::getAllOccupiedBoxes(BoxVector* occupied_boxes) const {
+  boxes(LS_LEAVES_OCCUPIED, NULL, NULL, occupied_boxes);
+}
+
+void OccupancyMap::getAllFreeBoxes(const kindr::minimal::Position& region_min, const kindr::minimal::Position& region_max,
+                                   BoxVector* free_boxes) const {
+  boxes(LS_LEAVES_FREE, &region_min, &region_max, free_boxes);
+}
+
+void OccupancyMap::getAllOccupiedBoxes(const kindr::minimal::Position& region_min,
+                                       const kindr::minimal::Position& region_max, BoxVector* occupied_boxes) const {
+  boxes(LS_LEAVES_OCCUPIED, &region_min, &region_max, occupied_boxes);
+}
+
+void OccupancyMap::generateMarkerArray(double min_z, double max_z, double color_factor,
+                                       std::vector<CubeList>* occupied_nodes, std::vector<CubeList>* free_nodes) const {
+  if (occupied_nodes == NULL || free_nodes == NULL) throw std::invalid_argument("null output");
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_leaf_stats st;
+  throwOnError(ctx_, ls_occupancy_build_leaves(map_, NULL, NULL, &st), "ls_occupancy_build_leaves");
+  const int64_t n = st.free_leaves + st.occupied_leaves;
+  const size_t m = (size_t)(n > 0 ? n : 1);
+  std::vector<float> c(4 * m), rgba(4 * m);
+  int64_t occ[18], fre[18], got = 0;
+  throwOnError(ctx_, ls_occupancy_marker_cubes(map_, min_z, max_z, color_factor, c.data(), rgba.data(), occ, fre, n, &got),
+               "ls_occupancy_marker_cubes");
+  occupied_nodes->assign(17, CubeList());
+  free_nodes->assign(17, CubeList());
+  for (int d = 0; d < 17; ++d) {
+    CubeList& o = (*occupied_nodes)[(size_t)d];
+    CubeList& f = (*free_nodes)[(size_t)d];
+    o.size = f.size = params_.resolution * std::ldexp(1.0, 16 - d);
+    for (int64_t i = occ[d]; i < occ[d + 1]; ++i) {
+      o.points.push_back(kindr::minimal::Position{c[4 * i], c[4 * i + 1], c[4 * i + 2]});
+      o.colors.push_back(std::array<float, 4>{rgba[4 * i], rgba[4 * i + 1], rgba[4 * i + 2], rgba[4 * i + 3]});
+    }
+    for (int64_t i = fre[d]; i < fre[d + 1]; ++i) f.points.push_back(kindr::minimal::Position{c[4 * i], c[4 * i + 1], c[4 * i + 2]});
+  }
+}
+
 // ---- queries ------------------------------------------------------------------------------------------------------
 OccupancyMap::CellStatus OccupancyMap::cellStatus(const kindr::minimal::Position& point, float* log_odds) const {
   std::lock_guard<std::mutex> lock(mutex_);

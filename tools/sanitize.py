@@ -153,6 +153,18 @@ xo = np.array([0, 10, 10, 40, 64], np.int64)
 for unknown in (True, False):
     xw = ocl.check_paths(xvox, xc, xo, (1.0, 1.0, 0.5), 0.2, oc.logodds(0.7), unknown)
     assert np.array_equal(om.check_paths(xc, xo, (1.0, 1.0, 0.5), unknown), xw)
+# leaf boxes and marker cubes of that map (the leaf kernels in ls_occupancy.cu): a whole-map and a region listing and one
+# marker call, against the reference walk of the map's .ot payload
+import leaf_boxes_ref as lbr
+lv = lbr.leaves(om.full_octree().payload, 0.2, oc.logodds(0.7))
+lreg = (truth[0][:3, 3] - 3.0, truth[0][:3, 3] + 3.0)
+for r in (None, lreg):
+    lw, lg = lbr.select(lv, r, 0.2), om.leaf_boxes(ls.LEAVES_ALL, r)
+    assert len(lg.depths) > 0 and np.array_equal(lg.centres.view(np.uint32), lw["centres"].view(np.uint32))
+    assert np.array_equal(lg.depths, lw["depths"]) and np.array_equal(lg.states, lw["states"])
+lcubes = om.marker_cubes(-1.0, 3.0, 0.8)
+assert np.array_equal(np.concatenate([c.colors for c in lcubes.occupied]).view(np.uint32),
+                      lbr.marker_cubes(lv, -1.0, 3.0, 0.8)[1].view(np.uint32))
 om.clear()
 assert om.size(ls.OCC_KNOWN) == 0
 om.close()
