@@ -431,8 +431,9 @@ LS_HD Best nn_search(const Grid& g, const GridView& v, float qx, float qy, float
 // ---- certified candidate lists ("Verlet lists") ------------------------------------------------------------------
 // Between two ICP iterations a query moves by far less than the distance to its match, so the search result rarely
 // changes -- but "rarely" is not "never", and the contract is the EXACT nearest neighbour every iteration.  A list
-// makes the repeat provable: after a full search at position q0 the kernel also records EVERY map point within
-// R_v = |match| * ratio (capped by |match| + skin) of q0.  At a later position q (moved by delta = |q - q0|) any
+// makes the repeat provable: during a full search at position q0 the kernel also records EVERY map point within
+// R_v = d * ratio (capped by d + skin) of q0, d being the distance of the search's first candidate, an upper bound of
+// the match distance (nn_search_collect).  At a later position q (moved by delta = |q - q0|) any
 // point NOT in the list is farther than R_v - delta from q, hence: if the best listed candidate lies within
 // R_c = R_v - delta (minus rounding slack) it is the exact nearest neighbour -- ties included, since every point at
 // that distance is listed too; and if nothing lies within sqrt(cap) <= R_c the capped search provably finds nothing.
@@ -448,7 +449,7 @@ LS_HD Best nn_search(const Grid& g, const GridView& v, float qx, float qy, float
 #define LS_VK 8  // candidates per list; a ball holding more is not listed
 #endif
 static_assert(LS_VK <= 15, "the list header keeps the candidate count in 4 bits");
-// tuning knobs of vlist_build (tests/sim sweeps them; results never depend on them)
+// tuning knobs of vlist_radius (tests/sim sweeps them; results never depend on them)
 #ifndef LS_VL_ABS
 #define LS_VL_ABS 0.0f   // floor of the list margin [m]
 #endif
@@ -532,35 +533,90 @@ LS_HD bool vlist_query(const VLists& L, const float4* pts, int i, const float4 v
   return b.d2 * 1.00001f <= Rc * Rc;
 }
 
-// After a full search at (qx,qy,qz) whose answer was `found_d2` (or nothing within cap_d2): record every point within
-// R_v -- if that can pay off.  `motion` bounds how far the last ICP step moved this query; steps shrink geometrically,
-// so a list is only worth its second traversal when its margin (R_v minus the match distance) covers about twice
-// that.  A list that is not rebuilt is left as it is: it remains a true statement about its own q0.
-LS_HD void vlist_build(const Grid& g, const GridView& v, const VLists& L, int i, float qx, float qy, float qz, bool found,
-                       float found_d2, float cap_d2, float motion) {
+// The radius of the list to build at a query whose match lies within sqrt(found_d2) (found) -- or of which nothing is
+// known inside cap_d2 (!found) -- or 0: no list, it would not pay off.  `motion` bounds how far the last ICP step moved
+// this query; steps shrink geometrically, so a list is only worth its collection when its margin (R_v minus the match
+// distance) covers about twice that.  A list that is not rebuilt is left as it is: it remains a true statement about
+// its own q0.  Any R_v gives a valid certificate (every point within it is listed), so `found_d2` may be any upper
+// bound of the match distance.
+LS_HD float vlist_radius(bool found, float found_d2, float cap_d2, float motion) {
   float Rv;
   if (found) {
     const float want = sqrtf(found_d2);
     const float margin = fmaxf(want * LS_VL_REL, LS_VL_ABS) + 1e-4f;
-    if (!(motion * LS_VL_GATE <= margin)) return;
+    if (!(motion * LS_VL_GATE <= margin)) return 0.0f;
     Rv = want + fminf(margin, fmaxf(0.002f, LS_VL_SKIN * motion));
   } else {
     const float want = sqrtf(cap_d2);  // the cap itself moves a little between iterations: 5 % head room
-    if (!(motion <= want * 0.125f)) return;
+    if (!(motion <= want * 0.125f)) return 0.0f;
     Rv = want * 1.05f + fminf(want * 0.25f, fmaxf(0.002f, 4.0f * motion));
   }
-  if (!(Rv < 3.0e38f)) return;
+  return Rv < 3.0e38f ? Rv : 0.0f;
+}
+
+// The list header of a collection of radius Rv at (qx,qy,qz) that saw `cnt` points within it.  Every point with
+// fl(d2) <= fl(Rv*Rv) is recorded; the stored radius is rounded down twice (1 ulp for the square's rounding, then the
+// count bits).  More than LS_VK points: no list.
+LS_HD void vlist_head(const VLists& L, int i, float qx, float qy, float qz, float Rv, int cnt) {
+  float4 head = make_float4(qx, qy, qz, 0.0f);
+  if (cnt <= LS_VK) head.w = i2f((int)((((unsigned int)f2i(Rv * 0.9999999f)) & ~15u) | (unsigned int)cnt));
+  st_state4(L.vq + i, head);
+}
+
+// The list build in a walk of its own after a search whose answer was `found_d2` (or nothing within cap_d2).  The
+// kernel collects in the search's walk instead (nn_search_collect); tests/sim replays this as the reference it compares
+// against.
+LS_HD void vlist_build(const Grid& g, const GridView& v, const VLists& L, int i, float qx, float qy, float qz, bool found,
+                       float found_d2, float cap_d2, float motion) {
+  const float Rv = vlist_radius(found, found_d2, cap_d2, motion);
+  if (!(Rv > 0.0f)) return;
   Collector c;
   c.r2 = Rv * Rv;
   c.cnt = 0;
   c.out = L.vpts + i;
   c.stride = L.n;
   ball_query(g, v, qx, qy, qz, c);
-  // every point with fl(d2) <= fl(Rv*Rv) is recorded; the stored radius is rounded down twice (1 ulp for the
-  // square's rounding, then the count bits).  More than LS_VK points: no list.
-  float4 head = make_float4(qx, qy, qz, 0.0f);
-  if (c.cnt <= LS_VK) head.w = i2f((int)((((unsigned int)f2i(Rv * 0.9999999f)) & ~15u) | (unsigned int)c.cnt));
-  st_state4(L.vq + i, head);
+  vlist_head(L, i, qx, qy, qz, Rv, c.cnt);
+}
+
+// The search and the list's collection in one walk: `best` is exactly nn_search's accumulator, `list` collects every
+// point within its radius.  The walk covers the larger of the two balls while the list is collecting; once it
+// overflows, or when no list is wanted (list.r2 < 0), only the search's ball is left to walk.
+struct SearchCollect {
+  Best best;
+  Collector list;
+  LS_HD float bound() const { return fmaxf(best.d2, list.r2); }
+  LS_HD void offer_pt(float d, const float4& c, int p) {
+    best.offer_pt(d, c, p);
+    list.offer_pt(d, c, p);
+  }
+};
+
+// nn_search(.., warm_pos, cap_d2) that also rebuilds list i at (qx,qy,qz) when that can pay off (vlist_radius).  The
+// list radius is fixed before the walk from the first candidate -- the warm start, or the seed -- whose distance bounds
+// the match's; walking the search's cells a second time for the list would double the dependent round trips.
+LS_HD Best nn_search_collect(const Grid& g, const GridView& v, const VLists& L, int i, float qx, float qy, float qz,
+                             int warm_pos, float cap_d2, float motion) {
+  SearchCollect s;
+  Best& b = s.best;
+  b.d2 = cap_d2;
+  b.idx = INT_MAX;
+  b.pos = -1;
+  if (g.m <= 0) { b.idx = -1; b.d2 = INFINITY; return b; }
+  // the first candidate goes to the search only: the walk offers it again, and the list must see each point once
+  if (warm_pos >= 0) consider(v.pts, warm_pos, qx, qy, qz, b);
+  else seed_query(g, v, qx, qy, qz, b);
+  const float Rv = vlist_radius(b.pos >= 0, b.d2, cap_d2, motion);
+  // No list wanted: r2 < 0 collects nothing and leaves the search's own bound.  The same walk either way, so that the
+  // lanes of a warp that build a list and those that do not walk together instead of one group after the other.
+  s.list.r2 = Rv > 0.0f ? Rv * Rv : -1.0f;
+  s.list.cnt = 0;
+  s.list.out = L.vpts + i;
+  s.list.stride = L.n;
+  ball_query(g, v, qx, qy, qz, s);
+  if (Rv > 0.0f) vlist_head(L, i, qx, qy, qz, Rv, s.list.cnt);
+  if (b.pos < 0) { b.idx = -1; b.d2 = INFINITY; }
+  return b;
 }
 
 // Exact K nearest neighbours (ties: lower index first) by verified expanding balls: a round searches the ball of

@@ -1217,11 +1217,12 @@ __device__ __forceinline__ void drain_pairs(PairQueue& Q, unsigned long long* sl
   __syncwarp();
 }
 
-// Slow path of phase A: the search itself (warm-started, inside the cap), then -- from the second iteration on -- the
-// list that lets later iterations skip it (vlist_build decides whether it can pay off from how far the last step moved
-// this query: T_prev is the previous iteration's T_iter).  Not inlined: the search wants the whole register budget
-// for itself, not the caller's loop state spilled into its inner loops.  Called by all 32 lanes (i < 0: nothing to do);
-// the outcome is left in the query's state (P.pos / P.d2), where the caller -- the same thread -- reads it back.
+// Slow path of phase A: the search itself (warm-started, inside the cap) -- from the second iteration on together with
+// the list that lets later iterations skip it, in the same walk (nn_search_collect decides whether a list can pay off
+// from how far the last step moved this query: T_prev is the previous iteration's T_iter).  Not inlined: the search
+// wants the whole register budget for itself, not the caller's loop state spilled into its inner loops.  Called by all
+// 32 lanes (i < 0: nothing to do); the outcome is left in the query's state (P.pos / P.d2), where the caller -- the
+// same thread -- reads it back.
 __device__ __noinline__ void phase_a_search(const Grid* gp, const IcpProblem* Pp, const float* T_iter, const float* T_prev,
                                             int i, float cap, SelHists* H, unsigned int pred_bin1, unsigned int pred_pref12) {
   if (i < 0) return;
@@ -1231,13 +1232,15 @@ __device__ __noinline__ void phase_a_search(const Grid* gp, const IcpProblem* Pp
   float sx, sy, sz;
   xform_point(T_iter, r.x, r.y, r.z, sx, sy, sz);
   const int warm = __ldcg(P.pos + i);
-  const Best b = nn_search(g, P.view, sx, sy, sz, warm, cap);
-  phase_a_record(P, i, b, H, pred_bin1, pred_pref12);
+  Best b;
   if (T_prev) {
     float px, py, pz;
     xform_point(T_prev, r.x, r.y, r.z, px, py, pz);
-    vlist_build(g, P.view, P.lists, i, sx, sy, sz, b.pos >= 0, b.d2, cap, sqrtf(dist2(sx, sy, sz, px, py, pz)));
+    b = nn_search_collect(g, P.view, P.lists, i, sx, sy, sz, warm, cap, sqrtf(dist2(sx, sy, sz, px, py, pz)));
+  } else {
+    b = nn_search(g, P.view, sx, sy, sz, warm, cap);
   }
+  phase_a_record(P, i, b, H, pred_bin1, pred_pref12);
 }
 
 // Warp-collective: the queries just searched (j < 0: none on this lane) whose match lies inside the accumulation
