@@ -2336,9 +2336,8 @@ int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]) {
   const double res = om->prm.res;
   for (int a = 0; a < 3; ++a) {
     // octomap's calcMinMax over depth-16 leaves: the lower corner, and the lower corner plus the voxel size
-    const auto centre = [res](int k) { return (double)(float)(((double)(k - 32768) + 0.5) * res); };
-    min3[a] = empty ? 0.0 : centre(kmin[a]) - res / 2.0;
-    max3[a] = empty ? 0.0 : (centre(kmax[a]) - res / 2.0) + res;
+    min3[a] = empty ? 0.0 : (double)lso::centre_of(kmin[a], res) - res / 2.0;
+    max3[a] = empty ? 0.0 : ((double)lso::centre_of(kmax[a], res) - res / 2.0) + res;
   }
   return LS_OK;
 }
@@ -2346,9 +2345,9 @@ int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]) {
 }  // extern "C"
 
 namespace {
-// The key of a region corner in double, clamped to the key range: floor(c * (1/res)) + 32768 in [0, 65535].
+// The key of a region corner in double (lso::key_of's floor and offset), clamped to [0, 65535] instead of refused.
 int clamped_key(double inv, double c) {
-  const double s = std::floor(c * inv) + 32768.0;
+  const double s = std::floor(c * inv) + (double)lso::kKeyOffset;
   return s < 0.0 ? 0 : s > 65535.0 ? 65535 : (int)s;
 }
 }  // namespace
@@ -2510,14 +2509,6 @@ struct ls_distance_map {
 };
 
 namespace {
-// The map's key of a float coordinate: floor((double)c * inv) + 32768; false when outside [0, 65535] (NaN included).
-bool corner_key(double inv, float c, int* k) {
-  const double s = std::floor((double)c * inv);
-  if (!(s >= -32768.0 && s < 32768.0)) return false;
-  *k = (int)s + 32768;
-  return true;
-}
-
 void distance_stats(const ls_distance_map* dm, float ms, ls_distance_map_stats* stats) {
   if (!stats) return;
   const lso::DistanceField& f = dm->field;
@@ -2586,7 +2577,7 @@ int ls_distance_map_update(ls_distance_map* dm, ls_occupancy* om, ls_distance_ma
   int kmin[3], kmax[3];
   long long cells = 1;
   for (int a = 0; a < 3; ++a) {
-    if (!corner_key(inv, p.bbx_min[a], &kmin[a]) || !corner_key(inv, p.bbx_max[a], &kmax[a]))
+    if (!lso::key_of(inv, p.bbx_min[a], kmin[a]) || !lso::key_of(inv, p.bbx_max[a], kmax[a]))
       return fail(ctx, LS_ERR_ARG, "a box corner has no valid key on axis %d at resolution %g", a, res);
     if (kmin[a] > kmax[a]) return fail(ctx, LS_ERR_ARG, "box min key above max key on axis %d", a);
     cells *= kmax[a] - kmin[a] + 1;

@@ -23,26 +23,7 @@
 namespace lso {
 namespace {
 
-constexpr int kKey0 = 32768;
 constexpr int kWords = 32;  // per baseline brick: 16 known words, then 16 occupied words
-
-int code(cudaError_t e) {
-  if (e == cudaSuccess) return LS_OK;
-  cudaGetLastError();
-  return e == cudaErrorMemoryAllocation ? LS_ERR_NOMEM : LS_ERR_CUDA;
-}
-
-#define CH_TRY(call)            \
-  do {                          \
-    const int rc_ = code(call); \
-    if (rc_) return rc_;        \
-  } while (0)
-
-#define CH_LAUNCHED()           \
-  do {                          \
-    ++*launches;                \
-    CH_TRY(cudaGetLastError()); \
-  } while (0)
 
 // (a): blockDim 512, warp w owns known word w of the brick.
 __global__ void __launch_bounds__(512) ch_capture_kernel(const unsigned long long* __restrict__ bkey,
@@ -94,9 +75,9 @@ __device__ __forceinline__ void emit(bool changed, unsigned long long bk, int t,
   base = __shfl_sync(0xffffffffu, base, 0);
   if (changed && out_key) {
     const unsigned long long pos = base + __popc(bal & ((1u << lane) - 1u));
-    const unsigned long long kx = (bk & 0x1fff) * 8 + (t & 7), ky = ((bk >> 13) & 0x1fff) * 8 + ((t >> 3) & 7),
-                             kz = ((bk >> 26) & 0x1fff) * 8 + (t >> 6);
-    out_key[pos] = kx | (ky << 16) | (kz << 32);
+    int k[3];
+    voxel_keys(bk, t, k);
+    out_key[pos] = pack(k[0], k[1], k[2]);
     out_val[pos] = (unsigned)now | ((unsigned)then << 2);
   }
 }
@@ -157,29 +138,27 @@ __global__ void ch_finish_kernel(const unsigned long long* __restrict__ keys, co
   const double res = now == LS_CELL_UNKNOWN ? res_base : res_now;
   const unsigned long long k = keys[i];
   float c[3];
-  for (int a = 0; a < 3; ++a) c[a] = (float)(((double)((int)((k >> (16 * a)) & 0xffff) - kKey0) + 0.5) * res);
+  for (int a = 0; a < 3; ++a) c[a] = centre_of((int)((k >> (16 * a)) & 0xffff), res);
   centres[i] = make_float4(c[0], c[1], c[2], 1.0f);
 }
-
-unsigned blocks(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
 // Grows an array of a group to at least `need` elements (an eighth more), after the stream's pending work.
 template <class T>
 int grow(ls::Buffer<T>& b, long long need, cudaStream_t st) {
   if ((size_t)need <= b.capacity()) return LS_OK;
-  CH_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return code(b.reserve((size_t)need, (size_t)(need + need / 8 + 64)));
 }
 
 int grow_cub(Changes& c, size_t bytes, cudaStream_t st) {
   if (bytes <= c.cub_tmp.capacity()) return LS_OK;
-  CH_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return code(c.cub_tmp.reserve(bytes, bytes + bytes / 8));
 }
 
 int read_count(Changes& c, cudaStream_t st, long long* n) {
-  CH_TRY(cudaMemcpyAsync(c.cnt_host.get(), c.cnt_dev.get(), sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CH_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemcpyAsync(c.cnt_host.get(), c.cnt_dev.get(), sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   *n = (long long)*c.cnt_host.get();
   return LS_OK;
 }
@@ -187,17 +166,17 @@ int read_count(Changes& c, cudaStream_t st, long long* n) {
 // One pass of (c) and (d): counts into cnt_dev, and with out_key emits.
 int diff_pass(Changes& c, const Map& m, const Params& P, unsigned long long* out_key, unsigned* out_val, cudaStream_t st,
               uint64_t* launches) {
-  CH_TRY(cudaMemsetAsync(c.cnt_dev.get(), 0, sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(c.cnt_dev.get(), 0, sizeof(unsigned long long), st));
   if (m.pool_n > 0) {
     ch_current_kernel<<<m.pool_n, 512, 0, st>>>(m.bkey.get(), m.known.get(), m.lo.get(), P.l_occ, c.base.keys.get(),
                                                 c.base.bits.get(), c.base.n, out_key, out_val, c.cnt_dev.get());
-    CH_LAUNCHED();
+    LSO_LAUNCHED();
   }
   if (c.base.n > 0) {
     ch_baseline_kernel<<<(unsigned)c.base.n, 512, 0, st>>>(m.tab_keys.get(), m.tab_vals.get(), (unsigned)m.tab_cap() - 1u,
                                                            c.base.keys.get(), c.base.bits.get(), out_key, out_val,
                                                            c.cnt_dev.get());
-    CH_LAUNCHED();
+    LSO_LAUNCHED();
   }
   return LS_OK;
 }
@@ -205,18 +184,18 @@ int diff_pass(Changes& c, const Map& m, const Params& P, unsigned long long* out
 }  // namespace
 
 int capture_baseline(Changes& c, const Map& m, const Params& P, cudaStream_t st, uint64_t* launches) {
-  CH_TRY(c.cnt_dev.reserve(1, 1));
-  CH_TRY(c.cnt_host.reserve(1, 1));
+  LSO_TRY(c.cnt_dev.reserve(1, 1));
+  LSO_TRY(c.cnt_host.reserve(1, 1));
   const long long nb = m.pool_n;
   int rc;
   if ((rc = grow(c.rec_key, nb, st)) || (rc = grow(c.rec_idx[0], nb, st)) ||
       (rc = grow(c.rec_idx[1], nb, st)) || (rc = grow(c.rec_bits, nb * kWords, st)))
     return rc;
-  CH_TRY(cudaMemsetAsync(c.cnt_dev.get(), 0, sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(c.cnt_dev.get(), 0, sizeof(unsigned long long), st));
   if (nb > 0) {
     ch_capture_kernel<<<(unsigned)nb, 512, 0, st>>>(m.bkey.get(), m.known.get(), m.lo.get(), P.l_occ, c.rec_key.get(),
                                                     c.rec_idx[0].get(), c.rec_bits.get(), c.cnt_dev.get());
-    CH_LAUNCHED();
+    LSO_LAUNCHED();
   }
   long long n = 0;
   if ((rc = read_count(c, st, &n))) return rc;
@@ -224,18 +203,18 @@ int capture_baseline(Changes& c, const Map& m, const Params& P, cudaStream_t st,
   if ((rc = grow(nx.keys, n, st)) || (rc = grow(nx.bits, n * kWords, st))) return rc;
   if (n > 0) {
     size_t bytes = 0;
-    CH_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, c.rec_key.get(), nx.keys.get(), c.rec_idx[0].get(),
+    LSO_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, c.rec_key.get(), nx.keys.get(), c.rec_idx[0].get(),
                                            c.rec_idx[1].get(), (int)n, 0, 39, st));
     if ((rc = grow_cub(c, bytes, st))) return rc;
     bytes = c.cub_tmp.capacity();
-    CH_TRY(cub::DeviceRadixSort::SortPairs(c.cub_tmp.get(), bytes, c.rec_key.get(), nx.keys.get(), c.rec_idx[0].get(),
+    LSO_TRY(cub::DeviceRadixSort::SortPairs(c.cub_tmp.get(), bytes, c.rec_key.get(), nx.keys.get(), c.rec_idx[0].get(),
                                            c.rec_idx[1].get(), (int)n, 0, 39, st));
     ++*launches;
     ch_gather_kernel<<<blocks(n * kWords, 256), 256, 0, st>>>(c.rec_idx[1].get(), c.rec_bits.get(), n * kWords,
                                                               nx.bits.get());
-    CH_LAUNCHED();
+    LSO_LAUNCHED();
   }
-  CH_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   nx.n = n;
   nx.res = P.res;
   std::swap(c.base, c.next);
@@ -257,23 +236,23 @@ int diff_changes(Changes& c, const Map& m, const Params& P, uint64_t* keys, int8
     return rc;
   if ((rc = diff_pass(c, m, P, c.out_key[0].get(), c.out_val[0].get(), st, launches))) return rc;
   size_t bytes = 0;
-  CH_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, c.out_key[0].get(), c.out_key[1].get(), c.out_val[0].get(),
+  LSO_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, c.out_key[0].get(), c.out_key[1].get(), c.out_val[0].get(),
                                          c.out_val[1].get(), (int)cnt, 0, 48, st));
   if ((rc = grow_cub(c, bytes, st))) return rc;
   bytes = c.cub_tmp.capacity();
-  CH_TRY(cub::DeviceRadixSort::SortPairs(c.cub_tmp.get(), bytes, c.out_key[0].get(), c.out_key[1].get(), c.out_val[0].get(),
+  LSO_TRY(cub::DeviceRadixSort::SortPairs(c.cub_tmp.get(), bytes, c.out_key[0].get(), c.out_key[1].get(), c.out_val[0].get(),
                                          c.out_val[1].get(), (int)cnt, 0, 48, st));
   ++*launches;
   signed char* st_now = c.out_st.get();
   ch_finish_kernel<<<blocks(cnt, 256), 256, 0, st>>>(c.out_key[1].get(), c.out_val[1].get(), cnt, P.res, c.base.res, st_now,
                                                      st_now + cnt, c.out_c.get());
-  CH_LAUNCHED();
+  LSO_LAUNCHED();
   const size_t N = (size_t)cnt;
-  if (keys) CH_TRY(cudaMemcpyAsync(keys, c.out_key[1].get(), 8 * N, cudaMemcpyDeviceToHost, st));
-  if (status) CH_TRY(cudaMemcpyAsync(status, st_now, N, cudaMemcpyDeviceToHost, st));
-  if (previous) CH_TRY(cudaMemcpyAsync(previous, st_now + cnt, N, cudaMemcpyDeviceToHost, st));
-  if (centres4) CH_TRY(cudaMemcpyAsync(centres4, c.out_c.get(), 16 * N, cudaMemcpyDeviceToHost, st));
-  CH_TRY(cudaStreamSynchronize(st));
+  if (keys) LSO_TRY(cudaMemcpyAsync(keys, c.out_key[1].get(), 8 * N, cudaMemcpyDeviceToHost, st));
+  if (status) LSO_TRY(cudaMemcpyAsync(status, st_now, N, cudaMemcpyDeviceToHost, st));
+  if (previous) LSO_TRY(cudaMemcpyAsync(previous, st_now + cnt, N, cudaMemcpyDeviceToHost, st));
+  if (centres4) LSO_TRY(cudaMemcpyAsync(centres4, c.out_c.get(), 16 * N, cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
 

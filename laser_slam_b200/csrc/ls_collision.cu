@@ -21,7 +21,6 @@
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
-#include <utility>
 #include <vector>
 
 #include <cub/cub.cuh>
@@ -33,7 +32,6 @@
 namespace lso {
 namespace {
 
-constexpr int kKey0 = 32768;
 constexpr long long kMaxAxisPoints = 1LL << 17;  // loop points per box axis
 constexpr unsigned kFlagOcc = 1u, kFlagUnk = 2u;
 constexpr unsigned kNone = 0xffffffffu;  // a path without a collision (yet)
@@ -48,24 +46,6 @@ struct CallCounters {
   double work;
 };
 
-int code(cudaError_t e) {
-  if (e == cudaSuccess) return LS_OK;
-  cudaGetLastError();
-  return e == cudaErrorMemoryAllocation ? LS_ERR_NOMEM : LS_ERR_CUDA;
-}
-
-#define CO_TRY(call)            \
-  do {                          \
-    const int rc_ = code(call); \
-    if (rc_) return rc_;        \
-  } while (0)
-
-#define CO_LAUNCHED()           \
-  do {                          \
-    ++*launches;                \
-    CO_TRY(cudaGetLastError()); \
-  } while (0)
-
 // One axis of one box after (a).  The passing keys [oa, ob] (empty when oa > ob) are those between the corner keys whose
 // cube meets [bmin, bmax]; `corners` is 0 when a corner key is invalid (no occupied pass for the box).  The axis's bricks
 // are b0 ... b0 + nb - 1.
@@ -75,33 +55,10 @@ struct Axis {
   int corners, invalid;  // invalid: some loop point has an invalid key
 };
 
-// floor(c * inv) + 32768, valid iff in [0, 65535]: the double rule (octomap's search(x, y, z)) and, with a float
-// argument, the float rule of every other key in the map
-__device__ __forceinline__ bool key_d(double inv, double c, int& k) {
-  const double s = floor(c * inv);
-  if (!(s >= -(double)kKey0 && s < (double)kKey0)) return false;
-  k = (int)s + kKey0;
-  return true;
-}
-__device__ __forceinline__ bool key_f(double inv, float c, int& k) { return key_d(inv, (double)c, k); }
-
-__device__ __forceinline__ unsigned long long brick_key3(int bx, int by, int bz) {
-  return (unsigned long long)bx | ((unsigned long long)by << 13) | ((unsigned long long)bz << 26);
-}
-
-// State (LS_CELL_*) of voxel k, reading the hash, the known bit and the log-odds.
-__device__ __forceinline__ int voxel_state(const unsigned long long* tab_keys, const int* tab_vals, unsigned mask,
-                                           const unsigned* known, const float* lo, float l_occ, const int k[3]) {
-  const int b = lookup_brick(tab_keys, tab_vals, mask, brick_key3(k[0] >> 3, k[1] >> 3, k[2] >> 3));
-  if (b < 0) return LS_CELL_UNKNOWN;
-  const int local = (k[0] & 7) | ((k[1] & 7) << 3) | ((k[2] & 7) << 6);
-  if (!((known[(size_t)b * 16 + (local >> 5)] >> (local & 31)) & 1u)) return LS_CELL_UNKNOWN;
-  return lo[(size_t)b * 512 + local] >= l_occ ? LS_CELL_OCCUPIED : LS_CELL_FREE;
-}
-
-// The centre of box i has a valid key on every axis by the double rule (step 1 can look it up).
+// The centre of box i has a valid key on every axis by the double rule, octomap's search(x, y, z) (step 1 can look it up).
+// Every other key of the call is a float coordinate's.
 __device__ __forceinline__ bool centre_keys(const double* c3, long long i, double inv, int k[3]) {
-  return key_d(inv, c3[3 * i], k[0]) && key_d(inv, c3[3 * i + 1], k[1]) && key_d(inv, c3[3 * i + 2], k[2]);
+  return key_of(inv, c3[3 * i], k[0]) && key_of(inv, c3[3 * i + 1], k[1]) && key_of(inv, c3[3 * i + 2], k[2]);
 }
 
 // (a): one thread per (box, axis).  s_stride 3: a size per box; 0: one size for every box (the robot's).
@@ -129,7 +86,7 @@ __global__ void co_axis_kernel(const double* __restrict__ c3, const double* __re
         atomicOr(refused, 2u);
         break;
       }
-      if (key_f(inv, (float)x, k)) {
+      if (key_of(inv, (float)x, k)) {
         if (first < 0) first = k;
         last = k;
       } else {
@@ -139,10 +96,10 @@ __global__ void co_axis_kernel(const double* __restrict__ c3, const double* __re
     if (points <= kMaxAxisPoints) {
       int kmin, kmax;
       const double half = res / 2;
-      if (key_f(inv, bmin, kmin) && key_f(inv, bmax, kmax)) {
+      if (key_of(inv, bmin, kmin) && key_of(inv, bmax, kmax)) {
         A.corners = 1;
         for (int q = kmin; q <= kmax; ++q) {  // the cube test of every key in the range
-          const double c = ((double)(q - kKey0) + 0.5) * res;
+          const double c = centre_d(q, res);
           if (c + half < (double)bmin || c - half > (double)bmax) continue;
           if (A.oa > A.ob) A.oa = q;
           A.ob = q;
@@ -180,10 +137,11 @@ __global__ void co_box_kernel(const double* __restrict__ c3, long long n, double
       st = LS_CELL_UNKNOWN;  // step 1: an invalid key is unknown
     } else {
       ++v;
-      const int s = voxel_state(tab_keys, tab_vals, tab_mask, known, lo, l_occ, k);
+      const int b = lookup_brick(tab_keys, tab_vals, tab_mask, brick_key(k));
+      const int s = b < 0 ? LS_CELL_UNKNOWN : voxel_state(known, lo, l_occ, b, local_of(k), nullptr);
       if (s != LS_CELL_FREE) st = s;
-      else if (!(key_f(inv, (float)c3[3 * i], k[0]) && key_f(inv, (float)c3[3 * i + 1], k[1]) &&
-                 key_f(inv, (float)c3[3 * i + 2], k[2])))
+      else if (!(key_of(inv, (float)c3[3 * i], k[0]) && key_of(inv, (float)c3[3 * i + 1], k[1]) &&
+                 key_of(inv, (float)c3[3 * i + 2], k[2])))
         st = LS_CELL_UNKNOWN;  // step 2: the float centre's key is invalid
     }
     const Axis X = axes[3 * i], Y = axes[3 * i + 1], Z = axes[3 * i + 2];
@@ -241,7 +199,7 @@ __global__ void co_mask_kernel(const double* __restrict__ c3, const double* __re
   int cur = -1, k;
   unsigned bits = 0;
   for (double x = bmin; x <= bmax; x += res) {  // (a) counted it: at most 2^17 points
-    if (!key_f(inv, (float)x, k)) continue;
+    if (!key_of(inv, (float)x, k)) continue;
     const int j = (k >> 3) - A.b0;
     if (j != cur) {
       if (cur >= 0) m[cur] |= (unsigned short)bits;
@@ -297,7 +255,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) co_voxel_kernel(
     const unsigned lx = loop_needed ? mx & 0xffu : 0u, ly = my & 0xffu, lz = mz & 0xffu;
     if (!(ox && oy && oz) && !(lx && ly && lz)) continue;
     int b = -1;
-    if (lane == 0) b = lookup_brick(tab_keys, tab_vals, tab_mask, brick_key3(X.b0 + (int)jx, Y.b0 + (int)jy, Z.b0 + (int)jz));
+    if (lane == 0) b = lookup_brick(tab_keys, tab_vals, tab_mask, brick_pack(X.b0 + (int)jx, Y.b0 + (int)jy, Z.b0 + (int)jz));
     b = __shfl_sync(0xffffffffu, b, 0);
     const unsigned kw = (b >= 0 && lane < 16) ? known[(size_t)b * 16 + lane] : 0u;
     const int x = lane & 7, ylo = (lane >> 3) & 3;
@@ -339,29 +297,6 @@ __global__ void co_result_kernel(long long n, const signed char* __restrict__ de
   status[i] = (signed char)(d >= 0 ? d : (f & kFlagOcc) ? LS_CELL_OCCUPIED : (f & kFlagUnk) ? LS_CELL_UNKNOWN : LS_CELL_FREE);
 }
 
-unsigned blocks(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
-
-size_t take(size_t& off, size_t bytes) {
-  const size_t o = off;
-  off += (bytes + 255) & ~(size_t)255;
-  return o;
-}
-
-// The query staging of at least `bytes`, grown by doubling; the first `keep` bytes survive a growth.
-int reserve_staging(Map& m, size_t bytes, size_t keep, cudaStream_t st) {
-  if (bytes <= m.qbuf.capacity()) return LS_OK;
-  CO_TRY(cudaStreamSynchronize(st));
-  size_t cap = m.qbuf.capacity() ? 2 * m.qbuf.capacity() : (size_t)1 << 16;
-  while (cap < bytes) cap *= 2;
-  if (keep == 0) return code(m.qbuf.reserve(bytes, cap));
-  ls::Buffer<char> grown;
-  CO_TRY(grown.reserve(bytes, cap));
-  CO_TRY(cudaMemcpyAsync(grown.get(), m.qbuf.get(), keep, cudaMemcpyDeviceToDevice, st));
-  CO_TRY(cudaStreamSynchronize(st));
-  m.qbuf = std::move(grown);
-  return LS_OK;
-}
-
 // Both calls: n boxes (centres c3, sizes s3 with stride s_stride) on the device; path mode when offsets is not NULL.
 int collide(Map& m, const Params& P, const double* c3, const double* s3, int s_stride, long long n, const int64_t* offsets,
             int n_paths, int unknown_occ, int8_t* status, int64_t* first, long long* visited, cudaStream_t st,
@@ -381,8 +316,8 @@ int collide(Map& m, const Params& P, const double* c3, const double* s3, int s_s
                o_flags = take(off, (size_t)n * sizeof(unsigned)), o_pid = take(off, paths ? (size_t)n * sizeof(int) : 0),
                o_best = take(off, paths ? (size_t)n_paths * sizeof(unsigned) : 0), o_ctr = take(off, sizeof(CallCounters));
   size_t cub_a = 0, cub_b = 0;
-  CO_TRY(cub::DeviceScan::InclusiveSum(nullptr, cub_a, (long long*)nullptr, (long long*)nullptr, (int64_t)n3, st));
-  CO_TRY(cub::DeviceScan::InclusiveSum(nullptr, cub_b, (long long*)nullptr, (long long*)nullptr, (int64_t)n, st));
+  LSO_TRY(cub::DeviceScan::InclusiveSum(nullptr, cub_a, (long long*)nullptr, (long long*)nullptr, (int64_t)n3, st));
+  LSO_TRY(cub::DeviceScan::InclusiveSum(nullptr, cub_b, (long long*)nullptr, (long long*)nullptr, (int64_t)n, st));
   const size_t cub_bytes = cub_a > cub_b ? cub_a : cub_b;
   const size_t o_cub = take(off, cub_bytes);
   int rc;
@@ -400,34 +335,34 @@ int collide(Map& m, const Params& P, const double* c3, const double* s3, int s_s
   unsigned* best = paths ? (unsigned*)(q + o_best) : nullptr;
   CallCounters* ctr = (CallCounters*)(q + o_ctr);
   unsigned long long* vis = (unsigned long long*)(q + o_vis);
-  CO_TRY(cudaMemcpyAsync(q + o_c, c3, n3 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CO_TRY(cudaMemcpyAsync(q + o_s, s3, (s_stride ? n3 : 3) * sizeof(double), cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_c, c3, n3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_s, s3, (s_stride ? n3 : 3) * sizeof(double), cudaMemcpyHostToDevice, st));
   if (paths) {
-    CO_TRY(cudaMemcpyAsync(q + o_off, offsets, ((size_t)n_paths + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-    CO_TRY(cudaMemsetAsync(best, 0xff, (size_t)n_paths * sizeof(unsigned), st));
+    LSO_TRY(cudaMemcpyAsync(q + o_off, offsets, ((size_t)n_paths + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+    LSO_TRY(cudaMemsetAsync(best, 0xff, (size_t)n_paths * sizeof(unsigned), st));
   }
-  CO_TRY(cudaMemsetAsync(vis, 0, sizeof(unsigned long long), st));
-  CO_TRY(cudaMemsetAsync(ctr, 0, sizeof(CallCounters), st));
+  LSO_TRY(cudaMemsetAsync(vis, 0, sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(ctr, 0, sizeof(CallCounters), st));
   const unsigned tab_mask = (unsigned)m.tab_cap() - 1u;
   co_axis_kernel<<<blocks(3 * n, 256), 256, 0, st>>>(dc, ds, s_stride, n, P.res, P.inv, ax, nb, ctr);
-  CO_LAUNCHED();
+  LSO_LAUNCHED();
   co_box_kernel<<<blocks(n, 256), 256, 0, st>>>(dc, n, P.inv, m.tab_keys.get(), m.tab_vals.get(), tab_mask, m.known.get(),
                                                 m.lo.get(), P.l_occ, ax, nb, items, dec, flags, doff, n_paths, unknown_occ,
                                                 pid, best, vis, ctr);
-  CO_LAUNCHED();
+  LSO_LAUNCHED();
   size_t bytes = cub_bytes;
-  CO_TRY(cub::DeviceScan::InclusiveSum(q + o_cub, bytes, nb, moff, (int64_t)n3, st));
+  LSO_TRY(cub::DeviceScan::InclusiveSum(q + o_cub, bytes, nb, moff, (int64_t)n3, st));
   bytes = cub_bytes;
-  CO_TRY(cub::DeviceScan::InclusiveSum(q + o_cub, bytes, items, iinc, (int64_t)n, st));
+  LSO_TRY(cub::DeviceScan::InclusiveSum(q + o_cub, bytes, items, iinc, (int64_t)n, st));
   *launches += 2;
   struct {
     CallCounters c;
     long long masks, total;
   } h{};
-  CO_TRY(cudaMemcpyAsync(&h.c, ctr, sizeof(CallCounters), cudaMemcpyDeviceToHost, st));
-  CO_TRY(cudaMemcpyAsync(&h.masks, moff + n3 - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
-  CO_TRY(cudaMemcpyAsync(&h.total, iinc + n - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
-  CO_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemcpyAsync(&h.c, ctr, sizeof(CallCounters), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaMemcpyAsync(&h.masks, moff + n3 - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaMemcpyAsync(&h.total, iinc + n - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   if (h.c.refused || !(h.c.work <= kMaxWork)) return LS_ERR_ARG;
   if (h.total > 0) {
     const size_t keep = off;
@@ -442,19 +377,19 @@ int collide(Map& m, const Params& P, const double* c3, const double* s3, int s_s
     vis = (unsigned long long*)(q + o_vis);
     unsigned short* masks = (unsigned short*)(q + o_mask);
     co_mask_kernel<<<blocks(3 * n, 256), 256, 0, st>>>(dc, ds, s_stride, n, P.res, P.inv, ax, nb, moff, masks);
-    CO_LAUNCHED();
+    LSO_LAUNCHED();
     const unsigned grid = (unsigned)std::min<long long>((h.total + kWarpsPerBlock - 1) / kWarpsPerBlock, kVoxelBlocks);
     co_voxel_kernel<<<grid, 32 * kWarpsPerBlock, 0, st>>>(
         h.total, n, iinc, ax, nb, moff, masks, m.tab_keys.get(), m.tab_vals.get(), tab_mask, m.known.get(), m.lo.get(),
         P.l_occ, paths ? unknown_occ : 1, flags, doff, pid, unknown_occ, best, vis);
-    CO_LAUNCHED();
+    LSO_LAUNCHED();
   }
   co_result_kernel<<<blocks(n_out, 256), 256, 0, st>>>(n_out, dec, flags, best, (signed char*)(q + o_res),
                                                        (long long*)(q + o_res));
-  CO_LAUNCHED();
+  LSO_LAUNCHED();
   std::vector<char> back(sizeof(unsigned long long) + (paths ? 8 * (size_t)n_out : (size_t)n_out));
-  CO_TRY(cudaMemcpyAsync(back.data(), q + o_vis, back.size(), cudaMemcpyDeviceToHost, st));
-  CO_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemcpyAsync(back.data(), q + o_vis, back.size(), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   unsigned long long v;
   std::memcpy(&v, back.data(), sizeof v);
   *visited = (long long)v;

@@ -29,26 +29,7 @@ namespace lso {
 namespace {
 
 constexpr int kNoSite = INT_MAX;  // the value of a cell without a site in (b) and (c)
-constexpr int kKey0 = 32768;
 constexpr unsigned kNanBits = 0x7fc00000u;
-
-int code(cudaError_t e) {
-  if (e == cudaSuccess) return LS_OK;
-  cudaGetLastError();
-  return e == cudaErrorMemoryAllocation ? LS_ERR_NOMEM : LS_ERR_CUDA;
-}
-
-#define DT_TRY(call)            \
-  do {                          \
-    const int rc_ = code(call); \
-    if (rc_) return rc_;        \
-  } while (0)
-
-#define DT_LAUNCHED()           \
-  do {                          \
-    ++*launches;                \
-    DT_TRY(cudaGetLastError()); \
-  } while (0)
 
 struct Box {
   int kmin[3], size[3];
@@ -58,8 +39,8 @@ __global__ void __launch_bounds__(512) dt_extract_kernel(const unsigned long lon
                                                          const unsigned* __restrict__ known, const float* __restrict__ lo,
                                                          Box B, float l_occ, int unknown_occ, unsigned char* __restrict__ grid) {
   const int b = blockIdx.x, t = threadIdx.x;
-  const unsigned long long bk = bkey[b];
-  const int base[3] = {(int)(bk & 0x1fff) * 8, (int)((bk >> 13) & 0x1fff) * 8, (int)((bk >> 26) & 0x1fff) * 8};
+  int base[3];  // the brick's first voxel
+  voxel_keys(bkey[b], 0, base);
   for (int a = 0; a < 3; ++a)
     if (base[a] + 7 < B.kmin[a] || base[a] > B.kmin[a] + B.size[a] - 1) return;  // the whole block: the brick misses the box
   const int c[3] = {base[0] + (t & 7) - B.kmin[0], base[1] + ((t >> 3) & 7) - B.kmin[1], base[2] + (t >> 6) - B.kmin[2]};
@@ -178,9 +159,7 @@ __global__ void dt_col_kernel(const int* __restrict__ gin, const int* __restrict
   }
 }
 
-__device__ __forceinline__ float centre_of(int k, double res) { return (float)(((double)(k - kKey0) + 0.5) * res); }
-
-// One thread per point: the key of each float coordinate, floor((double)c * inv) + 32768, inside the box or -1 / NaN.
+// One thread per point: the key of each float coordinate (key_of), inside the box or -1 / NaN.
 __global__ void dt_query_kernel(const float* __restrict__ pts3, int n, Box B, double inv, double res, const int* __restrict__ val,
                                 const int* __restrict__ site, float* __restrict__ dist, int* __restrict__ sq,
                                 float* __restrict__ obst3, unsigned long long* __restrict__ outside) {
@@ -190,12 +169,12 @@ __global__ void dt_query_kernel(const float* __restrict__ pts3, int n, Box B, do
     int c[3];
     bool in = true;
     for (int a = 0; a < 3; ++a) {
-      const double s = floor((double)pts3[3 * (size_t)i + a] * inv);
-      if (!(s >= -(double)kKey0 && s < (double)kKey0)) {
+      int k;
+      if (!key_of(inv, pts3[3 * (size_t)i + a], k)) {
         in = false;
         continue;
       }
-      c[a] = (int)s + kKey0 - B.kmin[a];
+      c[a] = k - B.kmin[a];
       if (c[a] < 0 || c[a] >= B.size[a]) in = false;
     }
     int s = -1, w = -1;
@@ -232,8 +211,7 @@ __global__ void dt_keys_kernel(const int* __restrict__ site, long long cells, Bo
     return;
   }
   const int wx = w % B.size[0], wy = (w / B.size[0]) % B.size[1], wz = w / B.size[0] / B.size[1];
-  keys[i] = (unsigned long long)(B.kmin[0] + wx) | ((unsigned long long)(B.kmin[1] + wy) << 16) |
-            ((unsigned long long)(B.kmin[2] + wz) << 32);
+  keys[i] = pack(B.kmin[0] + wx, B.kmin[1] + wy, B.kmin[2] + wz);
 }
 
 Box box_of(const DistanceField& f) {
@@ -241,8 +219,6 @@ Box box_of(const DistanceField& f) {
   for (int a = 0; a < 3; ++a) B.kmin[a] = f.kmin[a], B.size[a] = f.size[a];
   return B;
 }
-
-unsigned blocks(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
 }  // namespace
 
@@ -267,25 +243,25 @@ int distance_reserve(DistanceField& f, long long cells) {
 int distance_update(DistanceField& f, const Map& m, float l_occ, bool unknown_occ, cudaStream_t st, uint64_t* launches) {
   const Box B = box_of(f);
   const long long sx = f.size[0], sy = f.size[1], sz = f.size[2], cells = f.cells, M = f.M;
-  DT_TRY(cudaMemsetAsync(f.grid.get(), unknown_occ ? 1 : 0, (size_t)cells, st));
-  DT_TRY(cudaMemsetAsync(f.cnt_dev.get(), 0, sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(f.grid.get(), unknown_occ ? 1 : 0, (size_t)cells, st));
+  LSO_TRY(cudaMemsetAsync(f.cnt_dev.get(), 0, sizeof(unsigned long long), st));
   if (m.pool_n > 0) {
     dt_extract_kernel<<<m.pool_n, 512, 0, st>>>(m.bkey.get(), m.known.get(), m.lo.get(), B, l_occ, unknown_occ ? 1 : 0,
                                                 f.grid.get());
-    DT_LAUNCHED();
+    LSO_LAUNCHED();
   }
   dt_row_kernel<<<blocks(sy * sz * 32, 256), 256, 0, st>>>(f.grid.get(), (int)sx, sy * sz, M, f.val[0].get(), f.site[0].get(),
                                                            f.cnt_dev.get());
-  DT_LAUNCHED();
+  LSO_LAUNCHED();
   // y: columns (x, z), outer sx * sy; z: columns (x, y), outer sx
   dt_col_kernel<<<blocks(sx * sz, 128), 128, 0, st>>>(f.val[0].get(), f.site[0].get(), f.val[1].get(), f.site[1].get(),
                                                       f.stack.get(), sx * sz, (int)sx, sx * sy, sx, (int)sy, M, 0);
-  DT_LAUNCHED();
+  LSO_LAUNCHED();
   dt_col_kernel<<<blocks(sx * sy, 128), 128, 0, st>>>(f.val[1].get(), f.site[1].get(), f.val[0].get(), f.site[0].get(),
                                                       f.stack.get(), sx * sy, (int)sx, sx, sx * sy, (int)sz, M, 1);
-  DT_LAUNCHED();
-  DT_TRY(cudaMemcpyAsync(f.cnt_host.get(), f.cnt_dev.get(), sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  DT_TRY(cudaStreamSynchronize(st));
+  LSO_LAUNCHED();
+  LSO_TRY(cudaMemcpyAsync(f.cnt_host.get(), f.cnt_dev.get(), sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   f.obstacles = (long long)*f.cnt_host.get();
   return LS_OK;
 }
@@ -296,43 +272,38 @@ int distance_query(DistanceField& f, const float* pts3, int n, float* dist, int*
   if (n <= 0) return LS_OK;
   const size_t N = (size_t)n;
   size_t off = 0;
-  auto take = [&off](size_t bytes) {
-    const size_t o = off;
-    off += (bytes + 255) & ~(size_t)255;
-    return o;
-  };
-  const size_t o_cnt = take(sizeof(unsigned long long)), o_p = take(12 * N), o_d = dist ? take(4 * N) : 0,
-               o_s = sq ? take(4 * N) : 0, o_o = obst3 ? take(12 * N) : 0;
-  if (f.qbuf.capacity() < off) DT_TRY(f.qbuf.reserve(off, 2 * off));
+  const size_t o_cnt = take(off, sizeof(unsigned long long)), o_p = take(off, 12 * N), o_d = dist ? take(off, 4 * N) : 0,
+               o_s = sq ? take(off, 4 * N) : 0, o_o = obst3 ? take(off, 12 * N) : 0;
+  if (f.qbuf.capacity() < off) LSO_TRY(f.qbuf.reserve(off, 2 * off));
   char* q = f.qbuf.get();
   auto* cnt = reinterpret_cast<unsigned long long*>(q + o_cnt);
-  DT_TRY(cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), st));
-  DT_TRY(cudaMemcpyAsync(q + o_p, pts3, 12 * N, cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemsetAsync(cnt, 0, sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemcpyAsync(q + o_p, pts3, 12 * N, cudaMemcpyHostToDevice, st));
   dt_query_kernel<<<blocks(n, 256), 256, 0, st>>>(reinterpret_cast<const float*>(q + o_p), n, box_of(f), f.inv, f.res,
                                                   f.val[0].get(), f.site[0].get(), dist ? (float*)(q + o_d) : nullptr,
                                                   sq ? (int*)(q + o_s) : nullptr, obst3 ? (float*)(q + o_o) : nullptr, cnt);
-  DT_LAUNCHED();
-  if (dist) DT_TRY(cudaMemcpyAsync(dist, q + o_d, 4 * N, cudaMemcpyDeviceToHost, st));
-  if (sq) DT_TRY(cudaMemcpyAsync(sq, q + o_s, 4 * N, cudaMemcpyDeviceToHost, st));
-  if (obst3) DT_TRY(cudaMemcpyAsync(obst3, q + o_o, 12 * N, cudaMemcpyDeviceToHost, st));
+  LSO_LAUNCHED();
+  if (dist) LSO_TRY(cudaMemcpyAsync(dist, q + o_d, 4 * N, cudaMemcpyDeviceToHost, st));
+  if (sq) LSO_TRY(cudaMemcpyAsync(sq, q + o_s, 4 * N, cudaMemcpyDeviceToHost, st));
+  if (obst3) LSO_TRY(cudaMemcpyAsync(obst3, q + o_o, 12 * N, cudaMemcpyDeviceToHost, st));
   unsigned long long h = 0;
-  DT_TRY(cudaMemcpyAsync(&h, cnt, sizeof h, cudaMemcpyDeviceToHost, st));
-  DT_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemcpyAsync(&h, cnt, sizeof h, cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   *outside = (long long)h;
   return LS_OK;
 }
 
 int distance_download(DistanceField& f, int* sq, uint64_t* keys, cudaStream_t st, uint64_t* launches) {
   const size_t c = (size_t)f.cells;
-  if (sq) DT_TRY(cudaMemcpyAsync(sq, f.val[0].get(), 4 * c, cudaMemcpyDeviceToHost, st));
+  if (sq) LSO_TRY(cudaMemcpyAsync(sq, f.val[0].get(), 4 * c, cudaMemcpyDeviceToHost, st));
   if (keys) {
     // the stack is scratch between updates: 8 bytes per cell, as a key
     auto* k = reinterpret_cast<unsigned long long*>(f.stack.get());
     dt_keys_kernel<<<blocks(f.cells, 256), 256, 0, st>>>(f.site[0].get(), f.cells, box_of(f), k);
-    DT_LAUNCHED();
-    DT_TRY(cudaMemcpyAsync(keys, k, 8 * c, cudaMemcpyDeviceToHost, st));
+    LSO_LAUNCHED();
+    LSO_TRY(cudaMemcpyAsync(keys, k, 8 * c, cudaMemcpyDeviceToHost, st));
   }
-  DT_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
 

@@ -69,7 +69,6 @@ namespace {
 
 constexpr unsigned long long kEmpty = ~0ull;
 constexpr int kPending = -1, kFull = -2;
-constexpr int kKeyMax = 32768;
 constexpr long long kMaxEditAxis = 1LL << 17;    // loop points per box axis (the key space has 2^16 per axis)
 constexpr long long kMaxEditBricks = 1LL << 29;  // bricks of an edit plus those in use (the read's bound)
 constexpr int kOverflowTable = 1, kOverflowPool = 2;
@@ -104,18 +103,8 @@ Dev dev_of(const Map& m) {
              m.mfree.get(), m.mocc.get(), m.bkey.get(), m.touched.get(), m.tlist.get()};
 }
 
-// floor(c * (1/res)) + 32768, valid iff in [0, 65535]
-__device__ __forceinline__ bool key_of(double inv, float c, int& k) {
-  const double s = floor((double)c * inv);
-  if (!(s >= -(double)kKeyMax && s < (double)kKeyMax)) return false;
-  k = (int)s + kKeyMax;
-  return true;
-}
 __device__ __forceinline__ bool key3(double inv, const float p[3], int k[3]) {
   return key_of(inv, p[0], k[0]) && key_of(inv, p[1], k[1]) && key_of(inv, p[2], k[2]);
-}
-__device__ __forceinline__ unsigned long long pack(int kx, int ky, int kz) {
-  return (unsigned long long)kx | ((unsigned long long)ky << 16) | ((unsigned long long)kz << 32);
 }
 // |v|: squares and sums in float, the root in double
 __device__ __forceinline__ double norm3(const float v[3]) {
@@ -162,10 +151,6 @@ struct Cursor {
   int b = -1;
 };
 
-__device__ __forceinline__ unsigned long long brick_key(const int k[3]) {
-  return (unsigned long long)(k[0] >> 3) | ((unsigned long long)(k[1] >> 3) << 13) | ((unsigned long long)(k[2] >> 3) << 26);
-}
-
 // Set the free or occupied mark of voxel k; false when its brick could not be placed.
 __device__ __forceinline__ bool mark(const Dev& D, Counters* cnt, Cursor& cur, const int k[3], bool occ) {
   const unsigned long long bk = brick_key(k);
@@ -176,7 +161,7 @@ __device__ __forceinline__ bool mark(const Dev& D, Counters* cnt, Cursor& cur, c
     cur.b = b;
     if (D.touched[b] == 0u && atomicExch(&D.touched[b], 1u) == 0u) D.tlist[atomicAdd(&cnt->n_touched, 1)] = b;
   }
-  const int local = (k[0] & 7) | ((k[1] & 7) << 3) | ((k[2] & 7) << 6);
+  const int local = local_of(k);
   unsigned* w = (occ ? D.mocc : D.mfree) + (size_t)cur.b * 16 + (local >> 5);
   const unsigned bit = 1u << (local & 31);
   if (!(*w & bit)) atomicOr(w, bit);  // near the sensor thousands of rays share a voxel: read before the atomic
@@ -191,7 +176,7 @@ __device__ __forceinline__ void dda_setup(const int k[3], const float o[3], cons
   for (int i = 0; i < 3; ++i) {
     step[i] = dir[i] > 0.0f ? 1 : (dir[i] < 0.0f ? -1 : 0);
     if (step[i] != 0) {
-      double border = ((double)(k[i] - kKeyMax) + 0.5) * res;
+      double border = centre_d(k[i], res);
       const double half = (double)step[i] * res * 0.5;
       border += kFloatHalfStep ? (double)(float)half : half;
       tmax[i] = (border - (double)o[i]) / (double)dir[i];
@@ -391,9 +376,9 @@ __global__ void occ_select_kernel(Dev D, Params P, int which, long long nvox, un
       const unsigned long long pos = base + __popc(bal & ((1u << lane) - 1u));
       const unsigned long long bk = D.bkey[v >> 9];
       const int t = (int)(v & 511);
-      const int kx = (int)(bk & 0x1fff) * 8 + (t & 7), ky = (int)((bk >> 13) & 0x1fff) * 8 + ((t >> 3) & 7),
-                kz = (int)((bk >> 26) & 0x1fff) * 8 + (t >> 6);
-      keys[pos] = pack(kx, ky, kz);
+      int k[3];
+      voxel_keys(bk, t, k);
+      keys[pos] = pack(k[0], k[1], k[2]);
       vals[pos] = __float_as_uint(x);
     }
   }
@@ -403,7 +388,7 @@ __global__ void occ_centres_kernel(const unsigned long long* __restrict__ keys, 
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const unsigned long long k = keys[i];
     float c[3];
-    for (int a = 0; a < 3; ++a) c[a] = (float)(((double)((int)((k >> (16 * a)) & 0xffff) - kKeyMax) + 0.5) * res);
+    for (int a = 0; a < 3; ++a) c[a] = centre_of((int)((k >> (16 * a)) & 0xffff), res);
     out[i] = make_float4(c[0], c[1], c[2], 1.0f);
   }
 }
@@ -416,8 +401,7 @@ __device__ __forceinline__ int find_brick(const Dev& D, unsigned long long bk) {
   return lookup_brick(D.tab_keys, D.tab_vals, D.tab_mask, bk);
 }
 
-// State of voxel k (LS_CELL_*), the brick of the last lookup cached in cur.  The known bit decides "unknown", not the
-// brick's presence: a brick placed by a failed insert holds no known voxel.  *v: the log-odds of a known voxel.
+// State of voxel k (LS_CELL_*, voxel_state), the brick of the last lookup cached in cur.  *v: the log-odds of a known voxel.
 __device__ __forceinline__ int state_of(const Dev& D, const Params& P, Cursor& cur, const int k[3], float* v) {
   const unsigned long long bk = brick_key(k);
   if (bk != cur.bk) {
@@ -425,28 +409,13 @@ __device__ __forceinline__ int state_of(const Dev& D, const Params& P, Cursor& c
     cur.b = find_brick(D, bk);
   }
   if (cur.b < 0) return LS_CELL_UNKNOWN;
-  const int local = (k[0] & 7) | ((k[1] & 7) << 3) | ((k[2] & 7) << 6);
-  if (!((D.known[(size_t)cur.b * 16 + (local >> 5)] >> (local & 31)) & 1u)) return LS_CELL_UNKNOWN;
-  const float x = D.lo[(size_t)cur.b * 512 + local];
-  if (v) *v = x;
-  return x >= P.l_occ ? LS_CELL_OCCUPIED : LS_CELL_FREE;
+  return voxel_state(D.known, D.lo, P.l_occ, cur.b, local_of(k), v);
 }
-
-// octomap's keyToCoord(key): (float)(((double)(k - 32768) + 0.5) * res)
-__device__ __forceinline__ float centre_of(int k, double res) { return (float)(((double)(k - kKeyMax) + 0.5) * res); }
 
 // Every lane of the warp calls it: the warp's keys_visited into cnt->n_out.
 __device__ __forceinline__ void add_visited(Counters* cnt, unsigned long long v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
   if ((threadIdx.x & 31) == 0 && v) atomicAdd(&cnt->n_out, v);
-}
-
-// octomap's search(double x, double y, double z): the key of the double coordinate, valid iff in [0, 65535]
-__device__ __forceinline__ bool key_of_d(double inv, double c, int& k) {
-  const double s = floor(c * inv);
-  if (!(s >= -(double)kKeyMax && s < (double)kKeyMax)) return false;
-  k = (int)s + kKeyMax;
-  return true;
 }
 
 // getCellStatusPoint / getCellProbabilityPoint: one thread per point
@@ -458,8 +427,8 @@ __global__ void occ_cell_kernel(const double* __restrict__ pts3, int n, Dev D, P
     int k[3];
     int s = LS_CELL_UNKNOWN;
     float v = __uint_as_float(kNanBits);
-    if (key_of_d(P.inv, pts3[3 * (size_t)i], k[0]) && key_of_d(P.inv, pts3[3 * (size_t)i + 1], k[1]) &&
-        key_of_d(P.inv, pts3[3 * (size_t)i + 2], k[2])) {
+    if (key_of(P.inv, pts3[3 * (size_t)i], k[0]) && key_of(P.inv, pts3[3 * (size_t)i + 1], k[1]) &&
+        key_of(P.inv, pts3[3 * (size_t)i + 2], k[2])) {  // octomap's search(double x, double y, double z)
       Cursor cur;
       ++visited;
       s = state_of(D, P, cur, k, &v);
@@ -638,6 +607,7 @@ constexpr int kTreeThreads = 1024;  // (f) and (g)
 constexpr int kBrickDepth = 13;
 
 // .bt node states: 0 no known voxel below, 1 free leaf, 2 occupied leaf, 3 inner -- also the bit pair of the payload.
+static_assert(LS_CELL_FREE == 0 && LS_CELL_OCCUPIED == 1 && LS_CELL_UNKNOWN == 2, "a voxel's .bt state is (LS_CELL_* + 1) % 3");
 // octomap's isNodeCollapsible after toMaxLikelihood: all 8 children exist, are leaves and have one state.
 __device__ __forceinline__ int parent_state(int n_free, int n_occ, int n_any, bool may_prune) {
   if (may_prune && n_free == 8) return 1;
@@ -674,7 +644,7 @@ __device__ __forceinline__ int mask8(const unsigned char* s) {
 __device__ __forceinline__ float leaf_coord(int k0, int s, double res) {
   const int kc = k0 + (s > 0 ? 1 << (s - 1) : 0);
   const double scale = (double)(1 << s);
-  return (float)((floor(((double)kc - (double)kKeyMax) / scale) + 0.5) * (res * scale));
+  return (float)((floor(((double)kc - (double)kKeyOffset) / scale) + 0.5) * (res * scale));
 }
 
 __device__ __forceinline__ void put_leaf(float4* cen, unsigned char* dep, unsigned long long i, int kx, int ky, int kz,
@@ -758,9 +728,8 @@ struct BinaryTree {
                                 Levels& T) {
     const int t = threadIdx.x;
     const int v = morton_local(t);
-    int s = 0;
-    if ((known[(size_t)b * 16 + (v >> 5)] >> (v & 31)) & 1u) s = lo[(size_t)b * 512 + v] >= l_occ ? 2 : 1;
-    T.s16[t] = (unsigned char)s;
+    const int s = voxel_state(known, lo, l_occ, b, v, nullptr);
+    T.s16[t] = (unsigned char)((s + 1) % 3);  // LS_CELL_* (free 0, occupied 1, unknown 2) as the .bt state
     __syncthreads();
     if (t < 64) {
       int nf = 0, no = 0, na = 0;
@@ -1226,10 +1195,9 @@ __global__ void __launch_bounds__(512) oct_emit_kernel<BinaryTree>(const unsigne
   int idx;
   Scan(scan).ExclusiveSum(depth != 0 ? 1 : 0, idx);
   if (depth) {
-    const unsigned long long bk = bkey[b];
-    const int v = morton_local(t);
-    put_leaf(cen, dep, N.loff[r] + (unsigned long long)idx, (int)(bk & 0x1fff) * 8 + (v & 7),
-             (int)((bk >> 13) & 0x1fff) * 8 + ((v >> 3) & 7), (int)((bk >> 26) & 0x1fff) * 8 + (v >> 6), depth, res);
+    int k[3];
+    voxel_keys(bkey[b], morton_local(t), k);
+    put_leaf(cen, dep, N.loff[r] + (unsigned long long)idx, k[0], k[1], k[2], depth, res);
   }
 }
 
@@ -1352,11 +1320,9 @@ __global__ void __launch_bounds__(512) lv_emit_kernel(const unsigned* __restrict
   int idx;
   Scan(scan).ExclusiveSum(depth != 0 ? 1 : 0, idx);
   if (depth) {
-    const unsigned long long bk = bkey[b];
-    const int u = morton_local(t);
-    put_tree_leaf((int)(bk & 0x1fff) * 8 + (u & 7), (int)((bk >> 13) & 0x1fff) * 8 + ((u >> 3) & 7),
-                  (int)((bk >> 26) & 0x1fff) * 8 + (u >> 6), depth, v, l_occ, res, R, N.loff[r] + (unsigned long long)idx,
-                  cen, tag, keep);
+    int k[3];
+    voxel_keys(bkey[b], morton_local(t), k);
+    put_tree_leaf(k[0], k[1], k[2], depth, v, l_occ, res, R, N.loff[r] + (unsigned long long)idx, cen, tag, keep);
   }
 }
 
@@ -1592,7 +1558,7 @@ __device__ __forceinline__ unsigned long long edit_brick(const EditBox& B, const
   const unsigned ax = axes[B.off[0] + (int)(j / nyz)], ay = axes[B.off[1] + (int)((j / B.n[2]) % B.n[1])],
                  az = axes[B.off[2] + (int)(j % B.n[2])];
   m[0] = ax & 0xffu, m[1] = ay & 0xffu, m[2] = az & 0xffu;
-  return (unsigned long long)(ax >> 8) | ((unsigned long long)(ay >> 8) << 13) | ((unsigned long long)(az >> 8) << 26);
+  return brick_pack(ax >> 8, ay >> 8, az >> 8);
 }
 
 // One thread per (box, brick) item of the call.  kClaim false: the items whose brick the hash lacks, counted into
@@ -1665,10 +1631,9 @@ __global__ void ed_scatter_kernel(const int* __restrict__ keys, int nx, int ny, 
   if (i >= n || !flag[i]) return;
   const int k[3] = {keys[(int)(i / ((long long)ny * nz))], keys[nx + (int)((i / nz) % ny)], keys[nx + ny + (int)(i % nz)]};
   const int b = find_brick(D, brick_key(k));
-  const int local = (k[0] & 7) | ((k[1] & 7) << 3) | ((k[2] & 7) << 6);
   const int p = pos[i] - 1;
   ok[p] = pack(k[0], k[1], k[2]);
-  ov[p] = __float_as_uint(D.lo[(size_t)b * 512 + local]);
+  ov[p] = __float_as_uint(D.lo[(size_t)b * 512 + local_of(k)]);
   oc[p] = make_float4(centre_of(k[0], res), centre_of(k[1], res), centre_of(k[2], res), 1.0f);
 }
 
@@ -1679,9 +1644,8 @@ __global__ void __launch_bounds__(512) ed_bounds_kernel(Dev D, int* mm) {
   __shared__ typename Reduce::TempStorage tmp;
   const int b = blockIdx.x, t = threadIdx.x;
   const bool kn = (D.known[(size_t)b * 16 + (t >> 5)] >> (t & 31)) & 1u;
-  const unsigned long long bk = D.bkey[b];
-  const int k[3] = {(int)(bk & 0x1fff) * 8 + (t & 7), (int)((bk >> 13) & 0x1fff) * 8 + ((t >> 3) & 7),
-                    (int)((bk >> 26) & 0x1fff) * 8 + (t >> 6)};
+  int k[3];
+  voxel_keys(D.bkey[b], t, k);
   for (int a = 0; a < 3; ++a) {
     const int lo = Reduce(tmp).Reduce(kn ? k[a] : INT_MAX, cub::Min());
     __syncthreads();
@@ -1694,34 +1658,16 @@ __global__ void __launch_bounds__(512) ed_bounds_kernel(Dev D, int* mm) {
   }
 }
 
-int code(cudaError_t e) {
-  if (e == cudaSuccess) return LS_OK;
-  cudaGetLastError();
-  return e == cudaErrorMemoryAllocation ? LS_ERR_NOMEM : LS_ERR_CUDA;
-}
-
-#define OCC_TRY(call)           \
-  do {                          \
-    const int rc_ = code(call); \
-    if (rc_) return rc_;        \
-  } while (0)
-
-#define OCC_LAUNCHED()                        \
-  do {                                        \
-    ++*launches;                              \
-    OCC_TRY(cudaGetLastError());              \
-  } while (0)
-
 int upload_counters(Map& m, cudaStream_t st) {
   std::memset(m.cnt_host.get(), 0, sizeof(Counters));
   m.cnt_host.get()->pool_n = m.pool_n;
-  OCC_TRY(cudaMemcpyAsync(m.cnt_dev.get(), m.cnt_host.get(), sizeof(Counters), cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(m.cnt_dev.get(), m.cnt_host.get(), sizeof(Counters), cudaMemcpyHostToDevice, st));
   return LS_OK;
 }
 
 int read_counters(Map& m, cudaStream_t st) {
-  OCC_TRY(cudaMemcpyAsync(m.cnt_host.get(), m.cnt_dev.get(), sizeof(Counters), cudaMemcpyDeviceToHost, st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemcpyAsync(m.cnt_host.get(), m.cnt_dev.get(), sizeof(Counters), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
 
@@ -1796,14 +1742,14 @@ int rebuild_table(Map& m, int cap, cudaStream_t st, uint64_t* launches) {
 
 // The read's per-record scratch for n stream records of `bytes` payload bytes, grown all or nothing.
 int reserve_read(Map& m, int n, size_t bytes, cudaStream_t st) {
-  OCC_TRY(m.rd_cnt_dev.reserve(1, 1));
-  OCC_TRY(m.rd_cnt_host.reserve(1, 1));
+  LSO_TRY(m.rd_cnt_dev.reserve(1, 1));
+  LSO_TRY(m.rd_cnt_host.reserve(1, 1));
   if (bytes > m.rd_pay.capacity()) {
-    OCC_TRY(cudaStreamSynchronize(st));
-    OCC_TRY(m.rd_pay.reserve(bytes, bytes + bytes / 8));
+    LSO_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(m.rd_pay.reserve(bytes, bytes + bytes / 8));
   }
   if ((size_t)n + 1 <= m.rd_ex.capacity()) return LS_OK;
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   const size_t c = (size_t)n + n / 8 + 1, blocks = c / kReadThreads + 1;
   size_t b1 = 0, b2 = 0;
   cudaError_t e;
@@ -1826,7 +1772,7 @@ int reserve_read(Map& m, int n, size_t bytes, cudaStream_t st) {
 int reserve_points(Map& m, int n, cudaStream_t st) {
   cudaError_t e;
   if ((size_t)n > m.ends.capacity()) {
-    OCC_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(cudaStreamSynchronize(st));
     const size_t cap = (size_t)(n + n / 8);
     if ((e = m.ends.reserve(cap, cap)) || (e = m.pkey.reserve(cap, cap)) || (e = m.cls.reserve(cap, cap))) {
       m.ends.reset(), m.pkey.reset(), m.cls.reset();
@@ -1836,7 +1782,7 @@ int reserve_points(Map& m, int n, cudaStream_t st) {
   size_t ep = 1024;
   while (ep < 2 * (size_t)n) ep *= 2;
   if (ep > m.ep_keys.capacity()) {
-    OCC_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(cudaStreamSynchronize(st));
     if ((e = m.ep_keys.reserve(ep, ep)) || (e = m.ep_min.reserve(ep, ep))) {
       m.ep_keys.reset(), m.ep_min.reset();
       return code(e);
@@ -1847,7 +1793,7 @@ int reserve_points(Map& m, int n, cudaStream_t st) {
 
 int reserve_export(Map& m, long long n, cudaStream_t st) {
   if ((size_t)n <= m.ex_c.capacity()) return LS_OK;
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   const long long cap = n + n / 8 + 1024;
   const size_t c = (size_t)cap;
   size_t bytes = 0;
@@ -1874,7 +1820,7 @@ int select(Map& m, const Params& P, int which, unsigned long long* keys, unsigne
     long long blocks = (nvox + 255) / 256;
     if (blocks > 65536) blocks = 65536;
     occ_select_kernel<<<(int)blocks, 256, 0, st>>>(dev_of(m), P, which, nvox, keys, vals, m.cnt_dev.get());
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
   }
   return read_counters(m, st);
 }
@@ -1886,11 +1832,11 @@ Nodes nodes_of(const Octree& t) {
 
 // Records for n_b bricks and every upper node they can have: at most min(n_b, 8^d) at depth d.
 int reserve_tree(Octree& t, int n_b, cudaStream_t st) {
-  OCC_TRY(t.levels.reserve(2 * (kBrickDepth + 1), 2 * (kBrickDepth + 1)));
-  OCC_TRY(t.tot_dev.reserve(3, 3));
-  OCC_TRY(t.tot_host.reserve(3, 3));
+  LSO_TRY(t.levels.reserve(2 * (kBrickDepth + 1), 2 * (kBrickDepth + 1)));
+  LSO_TRY(t.tot_dev.reserve(3, 3));
+  LSO_TRY(t.tot_host.reserve(3, 3));
   if ((size_t)n_b <= t.pool.capacity()) return LS_OK;
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   const int cap = n_b + n_b / 8;
   long long nodes = cap, level = 1;
   for (int d = 0; d < kBrickDepth; ++d, level *= 8) nodes += level < cap ? level : cap;
@@ -1915,11 +1861,11 @@ int reserve_tree(Octree& t, int n_b, cudaStream_t st) {
 
 int reserve_tree_outputs(Octree& t, long long bytes, long long leaves, cudaStream_t st) {
   if ((size_t)bytes > t.payload.capacity()) {
-    OCC_TRY(cudaStreamSynchronize(st));
-    OCC_TRY(t.payload.reserve((size_t)bytes, (size_t)(bytes + bytes / 8)));
+    LSO_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(t.payload.reserve((size_t)bytes, (size_t)(bytes + bytes / 8)));
   }
   if ((size_t)leaves > t.centres.capacity()) {
-    OCC_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(cudaStreamSynchronize(st));
     const size_t cap = (size_t)(leaves + leaves / 8);
     cudaError_t e;
     if ((e = t.centres.reserve(cap, cap)) || (e = t.depths.reserve(cap, cap))) {
@@ -1934,8 +1880,8 @@ int reserve_tree_outputs(Octree& t, long long bytes, long long leaves, cudaStrea
 
 int init(Map& m, int initial_bricks, cudaStream_t st) {
   m = Map();
-  OCC_TRY(m.cnt_dev.reserve(1, 1));
-  OCC_TRY(m.cnt_host.reserve(1, 1));
+  LSO_TRY(m.cnt_dev.reserve(1, 1));
+  LSO_TRY(m.cnt_host.reserve(1, 1));
   int rc;
   if ((rc = grow_pool(m, initial_bricks, st))) return rc;
   int cap = 1024;
@@ -1965,8 +1911,8 @@ int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16],
   if ((rc = reserve_points(m, n, st))) return rc;
   if (2LL * m.pool_n > m.tab_cap() && (rc = rebuild_table(m, m.tab_cap() * 2, st, launches))) return rc;
   if ((rc = upload_counters(m, st))) return rc;
-  OCC_TRY(cudaMemsetAsync(m.ep_keys.get(), 0xff, m.ep_keys.capacity() * sizeof(unsigned long long), st));
-  OCC_TRY(cudaMemsetAsync(m.ep_min.get(), 0x7f, m.ep_keys.capacity() * sizeof(int), st));  // 0x7f7f7f7f: above any point index
+  LSO_TRY(cudaMemsetAsync(m.ep_keys.get(), 0xff, m.ep_keys.capacity() * sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(m.ep_min.get(), 0x7f, m.ep_keys.capacity() * sizeof(int), st));  // 0x7f7f7f7f: above any point index
   Xform16 x;
   std::memcpy(x.T, T, sizeof(x.T));
   const int blocks = (n + 255) / 256;
@@ -1974,14 +1920,14 @@ int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16],
     occ_classify_kernel<<<blocks, 256, 0, st>>>(pts, n, x, identity ? 1 : 0, P, m.ends.get(), m.pkey.get(), m.cls.get(),
                                                 m.ep_keys.get(), m.ep_min.get(),
                                                  (unsigned)m.ep_keys.capacity() - 1u);
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
   }
   for (;;) {
     if (n > 0) {
       occ_cast_kernel<<<blocks, 256, 0, st>>>(n, P, T[12], T[13], T[14], m.ends.get(), m.pkey.get(), m.cls.get(), m.ep_keys.get(),
                                               m.ep_min.get(),
                                               (unsigned)m.ep_keys.capacity() - 1u, dev_of(m), m.cnt_dev.get());
-      OCC_LAUNCHED();
+      LSO_LAUNCHED();
     }
     if ((rc = read_counters(m, st))) return rc;
     const Counters c = *m.cnt_host.get();
@@ -1989,9 +1935,9 @@ int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16],
     // Undo the marking: clear every mark and touched flag, keep the bricks that got a pool index, drop the rest from the
     // hash, grow what filled and mark again.
     m.pool_n = c.pool_n < m.pool_cap() ? c.pool_n : m.pool_cap();
-    OCC_TRY(cudaMemsetAsync(m.mfree.get(), 0, (size_t)m.pool_cap() * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mocc.get(), 0, (size_t)m.pool_cap() * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.touched.get(), 0, (size_t)m.pool_cap() * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.mfree.get(), 0, (size_t)m.pool_cap() * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.mocc.get(), 0, (size_t)m.pool_cap() * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.touched.get(), 0, (size_t)m.pool_cap() * sizeof(unsigned), st));
     int tab = m.tab_cap();
     if ((c.overflow & kOverflowTable) || 2LL * m.pool_n > tab) tab *= 2;
     if ((rc = rebuild_table(m, tab, st, launches))) return rc;
@@ -2001,7 +1947,7 @@ int insert(Map& m, const Params& P, const float4* pts, int n, const float T[16],
   m.pool_n = m.cnt_host.get()->pool_n;
   if (m.cnt_host.get()->n_touched > 0) {
     occ_update_kernel<<<m.cnt_host.get()->n_touched, 512, 0, st>>>(dev_of(m), P, m.cnt_dev.get());
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
     if ((rc = read_counters(m, st))) return rc;
   }
   m.n_known += (long long)m.cnt_host.get()->new_known;
@@ -2029,28 +1975,28 @@ int download(Map& m, const Params& P, int which, long long n, uint64_t* keys, fl
   if ((rc = select(m, P, which, m.ex_k[0].get(), m.ex_v[0].get(), st, launches))) return rc;
   if ((long long)m.cnt_host.get()->n_out != n) return LS_ERR_CUDA;
   size_t bytes = m.cub_bytes;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(m.cub_tmp.get(), bytes, m.ex_k[0].get(), m.ex_k[1].get(), m.ex_v[0].get(),
+  LSO_TRY(cub::DeviceRadixSort::SortPairs(m.cub_tmp.get(), bytes, m.ex_k[0].get(), m.ex_k[1].get(), m.ex_v[0].get(),
                                           m.ex_v[1].get(), (int)n, 0, 48, st));
   ++*launches;
   if (centres4) {
     long long blocks = (n + 255) / 256;
     if (blocks > 65536) blocks = 65536;
     occ_centres_kernel<<<(int)blocks, 256, 0, st>>>(m.ex_k[1].get(), n, P.res, m.ex_c.get());
-    OCC_LAUNCHED();
-    OCC_TRY(cudaMemcpyAsync(centres4, m.ex_c.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    LSO_LAUNCHED();
+    LSO_TRY(cudaMemcpyAsync(centres4, m.ex_c.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, st));
   }
-  if (keys) OCC_TRY(cudaMemcpyAsync(keys, m.ex_k[1].get(), (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, m.ex_v[1].get(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  if (keys) LSO_TRY(cudaMemcpyAsync(keys, m.ex_k[1].get(), (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  if (log_odds) LSO_TRY(cudaMemcpyAsync(log_odds, m.ex_v[1].get(), (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
 
 int download_octree(const Octree& t, unsigned char* payload, float* centres4, unsigned char* depths, cudaStream_t st) {
-  if (t.bytes > 0 && payload) OCC_TRY(cudaMemcpyAsync(payload, t.payload.get(), (size_t)t.bytes, cudaMemcpyDeviceToHost, st));
+  if (t.bytes > 0 && payload) LSO_TRY(cudaMemcpyAsync(payload, t.payload.get(), (size_t)t.bytes, cudaMemcpyDeviceToHost, st));
   if (t.leaves > 0 && centres4)
-    OCC_TRY(cudaMemcpyAsync(centres4, t.centres.get(), (size_t)t.leaves * sizeof(float4), cudaMemcpyDeviceToHost, st));
-  if (t.leaves > 0 && depths) OCC_TRY(cudaMemcpyAsync(depths, t.depths.get(), (size_t)t.leaves, cudaMemcpyDeviceToHost, st));
-  OCC_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(cudaMemcpyAsync(centres4, t.centres.get(), (size_t)t.leaves * sizeof(float4), cudaMemcpyDeviceToHost, st));
+  if (t.leaves > 0 && depths) LSO_TRY(cudaMemcpyAsync(depths, t.depths.get(), (size_t)t.leaves, cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
 
@@ -2086,13 +2032,13 @@ int replace_map(Map& m, int n_b, long long known, const std::function<int()>& ke
   if (n_b > 0 && (rc = fill(dev_of(m)))) return rc;
   if (m.pool_n > n_b) {  // bricks past the new pool start empty, as a grown pool's do
     const size_t a = (size_t)n_b, k = (size_t)(m.pool_n - n_b);
-    OCC_TRY(cudaMemsetAsync(m.lo.get() + a * 512, 0, k * 512 * sizeof(float), st));
-    OCC_TRY(cudaMemsetAsync(m.known.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mfree.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mocc.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.touched.get() + a, 0, k * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.lo.get() + a * 512, 0, k * 512 * sizeof(float), st));
+    LSO_TRY(cudaMemsetAsync(m.known.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.mfree.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.mocc.get() + a * 16, 0, k * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.touched.get() + a, 0, k * sizeof(unsigned), st));
   }
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   m.tab_keys = std::move(tkeys), m.tab_vals = std::move(tvals);
   m.pool_n = n_b;
   m.n_known = known;
@@ -2108,34 +2054,34 @@ int build_tree_as(const Map& m, const Params& P, Octree& t, cudaStream_t st, uin
   int rc;
   if ((rc = reserve_tree(t, n_b, st))) return rc;
   if (F::kValued && t.val.capacity() < t.code.capacity()) {
-    OCC_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(cudaStreamSynchronize(st));
     t.val.reset();
-    OCC_TRY(t.val.reserve(t.code.capacity(), t.code.capacity()));
+    LSO_TRY(t.val.reserve(t.code.capacity(), t.code.capacity()));
   }
   const Nodes N = nodes_of(t);
   oct_code_kernel<<<(n_b + 255) / 256, 256, 0, st>>>(m.bkey.get(), n_b, t.sort_k.get(), t.sort_v.get());
-  OCC_LAUNCHED();
+  LSO_LAUNCHED();
   size_t bytes = t.cub_bytes;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp.get(), bytes, t.sort_k.get(), t.code.get(), t.sort_v.get(), t.pool.get(), n_b,
+  LSO_TRY(cub::DeviceRadixSort::SortPairs(t.cub_tmp.get(), bytes, t.sort_k.get(), t.code.get(), t.sort_v.get(), t.pool.get(), n_b,
                                           0, 3 * kBrickDepth, st));
   ++*launches;
   oct_brick_kernel<F><<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), N, P.l_occ);
-  OCC_LAUNCHED();
+  LSO_LAUNCHED();
   oct_up_kernel<F><<<1, kTreeThreads, 0, st>>>(N, n_b, t.levels.get(), t.tot_dev.get());
-  OCC_LAUNCHED();
-  OCC_TRY(cudaMemcpyAsync(t.tot_host.get(), t.tot_dev.get(), F::kTotals * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+  LSO_LAUNCHED();
+  LSO_TRY(cudaMemcpyAsync(t.tot_host.get(), t.tot_dev.get(), F::kTotals * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
                           st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   const unsigned long long* tot = t.tot_host.get();
   const long long nodes = (long long)tot[0], leaves = (long long)tot[1], pay = F::payload_bytes(tot);
   if (nodes == 0) return LS_OK;
   if ((rc = reserve_tree_outputs(t, pay, F::kCentres ? leaves : 0, st))) return rc;
   oct_down_kernel<F><<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), P.res, t.payload.get(), t.centres.get(), t.depths.get());
-  OCC_LAUNCHED();
+  LSO_LAUNCHED();
   oct_emit_kernel<F><<<n_b, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, P.res, t.payload.get(),
                                           t.centres.get(), t.depths.get());
-  OCC_LAUNCHED();
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_LAUNCHED();
+  LSO_TRY(cudaStreamSynchronize(st));
   t.nodes = nodes, t.bytes = pay, t.leaves = leaves;
   t.bricks = n_b;
   return LS_OK;
@@ -2159,28 +2105,28 @@ int read_tree_as(Map& m, const Params& P, const unsigned char* payload, long lon
     ReadCounters init{};
     init.end = INT_MAX;
     *m.rd_cnt_host.get() = init;
-    OCC_TRY(cudaMemcpyAsync(cnt, m.rd_cnt_host.get(), sizeof(ReadCounters), cudaMemcpyHostToDevice, st));
-    OCC_TRY(cudaMemcpyAsync(m.rd_pay.get(), payload, pay, cudaMemcpyHostToDevice, st));
+    LSO_TRY(cudaMemcpyAsync(cnt, m.rd_cnt_host.get(), sizeof(ReadCounters), cudaMemcpyHostToDevice, st));
+    LSO_TRY(cudaMemcpyAsync(m.rd_pay.get(), payload, pay, cudaMemcpyHostToDevice, st));
     const int blocks = (n + kReadThreads) / kReadThreads;  // n + 1 items
     rd_excess_kernel<F><<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), n, m.rd_tmp.get());
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
     size_t tb = m.rd_cub_bytes;
-    OCC_TRY(cub::DeviceScan::InclusiveSum(m.rd_cub.get(), tb, m.rd_tmp.get(), m.rd_ex.get(), n + 1, st));
+    LSO_TRY(cub::DeviceScan::InclusiveSum(m.rd_cub.get(), tb, m.rd_tmp.get(), m.rd_ex.get(), n + 1, st));
     ++*launches;
     rd_end_kernel<<<blocks, kReadThreads, 0, st>>>(m.rd_ex.get(), n, m.rd_bmin.get(), cnt);
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
     rd_parent_kernel<F><<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_ex.get(), m.rd_bmin.get(), n, m.rd_par.get(),
                                                          m.rd_slot.get(), cnt);
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
     rd_node_kernel<F><<<blocks, kReadThreads, 0, st>>>(m.rd_pay.get(), m.rd_par.get(), m.rd_slot.get(), n, P.l_occ,
                                                        m.rd_depth.get(), m.rd_key.get(), m.rd_anc.get(), m.rd_nb.get(), cnt);
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
     tb = m.rd_cub_bytes;
-    OCC_TRY(cub::DeviceScan::ExclusiveSum(m.rd_cub.get(), tb, m.rd_nb.get(), m.rd_boff.get(), n + 1, st));
+    LSO_TRY(cub::DeviceScan::ExclusiveSum(m.rd_cub.get(), tb, m.rd_nb.get(), m.rd_boff.get(), n + 1, st));
     ++*launches;
-    OCC_TRY(cudaMemcpyAsync(&cnt->bricks, m.rd_boff.get() + n, sizeof(long long), cudaMemcpyDeviceToDevice, st));
-    OCC_TRY(cudaMemcpyAsync(m.rd_cnt_host.get(), cnt, sizeof(ReadCounters), cudaMemcpyDeviceToHost, st));
-    OCC_TRY(cudaStreamSynchronize(st));
+    LSO_TRY(cudaMemcpyAsync(&cnt->bricks, m.rd_boff.get() + n, sizeof(long long), cudaMemcpyDeviceToDevice, st));
+    LSO_TRY(cudaMemcpyAsync(m.rd_cnt_host.get(), cnt, sizeof(ReadCounters), cudaMemcpyDeviceToHost, st));
+    LSO_TRY(cudaStreamSynchronize(st));
     const ReadCounters c = *m.rd_cnt_host.get();
     if ((rc = F::check(c, count, nodes, why))) return rc;
     if (c.bricks > kMaxReadBricks) return *why = "the file covers more bricks than the map can index", LS_ERR_NOMEM;
@@ -2194,15 +2140,15 @@ int read_tree_as(Map& m, const Params& P, const unsigned char* payload, long lon
       [&]() -> int {
         rd_brick_kernel<F><<<(n_b + 255) / 256, 256, 0, st>>>(m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(),
                                                               m.rd_boff.get(), end, n_b, m.rd_bkey.get(), m.rd_bst.get());
-        OCC_LAUNCHED();
+        LSO_LAUNCHED();
         return LS_OK;
       },
       [&](const Dev& D) -> int {
         rd_fill_kernel<F><<<n_b, 512, 0, st>>>(D, P, m.rd_pay.get(), m.rd_boff.get(), end, m.rd_bkey.get(), m.rd_bst.get());
-        OCC_LAUNCHED();
+        LSO_LAUNCHED();
         rd_leaf_kernel<F><<<(end + 255) / 256, 256, 0, st>>>(D, P, m.rd_pay.get(), m.rd_depth.get(), m.rd_key.get(),
                                                              m.rd_anc.get(), m.rd_boff.get(), end);
-        OCC_LAUNCHED();
+        LSO_LAUNCHED();
         return LS_OK;
       },
       why, st, launches);
@@ -2225,11 +2171,11 @@ namespace {
 
 // Every buffer of a list of n leaves, all or nothing.
 int reserve_leaves(Leaves& L, long long n, cudaStream_t st) {
-  OCC_TRY(L.cnt_dev.reserve(kLeafBuckets, kLeafBuckets));
-  OCC_TRY(L.cnt_host.reserve(kLeafBuckets, kLeafBuckets));
+  LSO_TRY(L.cnt_dev.reserve(kLeafBuckets, kLeafBuckets));
+  LSO_TRY(L.cnt_host.reserve(kLeafBuckets, kLeafBuckets));
   if ((size_t)n <= L.raw_c.capacity()) return LS_OK;
   if (n > (1LL << 30)) return LS_ERR_NOMEM;  // CUB's item counts are int
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   const size_t c = (size_t)(n + n / 8);
   size_t scan = 0, sort = 0;
   cudaError_t e;
@@ -2254,7 +2200,7 @@ int grid_of(long long n) { return (int)std::min<long long>((n + 255) / 256, 4096
 // The list's positions stably sorted by tag bits [begin, 6) into L.sorted (tags into L.stag).
 int sort_leaves(Leaves& L, int begin, cudaStream_t st, uint64_t* launches) {
   size_t bytes = L.cub_bytes;
-  OCC_TRY(cub::DeviceRadixSort::SortPairs(L.cub_tmp.get(), bytes, L.tag.get(), L.stag.get(), L.idx.get(), L.sorted.get(),
+  LSO_TRY(cub::DeviceRadixSort::SortPairs(L.cub_tmp.get(), bytes, L.tag.get(), L.stag.get(), L.idx.get(), L.sorted.get(),
                                           (int)L.n, begin, 6, st));
   ++*launches;
   return LS_OK;
@@ -2266,13 +2212,13 @@ int gather_leaves(Leaves& L, long long first, long long n, long long n_col, doub
   if (n > 0) {
     lv_gather_kernel<<<grid_of(n), 256, 0, st>>>(L.cen.get(), L.tag.get(), L.sorted.get(), first, n, n_col, min_z, max_z,
                                                  color_factor, L.raw_c.get(), L.raw_tag.get(), L.rgba.get());
-    OCC_LAUNCHED();
-    if (centres4) OCC_TRY(cudaMemcpyAsync(centres4, L.raw_c.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, st));
-    if (tags) OCC_TRY(cudaMemcpyAsync(tags, L.raw_tag.get(), (size_t)n, cudaMemcpyDeviceToHost, st));
+    LSO_LAUNCHED();
+    if (centres4) LSO_TRY(cudaMemcpyAsync(centres4, L.raw_c.get(), (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    if (tags) LSO_TRY(cudaMemcpyAsync(tags, L.raw_tag.get(), (size_t)n, cudaMemcpyDeviceToHost, st));
     if (rgba4 && n_col > 0)
-      OCC_TRY(cudaMemcpyAsync(rgba4, L.rgba.get(), (size_t)n_col * sizeof(float4), cudaMemcpyDeviceToHost, st));
+      LSO_TRY(cudaMemcpyAsync(rgba4, L.rgba.get(), (size_t)n_col * sizeof(float4), cudaMemcpyDeviceToHost, st));
   }
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
 
@@ -2290,20 +2236,20 @@ int build_leaves(const Map& m, const Params& P, Octree& t, const int kmin[3], co
   const Nodes N = nodes_of(t);
   lv_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), P.l_occ, P.res, R, L.raw_c.get(), L.raw_tag.get(),
                                              L.keep.get());
-  OCC_LAUNCHED();
+  LSO_LAUNCHED();
   lv_emit_kernel<<<t.bricks, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, P.res, R, L.raw_c.get(),
                                            L.raw_tag.get(), L.keep.get());
-  OCC_LAUNCHED();
+  LSO_LAUNCHED();
   size_t bytes = L.cub_bytes;
-  OCC_TRY(cub::DeviceScan::ExclusiveSum(L.cub_tmp.get(), bytes, L.keep.get(), L.pos.get(), (int)nl, st));
+  LSO_TRY(cub::DeviceScan::ExclusiveSum(L.cub_tmp.get(), bytes, L.keep.get(), L.pos.get(), (int)nl, st));
   ++*launches;
-  OCC_TRY(cudaMemsetAsync(L.cnt_dev.get(), 0, kLeafBuckets * sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(L.cnt_dev.get(), 0, kLeafBuckets * sizeof(unsigned long long), st));
   lv_compact_kernel<<<grid_of(nl), 256, 0, st>>>(L.raw_c.get(), L.raw_tag.get(), L.keep.get(), L.pos.get(), (int)nl,
                                                  L.cen.get(), L.tag.get(), L.idx.get(), L.cnt_dev.get());
-  OCC_LAUNCHED();
-  OCC_TRY(cudaMemcpyAsync(L.cnt_host.get(), L.cnt_dev.get(), kLeafBuckets * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+  LSO_LAUNCHED();
+  LSO_TRY(cudaMemcpyAsync(L.cnt_host.get(), L.cnt_dev.get(), kLeafBuckets * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
                           st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   for (int d = 0; d < 17; ++d) {
     L.occupied[d] = (long long)L.cnt_host.get()[d], L.free[d] = (long long)L.cnt_host.get()[17 + d];
     L.n_occupied += L.occupied[d], L.n += L.occupied[d] + L.free[d];
@@ -2314,9 +2260,9 @@ int build_leaves(const Map& m, const Params& P, Octree& t, const int kmin[3], co
 int download_leaves(Leaves& L, int which, float* centres4, unsigned char* tags, cudaStream_t st, uint64_t* launches) {
   if (L.n == 0) return LS_OK;
   if (which == 3) {
-    if (centres4) OCC_TRY(cudaMemcpyAsync(centres4, L.cen.get(), (size_t)L.n * sizeof(float4), cudaMemcpyDeviceToHost, st));
-    if (tags) OCC_TRY(cudaMemcpyAsync(tags, L.tag.get(), (size_t)L.n, cudaMemcpyDeviceToHost, st));
-    OCC_TRY(cudaStreamSynchronize(st));
+    if (centres4) LSO_TRY(cudaMemcpyAsync(centres4, L.cen.get(), (size_t)L.n * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    if (tags) LSO_TRY(cudaMemcpyAsync(tags, L.tag.get(), (size_t)L.n, cudaMemcpyDeviceToHost, st));
+    LSO_TRY(cudaStreamSynchronize(st));
     return LS_OK;
   }
   int rc;
@@ -2336,38 +2282,19 @@ int marker_cubes(Leaves& L, double min_z, double max_z, double color_factor, flo
 
 namespace {
 
-// The next 256-byte aligned region of `bytes` in the query staging buffer.
-size_t take(size_t& off, size_t bytes) {
-  const size_t o = off;
-  off += (bytes + 255) & ~(size_t)255;
-  return o;
-}
-
-// Query staging of at least `bytes`, grown by doubling; the old buffer is dropped first (its contents are not needed).
-int reserve_query(Map& m, size_t bytes, cudaStream_t st) {
-  if (bytes <= m.qbuf.capacity()) return LS_OK;
-  OCC_TRY(cudaStreamSynchronize(st));
-  size_t cap = m.qbuf.capacity() ? 2 * m.qbuf.capacity() : (size_t)1 << 16;
-  while (cap < bytes) cap *= 2;
-  OCC_TRY(m.qbuf.reserve(bytes, cap));
-  return LS_OK;
-}
-
 int zero_visited(Map& m, cudaStream_t st) {
-  OCC_TRY(cudaMemsetAsync(&m.cnt_dev.get()->n_out, 0, sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(&m.cnt_dev.get()->n_out, 0, sizeof(unsigned long long), st));
   return LS_OK;
 }
 
 // The outputs' copies are queued; wait for them and the keys visited.
 int finish_query(Map& m, cudaStream_t st, long long* visited) {
-  OCC_TRY(cudaMemcpyAsync(&m.cnt_host.get()->n_out, &m.cnt_dev.get()->n_out, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+  LSO_TRY(cudaMemcpyAsync(&m.cnt_host.get()->n_out, &m.cnt_dev.get()->n_out, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
                           st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaStreamSynchronize(st));
   *visited = (long long)m.cnt_host.get()->n_out;
   return LS_OK;
 }
-
-int blocks_of(long long n) { return (int)((n + 255) / 256); }
 
 // One axis of getLineStatusBoundingBox's offset loop (at most cap values); false when it has more.
 bool box_axis(double size, double res, long long cap, std::vector<double>* out) {
@@ -2394,15 +2321,15 @@ int query_cells(Map& m, const Params& P, const double* pts3, int n, int8_t* stat
   const size_t o_in = take(off, (size_t)n * 3 * sizeof(double)), o_st = take(off, (size_t)n),
                o_lo = take(off, (size_t)n * sizeof(float));
   int rc;
-  if ((rc = reserve_query(m, off, st))) return rc;
+  if ((rc = reserve_staging(m, off, 0, st))) return rc;
   char* q = m.qbuf.get();
-  OCC_TRY(cudaMemcpyAsync(q + o_in, pts3, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_in, pts3, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
   if ((rc = zero_visited(m, st))) return rc;
-  occ_cell_kernel<<<blocks_of(n), 256, 0, st>>>((const double*)(q + o_in), n, dev_of(m), P, (signed char*)(q + o_st),
+  occ_cell_kernel<<<blocks(n, 256), 256, 0, st>>>((const double*)(q + o_in), n, dev_of(m), P, (signed char*)(q + o_st),
                                                 (float*)(q + o_lo), m.cnt_dev.get());
-  OCC_LAUNCHED();
-  OCC_TRY(cudaMemcpyAsync(status, q + o_st, (size_t)n, cudaMemcpyDeviceToHost, st));
-  if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, q + o_lo, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  LSO_LAUNCHED();
+  LSO_TRY(cudaMemcpyAsync(status, q + o_st, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (log_odds) LSO_TRY(cudaMemcpyAsync(log_odds, q + o_lo, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
   return finish_query(m, st, visited);
 }
 
@@ -2428,7 +2355,7 @@ int query_lines(Map& m, const Params& P, const double* starts3, const double* en
                o_st = take(off, (size_t)n), o_fk = take(off, (size_t)n * sizeof(uint64_t)),
                o_best = take(off, (size_t)n * sizeof(unsigned));
   int rc;
-  if ((rc = reserve_query(m, off, st))) return rc;
+  if ((rc = reserve_staging(m, off, 0, st))) return rc;
   char* q = m.qbuf.get();
   const double* s = (const double*)(q + o_s);
   const double* e = (const double*)(q + o_e);
@@ -2436,29 +2363,29 @@ int query_lines(Map& m, const Params& P, const double* starts3, const double* en
   signed char* dst = (signed char*)(q + o_st);
   unsigned long long* dfk = (unsigned long long*)(q + o_fk);
   unsigned* best = (unsigned*)(q + o_best);
-  OCC_TRY(cudaMemcpyAsync(q + o_s, starts3, seg_bytes, cudaMemcpyHostToDevice, st));
-  OCC_TRY(cudaMemcpyAsync(q + o_e, ends3, seg_bytes, cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_s, starts3, seg_bytes, cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_e, ends3, seg_bytes, cudaMemcpyHostToDevice, st));
   if ((rc = zero_visited(m, st))) return rc;
   if (!box3) {
-    occ_line_kernel<false><<<blocks_of(n), 256, 0, st>>>(s, e, n, 1, nullptr, 1, 1, 1, stop_at_unknown, dev_of(m), P, dst, dfk,
+    occ_line_kernel<false><<<blocks(n, 256), 256, 0, st>>>(s, e, n, 1, nullptr, 1, 1, 1, stop_at_unknown, dev_of(m), P, dst, dfk,
                                                          nullptr, m.cnt_dev.get());
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
   } else {
     std::vector<double> flat;
     for (int a = 0; a < 3; ++a) flat.insert(flat.end(), axes[a].begin(), axes[a].end());
-    OCC_TRY(cudaMemcpyAsync(offs, flat.data(), flat.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-    OCC_TRY(cudaMemsetAsync(best, 0, (size_t)n * sizeof(unsigned), st));  // 0: no line failed
+    LSO_TRY(cudaMemcpyAsync(offs, flat.data(), flat.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    LSO_TRY(cudaMemsetAsync(best, 0, (size_t)n * sizeof(unsigned), st));  // 0: no line failed
     const long long items = lines * n;
-    occ_line_kernel<true><<<blocks_of(items), 256, 0, st>>>(s, e, items, (int)lines, offs, nx, ny, nz, stop_at_unknown,
+    occ_line_kernel<true><<<blocks(items, 256), 256, 0, st>>>(s, e, items, (int)lines, offs, nx, ny, nz, stop_at_unknown,
                                                             dev_of(m), P, dst, dfk, best, m.cnt_dev.get());
-    OCC_LAUNCHED();
-    occ_box_result_kernel<<<blocks_of(n), 256, 0, st>>>(s, e, n, (int)lines, offs, nx, ny, nz, stop_at_unknown, dev_of(m), P,
+    LSO_LAUNCHED();
+    occ_box_result_kernel<<<blocks(n, 256), 256, 0, st>>>(s, e, n, (int)lines, offs, nx, ny, nz, stop_at_unknown, dev_of(m), P,
                                                          best, dst, dfk, m.cnt_dev.get());
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
     // the pageable copy of `flat` is staged before cudaMemcpyAsync returns, so it may go out of scope here
   }
-  OCC_TRY(cudaMemcpyAsync(status, dst, (size_t)n, cudaMemcpyDeviceToHost, st));
-  if (first_keys) OCC_TRY(cudaMemcpyAsync(first_keys, dfk, (size_t)n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaMemcpyAsync(status, dst, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (first_keys) LSO_TRY(cudaMemcpyAsync(first_keys, dfk, (size_t)n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   return finish_query(m, st, visited);
 }
 
@@ -2470,16 +2397,16 @@ int query_rays(Map& m, const Params& P, const float* origins3, const float* dire
   size_t off = 0;
   const size_t o_o = take(off, vec_bytes), o_d = take(off, vec_bytes), o_r = take(off, (size_t)n), o_e = take(off, vec_bytes);
   int rc;
-  if ((rc = reserve_query(m, off, st))) return rc;
+  if ((rc = reserve_staging(m, off, 0, st))) return rc;
   char* q = m.qbuf.get();
-  OCC_TRY(cudaMemcpyAsync(q + o_o, origins3, vec_bytes, cudaMemcpyHostToDevice, st));
-  OCC_TRY(cudaMemcpyAsync(q + o_d, directions3, vec_bytes, cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_o, origins3, vec_bytes, cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_d, directions3, vec_bytes, cudaMemcpyHostToDevice, st));
   if ((rc = zero_visited(m, st))) return rc;
-  occ_ray_kernel<<<blocks_of(n), 256, 0, st>>>((const float*)(q + o_o), (const float*)(q + o_d), n, ignore_unknown, max_range,
+  occ_ray_kernel<<<blocks(n, 256), 256, 0, st>>>((const float*)(q + o_o), (const float*)(q + o_d), n, ignore_unknown, max_range,
                                                dev_of(m), P, (signed char*)(q + o_r), (float*)(q + o_e), m.cnt_dev.get());
-  OCC_LAUNCHED();
-  OCC_TRY(cudaMemcpyAsync(result, q + o_r, (size_t)n, cudaMemcpyDeviceToHost, st));
-  if (ends3) OCC_TRY(cudaMemcpyAsync(ends3, q + o_e, vec_bytes, cudaMemcpyDeviceToHost, st));
+  LSO_LAUNCHED();
+  LSO_TRY(cudaMemcpyAsync(result, q + o_r, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (ends3) LSO_TRY(cudaMemcpyAsync(ends3, q + o_e, vec_bytes, cudaMemcpyDeviceToHost, st));
   return finish_query(m, st, visited);
 }
 
@@ -2496,8 +2423,8 @@ bool edit_axis(double p, double s, const Params& P, std::vector<int>* keys) {
   long long points = 0;
   for (double x = lo; x <= hi; x += P.res) {
     if (++points > kMaxEditAxis) return false;
-    const double f = std::floor((double)(float)x * P.inv);
-    if (f >= -(double)kKeyMax && f < (double)kKeyMax) keys->push_back((int)f + kKeyMax);
+    int k;
+    if (key_of(P.inv, (float)x, k)) keys->push_back(k);
   }
   return true;
 }
@@ -2546,12 +2473,12 @@ int set_boxes(Map& m, const Params& P, const double* centres3, const double* siz
   size_t off = 0;
   const size_t o_box = take(off, boxes.size() * sizeof(EditBox)), o_ax = take(off, axes.size() * sizeof(unsigned));
   int rc;
-  if ((rc = reserve_query(m, off, st))) return *why = "out of device memory for the boxes", rc;
+  if ((rc = reserve_staging(m, off, 0, st))) return *why = "out of device memory for the boxes", rc;
   char* q = m.qbuf.get();
   const EditBox* dbox = (const EditBox*)(q + o_box);
   const unsigned* dax = (const unsigned*)(q + o_ax);
-  OCC_TRY(cudaMemcpyAsync(q + o_box, boxes.data(), boxes.size() * sizeof(EditBox), cudaMemcpyHostToDevice, st));
-  OCC_TRY(cudaMemcpyAsync(q + o_ax, axes.data(), axes.size() * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_box, boxes.data(), boxes.size() * sizeof(EditBox), cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_ax, axes.data(), axes.size() * sizeof(unsigned), cudaMemcpyHostToDevice, st));
   const int blocks = (int)((items + 255) / 256);
   // Count the missing bricks, grow the pool and the hash for them, then place them (the insert's retry when a probe
   // sequence overflows).  A failure here (a growth refused after some bricks were placed) leaves the known voxels as they
@@ -2559,7 +2486,7 @@ int set_boxes(Map& m, const Params& P, const double* centres3, const double* siz
   // and no node, and the queries and the bounds test the known bits, so the cached trees and every answer stay current.
   if ((rc = upload_counters(m, st))) return rc;
   ed_bricks_kernel<false><<<blocks, 256, 0, st>>>(dbox, n, dax, items, dev_of(m), m.cnt_dev.get());
-  OCC_LAUNCHED();
+  LSO_LAUNCHED();
   if ((rc = read_counters(m, st))) return rc;
   const long long missing = (long long)m.cnt_host.get()->n_out;
   if (missing > 0) {
@@ -2575,7 +2502,7 @@ int set_boxes(Map& m, const Params& P, const double* centres3, const double* siz
     for (;;) {
       if ((rc = upload_counters(m, st))) return rc;
       ed_bricks_kernel<true><<<blocks, 256, 0, st>>>(dbox, n, dax, items, dev_of(m), m.cnt_dev.get());
-      OCC_LAUNCHED();
+      LSO_LAUNCHED();
       if ((rc = read_counters(m, st))) return rc;
       const Counters c = *m.cnt_host.get();
       m.pool_n = c.pool_n < m.pool_cap() ? c.pool_n : m.pool_cap();
@@ -2592,7 +2519,7 @@ int set_boxes(Map& m, const Params& P, const double* centres3, const double* siz
     if (nb == 0) continue;
     const float value = occupied[i] ? P.l_max : P.l_min;
     ed_write_kernel<<<(unsigned)nb, 512, 0, st>>>(B, dax, value, D, m.cnt_dev.get());
-    OCC_LAUNCHED();
+    LSO_LAUNCHED();
   }
   if ((rc = read_counters(m, st))) return rc;
   *new_known = (long long)m.cnt_host.get()->new_known;
@@ -2603,15 +2530,15 @@ int set_boxes(Map& m, const Params& P, const double* centres3, const double* siz
 int clear(Map& m, cudaStream_t st) {
   const size_t a = (size_t)m.pool_n;
   if (a > 0) {  // a claimed pool brick must start zeroed, as a grown pool's do
-    OCC_TRY(cudaMemsetAsync(m.lo.get(), 0, a * 512 * sizeof(float), st));
-    OCC_TRY(cudaMemsetAsync(m.known.get(), 0, a * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mfree.get(), 0, a * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.mocc.get(), 0, a * 16 * sizeof(unsigned), st));
-    OCC_TRY(cudaMemsetAsync(m.touched.get(), 0, a * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.lo.get(), 0, a * 512 * sizeof(float), st));
+    LSO_TRY(cudaMemsetAsync(m.known.get(), 0, a * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.mfree.get(), 0, a * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.mocc.get(), 0, a * 16 * sizeof(unsigned), st));
+    LSO_TRY(cudaMemsetAsync(m.touched.get(), 0, a * sizeof(unsigned), st));
   }
-  OCC_TRY(cudaMemsetAsync(m.tab_keys.get(), 0xff, (size_t)m.tab_cap() * sizeof(unsigned long long), st));
-  OCC_TRY(cudaMemsetAsync(m.tab_vals.get(), 0xff, (size_t)m.tab_cap() * sizeof(int), st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemsetAsync(m.tab_keys.get(), 0xff, (size_t)m.tab_cap() * sizeof(unsigned long long), st));
+  LSO_TRY(cudaMemsetAsync(m.tab_vals.get(), 0xff, (size_t)m.tab_cap() * sizeof(int), st));
+  LSO_TRY(cudaStreamSynchronize(st));
   m.pool_n = 0;
   m.n_known = 0;
   return LS_OK;
@@ -2632,36 +2559,36 @@ int box_voxels(Map& m, const Params& P, const double center3[3], const double si
   std::vector<int> flat;
   for (int a = 0; a < 3; ++a) flat.insert(flat.end(), axis[a].begin(), axis[a].end());
   size_t scan_bytes = 0;
-  OCC_TRY(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (int*)nullptr, (int*)nullptr, (int)pts, st));
+  LSO_TRY(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (int*)nullptr, (int*)nullptr, (int)pts, st));
   size_t off = 0;
   const size_t o_k = take(off, flat.size() * sizeof(int)), o_f = take(off, (size_t)pts * sizeof(int)),
                o_p = take(off, (size_t)pts * sizeof(int)), o_t = take(off, scan_bytes);
   int rc;
-  if ((rc = reserve_query(m, off, st))) return rc;
+  if ((rc = reserve_staging(m, off, 0, st))) return rc;
   char* q = m.qbuf.get();
   const int* dk = (const int*)(q + o_k);
   int* flag = (int*)(q + o_f);
   int* pos = (int*)(q + o_p);
-  OCC_TRY(cudaMemcpyAsync(q + o_k, flat.data(), flat.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  LSO_TRY(cudaMemcpyAsync(q + o_k, flat.data(), flat.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   const Dev D = dev_of(m);
-  ed_flag_kernel<<<blocks_of(pts), 256, 0, st>>>(dk, nx, ny, nz, pts, D, P, which, flag);
-  OCC_LAUNCHED();
-  OCC_TRY(cub::DeviceScan::InclusiveSum(q + o_t, scan_bytes, flag, pos, (int)pts, st));
+  ed_flag_kernel<<<blocks(pts, 256), 256, 0, st>>>(dk, nx, ny, nz, pts, D, P, which, flag);
+  LSO_LAUNCHED();
+  LSO_TRY(cub::DeviceScan::InclusiveSum(q + o_t, scan_bytes, flag, pos, (int)pts, st));
   ++*launches;
   int total = 0;
-  OCC_TRY(cudaMemcpyAsync(&total, pos + (pts - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemcpyAsync(&total, pos + (pts - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   *n = total;
   if (total > cap) return LS_ERR_ARG;
   if (total == 0 || (!keys && !log_odds && !centres4)) return LS_OK;
   if ((rc = reserve_export(m, total, st))) return rc;
-  ed_scatter_kernel<<<blocks_of(pts), 256, 0, st>>>(dk, nx, ny, nz, pts, D, P.res, flag, pos, m.ex_k[0].get(), m.ex_v[0].get(),
+  ed_scatter_kernel<<<blocks(pts, 256), 256, 0, st>>>(dk, nx, ny, nz, pts, D, P.res, flag, pos, m.ex_k[0].get(), m.ex_v[0].get(),
                                                     m.ex_c.get());
-  OCC_LAUNCHED();
-  if (keys) OCC_TRY(cudaMemcpyAsync(keys, m.ex_k[0].get(), (size_t)total * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  if (log_odds) OCC_TRY(cudaMemcpyAsync(log_odds, m.ex_v[0].get(), (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (centres4) OCC_TRY(cudaMemcpyAsync(centres4, m.ex_c.get(), (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_LAUNCHED();
+  if (keys) LSO_TRY(cudaMemcpyAsync(keys, m.ex_k[0].get(), (size_t)total * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  if (log_odds) LSO_TRY(cudaMemcpyAsync(log_odds, m.ex_v[0].get(), (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (centres4) LSO_TRY(cudaMemcpyAsync(centres4, m.ex_c.get(), (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   return LS_OK;
 }
 
@@ -2671,15 +2598,15 @@ int key_bounds(Map& m, int kmin[3], int kmax[3], bool* empty, cudaStream_t st, u
   size_t off = 0;
   const size_t o_mm = take(off, 6 * sizeof(int));
   int rc;
-  if ((rc = reserve_query(m, off, st))) return rc;
+  if ((rc = reserve_staging(m, off, 0, st))) return rc;
   int* mm = (int*)(m.qbuf.get() + o_mm);
-  OCC_TRY(cudaMemsetAsync(mm, 0x7f, 3 * sizeof(int), st));      // 0x7f7f7f7f: above any key
-  OCC_TRY(cudaMemsetAsync(mm + 3, 0xff, 3 * sizeof(int), st));  // -1
+  LSO_TRY(cudaMemsetAsync(mm, 0x7f, 3 * sizeof(int), st));      // 0x7f7f7f7f: above any key
+  LSO_TRY(cudaMemsetAsync(mm + 3, 0xff, 3 * sizeof(int), st));  // -1
   ed_bounds_kernel<<<m.pool_n, 512, 0, st>>>(dev_of(m), mm);
-  OCC_LAUNCHED();
+  LSO_LAUNCHED();
   int h[6];
-  OCC_TRY(cudaMemcpyAsync(h, mm, sizeof h, cudaMemcpyDeviceToHost, st));
-  OCC_TRY(cudaStreamSynchronize(st));
+  LSO_TRY(cudaMemcpyAsync(h, mm, sizeof h, cudaMemcpyDeviceToHost, st));
+  LSO_TRY(cudaStreamSynchronize(st));
   if (h[3] < 0) return LS_OK;
   for (int a = 0; a < 3; ++a) kmin[a] = h[a], kmax[a] = h[3 + a];
   *empty = false;

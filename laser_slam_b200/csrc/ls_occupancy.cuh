@@ -1,11 +1,14 @@
 // Resident occupancy map (ls_occupancy_*): laser_to_octomap's scan insertion on the device.  The rules are
 // oracle/OCCUPANCY.md; the layout and kernels are described in ls_occupancy.cu and DESIGN.md.
 #pragma once
+#include <cmath>
 #include <cstddef>
 #include <cstdint>
+#include <utility>
 
 #include <cuda_runtime.h>
 
+#include "../../include/ls_b200.h"
 #include "ls_buffer.cuh"
 
 namespace lso {
@@ -102,6 +105,107 @@ __device__ __forceinline__ int lookup_brick(const unsigned long long* tab_keys, 
     if (k == ~0ull) return -1;
   }
   return -1;
+}
+
+// ---- the map's keys and bricks ---------------------------------------------------------------------------------------
+// Every module that reads the map takes its key, centre, brick and voxel-state rules from here.  The key and centre rules
+// are octomap's (16 levels), bit for bit under -fmad=false.
+
+// A voxel key is floor(c / res) + kKeyOffset per axis, valid in [0, 65535].
+constexpr int kKeyOffset = 32768;
+
+// octomap's coordToKeyChecked: floor(c * inv) + 32768; false when outside [0, 65535] (NaN included).  A float coordinate
+// is widened to double before the multiply.
+__host__ __device__ __forceinline__ bool key_of(double inv, double c, int& k) {
+  const double s = floor(c * inv);
+  if (!(s >= -(double)kKeyOffset && s < (double)kKeyOffset)) return false;
+  k = (int)s + kKeyOffset;
+  return true;
+}
+
+// octomap's keyToCoord(key): the voxel centre on one axis in double (centre_d), and that rounded to float once (centre_of),
+// as every output centre is.
+__host__ __device__ __forceinline__ double centre_d(int k, double res) { return ((double)(k - kKeyOffset) + 0.5) * res; }
+__host__ __device__ __forceinline__ float centre_of(int k, double res) { return (float)centre_d(k, res); }
+
+// The packed key of a voxel: x | y << 16 | z << 32.
+__host__ __device__ __forceinline__ unsigned long long pack(int kx, int ky, int kz) {
+  return (unsigned long long)kx | ((unsigned long long)ky << 16) | ((unsigned long long)kz << 32);
+}
+
+// A brick key: the brick's coordinates (a voxel key >> 3 per axis), 13 bits each, x | y << 13 | z << 26.
+__host__ __device__ __forceinline__ unsigned long long brick_pack(unsigned long long bx, unsigned long long by,
+                                                                  unsigned long long bz) {
+  return bx | (by << 13) | (bz << 26);
+}
+__host__ __device__ __forceinline__ unsigned long long brick_key(const int k[3]) {
+  return brick_pack(k[0] >> 3, k[1] >> 3, k[2] >> 3);
+}
+
+// A voxel's local index in its brick, t = x | y << 3 | z << 6 of its key's low 3 bits, and back: the keys of voxel t of
+// brick bk (t in [0, 512)).
+__host__ __device__ __forceinline__ int local_of(const int k[3]) { return (k[0] & 7) | ((k[1] & 7) << 3) | ((k[2] & 7) << 6); }
+__host__ __device__ __forceinline__ void voxel_keys(unsigned long long bk, int t, int k[3]) {
+  k[0] = (int)(bk & 0x1fff) * 8 + (t & 7);
+  k[1] = (int)((bk >> 13) & 0x1fff) * 8 + ((t >> 3) & 7);
+  k[2] = (int)((bk >> 26) & 0x1fff) * 8 + (t >> 6);
+}
+
+// State (LS_CELL_*) of voxel `local` of pool brick b: unknown without its known bit, else occupied iff its log-odds >=
+// l_occ.  The known bit decides "unknown", not the brick's presence: a brick placed by a failed insert holds no known
+// voxel.  *v (when v is not NULL): the log-odds of a known voxel.
+__host__ __device__ __forceinline__ int voxel_state(const unsigned* known, const float* lo, float l_occ, int b, int local,
+                                                    float* v) {
+  if (!((known[(size_t)b * 16 + (local >> 5)] >> (local & 31)) & 1u)) return LS_CELL_UNKNOWN;
+  const float x = lo[(size_t)b * 512 + local];
+  if (v) *v = x;
+  return x >= l_occ ? LS_CELL_OCCUPIED : LS_CELL_FREE;
+}
+
+// ---- host: error codes, launches and staging -------------------------------------------------------------------------
+// LS_OK, LS_ERR_NOMEM for a failed allocation, else LS_ERR_CUDA; the error is cleared from cudaGetLastError.
+inline int code(cudaError_t e) {
+  if (e == cudaSuccess) return LS_OK;
+  cudaGetLastError();
+  return e == cudaErrorMemoryAllocation ? LS_ERR_NOMEM : LS_ERR_CUDA;
+}
+
+#define LSO_TRY(call)                \
+  do {                               \
+    const int rc_ = lso::code(call); \
+    if (rc_) return rc_;             \
+  } while (0)
+
+// After a launch: counts it in *launches and returns its error.
+#define LSO_LAUNCHED()           \
+  do {                           \
+    ++*launches;                 \
+    LSO_TRY(cudaGetLastError()); \
+  } while (0)
+
+inline unsigned blocks(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+
+// The next 256-byte aligned region of `bytes` in a staging buffer whose first `off` bytes are taken.
+inline size_t take(size_t& off, size_t bytes) {
+  const size_t o = off;
+  off += (bytes + 255) & ~(size_t)255;
+  return o;
+}
+
+// The query staging m.qbuf of at least `bytes`, grown by doubling from 64 KiB after the stream's pending work.  The first
+// `keep` bytes survive a growth; with keep 0 the old buffer is dropped first.
+inline int reserve_staging(Map& m, size_t bytes, size_t keep, cudaStream_t st) {
+  if (bytes <= m.qbuf.capacity()) return LS_OK;
+  LSO_TRY(cudaStreamSynchronize(st));
+  size_t cap = m.qbuf.capacity() ? 2 * m.qbuf.capacity() : (size_t)1 << 16;
+  while (cap < bytes) cap *= 2;
+  if (keep == 0) return code(m.qbuf.reserve(bytes, cap));
+  ls::Buffer<char> grown;
+  LSO_TRY(grown.reserve(bytes, cap));
+  LSO_TRY(cudaMemcpyAsync(grown.get(), m.qbuf.get(), keep, cudaMemcpyDeviceToDevice, st));
+  LSO_TRY(cudaStreamSynchronize(st));
+  m.qbuf = std::move(grown);
+  return LS_OK;
 }
 
 // Change detection (ls_changes.cu; DESIGN.md §4b'''''''''').  A baseline holds, per brick with a known voxel when it was
