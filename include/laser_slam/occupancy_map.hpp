@@ -9,6 +9,7 @@
 
 #include <array>
 #include <cstdint>
+#include <limits>
 #include <mutex>
 #include <string>
 #include <utility>
@@ -168,6 +169,25 @@ class OccupancyMap {
   // max_z, times color_factor), and for the free ones.  min_z < max_z, all finite, or it throws.
   void generateMarkerArray(double min_z, double max_z, double color_factor, std::vector<CubeList>* occupied_nodes,
                            std::vector<CubeList>* free_nodes) const;
+
+  // ---- 2D projection: octomap_server's projected_map and map_saver on the device map (ls_occupancy_build_projection /
+  // _download_projection; rules in DESIGN.md §4b''''''''''''').  octomap_server's occupancy_min_z / occupancy_max_z (NaN
+  // throws, infinities allowed) and min_x_size / min_y_size (finite, >= 0, or it throws).
+  struct ProjectedMapParams {
+    double occupancy_min_z = -std::numeric_limits<double>::infinity();
+    double occupancy_max_z = std::numeric_limits<double>::infinity();
+    double min_x_size = 0.0, min_y_size = 0.0;
+  };
+  // A nav_msgs/OccupancyGrid's content: cell (i, j) is data[j * width + i], -1 unknown, 0 free, 100 occupied; origin is the
+  // lower corner of cell (0, 0) (z and yaw 0).
+  struct ProjectedMap {
+    uint32_t width = 0, height = 0;
+    double resolution = 0.0, origin_x = 0.0, origin_y = 0.0;
+    std::vector<int8_t> data;
+  };
+  void getProjectedMap(const ProjectedMapParams& params, ProjectedMap* map) const;
+  // The projection written as map_saver writes it: stem + ".pgm" and stem + ".yaml".  False when a file cannot be written.
+  bool saveProjectedMap(const std::string& stem, const ProjectedMapParams& params) const;
 
   // ---- change detection: octomap's calls and volumetric_mapping's getChangedPoints on the device map
   // (ls_occupancy_track_changes / _changes; rules in DESIGN.md §4b'''''''''').  A change is a voxel whose state (free,

@@ -515,6 +515,41 @@ int ls_occupancy_download_leaves(ls_occupancy* om, int which, float* centres4, u
 int ls_occupancy_marker_cubes(ls_occupancy* om, double min_z, double max_z, double color_factor, float* centres4,
                               float* colors4, int64_t occupied_offsets[18], int64_t free_offsets[18], int64_t cap, int64_t* n);
 
+/* The map projected onto a 2D occupancy grid: octomap_server's projected_map (nav_msgs/OccupancyGrid) at m_maxTreeDepth = 16
+ * with a complete projection (DESIGN.md §4b''''''''''''').  Rules:
+ *   tree        the leaves of the .bt tree (toMaxLikelihood + prune, what ls_occupancy_write_octomap writes); every leaf is
+ *               free or occupied.  A map with no known voxel gives a 0 x 0 grid
+ *   bounds      octomap's calcMinMax over those leaves, in double: per axis the least centre - size/2 and the largest
+ *               (centre - size/2) + size, centre keyToCoord(key, d) and size res * 2^(16-d).  Unlike ls_occupancy_bounds,
+ *               which takes depth-16 leaves, a coarse leaf counts whole
+ *   padding     min x = min(min x, -min_size_x/2), max x = max(max x, min_size_x/2), the same in y
+ *   keys        paddedMinKey / paddedMaxKey = coordToKeyChecked of the padded corners as float points (z too)
+ *   geometry    width = paddedMaxKey.x - paddedMinKey.x + 1, height likewise in y, resolution = res, origin =
+ *               (float)keyToCoord(paddedMinKey) - res/2 in x and y (z and yaw 0).  Cell (i, j) is data[j * width + i]
+ *   band        a leaf takes part iff z + size/2 > min_z && z - size/2 < max_z, z = keyToCoord(key, d).z in double
+ *   paint       a taking-part leaf at depth d fills its 2^(16-d) x 2^(16-d) cells from (key.x - paddedMinKey.x, key.y -
+ *               paddedMinKey.y): an occupied leaf writes 100, a free one 0 where the cell is still -1; every cell starts
+ *               at -1.  So a cell is 100 if any occupied leaf covers it, else 0 if any free leaf does, else -1
+ * ls_occupancy_build_projection builds the .bt tree first unless its cached build is current (neither cached build is
+ * invalidated, and their outputs do not change), projects it and sets *info; the grid stays on the device until an insert,
+ * edit, read or reset of the map invalidates it, and a download then returns LS_ERR_STATE.  Calls run on the map's stream,
+ * are synchronous, never change the map and are legal between ls_icp_register_submap_batch_begin and _end.  Errors:
+ * LS_ERR_ARG for NULL info, a NaN min_z or max_z (infinities are allowed), a min_size that is negative, NaN or infinite, a
+ * padded corner outside the key space, a grid of more than 2^31 - 1 cells, a NULL data with cap > 0 or cap < width *
+ * height (nothing is copied); LS_ERR_NOMEM when the grid cannot be allocated.  A refused call leaves the map, both cached
+ * builds, the leaf list and the last projection as they were. */
+typedef struct ls_grid_info {
+  int64_t width, height;      /* cells along x and y; 0 x 0 for a map with no known voxel */
+  double resolution;          /* the map's resolution [m] (the message's float32 field holds it rounded) */
+  double origin_x, origin_y;  /* the lower corner of cell (0, 0) [m] */
+  int64_t unknown_cells, free_cells, occupied_cells; /* cells of -1, 0 and 100 */
+  float device_ms;            /* the call on the map's stream, a .bt build it needed included */
+} ls_grid_info;
+int ls_occupancy_build_projection(ls_occupancy* om, double min_z, double max_z, double min_size_x, double min_size_y,
+                                  ls_grid_info* info);
+/* The last projection's width * height cells (-1, 0 or 100), row j at data[j * width]. */
+int ls_occupancy_download_projection(ls_occupancy* om, int8_t* data, int64_t cap);
+
 /* Queries of the map: volumetric_mapping's WorldBase (getCellStatusPoint, getLineStatus, getVisibility,
  * getLineStatusBoundingBox) and octomap's castRay, batched, one device thread per query.  The rules (oracle/QUERIES.md):
  *   cell        the key of the double point (octomap's search(x, y, z): floor(c * (1/resolution)) + 32768, no float cast);

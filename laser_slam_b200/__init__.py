@@ -137,6 +137,14 @@ class LeafStats(ctypes.Structure):
                 ("device_ms", ctypes.c_float)]
 
 
+class GridInfo(ctypes.Structure):
+    """ls_grid_info: the 2D projection's width and height in cells, resolution, origin (the lower corner of cell (0, 0)),
+    the cells of -1, 0 and 100, and the call's device ms."""
+    _fields_ = [("width", ctypes.c_int64), ("height", ctypes.c_int64), ("resolution", ctypes.c_double),
+                ("origin_x", ctypes.c_double), ("origin_y", ctypes.c_double), ("unknown_cells", ctypes.c_int64),
+                ("free_cells", ctypes.c_int64), ("occupied_cells", ctypes.c_int64), ("device_ms", ctypes.c_float)]
+
+
 class OccupancyQueryStats(ctypes.Structure):
     _fields_ = [("keys_visited", ctypes.c_int64), ("device_ms", ctypes.c_float)]
 
@@ -293,6 +301,9 @@ def lib():
         L.ls_occupancy_download_leaves.argtypes = [vp, ci, vp, vp, vp, ctypes.c_int64, i64p]
         L.ls_occupancy_marker_cubes.argtypes = [vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp, vp, vp,
                                                 ctypes.c_int64, i64p]
+        L.ls_occupancy_build_projection.argtypes = [vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                                    ctypes.POINTER(GridInfo)]
+        L.ls_occupancy_download_projection.argtypes = [vp, vp, ctypes.c_int64]
         L.ls_distance_map_create.argtypes = [vp, ctypes.POINTER(DistanceMapParams), ctypes.POINTER(vp)]
         L.ls_distance_map_destroy.argtypes = [vp]
         L.ls_distance_map_destroy.restype = None
@@ -1253,6 +1264,43 @@ class OccupancyMap:
         free = [CubeList(res * 2.0 ** (16 - d), cen[free_off[d]:free_off[d + 1], :3].copy(), np.zeros((0, 4), np.float32))
                 for d in range(17)]
         return MarkerCubes(occ, free)
+
+    # ---- 2D projection (ls_occupancy_build_projection / _download_projection)
+    def projected_map(self, min_z=-math.inf, max_z=math.inf, min_size_x=0.0, min_size_y=0.0):
+        """octomap_server's projected_map (DESIGN.md §4b'''''''''''''): the .bt tree's leaves whose z extent meets the band
+        (min_z, max_z), painted into a 2D grid padded to at least min_size_x x min_size_y metres around the origin.
+        Returns (grid int8 (height, width) of -1 unknown, 0 free, 100 occupied, cell (i, j) at grid[j, i]; GridInfo)."""
+        info = GridInfo()
+        self.ctx._check(lib().ls_occupancy_build_projection(self._h, float(min_z), float(max_z), float(min_size_x),
+                                                            float(min_size_y), ctypes.byref(info)))
+        grid = np.empty((info.height, info.width), np.int8)
+        self.ctx._check(lib().ls_occupancy_download_projection(self._h, grid.ctypes.data if grid.size else None, grid.size))
+        return grid, info
+
+    def save_projected_map(self, stem, min_z=-math.inf, max_z=math.inf, min_size_x=0.0, min_size_y=0.0):
+        """projected_map(...) saved as map_saver saves it: stem.pgm and stem.yaml (save_map).  Returns the GridInfo."""
+        grid, info = self.projected_map(min_z, max_z, min_size_x, min_size_y)
+        save_map(stem, grid, info.resolution, info.origin_x, info.origin_y)
+        return info
+
+
+def save_map(stem, grid, resolution, origin_x, origin_y):
+    """map_saver's files of an occupancy grid (int8 (height, width), cell (i, j) at grid[j, i]): stem.pgm, a P5 image whose
+    rows run from j = height - 1 down to 0, 0 -> 254, 100 -> 0 and anything else -> 205; and stem.yaml naming it.  The
+    resolution is printed as the message's float32 holds it."""
+    grid = np.asarray(grid, np.int8)
+    height, width = grid.shape
+    res = float(np.float32(resolution))
+    pix = np.full(grid.shape, 205, np.uint8)
+    pix[grid == 0] = 254
+    pix[grid == 100] = 0
+    image = stem + ".pgm"
+    with open(image, "wb") as f:
+        f.write(b"P5\n# CREATOR: map_saver.cpp %.3f m/pix\n%d %d\n255\n" % (res, width, height))
+        f.write(pix[::-1].tobytes())
+    with open(stem + ".yaml", "w") as f:
+        f.write("image: %s\nresolution: %f\norigin: [%f, %f, %f]\nnegate: 0\noccupied_thresh: 0.65\nfree_thresh: 0.196\n\n"
+                % (image, res, origin_x, origin_y, 0.0))
 
 
 class DistanceMap:

@@ -1744,6 +1744,8 @@ struct ls_occupancy {
   bool tracking = false;
   lso::Leaves leaves;  // the last leaf list (ls_occupancy_build_leaves), current while it reflects every change to the map
   bool leaves_current = false;
+  lso::Projection projection;  // the last 2D projection (ls_occupancy_build_projection), current likewise
+  bool projection_current = false;
 };
 
 namespace {
@@ -1751,10 +1753,11 @@ using lso::TreeFormat;
 
 ls_occupancy::Tree& tree_of(ls_occupancy* om, TreeFormat f) { return om->trees[(int)f]; }
 
-// A change to the map invalidates both cached builds and the leaf list.
+// A change to the map invalidates both cached builds, the leaf list and the 2D projection.
 void trees_stale(ls_occupancy* om) {
   for (ls_occupancy::Tree& t : om->trees) t.current = false;
   om->leaves_current = false;
+  om->projection_current = false;
 }
 
 // The error texts' name of a format: "octree" or "full octree".
@@ -2441,6 +2444,54 @@ int ls_occupancy_marker_cubes(ls_occupancy* om, double min_z, double max_z, doub
   CU(cudaSetDevice(ctx->device));
   const int rc = lso::marker_cubes(om->leaves, min_z, max_z, color_factor, centres4, colors4, om->stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "marker cubes failed");
+  return LS_OK;
+}
+
+int ls_occupancy_build_projection(ls_occupancy* om, double min_z, double max_z, double min_size_x, double min_size_y,
+                                  ls_grid_info* info) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!info) return fail(ctx, LS_ERR_ARG, "bad argument");
+  if (std::isnan(min_z) || std::isnan(max_z)) return fail(ctx, LS_ERR_ARG, "band min_z %g, max_z %g has a NaN", min_z, max_z);
+  if (!std::isfinite(min_size_x) || !std::isfinite(min_size_y) || min_size_x < 0.0 || min_size_y < 0.0)
+    return fail(ctx, LS_ERR_ARG, "minimum size %g x %g (finite, >= 0)", min_size_x, min_size_y);
+  CU(cudaSetDevice(ctx->device));
+  ls_occupancy::Tree& t = tree_of(om, TreeFormat::Binary);
+  const bool build = !t.current;
+  int rc;
+  if (build && (rc = build_tree(om, TreeFormat::Binary))) return rc;
+  CU(cudaEventRecord(om->ev0, om->stream));
+  const char* why = "";
+  rc = lso::build_projection(om->map, om->prm, t.tree, lso::ProjectionArgs{min_z, max_z, min_size_x, min_size_y},
+                             om->projection, &why, om->stream, &ctx->launches);
+  if (rc == LS_ERR_ARG || (rc == LS_ERR_NOMEM && *why)) return fail(ctx, rc, "2D projection: %s", why);
+  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "2D projection: out of device memory" : "2D projection failed");
+  CU(cudaEventRecord(om->ev1, om->stream));
+  CU(cudaEventSynchronize(om->ev1));
+  om->projection_current = true;
+  float ms = 0.f;
+  CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+  const lso::Projection& p = om->projection;
+  info->width = p.width, info->height = p.height;
+  info->resolution = om->prm.res;
+  info->origin_x = p.origin[0], info->origin_y = p.origin[1];
+  info->unknown_cells = p.cells[0], info->free_cells = p.cells[1], info->occupied_cells = p.cells[2];
+  info->device_ms = ms + (build ? t.ms : 0.f);
+  return LS_OK;
+}
+
+int ls_occupancy_download_projection(ls_occupancy* om, int8_t* data, int64_t cap) {
+  if (!om) return LS_ERR_ARG;
+  ls_ctx* ctx = om->ctx;
+  if (!om->projection_current)
+    return fail(ctx, LS_ERR_STATE, "no current 2D projection: build it after the last change to the map");
+  const lso::Projection& p = om->projection;
+  const long long cells = p.width * p.height;
+  if (cap < cells || (cells > 0 && !data))
+    return fail(ctx, LS_ERR_ARG, "a buffer of %lld cells for %lld", (long long)cap, cells);
+  CU(cudaSetDevice(ctx->device));
+  const int rc = lso::download_projection(p, data, om->stream);
+  if (rc) return fail(ctx, rc, "2D projection download failed");
   return LS_OK;
 }
 

@@ -28,7 +28,8 @@
 //   (h) oct_emit_kernel      one block per inner brick: (e)'s levels again, its nodes below depth 13 written at the offset
 //                            (g) gave it, so no per-brick staging is kept; one specialisation per format
 // A brick without a known voxel (an insert that failed after placing it leaves one) has state 0 and adds nothing.
-// Leaf lists (DESIGN.md §4b''''''''''''), over the records of a current .ot build, reading them and the map only:
+// Leaf lists (DESIGN.md §4b''''''''''''), over the records of a current .ot build, reading them and the map only; (l1) and
+// (l2), templates over the format, also list the .bt build's leaves for the 2D projection (ls_projection.cu):
 //   (l1) lv_down_kernel      one block: levels 0 ... 12 as (g), each node's leaf offset; leaves above the bricks written
 //   (l2) lv_emit_kernel      one block per inner brick: (e)'s levels again, its leaves placed by a block scan
 //   (l3) lv_compact_kernel   after a CUB scan of the region flags: the kept leaves in order, counts per (state, depth)
@@ -641,11 +642,7 @@ __device__ __forceinline__ int mask8(const unsigned char* s) {
 }
 
 // octomap's keyToCoord(key, depth) of the node whose first voxel key is k0, s = 16 - depth
-__device__ __forceinline__ float leaf_coord(int k0, int s, double res) {
-  const int kc = k0 + (s > 0 ? 1 << (s - 1) : 0);
-  const double scale = (double)(1 << s);
-  return (float)((floor(((double)kc - (double)kKeyOffset) / scale) + 0.5) * (res * scale));
-}
+__device__ __forceinline__ float leaf_coord(int k0, int s, double res) { return (float)leaf_centre_d(k0, s, res); }
 
 __device__ __forceinline__ void put_leaf(float4* cen, unsigned char* dep, unsigned long long i, int kx, int ky, int kz,
                                          int depth, double res) {
@@ -799,6 +796,29 @@ struct BinaryTree {
       put_leaf(cen, dep, l, squeeze3(k) << sh, squeeze3(k >> 1) << sh, squeeze3(k >> 2) << sh, d, res);
     }
     o += N.tot[2][c], l += N.tot[1][c];
+  }
+  // The leaf walk (l1, l2): a leaf record's value is its state (1 free, 2 occupied); a subtree's leaves are its nodes less its
+  // inner nodes (2 payload bytes each).
+  __device__ __forceinline__ static bool walk_leaf(const Nodes& N, int c, unsigned& v) {
+    v = N.st[c];
+    return v == 1 || v == 2;
+  }
+  __device__ __forceinline__ static unsigned long long walk_leaves(const Nodes& N, int c) {
+    return N.tot[0][c] - N.tot[2][c] / 2;
+  }
+  // the leaf of a brick whose first voxel has Morton index t, if any: its depth (0: none) and state
+  __device__ __forceinline__ static int brick_leaf(const Levels& T, int t, unsigned& v) {
+    const int i14 = t >> 6, i15 = t >> 3;
+    int depth = 0;
+    v = 0;
+    if (T.s14[i14] != 3) {
+      if ((t & 63) == 0 && T.s14[i14]) depth = 14, v = T.s14[i14];
+    } else if (T.s15[i15] != 3) {
+      if ((t & 7) == 0 && T.s15[i15]) depth = 15, v = T.s15[i15];
+    } else if (T.s16[t]) {
+      depth = 16, v = T.s16[t];
+    }
+    return depth;
   }
 
   __device__ __forceinline__ static int pair(const unsigned char* pay, int i) {
@@ -991,6 +1011,26 @@ struct FullTree {
     N.off[c] = o;
     if (N.st[c] == 1) put_node(payload + o, N.val[c], 0);
     o += kNodeBytes * N.tot[0][c];
+  }
+  // The leaf walk (l1, l2): a leaf record's value is its log-odds bits.
+  __device__ __forceinline__ static bool walk_leaf(const Nodes& N, int c, unsigned& v) {
+    if (N.st[c] != 1) return false;
+    v = N.val[c];
+    return true;
+  }
+  __device__ __forceinline__ static unsigned long long walk_leaves(const Nodes& N, int c) { return N.tot[1][c]; }
+  __device__ __forceinline__ static int brick_leaf(const Levels& T, int t, unsigned& v) {
+    const int i14 = t >> 6, i15 = t >> 3;
+    int depth = 0;
+    v = 0;
+    if (T.s14[i14] != 3) {
+      if ((t & 63) == 0 && T.s14[i14] == 1) depth = 14, v = T.v14[i14];
+    } else if (T.s15[i15] != 3) {
+      if ((t & 7) == 0 && T.s15[i15] == 1) depth = 15, v = T.v15[i15];
+    } else if (T.s16[t]) {
+      depth = 16, v = T.v16[t];
+    }
+    return depth;
   }
 
   __device__ __forceinline__ static int mask(const unsigned char* pay, int i) { return pay[(size_t)kNodeBytes * i + 4]; }
@@ -1266,11 +1306,31 @@ __device__ __forceinline__ void put_tree_leaf(int kx, int ky, int kz, int depth,
             kz + side - 1 >= R.lo[2];
 }
 
+// What the walk writes per leaf: out(kx, ky, kz, depth, v, i) for the leaf whose first voxel key is (kx, ky, kz) and whose
+// place in pre-order is i, v its value (F::walk_leaf's).  The leaf list writes a box (BoxOut, over a .ot build); the 2D
+// projection a packed key (KeyOut, over a .bt build).
+struct BoxOut {
+  float l_occ;
+  double res;
+  KeyRange R;
+  float4* __restrict__ cen;
+  unsigned char* __restrict__ tag;
+  int* __restrict__ keep;
+  __device__ __forceinline__ void operator()(int kx, int ky, int kz, int depth, unsigned v, unsigned long long i) const {
+    put_tree_leaf(kx, ky, kz, depth, v, l_occ, res, R, i, cen, tag, keep);
+  }
+};
+struct KeyOut {
+  unsigned long long* __restrict__ rec;
+  __device__ __forceinline__ void operator()(int kx, int ky, int kz, int depth, unsigned v, unsigned long long i) const {
+    rec[i] = leaf_record(kx, ky, kz, depth, v == 2);
+  }
+};
+
 // (l1) levels 0 ... 12 as (g): each inner node gives its children their leaf offsets (its own + the earlier siblings'
 // leaves); a leaf child, bricks at depth 13 included, writes itself
-__global__ void __launch_bounds__(kTreeThreads) lv_down_kernel(Nodes N, const int* __restrict__ levels, float l_occ, double res,
-                                                               KeyRange R, float4* __restrict__ cen,
-                                                               unsigned char* __restrict__ tag, int* __restrict__ keep) {
+template <class F, class Out>
+__global__ void __launch_bounds__(kTreeThreads) lv_down_kernel(Nodes N, const int* __restrict__ levels, Out out) {
   const int t = threadIdx.x;
   if (t == 0) N.loff[levels[0]] = 0;
   __syncthreads();
@@ -1281,13 +1341,13 @@ __global__ void __launch_bounds__(kTreeThreads) lv_down_kernel(Nodes N, const in
       unsigned long long l = N.loff[p];
       for (int c = N.first[p]; c < N.end[p]; ++c) {
         N.loff[c] = l;
-        if (N.st[c] == 1) {
+        unsigned v;
+        if (F::walk_leaf(N, c, v)) {
           const unsigned long long k = N.code[c];
           const int sh = 15 - d;
-          put_tree_leaf(squeeze3(k) << sh, squeeze3(k >> 1) << sh, squeeze3(k >> 2) << sh, d + 1, N.val[c], l_occ, res, R, l,
-                        cen, tag, keep);
+          out(squeeze3(k) << sh, squeeze3(k >> 1) << sh, squeeze3(k >> 2) << sh, d + 1, v, l);
         }
-        l += N.tot[1][c];
+        l += F::walk_leaves(N, c);
       }
     }
     __syncthreads();
@@ -1296,33 +1356,26 @@ __global__ void __launch_bounds__(kTreeThreads) lv_down_kernel(Nodes N, const in
 
 // (l2) one block per inner brick: (e)'s levels again; thread t owns the leaf whose first voxel has Morton index t, if
 // any (a depth-14 leaf at t % 64 == 0, a depth-15 one at t % 8 == 0 or voxel t), and a block scan places it
+template <class F, class Out>
 __global__ void __launch_bounds__(512) lv_emit_kernel(const unsigned* __restrict__ known, const float* __restrict__ lo,
                                                       const unsigned long long* __restrict__ bkey, Nodes N, float l_occ,
-                                                      double res, KeyRange R, float4* __restrict__ cen,
-                                                      unsigned char* __restrict__ tag, int* __restrict__ keep) {
+                                                      Out out) {
   using Scan = cub::BlockScan<int, 512>;
-  __shared__ FullTree::Levels T;
+  __shared__ typename F::Levels T;
   __shared__ typename Scan::TempStorage scan;
   const int r = blockIdx.x;
   if (N.st[r] != 3) return;  // a leaf brick is written in (l1)
   const int b = N.pool[r];
-  FullTree::levels(known, lo, b, l_occ, T);
-  const int t = threadIdx.x, i14 = t >> 6, i15 = t >> 3;
-  int depth = 0;
-  unsigned v = 0;
-  if (T.s14[i14] != 3) {
-    if ((t & 63) == 0 && T.s14[i14] == 1) depth = 14, v = T.v14[i14];
-  } else if (T.s15[i15] != 3) {
-    if ((t & 7) == 0 && T.s15[i15] == 1) depth = 15, v = T.v15[i15];
-  } else if (T.s16[t]) {
-    depth = 16, v = T.v16[t];
-  }
+  F::levels(known, lo, b, l_occ, T);
+  const int t = threadIdx.x;
+  unsigned v;
+  const int depth = F::brick_leaf(T, t, v);
   int idx;
   Scan(scan).ExclusiveSum(depth != 0 ? 1 : 0, idx);
   if (depth) {
     int k[3];
     voxel_keys(bkey[b], morton_local(t), k);
-    put_tree_leaf(k[0], k[1], k[2], depth, v, l_occ, res, R, N.loff[r] + (unsigned long long)idx, cen, tag, keep);
+    out(k[0], k[1], k[2], depth, v, N.loff[r] + (unsigned long long)idx);
   }
 }
 
@@ -2234,11 +2287,10 @@ int build_leaves(const Map& m, const Params& P, Octree& t, const int kmin[3], co
   if ((rc = reserve_leaves(L, nl, st))) return rc;
   const KeyRange R{{kmin[0], kmin[1], kmin[2]}, {kmax[0], kmax[1], kmax[2]}};
   const Nodes N = nodes_of(t);
-  lv_down_kernel<<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), P.l_occ, P.res, R, L.raw_c.get(), L.raw_tag.get(),
-                                             L.keep.get());
+  const BoxOut out{P.l_occ, P.res, R, L.raw_c.get(), L.raw_tag.get(), L.keep.get()};
+  lv_down_kernel<FullTree><<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), out);
   LSO_LAUNCHED();
-  lv_emit_kernel<<<t.bricks, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, P.res, R, L.raw_c.get(),
-                                           L.raw_tag.get(), L.keep.get());
+  lv_emit_kernel<FullTree><<<t.bricks, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, out);
   LSO_LAUNCHED();
   size_t bytes = L.cub_bytes;
   LSO_TRY(cub::DeviceScan::ExclusiveSum(L.cub_tmp.get(), bytes, L.keep.get(), L.pos.get(), (int)nl, st));
@@ -2254,6 +2306,17 @@ int build_leaves(const Map& m, const Params& P, Octree& t, const int kmin[3], co
     L.occupied[d] = (long long)L.cnt_host.get()[d], L.free[d] = (long long)L.cnt_host.get()[17 + d];
     L.n_occupied += L.occupied[d], L.n += L.occupied[d] + L.free[d];
   }
+  return LS_OK;
+}
+
+int tree_leaf_records(const Map& m, const Params& P, Octree& t, unsigned long long* rec, cudaStream_t st, uint64_t* launches) {
+  if (t.nodes == 0) return LS_OK;
+  const Nodes N = nodes_of(t);
+  const KeyOut out{rec};
+  lv_down_kernel<BinaryTree><<<1, kTreeThreads, 0, st>>>(N, t.levels.get(), out);
+  LSO_LAUNCHED();
+  lv_emit_kernel<BinaryTree><<<t.bricks, 512, 0, st>>>(m.known.get(), m.lo.get(), m.bkey.get(), N, P.l_occ, out);
+  LSO_LAUNCHED();
   return LS_OK;
 }
 

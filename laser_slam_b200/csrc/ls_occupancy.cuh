@@ -127,6 +127,13 @@ __host__ __device__ __forceinline__ bool key_of(double inv, double c, int& k) {
 // as every output centre is.
 __host__ __device__ __forceinline__ double centre_d(int k, double res) { return ((double)(k - kKeyOffset) + 0.5) * res; }
 __host__ __device__ __forceinline__ float centre_of(int k, double res) { return (float)centre_d(k, res); }
+// octomap's keyToCoord(key, depth) in double of the node whose first voxel key is k0, s = 16 - depth (key + 2^(s-1) is the
+// node's key); at s = 0 it equals centre_d.
+__host__ __device__ __forceinline__ double leaf_centre_d(int k0, int s, double res) {
+  const int kc = k0 + (s > 0 ? 1 << (s - 1) : 0);
+  const double scale = (double)(1 << s);
+  return (floor(((double)kc - (double)kKeyOffset) / scale) + 0.5) * (res * scale);
+}
 
 // The packed key of a voxel: x | y << 16 | z << 32.
 __host__ __device__ __forceinline__ unsigned long long pack(int kx, int ky, int kz) {
@@ -308,6 +315,45 @@ int download_leaves(Leaves& L, int which, float* centres4, unsigned char* tags, 
 // height colour {r, g, b, 1} (min_z < max_z, finite: checked by the caller).
 int marker_cubes(Leaves& L, double min_z, double max_z, double color_factor, float* centres4, float* rgba4, cudaStream_t st,
                  uint64_t* launches);
+
+// A leaf of a tree walk as one word: its first voxel key packed (bits 0 ... 47), its depth (48 ... 55) and 1 when it is
+// occupied (bit 56).
+__host__ __device__ __forceinline__ unsigned long long leaf_record(int kx, int ky, int kz, int depth, bool occupied) {
+  return pack(kx, ky, kz) | ((unsigned long long)depth << 48) | ((unsigned long long)occupied << 56);
+}
+// The leaves of t, which must be the current .bt build of m (TreeFormat::Binary), in pre-order as leaf_record words: rec
+// holds t.nodes - t.bytes / 2 of them (every node less the inner ones).  Reads the map; of t it writes only t.loff, which
+// becomes each node's offset among all leaves (the .bt build leaves its occupied-leaf offsets there, read during the build
+// only, so loff is scratch between builds).  Asynchronous on st.
+int tree_leaf_records(const Map& m, const Params& P, Octree& t, unsigned long long* rec, cudaStream_t st, uint64_t* launches);
+
+// octomap_server's projected_map of the .bt tree (ls_projection.cu; DESIGN.md §4b''''''''''''').  rec / span / off: per
+// leaf, its record, the (leaf, row) spans it paints and their exclusive sum; stat: the ordered bounds (min x, y, z, max x,
+// y, z) and the spans in all; planes: the occupied and known-free bit-planes; grid: the last projection's cells, row j at
+// j * width, written only by a call that succeeds.
+struct Projection {
+  ls::Buffer<unsigned long long> rec, span, off, stat;
+  ls::PinnedBuffer<unsigned long long> stat_host;
+  ls::Buffer<unsigned char> cub_tmp;
+  size_t cub_bytes = 0;
+  ls::Buffer<unsigned> planes;
+  ls::Buffer<signed char> grid;
+  // the last projection: octomap_server's grid geometry and the cells per value (-1, 0, 100)
+  long long width = 0, height = 0, cells[3] = {0, 0, 0};
+  double origin[2] = {0.0, 0.0};
+};
+// The band, padding and map of one projection; the caller checks that the band has no NaN and that min_size is finite and
+// >= 0.
+struct ProjectionArgs {
+  double min_z, max_z, min_size_x, min_size_y;
+};
+// Projects t, the current .bt build of m, into p (synchronous).  LS_ERR_ARG (*why says why) when a padded corner has no key
+// or the grid has more than 2^31 - 1 cells; LS_ERR_NOMEM when its buffers cannot grow.  After any error p's last
+// projection is as it was.
+int build_projection(const Map& m, const Params& P, Octree& t, const ProjectionArgs& a, Projection& p, const char** why,
+                     cudaStream_t st, uint64_t* launches);
+// The last projection's width * height cells.
+int download_projection(const Projection& p, int8_t* cells, cudaStream_t st);
 
 // octomap's readBinary (.bt) or readData (.ot) of a payload (`bytes` bytes after "data\n", `nodes` the header's size) into
 // the map, replacing it (DESIGN.md §4b'''''' and §4b''''''').  P: the map's parameters at the file's resolution (P.l_occ

@@ -2,6 +2,7 @@
 laser_slam::IncrementalEstimator / LaserTrack the way the ROS worker's scanCallback does
 (reference laser_slam_ros/src/laser_slam_worker.cpp:124-173)."""
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -312,6 +313,13 @@ class OccupancyMap:
             L.lsh_occupancy_marker_array.argtypes = [vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, vp, vp, vp, vp,
                                                      i64]
             L.lsh_occupancy_marker_array.restype = i64
+            L.lsh_occupancy_projected_map.argtypes = [vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                                      vp]
+            L.lsh_occupancy_projected_map.restype = i64
+            L.lsh_occupancy_projected_cells.argtypes = [vp, vp, i64]
+            L.lsh_occupancy_projected_cells.restype = i64
+            L.lsh_occupancy_save_projected_map.argtypes = [vp, ctypes.c_char_p, ctypes.c_double, ctypes.c_double,
+                                                           ctypes.c_double, ctypes.c_double]
             L._occ_bound = True
         prm = np.array([resolution, prob_hit, prob_miss, clamp_min, clamp_max, occupancy_threshold, max_range,
                         float(bool(treat_unknown_as_occupied))], np.float64)
@@ -517,6 +525,21 @@ class OccupancyMap:
         lists = [(sizes[k], c[off[k]:off[k + 1]], rgba[off[k]:off[k + 1]] if k < 17 else np.zeros((0, 4), np.float32))
                  for k in range(34)]
         return lists[:17], lists[17:]
+
+    def projected_map(self, min_z=-math.inf, max_z=math.inf, min_x_size=0.0, min_y_size=0.0):
+        """getProjectedMap, called once: (grid int8 (height, width), (width, height, resolution, origin x, origin y))."""
+        geo = np.zeros(5, np.float64)
+        n = self._check(lib().lsh_occupancy_projected_map(self._h, float(min_z), float(max_z), float(min_x_size),
+                                                          float(min_y_size), geo.ctypes.data))
+        grid = np.zeros(max(n, 1), np.int8)
+        lib().lsh_occupancy_projected_cells(self._h, grid.ctypes.data, n)
+        w, h = int(geo[0]), int(geo[1])
+        return grid[:n].reshape(h, w), (w, h, float(geo[2]), float(geo[3]), float(geo[4]))
+
+    def save_projected_map(self, stem, min_z=-math.inf, max_z=math.inf, min_x_size=0.0, min_y_size=0.0):
+        """saveProjectedMap: True when stem.pgm and stem.yaml were written."""
+        return bool(self._check(lib().lsh_occupancy_save_projected_map(self._h, os.fsencode(stem), float(min_z), float(max_z),
+                                                                       float(min_x_size), float(min_y_size))))
 
     def box_status(self, centres, sizes, single=False):
         """The batched getCellStatusBoundingBox overload, or with single=True one call per box: int8 CELL_* per box."""

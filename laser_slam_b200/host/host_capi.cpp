@@ -1,6 +1,7 @@
 // C hooks over the C++ host layer so that tests (ctypes) can drive LaserTrack / IncrementalEstimator exactly the
 // way the ROS worker does (reference laser_slam_ros/src/laser_slam_worker.cpp:124-173): processPoseAndLaserScan,
 // then registerPrior or estimate, then updateFromGTSAMValues.  Not part of the drop-in boundary.
+#include <algorithm>
 #include <cstring>
 #include <memory>
 #include <string>
@@ -384,6 +385,7 @@ int lsh_assembler_add_packet(void* av, const float* pts4, int n, const float* T_
 struct OccupancyHandle {
   std::unique_ptr<OccupancyMap> map;
   std::string err;
+  OccupancyMap::ProjectedMap projected;  // the last getProjectedMap, held for lsh_occupancy_projected_cells
 };
 
 void* lsh_occupancy_create(void* hv, const double* prm, int initial_capacity_bricks, char* err, int errlen) {
@@ -779,6 +781,45 @@ int64_t lsh_occupancy_marker_array(void* ov, double min_z, double max_z, double 
         }
       }
     return n;
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// getProjectedMap of the band (min_z, max_z) padded to min_x_size x min_y_size, kept in the handle; returns width * height
+// and geo5 = {width, height, resolution, origin x, origin y}.  LS_ERR_STATE on an error
+int64_t lsh_occupancy_projected_map(void* ov, double min_z, double max_z, double min_x_size, double min_y_size, double* geo5) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    OccupancyMap::ProjectedMapParams p;
+    p.occupancy_min_z = min_z, p.occupancy_max_z = max_z, p.min_x_size = min_x_size, p.min_y_size = min_y_size;
+    h->map->getProjectedMap(p, &h->projected);
+    const OccupancyMap::ProjectedMap& m = h->projected;
+    geo5[0] = m.width, geo5[1] = m.height, geo5[2] = m.resolution, geo5[3] = m.origin_x, geo5[4] = m.origin_y;
+    return (int64_t)m.data.size();
+  } catch (const std::exception& e) {
+    h->err = e.what();
+    return LS_ERR_STATE;
+  }
+}
+
+// The cells of the last lsh_occupancy_projected_map, written when they fit in cap; returns their number
+int64_t lsh_occupancy_projected_cells(void* ov, int8_t* data, int64_t cap) {
+  const OccupancyHandle* h = static_cast<const OccupancyHandle*>(ov);
+  const int64_t n = (int64_t)h->projected.data.size();
+  if (n <= cap) std::copy(h->projected.data.begin(), h->projected.data.end(), data);
+  return n;
+}
+
+// saveProjectedMap: 1 written, 0 a file could not be written, LS_ERR_STATE on an error
+int lsh_occupancy_save_projected_map(void* ov, const char* stem, double min_z, double max_z, double min_x_size,
+                                     double min_y_size) {
+  OccupancyHandle* h = static_cast<OccupancyHandle*>(ov);
+  try {
+    OccupancyMap::ProjectedMapParams p;
+    p.occupancy_min_z = min_z, p.occupancy_max_z = max_z, p.min_x_size = min_x_size, p.min_y_size = min_y_size;
+    return h->map->saveProjectedMap(stem, p) ? 1 : 0;
   } catch (const std::exception& e) {
     h->err = e.what();
     return LS_ERR_STATE;

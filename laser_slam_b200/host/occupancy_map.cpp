@@ -3,6 +3,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
 #include <stdexcept>
 #include <string>
 #include <tuple>
@@ -229,6 +230,48 @@ void OccupancyMap::generateMarkerArray(double min_z, double max_z, double color_
     }
     for (int64_t i = fre[d]; i < fre[d + 1]; ++i) f.points.push_back(kindr::minimal::Position{c[4 * i], c[4 * i + 1], c[4 * i + 2]});
   }
+}
+
+// ---- 2D projection -------------------------------------------------------------------------------------------------
+void OccupancyMap::getProjectedMap(const ProjectedMapParams& params, ProjectedMap* map) const {
+  if (map == NULL) throw std::invalid_argument("null output");
+  std::lock_guard<std::mutex> lock(mutex_);
+  ls_grid_info info;
+  throwOnError(ctx_,
+               ls_occupancy_build_projection(map_, params.occupancy_min_z, params.occupancy_max_z, params.min_x_size,
+                                             params.min_y_size, &info),
+               "ls_occupancy_build_projection");
+  map->width = (uint32_t)info.width;
+  map->height = (uint32_t)info.height;
+  map->resolution = info.resolution;
+  map->origin_x = info.origin_x;
+  map->origin_y = info.origin_y;
+  map->data.resize((size_t)(info.width * info.height));
+  throwOnError(ctx_, ls_occupancy_download_projection(map_, map->data.data(), (int64_t)map->data.size()),
+               "ls_occupancy_download_projection");
+}
+
+bool OccupancyMap::saveProjectedMap(const std::string& stem, const ProjectedMapParams& params) const {
+  ProjectedMap m;
+  getProjectedMap(params, &m);
+  // map_saver: the message's float32 resolution; rows from the top (j = height - 1) down
+  const float res = (float)m.resolution;
+  const std::string image = stem + ".pgm";
+  FILE* out = std::fopen(image.c_str(), "wb");
+  if (!out) return false;
+  std::fprintf(out, "P5\n# CREATOR: map_saver.cpp %.3f m/pix\n%d %d\n255\n", res, (int)m.width, (int)m.height);
+  for (uint32_t y = 0; y < m.height; ++y)
+    for (uint32_t x = 0; x < m.width; ++x) {
+      const int8_t v = m.data[(size_t)x + (size_t)(m.height - y - 1) * m.width];
+      std::fputc(v == 0 ? 254 : v == 100 ? 0 : 205, out);
+    }
+  bool ok = std::fclose(out) == 0;
+  FILE* yaml = std::fopen((stem + ".yaml").c_str(), "w");
+  if (!yaml) return false;
+  std::fprintf(yaml, "image: %s\nresolution: %f\norigin: [%f, %f, %f]\nnegate: 0\noccupied_thresh: 0.65\nfree_thresh: 0.196\n\n",
+               image.c_str(), res, m.origin_x, m.origin_y, 0.0);
+  ok = std::fclose(yaml) == 0 && ok;
+  return ok;
 }
 
 // ---- queries ------------------------------------------------------------------------------------------------------

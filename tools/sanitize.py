@@ -165,6 +165,12 @@ for r in (None, lreg):
 lcubes = om.marker_cubes(-1.0, 3.0, 0.8)
 assert np.array_equal(np.concatenate([c.colors for c in lcubes.occupied]).view(np.uint32),
                       lbr.marker_cubes(lv, -1.0, 3.0, 0.8)[1].view(np.uint32))
+# the 2D projection of that map (ls_projection.cu and the .bt leaf walk in ls_occupancy.cu): the whole map and a padded
+# band, against the restatement over the map's .bt payload
+import projected_map_ref as pmr
+for band in (dict(), dict(min_z=0.3, max_z=2.0, min_size_x=30.0)):
+    pg_, pi_ = om.projected_map(**band)
+    assert np.array_equal(pg_, pmr.project(pmr.bt_leaves(om.octree().payload), 0.2, **band)[0]) and (pg_ >= 0).any()
 om.clear()
 assert om.size(ls.OCC_KNOWN) == 0
 om.close()
