@@ -920,6 +920,20 @@ class OccupancyMap:
         except Exception:
             pass
 
+    def _sized_output(self, call, *outputs):
+        """The ABI's sized outputs: call(out, cap, n) with no buffers and cap 0 counts them into n (LS_ERR_ARG with n > 0,
+        or OK with n == 0); with n > 0, the call is repeated into new arrays of n rows, one per (dtype, row shape) of
+        outputs.  Returns those arrays."""
+        n = ctypes.c_int64(0)
+        rc = call([None] * len(outputs), 0, ctypes.byref(n))
+        if rc != LS_ERR_ARG or n.value == 0:
+            self.ctx._check(rc)
+        m = n.value
+        arrays = tuple(np.empty((m,) + shape, dtype) for dtype, shape in outputs)
+        if m > 0:
+            self.ctx._check(call([a.ctypes.data for a in arrays], m, ctypes.byref(n)))
+        return arrays
+
     def insert_scan(self, ring, scan_id, T_w_scan):
         """Scan `scan_id` of `ring` at pose T_w_scan (4x4, cast to float32, not corrected).  Returns OccupancyStats."""
         t = colmajor(T_w_scan)
@@ -1154,19 +1168,9 @@ class OccupancyMap:
         in loop order with repeats: (keys uint64, log-odds float32, voxel centres (n,4) float32)."""
         c = np.ascontiguousarray(np.asarray(center, np.float64).reshape(3))
         s = np.ascontiguousarray(np.asarray(size, np.float64).reshape(3))
-        n = ctypes.c_int64(0)
-        rc = lib().ls_occupancy_box_voxels(self._h, c.ctypes.data, s.ctypes.data, int(which), None, None, None, 0,
-                                           ctypes.byref(n))
-        if rc != LS_ERR_ARG or n.value == 0:
-            self.ctx._check(rc)
-        m = n.value
-        keys = np.empty(max(m, 1), np.uint64)
-        lo = np.empty(max(m, 1), np.float32)
-        cen = np.empty((max(m, 1), 4), np.float32)
-        if m > 0:
-            self.ctx._check(lib().ls_occupancy_box_voxels(self._h, c.ctypes.data, s.ctypes.data, int(which), keys.ctypes.data,
-                                                          lo.ctypes.data, cen.ctypes.data, m, ctypes.byref(n)))
-        return keys[:m].copy(), lo[:m].copy(), cen[:m].copy()
+        return self._sized_output(
+            lambda out, cap, n: lib().ls_occupancy_box_voxels(self._h, c.ctypes.data, s.ctypes.data, int(which), *out, cap, n),
+            (np.uint64, ()), (np.float32, ()), (np.float32, (4,)))
 
     def bounds(self):
         """getMetricMin / getMetricMax over the known voxels: (min (3,) float64, max (3,) float64), zeros when empty."""
@@ -1184,22 +1188,11 @@ class OccupancyMap:
         """The voxels whose state (CELL_*) differs from the baseline's, by ascending packed key: (keys uint64, status int8
         now, previous int8 at the baseline, centres (n,4) float32).  reset=True then makes the map the new baseline
         (getChangedPoints followed by resetChangeDetection)."""
-        n = ctypes.c_int64(0)
         self.last_changes = OccupancyChangeStats()
-        rc = lib().ls_occupancy_changes(self._h, None, None, None, None, 0, ctypes.byref(n), int(bool(reset)),
-                                        ctypes.byref(self.last_changes))
-        if rc != LS_ERR_ARG or n.value == 0:
-            self.ctx._check(rc)
-        m = n.value
-        keys = np.empty(max(m, 1), np.uint64)
-        st = np.empty(max(m, 1), np.int8)
-        prev = np.empty(max(m, 1), np.int8)
-        cen = np.empty((max(m, 1), 4), np.float32)
-        if m > 0:
-            self.ctx._check(lib().ls_occupancy_changes(self._h, keys.ctypes.data, st.ctypes.data, prev.ctypes.data,
-                                                       cen.ctypes.data, m, ctypes.byref(n), int(bool(reset)),
-                                                       ctypes.byref(self.last_changes)))
-        return keys[:m].copy(), st[:m].copy(), prev[:m].copy(), cen[:m].copy()
+        return self._sized_output(
+            lambda out, cap, n: lib().ls_occupancy_changes(self._h, *out, cap, n, int(bool(reset)),
+                                                           ctypes.byref(self.last_changes)),
+            (np.uint64, ()), (np.int8, ()), (np.int8, ()), (np.float32, (4,)))
 
     # ---- leaf boxes and marker cubes (ls_occupancy_build_leaves / _download_leaves / _marker_cubes)
     def build_leaves(self, region=None):
@@ -1218,18 +1211,9 @@ class OccupancyMap:
     def download_leaves(self, which=LEAVES_ALL):
         """The last list's leaves of `which` (LEAVES_*) in octomap's leaf order: (centres (n,4) float32, depths uint8,
         states int8 CELL_*)."""
-        n = ctypes.c_int64(0)
-        rc = lib().ls_occupancy_download_leaves(self._h, int(which), None, None, None, 0, ctypes.byref(n))
-        if rc != LS_ERR_ARG or n.value == 0:
-            self.ctx._check(rc)
-        m = n.value
-        cen = np.empty((max(m, 1), 4), np.float32)
-        dep = np.empty(max(m, 1), np.uint8)
-        st = np.empty(max(m, 1), np.int8)
-        if m > 0:
-            self.ctx._check(lib().ls_occupancy_download_leaves(self._h, int(which), cen.ctypes.data, dep.ctypes.data,
-                                                               st.ctypes.data, m, ctypes.byref(n)))
-        return cen[:m].copy(), dep[:m].copy(), st[:m].copy()
+        return self._sized_output(
+            lambda out, cap, n: lib().ls_occupancy_download_leaves(self._h, int(which), *out, cap, n),
+            (np.float32, (4,)), (np.uint8, ()), (np.int8, ()))
 
     def leaf_boxes(self, which=LEAVES_ALL, region=None):
         """getAllFreeBoxes (which=LEAVES_FREE) / getAllOccupiedBoxes (LEAVES_OCCUPIED), or both in one list, optionally
@@ -1246,18 +1230,10 @@ class OccupancyMap:
         carry no colours (an empty (0,4) array).  self.last_leaves holds the build's LeafStats."""
         self.last_leaves = self.build_leaves(region)
         occ_off, free_off = np.zeros(18, np.int64), np.zeros(18, np.int64)
-        n = ctypes.c_int64(0)
-        rc = lib().ls_occupancy_marker_cubes(self._h, float(min_z), float(max_z), float(color_factor), None, None,
-                                             occ_off.ctypes.data, free_off.ctypes.data, 0, ctypes.byref(n))
-        if rc != LS_ERR_ARG or n.value == 0:
-            self.ctx._check(rc)
-        m = n.value
-        cen = np.empty((max(m, 1), 4), np.float32)
-        rgba = np.empty((max(m, 1), 4), np.float32)
-        if m > 0:
-            self.ctx._check(lib().ls_occupancy_marker_cubes(self._h, float(min_z), float(max_z), float(color_factor),
-                                                            cen.ctypes.data, rgba.ctypes.data, occ_off.ctypes.data,
-                                                            free_off.ctypes.data, m, ctypes.byref(n)))
+        cen, rgba = self._sized_output(
+            lambda out, cap, n: lib().ls_occupancy_marker_cubes(self._h, float(min_z), float(max_z), float(color_factor), *out,
+                                                                occ_off.ctypes.data, free_off.ctypes.data, cap, n),
+            (np.float32, (4,)), (np.float32, (4,)))
         res = self.params.resolution
         occ = [CubeList(res * 2.0 ** (16 - d), cen[occ_off[d]:occ_off[d + 1], :3].copy(),
                         rgba[occ_off[d]:occ_off[d + 1]].copy()) for d in range(17)]

@@ -130,6 +130,11 @@ int fail(ls_ctx* ctx, int code, const char* fmt, ...) {
   return code;
 }
 
+// A failed lso:: call (the occupancy map's modules): "<what>: out of device memory" for LS_ERR_NOMEM, else "<what> failed".
+int fail_lso(ls_ctx* ctx, int rc, const char* what) {
+  return fail(ctx, rc, rc == LS_ERR_NOMEM ? "%s: out of device memory" : "%s failed", what);
+}
+
 // the workspaces are single-tenant: nothing that uses them may run between a batch's begin and end
 #define BUSY_CHECK(ctx)                                                                                       \
   do {                                                                                                        \
@@ -1727,25 +1732,61 @@ int ls_local_map_clear(ls_local_map* lm) {
 }  // extern "C"
 
 // ---- resident occupancy map (laser_to_octomap's insertion loop; kernels in ls_occupancy.cu) ------------------------------
+namespace {
+// A stream and the two events that time work on it: start() .. stop(&ms).  The calls return the CUDA status for CU.
+struct DeviceClock {
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  // All three or none: false, with whatever was created destroyed again, when one cannot be created.
+  bool create() {
+    if (cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) == cudaSuccess && cudaEventCreate(&ev0) == cudaSuccess &&
+        cudaEventCreate(&ev1) == cudaSuccess)
+      return true;
+    cudaGetLastError();
+    destroy();
+    return false;
+  }
+  // The stream's work finishes first.
+  void destroy() {
+    if (stream) cudaStreamSynchronize(stream);
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (stream) cudaStreamDestroy(stream);
+    stream = nullptr, ev0 = ev1 = nullptr;
+  }
+  cudaError_t start() { return cudaEventRecord(ev0, stream); }
+  // Waits for the work since start(); *ms: its device time.
+  cudaError_t stop(float* ms) {
+    cudaError_t e = cudaEventRecord(ev1, stream);
+    if (e == cudaSuccess) e = cudaEventSynchronize(ev1);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(ms, ev0, ev1);
+    return e;
+  }
+};
+
+constexpr uint64_t kNoVersion = ~0ull;
+}  // namespace
+
 struct ls_occupancy {
   ls_ctx* ctx = nullptr;
   lso::Params prm{};
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  DeviceClock clock;
   lso::Map map;
-  // The last build of each tree format (indexed by lso::TreeFormat), cached apart; current while it reflects every change
-  // to the map.
+  // Every change to the map increments `version`.  Each cached product below records the version it reflects (kNoVersion:
+  // none) and is current while that equals `version`.
+  uint64_t version = 0;
+  // The last build of each tree format (indexed by lso::TreeFormat), cached apart.
   struct Tree {
     lso::Octree tree;
-    bool current = false;
+    uint64_t version = kNoVersion;
     float ms = 0.f;
   } trees[2];
   lso::Changes changes;  // change detection's baseline and scratch (ls_changes.cu)
   bool tracking = false;
-  lso::Leaves leaves;  // the last leaf list (ls_occupancy_build_leaves), current while it reflects every change to the map
-  bool leaves_current = false;
-  lso::Projection projection;  // the last 2D projection (ls_occupancy_build_projection), current likewise
-  bool projection_current = false;
+  lso::Leaves leaves;  // the last leaf list (ls_occupancy_build_leaves)
+  uint64_t leaves_version = kNoVersion;
+  lso::Projection projection;  // the last 2D projection (ls_occupancy_build_projection)
+  uint64_t projection_version = kNoVersion;
 };
 
 namespace {
@@ -1753,28 +1794,25 @@ using lso::TreeFormat;
 
 ls_occupancy::Tree& tree_of(ls_occupancy* om, TreeFormat f) { return om->trees[(int)f]; }
 
-// A change to the map invalidates both cached builds, the leaf list and the 2D projection.
-void trees_stale(ls_occupancy* om) {
-  for (ls_occupancy::Tree& t : om->trees) t.current = false;
-  om->leaves_current = false;
-  om->projection_current = false;
-}
-
 // The error texts' name of a format: "octree" or "full octree".
 const char* tree_name(TreeFormat f) { return f == TreeFormat::Full ? "full octree" : "octree"; }
 
 int build_tree(ls_occupancy* om, TreeFormat f) {
   ls_ctx* ctx = om->ctx;
   ls_occupancy::Tree& t = tree_of(om, f);
-  t.current = false;
-  CU(cudaEventRecord(om->ev0, om->stream));
-  const int rc = lso::build_tree(om->map, om->prm, f, t.tree, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "%s export: out of device memory" : "%s export failed", tree_name(f));
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
-  CU(cudaEventElapsedTime(&t.ms, om->ev0, om->ev1));
-  t.current = true;
+  t.version = kNoVersion;
+  CU(om->clock.start());
+  const int rc = lso::build_tree(om->map, om->prm, f, t.tree, om->clock.stream, &ctx->launches);
+  if (rc) return fail_lso(ctx, rc, f == TreeFormat::Full ? "full octree export" : "octree export");
+  CU(om->clock.stop(&t.ms));
+  t.version = om->version;
   return LS_OK;
+}
+
+// Makes the build of format f current, building it now unless it already is; *built: whether it was built now.
+int current_tree(ls_occupancy* om, TreeFormat f, bool* built) {
+  *built = tree_of(om, f).version != om->version;
+  return *built ? build_tree(om, f) : LS_OK;
 }
 
 void full_stats(const ls_occupancy* om, ls_full_octree_stats* stats) {
@@ -1857,7 +1895,7 @@ const char* parse_bt_header(const std::vector<uint8_t>& d, size_t* off, long lon
 int download_tree(ls_occupancy* om, TreeFormat f, uint8_t* payload, int64_t payload_cap, float* centres4, uint8_t* depths,
                   int64_t leaf_cap) {
   ls_ctx* ctx = om->ctx;
-  if (!tree_of(om, f).current)
+  if (tree_of(om, f).version != om->version)
     return fail(ctx, LS_ERR_STATE, f == TreeFormat::Full ? "no current full octree: build it after the last insert or read"
                                                          : "no current octree: build it after the last insert");
   const lso::Octree& t = tree_of(om, f).tree;
@@ -1866,7 +1904,7 @@ int download_tree(ls_occupancy* om, TreeFormat f, uint8_t* payload, int64_t payl
   if ((centres4 || depths) && leaf_cap < t.leaves)
     return fail(ctx, LS_ERR_ARG, "leaf buffers of %lld for %lld occupied leaves", (long long)leaf_cap, t.leaves);
   CU(cudaSetDevice(ctx->device));
-  const int rc = lso::download_octree(t, payload, centres4, depths, om->stream);
+  const int rc = lso::download_octree(t, payload, centres4, depths, om->clock.stream);
   if (rc) return fail(ctx, rc, "%s download failed", tree_name(f));
   return LS_OK;
 }
@@ -1876,11 +1914,12 @@ int write_tree(ls_occupancy* om, TreeFormat f, const char* path) {
   ls_ctx* ctx = om->ctx;
   if (!path) return fail(ctx, LS_ERR_ARG, "bad argument");
   CU(cudaSetDevice(ctx->device));
-  ls_occupancy::Tree& t = tree_of(om, f);
-  int rc;
-  if (!t.current && (rc = build_tree(om, f))) return rc;
+  bool built;
+  int rc = current_tree(om, f, &built);
+  if (rc) return rc;
+  const ls_occupancy::Tree& t = tree_of(om, f);
   std::vector<uint8_t> payload((size_t)t.tree.bytes);
-  if ((rc = lso::download_octree(t.tree, payload.data(), nullptr, nullptr, om->stream)))
+  if ((rc = lso::download_octree(t.tree, payload.data(), nullptr, nullptr, om->clock.stream)))
     return fail(ctx, rc, "%s download failed", tree_name(f));
   // the resolution as a default std::ostream prints a double (%g)
   char head[256];
@@ -1905,22 +1944,20 @@ int read_tree(ls_occupancy* om, TreeFormat f, const uint8_t* payload, int64_t pa
   if (!(resolution > 0.0) || !std::isfinite(resolution))
     return fail(ctx, LS_ERR_ARG, "octomap resolution %g (finite and > 0)", resolution);
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   lso::Params P = om->prm;
   P.res = resolution;
   P.inv = 1.0 / resolution;
   lso::ReadCounters c;
   const char* why = "";
-  const int rc = lso::read_tree(om->map, P, f, payload, payload_bytes, nodes, &c, &why, om->stream, &ctx->launches);
+  const int rc = lso::read_tree(om->map, P, f, payload, payload_bytes, nodes, &c, &why, om->clock.stream, &ctx->launches);
   if (rc)
     return fail(ctx, rc, "octomap %sread refused, the map is unchanged: %s", f == TreeFormat::Full ? "full tree " : "", why);
   om->prm = P;
-  trees_stale(om);
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
+  ++om->version;
+  float ms = 0.f;
+  CU(om->clock.stop(&ms));
   if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
     stats->nodes = (int64_t)c.nodes;
     stats->inner_nodes = (int64_t)c.inner;
     stats->free_leaves = (int64_t)c.free_leaves;
@@ -1979,13 +2016,7 @@ int ls_occupancy_create(ls_ctx* ctx, const ls_occupancy_params* params, ls_occup
                         logodds(p.clamp_min), logodds(p.clamp_max), logodds(p.occupancy_threshold)};
   int bricks = 32768;
   if (p.initial_capacity > 0) bricks = p.initial_capacity < (1 << 24) ? p.initial_capacity : (1 << 24);
-  int rc = LS_OK;
-  if (cudaStreamCreateWithFlags(&om->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreate(&om->ev0) != cudaSuccess || cudaEventCreate(&om->ev1) != cudaSuccess) {
-    cudaGetLastError();
-    rc = LS_ERR_NOMEM;
-  }
-  if (!rc) rc = lso::init(om->map, bricks, om->stream);
+  const int rc = om->clock.create() ? lso::init(om->map, bricks, om->clock.stream) : LS_ERR_NOMEM;
   if (rc) {
     ls_occupancy_destroy(om);
     return fail(ctx, rc, "occupancy map creation failed");
@@ -1997,10 +2028,7 @@ int ls_occupancy_create(ls_ctx* ctx, const ls_occupancy_params* params, ls_occup
 void ls_occupancy_destroy(ls_occupancy* om) {
   if (!om) return;
   cudaSetDevice(om->ctx->device);
-  if (om->stream) cudaStreamSynchronize(om->stream);
-  if (om->ev0) cudaEventDestroy(om->ev0);
-  if (om->ev1) cudaEventDestroy(om->ev1);
-  if (om->stream) cudaStreamDestroy(om->stream);
+  om->clock.destroy();
   delete om;
 }
 
@@ -2014,18 +2042,16 @@ int ls_occupancy_insert_scan(ls_occupancy* om, const ls_map* ring, uint64_t scan
   CU(cudaSetDevice(ctx->device));
   const ls_scan_slot* s = find_slot(ring, scan_id);
   if (!s) return fail(ctx, LS_ERR_STATE, "scan %llu is not resident (evicted or never pushed)", (unsigned long long)scan_id);
-  if (wait_slot(s, om->stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
-  CU(cudaEventRecord(om->ev0, om->stream));
-  trees_stale(om);
+  if (wait_slot(s, om->clock.stream) != LS_OK) return fail(ctx, LS_ERR_CUDA, "cudaStreamWaitEvent failed");
+  CU(om->clock.start());
+  ++om->version;  // before the insert: a failed one may have changed voxels
   lso::Counters c;
-  const int rc = lso::insert(om->map, om->prm, s->pts.get(), s->n, T_w_scan, is_identity16(T_w_scan), om->stream, &c,
-                             &ctx->launches);
+  const int rc = lso::insert(om->map, om->prm, s->pts.get(), s->n, T_w_scan, is_identity16(T_w_scan), om->clock.stream,
+                             &c, &ctx->launches);
   if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "occupancy map growth failed" : "occupancy map insert failed");
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
+  float ms = 0.f;
+  CU(om->clock.stop(&ms));
   if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
     stats->rays_cast = c.rays_cast;
     stats->rays_skipped = c.rays_skipped;
     stats->free_updates = (int64_t)c.free_upd;
@@ -2044,7 +2070,7 @@ int ls_occupancy_size(ls_occupancy* om, int which, int64_t* n) {
   if (!n || (which != LS_OCC_KNOWN && which != LS_OCC_OCCUPIED)) return fail(ctx, LS_ERR_ARG, "bad argument");
   CU(cudaSetDevice(ctx->device));
   long long m = 0;
-  const int rc = lso::count(om->map, om->prm, which, &m, om->stream, &ctx->launches);
+  const int rc = lso::count(om->map, om->prm, which, &m, om->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "occupancy map count failed");
   *n = m;
   return LS_OK;
@@ -2057,10 +2083,10 @@ int ls_occupancy_download(ls_occupancy* om, int which, uint64_t* keys, float* lo
   if (!n || (which != LS_OCC_KNOWN && which != LS_OCC_OCCUPIED)) return fail(ctx, LS_ERR_ARG, "bad argument");
   CU(cudaSetDevice(ctx->device));
   long long m = 0;
-  int rc = lso::count(om->map, om->prm, which, &m, om->stream, &ctx->launches);
+  int rc = lso::count(om->map, om->prm, which, &m, om->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "occupancy map count failed");
   if (m > cap) return fail(ctx, LS_ERR_ARG, "buffers of %lld voxels for %lld", (long long)cap, m);
-  rc = lso::download(om->map, om->prm, which, m, keys, log_odds, centres4, om->stream, &ctx->launches);
+  rc = lso::download(om->map, om->prm, which, m, keys, log_odds, centres4, om->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "occupancy map download failed");
   *n = m;
   return LS_OK;
@@ -2134,14 +2160,12 @@ int ls_occupancy_read_octomap_full(ls_occupancy* om, const char* path, ls_octoma
 }  // extern "C"
 
 namespace {
-// The query's device time (ev0 .. ev1 around it on the map's stream) and its keys visited into *stats.
+// The query's device time (the map's clock, started before it) and its keys visited into *stats.
 int query_done(ls_occupancy* om, long long visited, ls_occupancy_query_stats* stats) {
   ls_ctx* ctx = om->ctx;
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
+  float ms = 0.f;
+  CU(om->clock.stop(&ms));
   if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
     stats->keys_visited = visited;
     stats->device_ms = ms;
   }
@@ -2162,10 +2186,10 @@ int ls_occupancy_cell_status(ls_occupancy* om, const double* points3, int n, int
   if (n < 0 || (n > 0 && (!points3 || !status))) return fail(ctx, LS_ERR_ARG, "bad argument");
   if (n == 0) return query_none(stats), LS_OK;
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   long long visited = 0;
-  const int rc = lso::query_cells(om->map, om->prm, points3, n, status, log_odds, &visited, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "cell query: out of device memory" : "cell query failed");
+  const int rc = lso::query_cells(om->map, om->prm, points3, n, status, log_odds, &visited, om->clock.stream, &ctx->launches);
+  if (rc) return fail_lso(ctx, rc, "cell query");
   return query_done(om, visited, stats);
 }
 
@@ -2180,12 +2204,12 @@ int ls_occupancy_line_status(ls_occupancy* om, const double* starts3, const doub
         return fail(ctx, LS_ERR_ARG, "bounding box size %g on axis %d (finite and >= 0)", box3[a], a);
   if (n == 0) return query_none(stats), LS_OK;
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   long long visited = 0;
   const int rc = lso::query_lines(om->map, om->prm, starts3, ends3, n, box3, stop_at_unknown, status, first_keys, &visited,
-                                  om->stream, &ctx->launches);
+                                  om->clock.stream, &ctx->launches);
   if (rc == LS_ERR_ARG) return fail(ctx, rc, "%d segments with this bounding box make more than 2^31 - 1 lines", n);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "line query: out of device memory" : "line query failed");
+  if (rc) return fail_lso(ctx, rc, "line query");
   return query_done(om, visited, stats);
 }
 
@@ -2196,11 +2220,11 @@ int ls_occupancy_cast_rays(ls_occupancy* om, const float* origins3, const float*
   if (n < 0 || (n > 0 && (!origins3 || !directions3 || !result))) return fail(ctx, LS_ERR_ARG, "bad argument");
   if (n == 0) return query_none(stats), LS_OK;
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   long long visited = 0;
   const int rc = lso::query_rays(om->map, om->prm, origins3, directions3, n, ignore_unknown, max_range, result, ends3, &visited,
-                                 om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "ray query: out of device memory" : "ray query failed");
+                                 om->clock.stream, &ctx->launches);
+  if (rc) return fail_lso(ctx, rc, "ray query");
   return query_done(om, visited, stats);
 }
 
@@ -2211,13 +2235,13 @@ int ls_occupancy_box_status(ls_occupancy* om, const double* centres3, const doub
   if (n < 0 || (n > 0 && (!centres3 || !sizes3 || !status))) return fail(ctx, LS_ERR_ARG, "bad argument");
   if (n == 0) return query_none(stats), LS_OK;
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   long long visited = 0;
-  const int rc = lso::box_status(om->map, om->prm, centres3, sizes3, n, status, &visited, om->stream, &ctx->launches);
+  const int rc = lso::box_status(om->map, om->prm, centres3, sizes3, n, status, &visited, om->clock.stream, &ctx->launches);
   if (rc == LS_ERR_ARG)
     return fail(ctx, rc, "box status refused: a size is negative or not finite, a box axis has more than 2^17 loop points, "
                          "or the boxes span more than 2^36 (box, brick) items");
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "box status: out of device memory" : "box status failed");
+  if (rc) return fail_lso(ctx, rc, "box status");
   return query_done(om, visited, stats);
 }
 
@@ -2238,14 +2262,14 @@ int ls_occupancy_check_paths(ls_occupancy* om, const double* positions3, const i
   if (offsets[n_paths] > 0x7fffffffLL) return fail(ctx, LS_ERR_ARG, "%lld poses (at most 2^31 - 1)", (long long)offsets[n_paths]);
   if (offsets[n_paths] > 0 && !positions3) return fail(ctx, LS_ERR_ARG, "bad argument");
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   long long visited = 0;
   const int rc = lso::check_paths(om->map, om->prm, positions3, offsets, n_paths, robot_size3, unknown_as_occupied,
-                                  first_collision, &visited, om->stream, &ctx->launches);
+                                  first_collision, &visited, om->clock.stream, &ctx->launches);
   if (rc == LS_ERR_ARG)
     return fail(ctx, rc, "path check refused: the robot box has more than 2^17 loop points on an axis, or the poses span "
                          "more than 2^36 (box, brick) items");
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "path check: out of device memory" : "path check failed");
+  if (rc) return fail_lso(ctx, rc, "path check");
   return query_done(om, visited, stats);
 }
 
@@ -2274,18 +2298,16 @@ int ls_occupancy_set_boxes(ls_occupancy* om, const double* centres3, const doubl
     if (why) return fail(ctx, LS_ERR_ARG, "box %d: %s", i, why);
   }
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   long long set = 0, added = 0;
   const char* why = "";
-  const int rc = lso::set_boxes(om->map, om->prm, centres3, sizes3, occupied, n, &set, &added, &why, om->stream,
+  const int rc = lso::set_boxes(om->map, om->prm, centres3, sizes3, occupied, n, &set, &added, &why, om->clock.stream,
                                 &ctx->launches);
   if (rc) return fail(ctx, rc, "set boxes refused, the map's voxels are unchanged: %s", why);
-  if (set > 0) trees_stale(om);
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
+  if (set > 0) ++om->version;
+  float ms = 0.f;
+  CU(om->clock.stop(&ms));
   if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
     stats->voxels_set = set;
     stats->new_known = added;
     stats->known_voxels = om->map.n_known;
@@ -2300,8 +2322,8 @@ int ls_occupancy_clear(ls_occupancy* om) {
   if (!om) return LS_ERR_ARG;
   ls_ctx* ctx = om->ctx;
   CU(cudaSetDevice(ctx->device));
-  const int rc = lso::clear(om->map, om->stream);
-  trees_stale(om);
+  const int rc = lso::clear(om->map, om->clock.stream);
+  ++om->version;
   if (rc) return fail(ctx, rc, "occupancy map reset failed");
   return LS_OK;
 }
@@ -2318,12 +2340,12 @@ int ls_occupancy_box_voxels(ls_occupancy* om, const double center3[3], const dou
   if (why) return fail(ctx, LS_ERR_ARG, "%s", why);
   CU(cudaSetDevice(ctx->device));
   long long m = 0;
-  const int rc = lso::box_voxels(om->map, om->prm, center3, size3, which, keys, log_odds, centres4, cap, &m, om->stream,
+  const int rc = lso::box_voxels(om->map, om->prm, center3, size3, which, keys, log_odds, centres4, cap, &m, om->clock.stream,
                                  &ctx->launches);
   *n = m;
   if (rc == LS_ERR_ARG && m > cap) return fail(ctx, rc, "buffers of %lld voxels for %lld", (long long)cap, m);
   if (rc == LS_ERR_ARG) return fail(ctx, rc, "the box has more than 2^17 loop points on an axis or 2^31 - 1 in all");
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "box voxels: out of device memory" : "box voxels failed");
+  if (rc) return fail_lso(ctx, rc, "box voxels");
   return LS_OK;
 }
 
@@ -2334,8 +2356,8 @@ int ls_occupancy_bounds(ls_occupancy* om, double min3[3], double max3[3]) {
   CU(cudaSetDevice(ctx->device));
   int kmin[3], kmax[3];
   bool empty = true;
-  const int rc = lso::key_bounds(om->map, kmin, kmax, &empty, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "bounds: out of device memory" : "bounds failed");
+  const int rc = lso::key_bounds(om->map, kmin, kmax, &empty, om->clock.stream, &ctx->launches);
+  if (rc) return fail_lso(ctx, rc, "bounds");
   const double res = om->prm.res;
   for (int a = 0; a < 3; ++a) {
     // octomap's calcMinMax over depth-16 leaves: the lower corner, and the lower corner plus the voxel size
@@ -2372,25 +2394,23 @@ int ls_occupancy_build_leaves(ls_occupancy* om, const double* region_min3, const
     }
   }
   CU(cudaSetDevice(ctx->device));
-  om->leaves_current = false;
+  om->leaves_version = kNoVersion;
+  bool built;
+  int rc = current_tree(om, TreeFormat::Full, &built);
+  if (rc) return rc;
   ls_occupancy::Tree& t = tree_of(om, TreeFormat::Full);
-  const bool build = !t.current;
-  int rc;
-  if (build && (rc = build_tree(om, TreeFormat::Full))) return rc;
-  CU(cudaEventRecord(om->ev0, om->stream));
-  rc = lso::build_leaves(om->map, om->prm, t.tree, kmin, kmax, om->leaves, om->stream, &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "leaf list: out of device memory" : "leaf list failed");
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
-  om->leaves_current = true;
+  CU(om->clock.start());
+  rc = lso::build_leaves(om->map, om->prm, t.tree, kmin, kmax, om->leaves, om->clock.stream, &ctx->launches);
+  if (rc) return fail_lso(ctx, rc, "leaf list");
+  float ms = 0.f;
+  CU(om->clock.stop(&ms));
+  om->leaves_version = om->version;
   if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
     const lso::Leaves& L = om->leaves;
     stats->free_leaves = L.n - L.n_occupied;
     stats->occupied_leaves = L.n_occupied;
     for (int d = 0; d < 17; ++d) stats->free_by_depth[d] = L.free[d], stats->occupied_by_depth[d] = L.occupied[d];
-    stats->device_ms = ms + (build ? t.ms : 0.f);
+    stats->device_ms = ms + (built ? t.ms : 0.f);
   }
   return LS_OK;
 }
@@ -2404,7 +2424,8 @@ int ls_occupancy_download_leaves(ls_occupancy* om, int which, float* centres4, u
   if (cap < 0 || (which != LS_LEAVES_FREE && which != LS_LEAVES_OCCUPIED && which != LS_LEAVES_ALL) ||
       (cap > 0 && (!centres4 || !depths || !states)))
     return fail(ctx, LS_ERR_ARG, "bad argument");
-  if (!om->leaves_current) return fail(ctx, LS_ERR_STATE, "no current leaf list: build it after the last change to the map");
+  if (om->leaves_version != om->version)
+    return fail(ctx, LS_ERR_STATE, "no current leaf list: build it after the last change to the map");
   const lso::Leaves& L = om->leaves;
   const long long m = which == LS_LEAVES_ALL ? L.n : which == LS_LEAVES_OCCUPIED ? L.n_occupied : L.n - L.n_occupied;
   *n = m;
@@ -2412,7 +2433,7 @@ int ls_occupancy_download_leaves(ls_occupancy* om, int which, float* centres4, u
   if (m == 0) return LS_OK;
   CU(cudaSetDevice(ctx->device));
   std::vector<uint8_t> tags((size_t)m);
-  const int rc = lso::download_leaves(om->leaves, which, centres4, tags.data(), om->stream, &ctx->launches);
+  const int rc = lso::download_leaves(om->leaves, which, centres4, tags.data(), om->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "leaf download failed");
   for (long long i = 0; i < m; ++i) {
     depths[i] = tags[i] & 31;
@@ -2433,7 +2454,8 @@ int ls_occupancy_marker_cubes(ls_occupancy* om, double min_z, double max_z, doub
       !std::isfinite(max_z - min_z))
     return fail(ctx, LS_ERR_ARG, "colour arguments min_z %g, max_z %g, color_factor %g (finite, min_z < max_z)", min_z, max_z,
                 color_factor);
-  if (!om->leaves_current) return fail(ctx, LS_ERR_STATE, "no current leaf list: build it after the last change to the map");
+  if (om->leaves_version != om->version)
+    return fail(ctx, LS_ERR_STATE, "no current leaf list: build it after the last change to the map");
   const lso::Leaves& L = om->leaves;
   occupied_offsets[0] = 0;
   for (int d = 0; d < 17; ++d) occupied_offsets[d + 1] = occupied_offsets[d] + L.occupied[d];
@@ -2442,7 +2464,7 @@ int ls_occupancy_marker_cubes(ls_occupancy* om, double min_z, double max_z, doub
   *n = free_offsets[17];
   if (*n > cap) return fail(ctx, LS_ERR_ARG, "buffers of %lld cubes for %lld", (long long)cap, (long long)*n);
   CU(cudaSetDevice(ctx->device));
-  const int rc = lso::marker_cubes(om->leaves, min_z, max_z, color_factor, centres4, colors4, om->stream, &ctx->launches);
+  const int rc = lso::marker_cubes(om->leaves, min_z, max_z, color_factor, centres4, colors4, om->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "marker cubes failed");
   return LS_OK;
 }
@@ -2456,41 +2478,41 @@ int ls_occupancy_build_projection(ls_occupancy* om, double min_z, double max_z, 
   if (!std::isfinite(min_size_x) || !std::isfinite(min_size_y) || min_size_x < 0.0 || min_size_y < 0.0)
     return fail(ctx, LS_ERR_ARG, "minimum size %g x %g (finite, >= 0)", min_size_x, min_size_y);
   CU(cudaSetDevice(ctx->device));
+  // The projection's version is not reset first: on a failure here or in the .bt build, the last projection stays as it
+  // was, and current if it was.
+  bool built;
+  int rc = current_tree(om, TreeFormat::Binary, &built);
+  if (rc) return rc;
   ls_occupancy::Tree& t = tree_of(om, TreeFormat::Binary);
-  const bool build = !t.current;
-  int rc;
-  if (build && (rc = build_tree(om, TreeFormat::Binary))) return rc;
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   const char* why = "";
   rc = lso::build_projection(om->map, om->prm, t.tree, lso::ProjectionArgs{min_z, max_z, min_size_x, min_size_y},
-                             om->projection, &why, om->stream, &ctx->launches);
+                             om->projection, &why, om->clock.stream, &ctx->launches);
   if (rc == LS_ERR_ARG || (rc == LS_ERR_NOMEM && *why)) return fail(ctx, rc, "2D projection: %s", why);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "2D projection: out of device memory" : "2D projection failed");
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
-  om->projection_current = true;
+  if (rc) return fail_lso(ctx, rc, "2D projection");
   float ms = 0.f;
-  CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
+  CU(om->clock.stop(&ms));
+  om->projection_version = om->version;
   const lso::Projection& p = om->projection;
   info->width = p.width, info->height = p.height;
   info->resolution = om->prm.res;
   info->origin_x = p.origin[0], info->origin_y = p.origin[1];
   info->unknown_cells = p.cells[0], info->free_cells = p.cells[1], info->occupied_cells = p.cells[2];
-  info->device_ms = ms + (build ? t.ms : 0.f);
+  info->device_ms = ms + (built ? t.ms : 0.f);
   return LS_OK;
 }
 
 int ls_occupancy_download_projection(ls_occupancy* om, int8_t* data, int64_t cap) {
   if (!om) return LS_ERR_ARG;
   ls_ctx* ctx = om->ctx;
-  if (!om->projection_current)
+  if (om->projection_version != om->version)
     return fail(ctx, LS_ERR_STATE, "no current 2D projection: build it after the last change to the map");
   const lso::Projection& p = om->projection;
   const long long cells = p.width * p.height;
   if (cap < cells || (cells > 0 && !data))
     return fail(ctx, LS_ERR_ARG, "a buffer of %lld cells for %lld", (long long)cap, cells);
   CU(cudaSetDevice(ctx->device));
-  const int rc = lso::download_projection(p, data, om->stream);
+  const int rc = lso::download_projection(p, data, om->clock.stream);
   if (rc) return fail(ctx, rc, "2D projection download failed");
   return LS_OK;
 }
@@ -2500,12 +2522,12 @@ int ls_occupancy_track_changes(ls_occupancy* om, int enable) {
   ls_ctx* ctx = om->ctx;
   CU(cudaSetDevice(ctx->device));
   if (!enable) {
-    CU(cudaStreamSynchronize(om->stream));
+    CU(cudaStreamSynchronize(om->clock.stream));
     lso::release_changes(om->changes);
     om->tracking = false;
     return LS_OK;
   }
-  const int rc = lso::capture_baseline(om->changes, om->map, om->prm, om->stream, &ctx->launches);
+  const int rc = lso::capture_baseline(om->changes, om->map, om->prm, om->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "change detection: out of device memory for the baseline" :
                                                     "change detection: baseline capture failed");
   om->tracking = true;
@@ -2521,22 +2543,20 @@ int ls_occupancy_changes(ls_occupancy* om, uint64_t* keys, int8_t* status, int8_
   if (cap < 0) return fail(ctx, LS_ERR_ARG, "bad argument");
   if (!om->tracking) return fail(ctx, LS_ERR_STATE, "change detection is off: enable it with ls_occupancy_track_changes");
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(om->ev0, om->stream));
+  CU(om->clock.start());
   const long long compared = (long long)om->map.pool_n + om->changes.base.n;
   long long m = 0;
-  int rc = lso::diff_changes(om->changes, om->map, om->prm, keys, status, previous, centres4, cap, &m, om->stream,
+  int rc = lso::diff_changes(om->changes, om->map, om->prm, keys, status, previous, centres4, cap, &m, om->clock.stream,
                              &ctx->launches);
   *n = m;
   if (rc == LS_ERR_ARG) return fail(ctx, rc, "buffers of %lld changes for %lld", (long long)cap, m);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "changes: out of device memory" : "changes failed");
-  if (reset && (rc = lso::capture_baseline(om->changes, om->map, om->prm, om->stream, &ctx->launches)))
+  if (rc) return fail_lso(ctx, rc, "changes");
+  if (reset && (rc = lso::capture_baseline(om->changes, om->map, om->prm, om->clock.stream, &ctx->launches)))
     return fail(ctx, rc, rc == LS_ERR_NOMEM ? "changes copied, the reset is refused: out of device memory for the baseline"
                                             : "changes copied, the reset failed");
-  CU(cudaEventRecord(om->ev1, om->stream));
-  CU(cudaEventSynchronize(om->ev1));
+  float ms = 0.f;
+  CU(om->clock.stop(&ms));
   if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, om->ev0, om->ev1));
     stats->bricks_compared = compared;
     stats->changed = m;
     stats->baseline_bricks = om->changes.base.n;
@@ -2552,8 +2572,7 @@ int ls_occupancy_changes(ls_occupancy* om, uint64_t* keys, int8_t* status, int8_
 struct ls_distance_map {
   ls_ctx* ctx = nullptr;
   ls_distance_map_params prm{};
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  DeviceClock clock;
   lso::DistanceField field;
   bool has_field = false;
   float max_dist = 0.f;  // getMaxDist of the field
@@ -2593,9 +2612,7 @@ int ls_distance_map_create(ls_ctx* ctx, const ls_distance_map_params* params, ls
   ls_distance_map* dm = new ls_distance_map();
   dm->ctx = ctx;
   dm->prm = p;
-  if (cudaStreamCreateWithFlags(&dm->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreate(&dm->ev0) != cudaSuccess || cudaEventCreate(&dm->ev1) != cudaSuccess) {
-    cudaGetLastError();
+  if (!dm->clock.create()) {
     ls_distance_map_destroy(dm);
     return fail(ctx, LS_ERR_NOMEM, "distance map creation failed");
   }
@@ -2606,10 +2623,7 @@ int ls_distance_map_create(ls_ctx* ctx, const ls_distance_map_params* params, ls
 void ls_distance_map_destroy(ls_distance_map* dm) {
   if (!dm) return;
   cudaSetDevice(dm->ctx->device);
-  if (dm->stream) cudaStreamSynchronize(dm->stream);
-  if (dm->ev0) cudaEventDestroy(dm->ev0);
-  if (dm->ev1) cudaEventDestroy(dm->ev1);
-  if (dm->stream) cudaStreamDestroy(dm->stream);
+  dm->clock.destroy();
   delete dm;
 }
 
@@ -2644,14 +2658,12 @@ int ls_distance_map_update(ls_distance_map* dm, ls_occupancy* om, ls_distance_ma
   f.res = res, f.inv = inv;
   f.M = m * m;
   dm->max_dist = (float)(m * res);
-  CU(cudaEventRecord(dm->ev0, dm->stream));
-  rc = lso::distance_update(f, om->map, om->prm.l_occ, p.treat_unknown_as_occupied != 0, dm->stream, &ctx->launches);
+  CU(dm->clock.start());
+  rc = lso::distance_update(f, om->map, om->prm.l_occ, p.treat_unknown_as_occupied != 0, dm->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "distance map update failed");
-  CU(cudaEventRecord(dm->ev1, dm->stream));
-  CU(cudaEventSynchronize(dm->ev1));
-  dm->has_field = true;
   float ms = 0.f;
-  CU(cudaEventElapsedTime(&ms, dm->ev0, dm->ev1));
+  CU(dm->clock.stop(&ms));
+  dm->has_field = true;
   distance_stats(dm, ms, stats);
   return LS_OK;
 }
@@ -2663,16 +2675,14 @@ int ls_distance_map_query(ls_distance_map* dm, const float* points3, int n, floa
   if (n < 0 || (n > 0 && !points3)) return fail(ctx, LS_ERR_ARG, "bad argument");
   if (!dm->has_field) return fail(ctx, LS_ERR_STATE, "the distance map has no field: update it first");
   CU(cudaSetDevice(ctx->device));
-  CU(cudaEventRecord(dm->ev0, dm->stream));
+  CU(dm->clock.start());
   long long outside = 0;
-  const int rc = lso::distance_query(dm->field, points3, n, distance, sqdist_cells, obstacles3, &outside, dm->stream,
+  const int rc = lso::distance_query(dm->field, points3, n, distance, sqdist_cells, obstacles3, &outside, dm->clock.stream,
                                      &ctx->launches);
-  if (rc) return fail(ctx, rc, rc == LS_ERR_NOMEM ? "distance query: out of device memory" : "distance query failed");
-  CU(cudaEventRecord(dm->ev1, dm->stream));
-  CU(cudaEventSynchronize(dm->ev1));
+  if (rc) return fail_lso(ctx, rc, "distance query");
+  float ms = 0.f;
+  CU(dm->clock.stop(&ms));
   if (stats) {
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, dm->ev0, dm->ev1));
     stats->outside = outside;
     stats->device_ms = ms;
   }
@@ -2689,7 +2699,7 @@ int ls_distance_map_download(ls_distance_map* dm, int32_t* sqdist, uint64_t* obs
   if (cap_cells < dm->field.cells)
     return fail(ctx, LS_ERR_ARG, "buffers of %lld cells for %lld", (long long)cap_cells, dm->field.cells);
   CU(cudaSetDevice(ctx->device));
-  const int rc = lso::distance_download(dm->field, sqdist, obstacle_keys, dm->stream, &ctx->launches);
+  const int rc = lso::distance_download(dm->field, sqdist, obstacle_keys, dm->clock.stream, &ctx->launches);
   if (rc) return fail(ctx, rc, "distance map download failed");
   return LS_OK;
 }
